@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """bench.py -- L-BFGS iterations/s (and apply_Hv HBM GB/s) on the BASELINE configs, default config 2:
-paired Rosenbrock, n = 1e7, fp64, m = 10, More-Thuente line search, x0 = 0, on N B200s.
+paired Rosenbrock, n = 1e7, fp64, m = 10, More-Thuente line search, x0 = 0, on N H100s.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config c2|c3|c4|c5] [--solver-loop resident|host]
+                  [--dump-outputs DIR]
   (N > 1: launched under torchrun, one rank per GPU; c2/c3: n is sharded over the ranks ("strong" scaling);
    c5: --sharding problems (default; ranks take whole problems, no communication) or n (every problem split along n);
    c4: replicas only, N = 1)
@@ -14,6 +15,8 @@ device-resident solve: ONE persistent kernel launch per minimize() (lbfgspp_b200
 algorithmic bytes of its passes (accounted by the kernel itself, include/lbfgs_b200.h: lbfgs_b200_solver_profile) divided by its
 duration measured with CUDA events around the launch on the launching stream.  `cpu_baseline` / `--impl reference` time the CPU
 restatement of the reference (oracle/; the reference itself cannot be built: Eigen is absent) on this box's host cores.
+--dump-outputs DIR: after the timed steps, what the last timed step computed is written as DIR/<name>.npy (float64, see dump_outputs);
+the inputs are fixed (zeros, constants or seeded), so two builds can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -21,6 +24,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -58,19 +62,11 @@ def load_peaks():
     if os.path.exists(path):
         with open(path) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def load_traffic(key):
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tpath):
-        with open(tpath) as fh:
-            return json.load(fh).get(key)
-    return None
+    return 3350.0, "fallback (NVIDIA H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 class ClockSampler(threading.Thread):
-    """SM clock and throttle reasons DURING the timed region (B200_PROFILING.md's clocks line).  Sampled in-process through NVML -- the
+    """SM clock and throttle reasons DURING the timed region.  Sampled in-process through NVML -- the
     library nvidia-smi itself reads -- every 50 ms: starting an nvidia-smi per sample re-initialises NVML every time and was seen to
     stall the solver's own driver calls (a 14 ms solve took 39 ms of wall clock on one box), and `nvidia-smi -lms` block-buffers its
     output into a pipe.  Falls back to one nvidia-smi process per sample when NVML cannot be loaded."""
@@ -148,17 +144,47 @@ class ClockSampler(threading.Thread):
                 "reasons": sorted(reasons), "samples": len(self.samples), "source": self.source}
 
 
+DUMP_SAMPLE = 1 << 20      # longest vector written whole by --dump-outputs (8 MB of float64)
+
+
+def dump_outputs(dirname, arrays, rank=0, world=1):
+    """Write each of `arrays` (name -> array or scalar) as dirname/<name>.npy in float64 (per rank: <name>_rank<r>.npy when
+    world > 1).  An array with more than DUMP_SAMPLE elements is written as <name>_sample.npy: its flattened elements at
+    DUMP_SAMPLE indices drawn without replacement by numpy.random.default_rng(0), in ascending order -- the same indices in every
+    run for the same shape."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    sfx = "_rank%d" % rank if world > 1 else ""
+    for name, a in arrays.items():
+        a = np.asarray(a, dtype=np.float64)
+        if a.size > DUMP_SAMPLE:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, DUMP_SAMPLE, replace=False))
+            a, name = a.reshape(-1)[idx], name + "_sample"
+        np.save(os.path.join(dirname, name + sfx + ".npy"), np.atleast_1d(a))
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # CPU legs (oracle/ is executed only here, in tests/ and in smoke())
 # ---------------------------------------------------------------------------------------------------------------------
+_native_dir = None
+
+
 def load_oracle(native=True):
+    """The CPU checker.  native=True: its -O3 -march=native build, compiled on the host it is timed on into a temporary directory
+    (the tree may be read-only); the portable oracle/liboracle.so that build() made when that fails."""
+    global _native_dir
     sys.path.insert(0, os.path.join(ROOT, "oracle"))
     import pyoracle as po
-    try:
-        po.build(native=native)   # native build happens on the box it is timed on
-        return po, po.Oracle("orc", native=native)
-    except Exception:
-        return po, po.Oracle("orc", native=False)
+    if native:
+        try:
+            if _native_dir is None:
+                _native_dir = tempfile.TemporaryDirectory(prefix="lbfgspp_bench_")
+            path = os.path.join(_native_dir.name, "liboracle_native.so")
+            po.build_native(path)
+            return po, po.Oracle("orc", path=path)
+        except Exception:
+            pass
+    return po, po.Oracle("orc")
 
 
 def cpu_solve(po, orc, name, sum_mode, problem=0, max_iterations=None):
@@ -216,7 +242,7 @@ def run_reference_arm(args, rank):
     all_cores = {"value": allc["niter"] / allc["seconds"], "unit": "iters/s", "cores": orc.hw_threads(),
                  "note": "the same full solve by the OpenMP build of the restatement on all host threads (the reference has no such mode)"}
     sample = ("%d x the full minimize() of the config (%d iterations, %d evaluations each), 1 thread; warm-up = one 1-iteration solve; "
-              "restatement of the reference (oracle/liboracle_native.so, -O3 -march=native, 8-lane partial sums)" % (nsolves, last["niter"], last["nfev"]))
+              "restatement of the reference (oracle/, -O3 -march=native, 8-lane partial sums)" % (nsolves, last["niter"], last["nfev"]))
     ref_headers = None
     if name == "c2":
         try:   # for the record: the unmodified reference headers themselves (over the minieigen stand-in), 3 iterations of the same solve
@@ -254,7 +280,8 @@ def main():
                     help="device-resident solve (one persistent kernel launch per minimize; default) or the host-driven loop (one launch per pass)")
     ap.add_argument("--sharding", default="problems", choices=["problems", "n"], help="c5 on N > 1 GPUs")
     ap.add_argument("--no-cpu-baseline", action="store_true")
-    ap.add_argument("--profile-mode", action="store_true", help="timed region only (for runs under ncu; numbers are not bench values)")
+    ap.add_argument("--profile-mode", action="store_true", help="timed region only (for runs under a profiler; numbers are not bench values)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last timed step computed as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else max(args.warmup, 1)
 
@@ -270,7 +297,7 @@ def main():
     import torch
     import lbfgspp_b200 as lb
 
-    assert torch.cuda.is_available(), "bench.py needs a B200 (there is no CPU fallback)"
+    assert torch.cuda.is_available(), "bench.py needs an H100 (there is no CPU fallback)"
     torch.cuda.set_device(local_rank)
     dist = None
     if world > 1:
@@ -342,7 +369,7 @@ def main():
         barrier()
         return outs, max_over_ranks(ms.value * 1e-3)
 
-    def roofline_from_profiles(profs, kernel_name, traffic_key):
+    def roofline_from_profiles(profs, kernel_name):
         """profs: Session.profile() of every timed solve.  achieved = algorithmic bytes of the launch / its CUDA-event duration."""
         nbytes = sum(sum(v["alg_bytes"] for v in p["ops"].values()) for p in profs)
         ms = sum(p["kernel_ms"] for p in profs)
@@ -353,7 +380,7 @@ def main():
                 o["ms"] += v["ms"]; o["rounds"] += v["rounds"]; o["alg_bytes"] += v["alg_bytes"]
         ach = nbytes / (ms * 1e-3) / 1e9 if ms > 0 else 0.0
         return {"kernel": kernel_name, "bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                "traffic": load_traffic(traffic_key), "peak_source": peak_src,
+                "traffic": None, "peak_source": peak_src,
                 "algorithmic_bytes": "per launch (= one minimize): sum over the kernel's passes of whole vectors read + written, 8 n x "
                                      "{first 3, trial 4, pair-forming dots 2c+4, combination + first trial 2c+3 (+2 when its x, g are stored), plain dots 2c+1, "
                                      "materialise 4}, c = pairs taking part in that pass; one iteration with T trials moves (4c+9) + 4(T-1) words per "
@@ -392,6 +419,10 @@ def main():
         outs, dev_seconds = device_timed(one, args.steps)
         iters = sum(o["niter"] for o in outs)
         launches = sum(o["launches"] for o in outs)
+        if args.dump_outputs:
+            last = outs[-1]
+            dump_outputs(args.dump_outputs, {"x": sess.solution(), "fx": last["fx"], "gnorm": last["gnorm"], "niter": last["niter"],
+                                             "nfev": last["nfev"]}, rank, world)
         # ---- end to end: pinned host -> device every step, result back to the host ----
         for _ in range(0 if args.profile_mode else 2):
             sess.solve(from_host=True, to_host=True)
@@ -415,7 +446,7 @@ def main():
                              world, "inside the kernel over NVLink peer memory" if args.comm == "p2p" else "with ncclAllReduce"),
                          "l2": "inputs larger than L2 (S,Y = %.2f GB per GPU)" % (2 * 8 * n_local * (m_hist + 1) / 1e9)}
         if resident:
-            line["roofline"] = roofline_from_profiles(profs, "k_persist (device-resident solve)", "k_persist_dram_bytes_per_launch_%s" % name)
+            line["roofline"] = roofline_from_profiles(profs, "k_persist (device-resident solve)")
         # ---- the other loop, for comparison (not the headline) ----
         if not args.profile_mode and world == 1:
             other = lb.Session(objective, x0, prm, cfg["ls"], device=local_rank, hv_algo=hv, data0=data0, data1=data1, resident=not resident)
@@ -467,6 +498,8 @@ def main():
             secs += r["seconds"]; e2e_secs += r["seconds_e2e"]; iters += r["niter"]; launches += r["launches"]
         barrier()
         clocks = sampler.summary()
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, {k: r[k] for k in ("x", "grad", "fx", "gnorm", "niter", "nfev")})
         # algorithmic bytes of one L-BFGS-B iteration at c pairs (DESIGN.md section 9): line-search trials 4n each, breakpoints + classes 5n,
         # W'd and the Cauchy build ~(2c+4)n, subspace minimisation >= (4c+8)n per BOXCQP sweep: reported as a lower bound with T trials
         nfev = r["nfev"]
@@ -503,7 +536,7 @@ def main():
             X0 = np.stack([np.random.default_rng(1000 + b).uniform(-1, 1, n_global) for b in mine])
         prm = lb.LBFGSParam(m=m_hist)
         bs = lb.BatchSession(lb.OBJ_ROSENBROCK_PAIRED, X0, prm, cfg["ls"], device=local_rank)
-        steps = max(1, min(args.steps, 3))
+        steps = args.steps
         for _ in range(max(1, min(args.warmup, 2))):
             res, _, _ = bs.solve(return_x=False)
         sampler.start()
@@ -516,6 +549,9 @@ def main():
                 profs.append(pr)
             return rr
         outs, dev_seconds = device_timed(one_batch, steps)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, dict({"X": bs.solution()}, **{k: [p[k] for p in outs[-1]] for k in ("fx", "gnorm", "niter", "nfev")}),
+                         rank, world)
         iters_rank = sum(sum(p["niter"] for p in o) for o in outs)
         iters = iters_rank if shard_n else sum_over_ranks(iters_rank)
         barrier()
@@ -541,7 +577,7 @@ def main():
                                        % (len(its), min(its), float(np.mean(its)), max(its), max(rounds)),
                                "converged": int(sum(p["status"] == "ok" for p in outs[-1]))}})
         if profs:
-            line["roofline"] = roofline_from_profiles(profs, "k_persist (device-resident solve, %d problems in one launch)" % len(mine), "k_persist_dram_bytes_per_launch_c5")
+            line["roofline"] = roofline_from_profiles(profs, "k_persist (device-resident solve, %d problems in one launch)" % len(mine))
         if not args.no_cpu_baseline and rank == 0 and world == 1:
             line["cpu_baseline"] = cpu_baseline_block(name)
         bs.close()

@@ -1,5 +1,5 @@
 // The reference's two self-checking examples (examples/example-rosenbrock-comparison.cpp and
-// example-rosenbrock-bracketing.cpp) on the B200 front: for n = 2, 4, .., 24 and `trials` seeded random starts in
+// example-rosenbrock-bracketing.cpp) on the GPU front: for n = 2, 4, .., 24 and `trials` seeded random starts in
 // [-1,1]^n, minimise the paired Rosenbrock function with all four line searches (max_linesearch = 256), check
 // |x - 1|_inf <= 1e-4 like validate_solution() there, and report the average evaluation / iteration counts.
 #include <cmath>

@@ -1,4 +1,4 @@
-// examples/example-quadratic.cpp of the reference on the B200 front: a free function over host vectors,
+// examples/example-quadratic.cpp of the reference on the GPU front: a free function over host vectors,
 // f(x) = |x - (0,1,...,n-1)|^2, double precision, default parameters.
 #include <cmath>
 #include <iostream>

@@ -1,4 +1,4 @@
-// examples/example-rosenbrock-box.cpp of the reference on the B200 front: chained Rosenbrock, n = 25, bounds [2, 4] with the
+// examples/example-rosenbrock-box.cpp of the reference on the GPU front: chained Rosenbrock, n = 25, bounds [2, 4] with the
 // third variable unbounded and some start values on the bounds, LBFGSBSolver with default LBFGSBParam.  Vectors live on the
 // device; the objective is the built-in device kernel for this function.
 #include <cmath>

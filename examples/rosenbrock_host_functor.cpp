@@ -1,4 +1,4 @@
-// The reference's first example (examples/example-rosenbrock.cpp) on the B200 front, host-vector compatibility mode:
+// The reference's first example (examples/example-rosenbrock.cpp) on the GPU front, host-vector compatibility mode:
 // the objective is an ordinary host functor, exactly as an LBFGSpp user writes it; only the vector type changed
 // (Eigen::VectorXf -> LBFGSpp::HostVector<float>; with Eigen installed, Eigen::VectorXf works unchanged).
 #include <iostream>

@@ -1,4 +1,4 @@
-// LBFGS.h -- LBFGSSolver<Scalar, LineSearch>: unconstrained L-BFGS with every n-vector in B200 HBM.
+// LBFGS.h -- LBFGSSolver<Scalar, LineSearch>: unconstrained L-BFGS with every n-vector in H100 HBM.
 //
 // Drop-in for the reference's include/LBFGS.h: same class template, same constructor / minimize() /
 // final_grad() / final_grad_norm() surface, same convergence rules and return values (reference LBFGS.h:78-173).

@@ -1,4 +1,4 @@
-// LBFGSB.h -- LBFGSBSolver<Scalar, LineSearch>: bound-constrained L-BFGS-B with every n-vector in B200 HBM.
+// LBFGSB.h -- LBFGSBSolver<Scalar, LineSearch>: bound-constrained L-BFGS-B with every n-vector in H100 HBM.
 //
 // Drop-in for the reference's include/LBFGSB.h (reference LBFGSB.h:116-262): same class template, constructor, minimize(f, x,
 // fx, lb, ub) / final_grad() / final_grad_norm(), same convergence tests (projected-gradient infinity norm against epsilon and

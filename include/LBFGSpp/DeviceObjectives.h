@@ -1,7 +1,7 @@
 // LBFGSpp/DeviceObjectives.h -- objective functors whose f/grad run on the GPU.
 //
 // The reference's users write `Scalar operator()(const Vector& x, Vector& grad)` over host vectors
-// (reference LBFGS.h:69-71; examples/example-rosenbrock.cpp:15-27).  On the B200 front x and grad are device
+// (reference LBFGS.h:69-71; examples/example-rosenbrock.cpp:15-27).  On the GPU front x and grad are device
 // vectors, so an objective is a functor that launches kernels.  BuiltinObjective wraps the four objective kernels
 // compiled into liblbfgs_b200 (the reference's example functions + the SPD quadratic of the benchmark configs) and
 // exposes, besides operator(), the two fused entry points LineSearchDriver.h looks for:

@@ -1,4 +1,4 @@
-// LBFGSpp/DeviceVector.h -- the `Vector` type of the B200 front: an n-vector that lives in HBM.
+// LBFGSpp/DeviceVector.h -- the `Vector` type of the GPU front: an n-vector that lives in HBM.
 //
 // The reference's Vector is Eigen::Matrix<Scalar, Dynamic, 1> (reference LBFGS.h:25); here it is a handle to
 // device memory obtained through the C ABI (include/lbfgs_b200.h).  The members the reference's solver and

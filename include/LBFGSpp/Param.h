@@ -1,4 +1,4 @@
-// LBFGSpp/Param.h -- solver options of the B200 L-BFGS / L-BFGS-B front.
+// LBFGSpp/Param.h -- solver options of the H100 L-BFGS / L-BFGS-B front.
 //
 // Drop-in for the reference's include/LBFGSpp/Param.h: same struct names, same public fields, same
 // defaults (reference Param.h:171-182 and :330-341), same enum values (:23-62) and the same

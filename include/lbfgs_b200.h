@@ -1,4 +1,4 @@
-/* lbfgs_b200.h -- C ABI of liblbfgs_b200.so: the L-BFGS hot path of LBFGSpp on NVIDIA B200 (sm_100a).
+/* lbfgs_b200.h -- C ABI of liblbfgs_b200.so: the L-BFGS hot path of LBFGSpp on NVIDIA H100 (sm_90a).
  *
  * The reference (yixuan/LBFGSpp @ ebef584) has no FFI: its boundary is a C++ template API whose
  * floating-point work happens inside Eigen expressions.  This header is the contract between the

@@ -1,14 +1,14 @@
-"""lbfgspp_b200 -- B200-native L-BFGS hot path behind LBFGSpp's solver interface.
+"""lbfgspp_b200 -- H100-native L-BFGS hot path behind LBFGSpp's solver interface.
 
 Layers (top to bottom):
   LBFGSParam / LBFGSSolver (this module)   Python mirror of the reference's classes for tests and bench.py;
                                            calls the C++ front through liblbfgs_b200_driver.so
   include/LBFGS.h, include/LBFGSpp/*.h     header-only C++ front = the drop-in (same class names as the reference)
   include/lbfgs_b200.h                     C ABI
-  csrc/*.cu                                hand-written sm_100a kernels (liblbfgs_b200.so)
+  csrc/*.cu                                hand-written sm_90a kernels (liblbfgs_b200.so)
 
 There is no CPU fallback: importing works anywhere, but creating a Context / solving raises unless the CUDA
-library is built (lbfgspp_b200.build.build_all()) and a B200 is present.
+library is built (lbfgspp_b200.build.build_all()) and an H100 is present.
 """
 import ctypes as C
 import os
@@ -168,6 +168,8 @@ def driver():
     lib.lbfgsb200_drv_session_solve.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(_DrvResult)]
     lib.lbfgsb200_drv_session_result.restype = dp
     lib.lbfgsb200_drv_session_result.argtypes = [C.c_void_p]
+    lib.lbfgsb200_drv_session_download.argtypes = [C.c_void_p, dp]
+    lib.lbfgsb200_drv_batch_session_download.argtypes = [C.c_void_p, dp]
     lib.lbfgsb200_drv_batch_session_create.restype = C.c_void_p
     lib.lbfgsb200_drv_batch_session_create.argtypes = [C.c_int, C.c_int, C.c_long, C.c_int, dp, C.c_int, C.POINTER(_DrvParam), C.c_char_p, C.c_int]
     lib.lbfgsb200_drv_batch_session_destroy.argtypes = [C.c_void_p]
@@ -543,6 +545,13 @@ class Session:
         p = self.drv.lbfgsb200_drv_session_result(self.h)
         return np.ctypeslib.as_array(p, shape=(self.n,)).copy()
 
+    def solution(self):
+        """x of the last solve(), copied from the device (the solve itself need not have asked for to_host)."""
+        x = np.empty(self.n)
+        if self.drv.lbfgsb200_drv_session_download(self.h, x.ctypes.data_as(C.POINTER(C.c_double))):
+            raise RuntimeError("session download failed")
+        return x
+
     def close(self):
         if self.h:
             self.drv.lbfgsb200_drv_session_destroy(self.h)
@@ -613,6 +622,13 @@ class BatchSession:
         if self.drv.lbfgsb200_drv_batch_session_upload(self.h, X0.ctypes.data_as(C.POINTER(C.c_double)), err, 256):
             raise RuntimeError("batch upload failed: " + err.value.decode())
         return X0.nbytes
+
+    def solution(self):
+        """X (B x n) of the last solve(), copied from the device (also after solve(return_x=False))."""
+        X = np.empty((self.B, self.n))
+        if self.drv.lbfgsb200_drv_batch_session_download(self.h, X.ctypes.data_as(C.POINTER(C.c_double))):
+            raise RuntimeError("batch session download failed")
+        return X
 
     def profile(self):
         """Accounting of the last batched solve (one kernel launch for the whole batch): same dict as Session.profile()."""

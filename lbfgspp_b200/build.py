@@ -1,6 +1,6 @@
 """Build the two in-tree shared objects of the product (no JIT cache: the .so files travel with the snapshot).
 
-  liblbfgs_b200.so         hand-written sm_100a kernels + C ABI  (nvcc; include/lbfgs_b200.h)
+  liblbfgs_b200.so         hand-written sm_90a kernels + C ABI  (nvcc; include/lbfgs_b200.h)
   liblbfgs_b200_driver.so  header-only C++ front (include/LBFGS.h ...) behind host-buffer entry points (g++)
 
 `python -m lbfgspp_b200.build` or lbfgspp_b200.build.build_all().
@@ -20,7 +20,8 @@ CXX = "/usr/bin/g++"
 # -fmad=false: IEEE multiply/add without FMA contraction.  The scalar line-search cores then take bit-identical decisions on
 # the device and on the host (g++ does not contract either), element-wise kernels reproduce the CPU checker bit for bit, and
 # the streaming kernels stay HBM-bound (FP64 pipe < 30 % busy), so it costs nothing measurable.
-NVCC_FLAGS = ["-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-fmad=false",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]     # H100 only: the kernels use sm_90a PTX (TMA bulk copies, mbarrier)
+NVCC_FLAGS = ["-std=c++17"] + ARCH + ["-O3", "-lineinfo", "-fmad=false",
               "-Xcompiler", "-fPIC", "-shared", "-ccbin", CXX]
 
 
@@ -58,7 +59,7 @@ def build_kernels(force=False, verbose=False):
     for cmd, p in procs:
         if p.wait() != 0:
             raise subprocess.CalledProcessError(p.returncode, cmd)
-    subprocess.run([NVCC, "-shared", "-ccbin", CXX, "-o", LIB] + objs + ["-lnccl"], check=True)
+    subprocess.run([NVCC, "-shared"] + ARCH + ["-ccbin", CXX, "-o", LIB] + objs + ["-lnccl"], check=True)
     return LIB
 
 

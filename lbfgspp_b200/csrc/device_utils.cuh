@@ -1,12 +1,11 @@
 // device_utils.cuh -- wide global-memory accessors and the deterministic grid reduction used by every
-// kernel of liblbfgs_b200.so (sm_100a only).
+// kernel of liblbfgs_b200.so (sm_90a only).
 //
 // Memory model of the path: all operands are long contiguous fp64/fp32 vectors streamed once per kernel,
-// so the kernels are HBM-bound.  Rules applied here (B200 guide, "HBM3e + on-chip memory"):
-//   * 256-bit accesses (LDG.E.256 / STG.E.256, new on sm_100): one pack = 4 doubles (or 8 floats handled as
-//     two 128-bit halves is not needed: fp32 packs are 4 floats = 128 bit);
+// so the kernels are HBM-bound.  Rules applied here:
+//   * one pack = 4 elements: two 128-bit accesses for fp64 (the widest global access on sm_90), one for fp32;
 //   * history columns are read with L1::no_allocate + L2::evict_first (touched once per pass), the running
-//     vector q/r with L2::evict_last so that it can survive in the 126 MB L2 between consecutive stages;
+//     vector q/r with L2::evict_last so that it can survive in the 50 MB L2 between consecutive stages;
 //   * grids are a multiple of the SM count; every thread keeps several independent packs in flight.
 #pragma once
 
@@ -17,40 +16,57 @@ namespace lb {
 
 constexpr int kThreads = 256;        // threads per CTA for all streaming kernels
 constexpr int kMaxRed = 8;           // max simultaneous reductions per kernel launch
-constexpr int kMaxBlocks = 148 * 8;  // upper bound on any reducing grid (partials buffer size)
+constexpr int kMaxBlocks = 132 * 8;  // H100 SXM: 132 SMs; upper bound on any reducing grid (partials buffer size)
 
 // ----------------------------------------------------------------------------- packs of 4 elements
 template <class T> struct Pack { T v[4]; };
 
 enum class Hint { Stream, Keep, Plain };
 
+// sm_90 has neither 256-bit global accesses nor the .L2::evict_* qualifiers of ld/st: a pack of 4 doubles is two 128-bit
+// accesses to adjacent 16-byte halves, and the L2 eviction priority travels as a cache policy (createpolicy + .L2::cache_hint)
+template <Hint H> __device__ __forceinline__ uint64_t l2_policy()
+{
+    uint64_t pol;
+    if (H == Hint::Stream) asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    else asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+#define LB_LD2H(p, a, b, pol) asm("ld.global.L1::no_allocate.L2::cache_hint.v2.f64 {%0,%1}, [%2], %3;" : "=d"(a), "=d"(b) : "l"(p), "l"(pol))
+#define LB_ST2H(p, a, b, pol) asm volatile("st.global.L1::no_allocate.L2::cache_hint.v2.f64 [%0], {%1,%2}, %3;" :: "l"(p), "d"(a), "d"(b), "l"(pol) : "memory")
 template <Hint H> __device__ __forceinline__ Pack<double> ld_pack(const double* p)
 {
     Pack<double> r;
-    if (H == Hint::Stream)
-        asm("ld.global.L1::no_allocate.L2::evict_first.v4.f64 {%0,%1,%2,%3}, [%4];"
-                     : "=d"(r.v[0]), "=d"(r.v[1]), "=d"(r.v[2]), "=d"(r.v[3]) : "l"(p));
-    else if (H == Hint::Keep)
-        asm("ld.global.L1::no_allocate.L2::evict_last.v4.f64 {%0,%1,%2,%3}, [%4];"
-                     : "=d"(r.v[0]), "=d"(r.v[1]), "=d"(r.v[2]), "=d"(r.v[3]) : "l"(p));
+    if (H == Hint::Plain)
+    {
+        asm("ld.global.v2.f64 {%0,%1}, [%2];" : "=d"(r.v[0]), "=d"(r.v[1]) : "l"(p));
+        asm("ld.global.v2.f64 {%0,%1}, [%2];" : "=d"(r.v[2]), "=d"(r.v[3]) : "l"(p + 2));
+    }
     else
-        asm("ld.global.v4.f64 {%0,%1,%2,%3}, [%4];"
-                     : "=d"(r.v[0]), "=d"(r.v[1]), "=d"(r.v[2]), "=d"(r.v[3]) : "l"(p));
+    {
+        const uint64_t pol = l2_policy<H>();
+        LB_LD2H(p, r.v[0], r.v[1], pol);
+        LB_LD2H(p + 2, r.v[2], r.v[3], pol);
+    }
     return r;
 }
 template <Hint H> __device__ __forceinline__ void st_pack(double* p, const Pack<double>& r)
 {
-    if (H == Hint::Stream)
-        asm volatile("st.global.L1::no_allocate.L2::evict_first.v4.f64 [%0], {%1,%2,%3,%4};"
-                     :: "l"(p), "d"(r.v[0]), "d"(r.v[1]), "d"(r.v[2]), "d"(r.v[3]) : "memory");
-    else if (H == Hint::Keep)
-        asm volatile("st.global.L1::no_allocate.L2::evict_last.v4.f64 [%0], {%1,%2,%3,%4};"
-                     :: "l"(p), "d"(r.v[0]), "d"(r.v[1]), "d"(r.v[2]), "d"(r.v[3]) : "memory");
+    if (H == Hint::Plain)
+    {
+        asm volatile("st.global.v2.f64 [%0], {%1,%2};" :: "l"(p), "d"(r.v[0]), "d"(r.v[1]) : "memory");
+        asm volatile("st.global.v2.f64 [%0], {%1,%2};" :: "l"(p + 2), "d"(r.v[2]), "d"(r.v[3]) : "memory");
+    }
     else
-        asm volatile("st.global.v4.f64 [%0], {%1,%2,%3,%4};"
-                     :: "l"(p), "d"(r.v[0]), "d"(r.v[1]), "d"(r.v[2]), "d"(r.v[3]) : "memory");
+    {
+        const uint64_t pol = l2_policy<H>();
+        LB_ST2H(p, r.v[0], r.v[1], pol);
+        LB_ST2H(p + 2, r.v[2], r.v[3], pol);
+    }
 }
-// fp32: 128-bit packs (L2 eviction-priority qualifiers exist only on the 256-bit forms)
+#undef LB_LD2H
+#undef LB_ST2H
+// fp32: 128-bit packs (no L2 eviction hint)
 template <Hint H> __device__ __forceinline__ Pack<float> ld_pack(const float* p)
 {
     Pack<float> r;

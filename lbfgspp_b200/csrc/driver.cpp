@@ -422,6 +422,14 @@ int lbfgsb200_drv_session_solve(void* handle, int from_host, int to_host, drv_re
 
 const double* lbfgsb200_drv_session_result(void* handle) { return static_cast<Session*>(handle)->pinned_out; }
 
+// the solution of the last solve (device-resident, n doubles) copied to x_out_host; 0 on success
+int lbfgsb200_drv_session_download(void* handle, double* x_out_host)
+{
+    Session* s = static_cast<Session*>(handle);
+    drv_result res{};
+    return guarded(&res, [&]() { s->x.copy_to_host(x_out_host); });
+}
+
 // accounting of the session's last device-resident solve (lbfgs_b200_solver_profile; sync_ms has 3 slots); returns 1 when the
 // session runs the host-driven loop
 int lbfgsb200_drv_session_profile(void* handle, double* kernel_ms, double* ms_by_op10, unsigned long long* rounds_by_op10, double* alg_bytes_by_op10,
@@ -737,6 +745,14 @@ extern "C" void* lbfgsb200_drv_batch_session_create(int device_ordinal, int obje
     }
 }
 extern "C" void lbfgsb200_drv_batch_session_destroy(void* handle) { delete static_cast<BatchSession*>(handle); }
+
+// the solutions of the last batched solve (device-resident, B*n doubles) copied to xs_out_host; 0 on success
+extern "C" int lbfgsb200_drv_batch_session_download(void* handle, double* xs_out_host)
+{
+    BatchSession* s = static_cast<BatchSession*>(handle);
+    drv_result res{};
+    return guarded(&res, [&]() { s->X.copy_to_host(xs_out_host); });
+}
 
 // new start points for the next solve(s), from host memory (B*n doubles): the end-to-end path of a batch
 extern "C" int lbfgsb200_drv_batch_session_upload(void* handle, const double* x0s_host, char* err, int errlen)

@@ -31,7 +31,7 @@ struct lbfgs_b200_ctx
     int device = 0;
     cudaStream_t stream = nullptr;
     bool own_stream = false;
-    int sm_count = 148;
+    int sm_count = 132;
     int ctas_per_sm_cap = 8;       // streaming grids: at most this many CTAs per SM (tuning knob LBFGS_B200_CTAS_PER_SM, 1..8)
     ReduceBuf rb{};                // device scratch for grid_reduce
     double* h_result = nullptr;    // pinned mirror of rb.result (+ extra slots)

@@ -1,7 +1,7 @@
 // lbfgs_b200.cu -- kernels + C ABI of liblbfgs_b200.so (declared in include/lbfgs_b200.h).
 //
 // Build (see lbfgspp_b200/build.py):
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -shared -Xcompiler -fPIC ... -lnccl
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -shared -Xcompiler -fPIC ... -lnccl
 //
 // Kernel inventory (all HBM-bound streaming kernels; algorithmic words moved per element in brackets):
 //   k_trial<OBJ>      x = xp + step*d ; g = grad f(x) ; {f, g.d, g.g, x.x}      [R 2 + W 2 (+data)]
@@ -468,7 +468,7 @@ __global__ void __launch_bounds__(kThreads) k_hv_stage(StageArgs<T> s, ReduceBuf
 // =====================================================================================================
 extern "C" {
 
-const char* lbfgs_b200_version(void) { return "lbfgs_b200 0.1 (sm_100a)"; }
+const char* lbfgs_b200_version(void) { return "lbfgs_b200 0.1 (sm_90a)"; }
 
 lbfgs_b200_status lbfgs_b200_ctx_create(lbfgs_b200_ctx** out, int device, void* stream)
 {
@@ -495,9 +495,9 @@ lbfgs_b200_status lbfgs_b200_ctx_create(lbfgs_b200_ctx** out, int device, void* 
     CUC(cudaSetDevice(device));
     cudaDeviceProp prop;
     CUC(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10)
+    if (prop.major != 9 || prop.minor != 0)
     {
-        fail(nullptr, LBFGS_B200_ERR_CUDA, "device %d is sm_%d%d; this library contains sm_100a code only", device, prop.major, prop.minor);
+        fail(nullptr, LBFGS_B200_ERR_CUDA, "device %d is sm_%d%d; this library contains sm_90a code only", device, prop.major, prop.minor);
         lbfgs_b200_ctx_destroy(ctx);
         return LBFGS_B200_ERR_CUDA;
     }

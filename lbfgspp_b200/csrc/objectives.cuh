@@ -1,7 +1,7 @@
 // objectives.cuh -- device versions of the benchmark objective functions (SURVEY.md 8a row A12).
 //
 // Each functor evaluates 4 consecutive coordinates at once ("pack") so that it can sit inside the fused
-// line-search trial kernel between the 256-bit loads of xp/d and the 256-bit stores of x/g.
+// line-search trial kernel between the wide loads of xp/d and the wide stores of x/g.
 //   eval(i0, cnt, x[4], xl, xr, g[4]) -> this pack's contribution to f
 //     i0   local index of x[0];  cnt valid lanes (ragged tail);  xl = x_{i0-1}, xr = x_{i0+4} (0 outside the GLOBAL vector)
 // n-sharding: a functor whose coordinates couple to their neighbours (kHalo) also carries the global position of its block

@@ -27,7 +27,7 @@
 // Data movement: ALL operands of the dots and combination passes -- the right-hand vectors and the 2c history columns, which live in
 // a tiled layout (PHist) so that the columns of a tile are one or two contiguous runs -- are staged into shared memory by TMA bulk
 // copies (cp.async.bulk + mbarrier) in a two-stage ring of ~90 KB stages: the bytes in flight per SM are set by the ring, not by
-// registers.  The trial pass streams through registers (256-bit loads / stores).  Vectors owned by the solver are padded to whole
+// registers.  The trial pass streams through registers (128-bit loads / stores).  Vectors owned by the solver are padded to whole
 // 256-byte lines, so every tile -- the ragged end of a vector included -- is a legal bulk copy; lanes past n are masked in the
 // arithmetic.  The coefficient recursion of a combination pass runs from a scratch area of its own while the pass's first tiles
 // are in flight.  DESIGN.md section 10 has what was measured about the limits of this arrangement.
@@ -281,7 +281,7 @@ template <int NV> __device__ __forceinline__ void block_sums(const double (&acc)
 
 // ---- FIRST / TRIAL -------------------------------------------------------------------------------------------------------------
 // MODE 0: FIRST (evaluate at x, write g and d = -g) ; MODE 1: TRIAL (x = xp + step*d, write x and g).  Operands stream through
-// registers with 256-bit loads/stores (a shared-memory staged variant measured slower for this 1:1 read/write pass).
+// registers with 128-bit loads/stores (a shared-memory staged variant measured slower for this 1:1 read/write pass).
 template <class T, class OBJ, int MODE>
 __device__ __forceinline__ void p_trial(const OBJ& obj, const Own& own, const T* __restrict__ xp, const T* __restrict__ d, T step,
                                         T* __restrict__ x, T* __restrict__ g, T* __restrict__ dout, PShared& sh, double* dst, int G, int tune)

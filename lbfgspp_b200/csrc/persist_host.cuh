@@ -165,7 +165,7 @@ static lbfgs_b200_status solver_minimize(lbfgs_b200_solver* s, int objective, co
     a.index_offset = index_offset; a.n_global = n_global;
     a.wait_cycles = kPWaitCycles;
     if (const char* e = getenv("LBFGS_B200_WATCHDOG_SCALE")) { const long long k = atoll(e); if (k >= 1 && k <= 100000) a.wait_cycles *= k; }
-    a.tune = ((size_t)s->n * sizeof(T) * 4 > ((size_t)96 << 20)) ? 4 : 0;     // x, xp, g, d of one problem exceed what L2 can hold between rounds
+    a.tune = ((size_t)s->n * sizeof(T) * 4 > ((size_t)36 << 20)) ? 4 : 0;     // x, xp, g, d of one problem exceed ~3/4 of the 50 MB L2
     if (const char* e = getenv("LBFGS_B200_TUNE")) a.tune = atoi(e);
     void* kargs[] = {&a};
     CU(ctx, cudaEventRecord(s->ev0, ctx->stream));

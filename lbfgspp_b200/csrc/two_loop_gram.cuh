@@ -16,7 +16,7 @@
 // k_gram_dots: tall-skinny [S Y]'[v s_new y_new].  One warp (or `split` warps) per history column pair;
 // the three right-hand vectors are staged tile by tile into shared memory with TMA bulk copies
 // (cp.async.bulk + mbarrier, 3-stage ring) and shared by all warps of the CTA; the S/Y columns stream from
-// HBM straight into registers with 256-bit evict-first loads.  Deterministic: fixed-slot block partials,
+// HBM straight into registers with 128-bit evict-first loads.  Deterministic: fixed-slot block partials,
 // fixed-order final sum, integer ticket only.
 #pragma once
 
@@ -53,7 +53,7 @@ template <class T> struct GramDotsArgs
     T* y_out;
 };
 
-// ---- mbarrier / TMA helpers (sm_90+ PTX, assembled for sm_100a) -------------------------------------
+// ---- mbarrier / TMA helpers (sm_90 PTX) -----------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, unsigned count)
 {

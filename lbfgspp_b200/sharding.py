@@ -2,7 +2,7 @@
 
 Rank r of N owns the contiguous block [lo, hi) of every n-vector and of every S/Y column; all scalars are replicated.
 Blocks are even-length (the paired Rosenbrock couples coordinates (2i, 2i+1)) and 4-aligned where possible so that
-every shard keeps the 256-bit access path.  A reduction is: local deterministic partial -> sum over ranks in rank order
+every shard keeps the 4-element pack access path.  A reduction is: local deterministic partial -> sum over ranks in rank order
 (NCCL all-reduce on the GPU; tests use gloo) -> identical scalar on every rank -> identical host decisions everywhere.
 """
 

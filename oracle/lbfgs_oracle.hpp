@@ -3,7 +3,7 @@
 // This file is a checker, never a product path: only tests/, __graft_entry__.smoke()
 // and bench.py's cpu_baseline / "--impl reference" legs may execute it.
 //
-// What it restates (reference @ ebef584, paths relative to /root/reference):
+// What it restates (reference @ ebef584, paths relative to the reference checkout):
 //   History<T>::reset/add/apply_Hv   include/LBFGSpp/BFGSMat.h:61-97, 276-302
 //   ls_backtracking                  include/LBFGSpp/LineSearchBacktracking.h:44-121
 //   ls_bracketing                    include/LBFGSpp/LineSearchBracketing.h:48-128

@@ -1,6 +1,6 @@
 // lbfgsb_oracle.hpp -- TEST INFRASTRUCTURE ONLY.  CPU restatement of the bound-constrained solver of LBFGSpp.
 //
-// What it restates (reference @ ebef584, paths relative to /root/reference/include):
+// What it restates (reference @ ebef584, paths relative to the reference's include/):
 //   PackedLDLT<T>                    LBFGSpp/BKLDLT.h:30-530     (Bunch-Kaufman LDL' of the 2m x 2m middle matrices)
 //   BoxHistory<T>                    LBFGSpp/BFGSMat.h:81-146, 307-615  (BFGSMat<Scalar, true>)
 //   cauchy_point                     LBFGSpp/Cauchy.h:31-50, 86-284

@@ -1,8 +1,8 @@
 /* oracle_api.h -- TEST INFRASTRUCTURE ONLY.
  *
  * One C ABI implemented twice:
- *   - oracle/_ref/libref_lbfgspp.so : the UNMODIFIED reference headers (/root/reference/include)
- *     compiled over oracle/minieigen (built only where /root/reference exists), prefix "ref_";
+ *   - oracle/_ref/libref_lbfgspp.so : the UNMODIFIED reference headers (LBFGSpp's include/)
+ *     compiled over oracle/minieigen (built only when REF names a checkout), prefix "ref_";
  *   - oracle/liboracle.so           : the plain-C++ restatement (oracle/lbfgs_oracle.hpp),
  *     prefix "orc_".
  * Both are checkers.  Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline /

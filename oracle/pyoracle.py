@@ -1,8 +1,8 @@
 """ctypes bindings for the two CPU checkers (TEST INFRASTRUCTURE ONLY).
 
-  Oracle("orc")  -> oracle/liboracle.so            plain-C++ restatement (travels to the GPU box)
+  Oracle("orc")  -> oracle/liboracle.so            plain-C++ restatement (built by build() on every machine)
   Oracle("ref")  -> oracle/_ref/libref_lbfgspp.so  unmodified reference headers over minieigen
-                                                    (built only in the container that has /root/reference)
+                                                    (built only when oracle/Makefile is given REF=<LBFGSpp checkout>)
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may import
 this module; nothing under lbfgspp_b200/ or include/ does.
@@ -33,10 +33,14 @@ class Result(C.Structure):
                 ("fx", C.c_double), ("gnorm", C.c_double), ("trace_len", C.c_long), ("seconds", C.c_double)]
 
 
-def build(native=False):
+def build():
     """(Re)build the checkers with oracle/Makefile.  Building the checker is not using it."""
-    targets = ["all"] + (["native"] if native else [])
-    subprocess.run(["make", "-s", "-C", HERE] + targets, check=True)
+    subprocess.run(["make", "-s", "-C", HERE, "all"], check=True)
+
+
+def build_native(path):
+    """The -O3 -march=native timing build of the restatement, written to `path` (nothing is written under oracle/)."""
+    subprocess.run(["make", "-s", "-C", HERE, "native", "NATIVE_OUT=" + os.path.abspath(path)], check=True)
 
 
 def _ptr(a, ctype):
@@ -44,13 +48,12 @@ def _ptr(a, ctype):
 
 
 class Oracle:
-    def __init__(self, which="orc", native=False):
+    def __init__(self, which="orc", path=None):
+        """path: a library other than the default one of `which` (e.g. a build_native() output)."""
         assert which in ("orc", "ref")
         self.prefix = which + "_"
-        if which == "ref":
-            path = os.path.join(HERE, "_ref", "libref_lbfgspp.so")
-        else:
-            path = os.path.join(HERE, "liboracle_native.so" if native else "liboracle.so")
+        if path is None:
+            path = os.path.join(HERE, "_ref", "libref_lbfgspp.so") if which == "ref" else os.path.join(HERE, "liboracle.so")
         if not os.path.exists(path):
             raise FileNotFoundError(path)
         self.path = path

@@ -1,8 +1,8 @@
 // ref_capi.cpp -- TEST INFRASTRUCTURE ONLY.
 //
 // C-ABI wrapper ("ref_" prefix of oracle_api.h) around the UNMODIFIED reference headers.
-// Compiled ONLY where /root/reference exists (this container), by oracle/Makefile:
-//     g++ -I oracle/minieigen -I /root/reference/include ... -o oracle/_ref/libref_lbfgspp.so
+// Compiled ONLY when a reference checkout is named (make -C oracle ref REF=<LBFGSpp checkout>):
+//     g++ -I oracle/minieigen -I $(REF)/include ... -o oracle/_ref/libref_lbfgspp.so
 // No reference source is copied: <LBFGS.h>/<LBFGSB.h> are included from where they lie.
 // Arithmetic comes from oracle/minieigen (strictly sequential sums), control flow is the
 // reference's own.  Used to (1) pin the restatement bit-for-bit and (2) generate

@@ -2,9 +2,9 @@
 the CPU by the unmodified reference headers (oracle/_ref, built over minieigen: sequential sums) and by the restatement
 (oracle/liboracle.so) under three summation orders (sequential = what _ref does, 8-lane partial sums = what an AVX-512 Eigen
 redux does, and the Gram-form twin of apply_Hv with 8-lane sums = the GPU's re-association).  The spread BETWEEN the CPU
-columns is what a different reduction order does to the reference itself; the GPU tests hold the B200 to these tables.
+columns is what a different reduction order does to the reference itself; the GPU tests hold the H100 to these tables.
 
-Run from the repo root in the build container (needs /root/reference for oracle/_ref):
+Run from the repo root (needs oracle/_ref: make -C oracle ref REF=<LBFGSpp checkout>):
     python tests/golden/make_fullsize.py [c3] [c4] [c5] [--procs 7]
 C5 is 64 solves of 150-260 iterations at n = 1e6 in each of four CPU variants: about 15 minutes on 7 cores.
 Floats are stored as hex strings.

@@ -1,6 +1,6 @@
 """Generate tests/golden/lbfgs_ref.json from the UNMODIFIED reference headers (oracle/_ref, built over minieigen).
 
-Run in the container that has /root/reference:   python tests/golden/make_golden.py
+Needs oracle/_ref (make -C oracle ref REF=<LBFGSpp checkout>):   python tests/golden/make_golden.py
 The reference ships no golden vectors of its own (SURVEY.md section 4); these freeze what its headers compute
 (sequential summation, no FMA contraction) so that the travelling restatement can be checked on any machine.
 Floats are stored as hex strings: comparisons are bit-exact.

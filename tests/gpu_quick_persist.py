@@ -1,4 +1,4 @@
-"""Development check of the device-resident (persistent kernel) solve on a GPU box: parity against the CPU checker at a few sizes,
+"""Development check of the device-resident (persistent kernel) solve on a GPU: parity against the CPU checker at a few sizes,
 timing at config 2's size, batch == lone solves.  Not collected by pytest (no test_ prefix); run: python tests/gpu_quick_persist.py"""
 import json
 import os

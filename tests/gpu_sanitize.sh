@@ -1,6 +1,6 @@
 #!/bin/bash
-# compute-sanitizer passes over a small end-to-end solve and the kernel-level tests (run on a GPU box; not part of pytest):
-#     gpurun --timeout 900 -- 'bash tests/gpu_sanitize.sh > gpurun_out/sanitize.log 2>&1'
+# compute-sanitizer passes over a small end-to-end solve and the kernel-level tests (on a machine with an H100; not part of pytest):
+#     bash tests/gpu_sanitize.sh > sanitize.log 2>&1
 # memcheck: out-of-bounds / misaligned accesses; racecheck: shared-memory hazards (the TMA ring, the pair-forming tiles);
 # synccheck: barrier misuse; initcheck: reads of uninitialised device memory.  Kernels run 10-100x slower under the tools,
 # so the inputs are small; the multi-GPU exchange kernels spin on peer flags and are not run under the tools.

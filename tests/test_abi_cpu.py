@@ -64,7 +64,7 @@ def test_no_cpu_fallback_solver_reports_runtime_error():
 
 
 def test_version_string():
-    assert b"sm_100a" in lb.abi().lbfgs_b200_version()
+    assert b"sm_90a" in lb.abi().lbfgs_b200_version()
 
 
 def test_header_is_plain_c_and_links_from_c(tmp_path):

@@ -83,4 +83,4 @@ def test_peak_lookup(bench):
     if os.path.exists(path):
         assert peak == float(json.load(open(path))["hbm_gbs"]) and src.startswith("measured")
     else:
-        assert peak == 6650.0 and src.startswith("fallback")
+        assert peak == 3350.0 and src.startswith("fallback")

@@ -77,7 +77,7 @@ def test_apply_Hv_full_size_properties(gpu_ctx):
 # headers (sequential sums) and the restatement under two more summation orders.  Where the reference's own result depends on the
 # summation order (C3's last line search, C5's 150-400-iteration random starts) the test holds the GPU to what is order-independent
 # (the trace of f while it is well conditioned, the optimum, the error text) and to the spread the CPU columns show among
-# themselves; every comparison is also written to gpurun_out/parity_fullsize.json (copied to profiles/ per round).
+# themselves; with LBFGSPP_PARITY_REPORT=<file.json> set, every comparison is also written to that file.
 # ---------------------------------------------------------------------------------------------------------------------------------
 def _golden(name):
     with open(os.path.join(HERE, "golden", name)) as fh:
@@ -85,7 +85,10 @@ def _golden(name):
 
 
 def _report(key, value):
-    path = os.path.join(os.path.dirname(HERE), "gpurun_out", "parity_fullsize.json")
+    path = os.environ.get("LBFGSPP_PARITY_REPORT")
+    if not path:
+        return
+    path = os.path.abspath(path)
     try:
         os.makedirs(os.path.dirname(path), exist_ok=True)
         data = {}
@@ -163,7 +166,7 @@ def test_config5_full_size_batch_of_64():
     """One persistent kernel launch for the 64 problems of BASELINE config 5 at n = 1e6.  These are 140-620-iteration runs from
     random starts in which the reference's own iteration count moves by 15 % on average (up to a factor 1.45) between summation
     orders, and the distance to x* at the stop by up to 50x (columns of c5_full.json: the stop rule gnorm <= 1e-5 |x| is met at
-    different points of a flat valley).  So the per-seed table is reported (gpurun_out/parity_fullsize.json -> profiles/) and the
+    different points of a flat valley).  So the per-seed table is reported (LBFGSPP_PARITY_REPORT) and the
     assertions are: (a) every problem stops on the reference's own criterion, near x* = 1; (b) per seed the GPU count lies within
     the CPU columns' range widened by the factor the columns show among themselves; (c) over the 64 seeds the mean count is
     within 8 % of the CPU columns' mean (2.7 % apart among themselves); (d) a batch member is bit-identical to the same problem

@@ -1,5 +1,5 @@
 """n-sharded (multi-GPU) parity: launches tests/multi_gpu_check.py under torchrun on 2 GPUs of this box, once with the
-in-kernel NVLink exchange and once with NCCL.  Skipped on a single-GPU box (the host-side sharding logic is covered on CPU by
+in-kernel NVLink exchange and once with NCCL.  Skipped on a single-GPU machine (the host-side sharding logic is covered on CPU by
 tests/test_sharding_cpu.py with the gloo backend)."""
 import os
 import subprocess

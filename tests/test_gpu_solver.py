@@ -1,4 +1,4 @@
-"""GPU parity tests, solver level: LBFGSSolver<Scalar, LineSearch>::minimize on the B200 against the CPU checker.
+"""GPU parity tests, solver level: LBFGSSolver<Scalar, LineSearch>::minimize on the H100 against the CPU checker.
 
 Parity definition (SURVEY.md 8c): same return value (iterations), same number of objective evaluations,
 |fx_gpu - fx_cpu| <= 1e-10 * max(1, |fx_cpu|), |x_gpu - x_cpu|_inf <= 1e-8 * max(1, |x|_inf), and the per-evaluation

@@ -22,7 +22,7 @@ def test_shards_tile_the_vector(n, nranks):
     for (lo, hi), (lo2, _) in zip(sh, sh[1:]):
         assert hi == lo2 and lo <= hi
     for lo, hi in sh[:-1]:
-        assert lo % 4 == 0 and hi % 4 == 0          # 256-bit path and Rosenbrock pairs stay intact
+        assert lo % 4 == 0 and hi % 4 == 0          # 4-element packs and Rosenbrock pairs stay intact
     sizes = [hi - lo for lo, hi in sh[:-1]]
     if sizes:
         assert max(sizes) - min(sizes) <= 4
