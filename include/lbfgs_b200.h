@@ -51,11 +51,8 @@ enum {
     LBFGS_B200_HV_AUTO = 0,      /* currently GRAM                                                             */
     LBFGS_B200_HV_TWO_LOOP = 1,  /* literal two-loop recursion, one fused AXPY+dot stage kernel per history column:
                                     (8c+4) n words of traffic, 2c+1 launches, 2c collectives when sharded      */
-    LBFGS_B200_HV_GRAM = 2,      /* the same recursion carried out on 2c coefficients: two passes over S,Y,
+    LBFGS_B200_HV_GRAM = 2       /* the same recursion carried out on 2c coefficients: two passes over S,Y,
                                     (4c+3) n words, 3 launches, 1 collective; differs from TWO_LOOP by rounding */
-    LBFGS_B200_HV_GRAM_UNFUSED = 3 /* GRAM, but hist_update_apply_Hv keeps the separate update kernel (s'y, y'y from
-                                    its own reduction): the exact arithmetic of the device-resident solve, kept so
-                                    that the two solver loops can be compared bit for bit                       */
 };
 
 /* ---------------------------------------------------------------- context, memory, communicator */
@@ -284,9 +281,9 @@ void lbfgs_b200_solver_destroy(lbfgs_b200_solver* s);
 int lbfgs_b200_solver_batch(const lbfgs_b200_solver* s);
 /* Accounting of the last solve.  kernel_ms: device time of the one kernel (CUDA events around its launch).  The arrays have 10 slots
  * indexed by the pass a round ran: 0 = rounds in which the problems of a batch ran different passes, 1 FIRST, 2 TRIAL, 3 DOTS_FORM,
- * 4 DOTS_PLAIN, 5 COMBINE, 6 COMBINE_TRIAL, 7 RESTORE, 8 MATERIALIZE (9 unused).  ms_by_op10: the kernel's time split by round (CTA 0's cycle counter scaled
+ * 4 DOTS_PLAIN, 5 COMBINE, 6 COMBINE_TRIAL, 7 RESTORE (8, 9 unused).  ms_by_op10: the kernel's time split by round (CTA 0's cycle counter scaled
  * to kernel_ms; includes each round's synchronisation); alg_bytes_by_op10: algorithmic bytes of those passes (whole vectors read and
- * written: FIRST 3n, TRIAL 4n, DOTS_FORM (2c+4)n, DOTS_PLAIN (2c+1)n, COMBINE (2c+2)n, COMBINE_TRIAL (2c+3)n words or (2c+5)n when the first trial's x, g are stored, MATERIALIZE 4n words, + the objective's
+ * written: FIRST 3n, TRIAL 4n, DOTS_FORM (2c+4)n, DOTS_PLAIN (2c+1)n, COMBINE (2c+2)n, COMBINE_TRIAL (2c+5)n, RESTORE 4n words, + the objective's
  * data vectors per evaluation); sync_ms[3]: { the part of kernel_ms between CTA 0's arrival at a grid barrier and its release, the part of that spent waiting for
  * the last CTA to arrive, the part spent in the cross-rank exchange }. */
 lbfgs_b200_status lbfgs_b200_solver_profile(const lbfgs_b200_solver* s, double* kernel_ms, double* ms_by_op10, unsigned long long* rounds_by_op10,

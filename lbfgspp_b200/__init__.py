@@ -20,7 +20,7 @@ from . import build as _build
 PKG = os.path.dirname(os.path.abspath(__file__))
 
 OBJ_ROSENBROCK_PAIRED, OBJ_QUAD_SHIFT, OBJ_ROSENBROCK_CHAINED, OBJ_QUAD_TRIDIAG = 0, 1, 2, 3
-HV_AUTO, HV_TWO_LOOP, HV_GRAM, HV_GRAM_UNFUSED = 0, 1, 2, 3
+HV_AUTO, HV_TWO_LOOP, HV_GRAM = 0, 1, 2
 LINE_SEARCHES = {"Backtracking": 0, "Bracketing": 1, "NocedalWright": 2, "MoreThuente": 3}
 LBFGS_LINESEARCH_BACKTRACKING_ARMIJO = 1
 LBFGS_LINESEARCH_BACKTRACKING = 2
@@ -528,7 +528,7 @@ class Session:
         return dict(niter=res.niter, nfev=res.nfev, fx=res.fx, gnorm=res.gnorm, launches=res.launches,
                     h2d_bytes=res.h2d_bytes, d2h_bytes=res.d2h_bytes)
 
-    OPS = ("mixed", "first", "trial", "dots_form", "dots_plain", "combine", "combine_trial", "restore", "materialize", "-")
+    OPS = ("mixed", "first", "trial", "dots_form", "dots_plain", "combine", "combine_trial", "restore", "-", "-")   # slots 8, 9 unused
 
     def profile(self):
         """Accounting of the last device-resident solve: dict(kernel_ms, sync_ms, ops={name: dict(ms, rounds, alg_bytes)}); None for

@@ -9,7 +9,7 @@
 //   k_axpy_out, k_scale_out                                                      [R 2 W 1 / R 1 W 1]
 //   k_update          s = x-xp, y = g-gp -> ring slot ; {s.y, y.y}               [R 4 + W 2]
 //   k_hv_stage<KIND>  one fused AXPY+dot stage of the two-loop recursion         [R 3 + W 1]
-//   (k_gram_*, k_hv_resident live in two_loop_fast.cuh)
+//   (k_gram_dots, k_gram_fold, k_gram_combine live in two_loop_gram.cuh; the device-resident solve in persist.cuh)
 #include "internal.cuh"
 #include "two_loop_gram.cuh"
 
@@ -17,11 +17,12 @@ using namespace lb;
 
 // grid for a streaming kernel over n elements: a multiple of the SM count, capped so that every CTA has
 // at least a few packs; 4 CTAs of 256 threads per SM are resident (register budget <= 64/thread).
+constexpr int kCtasPerSmCap = 8;   // streaming grids: at most this many CTAs per SM
 static int grid_for(const lbfgs_b200_ctx* ctx, int64_t n, int packs_per_thread = 4)
 {
     const int64_t packs = (n + 3) / 4;
     const int64_t want = (packs + (int64_t)kThreads * packs_per_thread - 1) / ((int64_t)kThreads * packs_per_thread);
-    const int64_t cap = (int64_t)ctx->sm_count * ctx->ctas_per_sm_cap;
+    const int64_t cap = (int64_t)ctx->sm_count * kCtasPerSmCap;
     int64_t g = want < 1 ? 1 : want;
     if (g > cap) g = cap;
     if (g > ctx->sm_count) g = (g / ctx->sm_count) * ctx->sm_count;  // whole waves
@@ -75,13 +76,19 @@ static lbfgs_b200_status wait_mail(lbfgs_b200_ctx* ctx, int count)
     return LBFGS_B200_OK;
 }
 
+// copy result slots to the host and wait
+static lbfgs_b200_status fetch_result(lbfgs_b200_ctx* ctx, int count)
+{
+    CU(ctx, cudaMemcpyAsync(ctx->h_result, ctx->rb.result, sizeof(double) * count, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(ctx, cudaStreamSynchronize(ctx->stream));
+    return LBFGS_B200_OK;
+}
+
 // host receives `count` result slots: mailbox when the kernel delivered there, else memcpy + synchronise
 static lbfgs_b200_status receive(lbfgs_b200_ctx* ctx, int count)
 {
     if (mail_ok(ctx)) return wait_mail(ctx, count);
-    CU(ctx, cudaMemcpyAsync(ctx->h_result, ctx->rb.result, sizeof(double) * count, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(ctx, cudaStreamSynchronize(ctx->stream));
-    return LBFGS_B200_OK;
+    return fetch_result(ctx, count);
 }
 
 // sum the first `count` result slots over all ranks (no-op on one GPU, and in p2p mode where the kernel did it)
@@ -89,14 +96,6 @@ static lbfgs_b200_status allreduce_result(lbfgs_b200_ctx* ctx, int count)
 {
     if (ctx->nranks > 1 && !ctx->x_active)
         NC(ctx, ncclAllReduce(ctx->rb.result, ctx->rb.result, count, ncclDouble, ncclSum, ctx->comm, ctx->stream));
-    return LBFGS_B200_OK;
-}
-
-// copy result slots to the host and wait
-static lbfgs_b200_status fetch_result(lbfgs_b200_ctx* ctx, int count)
-{
-    CU(ctx, cudaMemcpyAsync(ctx->h_result, ctx->rb.result, sizeof(double) * count, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(ctx, cudaStreamSynchronize(ctx->stream));
     return LBFGS_B200_OK;
 }
 
@@ -213,10 +212,9 @@ __global__ void k_halo_exchange(int64_t n, const T* __restrict__ a, const T* __r
 // fused line-search trial  (x = xp + step*d ; g = grad f(x) ; {f, g.d, g.g, x.x})
 //   TRIAL = false: plain objective evaluation at x (no xp/d, no x store), reduces {f, -, g.g, x.x}
 // =====================================================================================================
-// body shared by the stand-alone kernel and the device-resident solve; returns true in the last CTA once result[0..4) is final
 template <class T, class OBJ, bool TRIAL, bool VEC>
-__device__ __forceinline__ bool trial_body(const OBJ& obj, int64_t n, const T* __restrict__ xp, const T* __restrict__ d,
-                                           T step, T* __restrict__ x, T* __restrict__ g, const ReduceBuf& rb)
+__global__ void __launch_bounds__(kThreads) k_trial(OBJ obj, int64_t n, const T* __restrict__ xp, const T* __restrict__ d,
+                                                    T step, T* __restrict__ x, T* __restrict__ g, ReduceBuf rb)
 {
     T acc[4] = {T(0), T(0), T(0), T(0)};
     const int64_t packs = (n + 3) >> 2, stride = (int64_t)gridDim.x * kThreads;
@@ -268,14 +266,7 @@ __device__ __forceinline__ bool trial_body(const OBJ& obj, int64_t n, const T* _
         store4<T, Hint::Plain, VEC>(g, i0, cnt, pg);
     }
     double dacc[4] = {(double)acc[0], (double)acc[1], (double)acc[2], (double)acc[3]};
-    return grid_reduce<4>(dacc, rb);
-}
-
-template <class T, class OBJ, bool TRIAL, bool VEC>
-__global__ void __launch_bounds__(kThreads) k_trial(OBJ obj, int64_t n, const T* __restrict__ xp, const T* __restrict__ d,
-                                                    T step, T* __restrict__ x, T* __restrict__ g, ReduceBuf rb)
-{
-    trial_body<T, OBJ, TRIAL, VEC>(obj, n, xp, d, step, x, g, rb);
+    grid_reduce<4>(dacc, rb);
 }
 
 // =====================================================================================================
@@ -285,21 +276,12 @@ __global__ void __launch_bounds__(kThreads) k_trial(OBJ obj, int64_t n, const T*
 // The ring has M = m+1 physical columns so that the pair of an iteration can be written speculatively into
 // the free slot `head` before the curvature gate (LBFGS.h:161) is known; a rejected pair simply leaves
 // `head` where it was and the m older pairs untouched (the reference would not have called add_correction).
-template <class T> struct HistDev
-{
-    T* S;         // [M][ld]
-    T* Y;         // [M][ld]
-    T* ys;        // [M]
-    T* alpha;     // [M]
-    T* theta;     // [1]
-};
-
 
 // s = x - xp ; y = g - gp -> slot ; {s.y, y.y}
 template <class T, bool VEC>
-__device__ __forceinline__ bool update_body(int64_t n, const T* __restrict__ x, const T* __restrict__ xp,
-                                            const T* __restrict__ g, const T* __restrict__ gp,
-                                            T* __restrict__ s_out, T* __restrict__ y_out, const ReduceBuf& rb)
+__global__ void __launch_bounds__(kThreads) k_update(int64_t n, const T* __restrict__ x, const T* __restrict__ xp,
+                                                     const T* __restrict__ g, const T* __restrict__ gp,
+                                                     T* __restrict__ s_out, T* __restrict__ y_out, ReduceBuf rb)
 {
     T acc[2] = {T(0), T(0)};
     const int64_t packs = (n + 3) >> 2, stride = (int64_t)gridDim.x * kThreads;
@@ -323,15 +305,7 @@ __device__ __forceinline__ bool update_body(int64_t n, const T* __restrict__ x, 
         store4<T, Hint::Plain, VEC>(y_out, i0, cnt, y);
     }
     double dacc[2] = {(double)acc[0], (double)acc[1]};
-    return grid_reduce<2>(dacc, rb);
-}
-
-template <class T, bool VEC>
-__global__ void __launch_bounds__(kThreads) k_update(int64_t n, const T* __restrict__ x, const T* __restrict__ xp,
-                                                     const T* __restrict__ g, const T* __restrict__ gp,
-                                                     T* __restrict__ s_out, T* __restrict__ y_out, ReduceBuf rb)
-{
-    update_body<T, VEC>(n, x, xp, g, gp, s_out, y_out, rb);
+    grid_reduce<2>(dacc, rb);
 }
 
 // {s.y, y.y} of an explicitly given pair while copying it into the slot (BFGSMat::add_correction)
@@ -502,11 +476,6 @@ lbfgs_b200_status lbfgs_b200_ctx_create(lbfgs_b200_ctx** out, int device, void* 
         return LBFGS_B200_ERR_CUDA;
     }
     ctx->sm_count = prop.multiProcessorCount;
-    if (const char* e = getenv("LBFGS_B200_CTAS_PER_SM"))
-    {
-        const int v = atoi(e);
-        if (v >= 1 && v <= 8) ctx->ctas_per_sm_cap = v;
-    }
     if (stream) ctx->stream = static_cast<cudaStream_t>(stream);
     else { CUC(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking)); ctx->own_stream = true; }
     CUC(cudaMalloc(&ctx->rb.partials, sizeof(double) * kMaxBlocks * kMaxRed));
@@ -1083,6 +1052,24 @@ template <class T> static void fill_slots(const lbfgs_b200_hist* h, unsigned cha
 // h->head and takes part as the newest column, exactly as if it had been appended already; the caller commits or discards it.
 template <class T> struct PairForm { const T* x; const T* xp; const T* gp; };
 
+// k_gram_dots for `rounds` rounds of column pairs.  The opt-in for > 48 KB of dynamic shared memory is per device and
+// instantiation: the context remembers which instantiations have it.
+template <class T, bool FORM>
+static lbfgs_b200_status launch_gram_dots(lbfgs_b200_ctx* ctx, const GramDotsArgs<T>& a, int rounds, int grid, int threads, size_t smem,
+                                          const XComm* xc, unsigned long long epoch)
+{
+    const int r = rounds <= 1 ? 1 : rounds == 2 ? 2 : 3;
+    const auto kernel = r == 1 ? k_gram_dots<T, 1, FORM> : r == 2 ? k_gram_dots<T, 2, FORM> : k_gram_dots<T, 3, FORM>;
+    const unsigned bit = 1u << ((FORM ? 8 : 0) + (sizeof(T) == 8 ? 0 : 4) + r);
+    if (!(ctx->smem_optin & bit))
+    {
+        CU(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ctx->smem_optin |= bit;
+    }
+    kernel<<<grid, threads, smem, ctx->stream>>>(a, ctx->gram_partials, ctx->rb.ticket, ctx->gram_raw, xc, epoch);
+    return post_launch(ctx, FORM ? "k_gram_dots<FORM>" : "k_gram_dots");
+}
+
 template <class T>
 static lbfgs_b200_status gram_dots(lbfgs_b200_hist* h, const T* v, const PairForm<T>* form = nullptr)
 {
@@ -1117,30 +1104,8 @@ static lbfgs_b200_status gram_dots(lbfgs_b200_hist* h, const T* v, const PairFor
     const size_t smem = (size_t)kGramStages * (form ? 4 : 3) * kGramTE * sizeof(T);
     const XComm* xc = ctx->x_active ? ctx->x_comm : nullptr;
     const unsigned long long epoch = ctx->x_active ? ++ctx->x_epoch : 0ull;
-#define LAUNCH_GRAM(KERNEL, R, BASE)                                                                         \
-    do {                                                                                                     \
-        /* the opt-in for > 48 KB of dynamic shared memory is per device: remember it per context */        \
-        const unsigned bit = 1u << (BASE + (sizeof(T) == 8 ? 0 : 4) + R);                                    \
-        if (!(ctx->smem_optin & bit)) {                                                                      \
-            CU(ctx, cudaFuncSetAttribute(KERNEL<T, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-            ctx->smem_optin |= bit;                                                                          \
-        }                                                                                                    \
-        KERNEL<T, R><<<grid, threads, smem, ctx->stream>>>(a, ctx->gram_partials, ctx->rb.ticket, ctx->gram_raw, xc, epoch); \
-    } while (0)
-    if (form)
-    {
-        if (rounds <= 1) LAUNCH_GRAM(k_pair_dots, 1, 8);
-        else if (rounds == 2) LAUNCH_GRAM(k_pair_dots, 2, 8);
-        else LAUNCH_GRAM(k_pair_dots, 3, 8);
-    }
-    else
-    {
-        if (rounds <= 1) LAUNCH_GRAM(k_gram_dots, 1, 0);
-        else if (rounds == 2) LAUNCH_GRAM(k_gram_dots, 2, 0);
-        else LAUNCH_GRAM(k_gram_dots, 3, 0);
-    }
-#undef LAUNCH_GRAM
-    if (auto st = post_launch(ctx, form ? "k_pair_dots" : "k_gram_dots")) return st;
+    if (auto st = form ? launch_gram_dots<T, true>(ctx, a, rounds, grid, threads, smem, xc, epoch)
+                       : launch_gram_dots<T, false>(ctx, a, rounds, grid, threads, smem, xc, epoch)) return st;
     if (ctx->nranks > 1 && !ctx->x_active)
         NC(ctx, ncclAllReduce(ctx->gram_raw, ctx->gram_raw, c * kGramVals, ncclDouble, ncclSum, ctx->comm, ctx->stream));
     return LBFGS_B200_OK;
@@ -1159,8 +1124,6 @@ template <class T> static GramSolveArgs<T> make_solve_args(lbfgs_b200_hist* h, T
     g.SS_out = static_cast<T*>(h->SS[out]);
     g.ys = static_cast<const T*>(h->ys); g.alpha = static_cast<T*>(h->alpha);
     g.theta = static_cast<const T*>(h->theta);
-    g.ov_slot = -1;
-    g.ov_theta_on = 0;
     fill_slots<T>(h, g.slots);
     return g;
 }
@@ -1229,7 +1192,7 @@ static lbfgs_b200_status do_hist_apply_Hv(lbfgs_b200_hist* h, const T* v, T a, T
     if (auto st = hist_check<T>(h)) return st;
     lbfgs_b200_ctx* ctx = h->ctx;
     REQUIRE(ctx, v && res && v != res, "apply_Hv: v/res NULL or aliased");
-    REQUIRE(ctx, algo >= LBFGS_B200_HV_AUTO && algo <= LBFGS_B200_HV_GRAM_UNFUSED, "apply_Hv: unknown algorithm %d", algo);
+    REQUIRE(ctx, algo >= LBFGS_B200_HV_AUTO && algo <= LBFGS_B200_HV_GRAM, "apply_Hv: unknown algorithm %d", algo);
     const bool gram = (algo != LBFGS_B200_HV_TWO_LOOP) && h->ncorr > 0;
     ProfSpan span(ctx, PH_APPLY_HV, double(sizeof(T)) * double(h->n) * (4.0 * h->ncorr + 2.0));
     lbfgs_b200_status st = gram ? hv_gram<T>(h, v, a, res, vdot_host != nullptr)
@@ -1245,7 +1208,7 @@ static lbfgs_b200_status do_hist_apply_Hv(lbfgs_b200_hist* h, const T* v, T a, T
 }
 
 // LBFGS.h:159-165 as one call: { s = x - xp; y = g - gp; if (s'y > eps*y'y) add_correction(s, y); res = a*H*g } (+ g.res).
-// With the Gram form the pair is formed inside the dots pass (k_pair_dots): no separate update kernel, x/xp/g/gp are read
+// With the Gram form the pair is formed inside the dots pass (k_gram_dots<FORM>): no separate update kernel, x/xp/g/gp are read
 // once, s and y are written once.  The pair is committed only after the gate has seen s'y, y'y (its own dots); a rejected
 // pair leaves the history untouched and the old history answers, as in the reference.
 template <class T>
@@ -1256,8 +1219,8 @@ static lbfgs_b200_status do_hist_update_apply_Hv(lbfgs_b200_hist* h, const T* x,
     lbfgs_b200_ctx* ctx = h->ctx;
     REQUIRE(ctx, x && xp && g && gp && res, "update_apply_Hv: NULL vector");
     REQUIRE(ctx, res != g && res != x && res != xp && res != gp, "update_apply_Hv: res aliases an input");
-    REQUIRE(ctx, algo >= LBFGS_B200_HV_AUTO && algo <= LBFGS_B200_HV_GRAM_UNFUSED, "update_apply_Hv: unknown algorithm %d", algo);
-    if (algo == LBFGS_B200_HV_TWO_LOOP || algo == LBFGS_B200_HV_GRAM_UNFUSED || !all_aligned<T>({x, xp, g, gp}))
+    REQUIRE(ctx, algo >= LBFGS_B200_HV_AUTO && algo <= LBFGS_B200_HV_GRAM, "update_apply_Hv: unknown algorithm %d", algo);
+    if (algo == LBFGS_B200_HV_TWO_LOOP || !all_aligned<T>({x, xp, g, gp}))
     {
         if (auto st = do_hist_update<T>(h, x, xp, g, gp, eps, accepted_host, nullptr)) return st;
         return do_hist_apply_Hv<T>(h, g, a, res, algo, vdot_host);

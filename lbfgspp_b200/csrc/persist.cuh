@@ -12,8 +12,6 @@
 //     COMBINE_TRIAL  COMBINE + the first trial of the next line search in the same pass: the reference restarts every search
 //                    at step = 1 (LBFGS.h:168), so x1 = x + d, g1 = grad f(x1) ; {g.d, f1, g1.d, g1.g1, x1.x1}
 //     RESTORE        x = xp, g = gp (a search that never improved on its start point; LineSearchMoreThuente.h:602-614)
-//     MATERIALIZE    x = xp + step*d, g = grad f(x) for a trial whose sums are already known: optional policy in which the fused first trial
-//                    does not store x1, g1 while first trials keep being rejected (see digest_trial; off by default)
 // Every CTA owns the same contiguous chunk (granularity: the block length of the tiled history) of EVERY vector in EVERY pass, so a CTA only ever reads vector
 // elements it wrote itself (halo coordinates excepted, those are read through L2) and streams long contiguous runs.  Between rounds there is one
 // grid-wide synchronisation: CTAs deposit their partial sums in fixed slots, CTA 0 adds them in a fixed order (deterministic: no
@@ -44,9 +42,8 @@ constexpr int kPStageBytes = kGramStages * 4 * kGramTE * 8;   // dynamic shared 
 constexpr int kPMaxStages = 4;
 constexpr int kPCache = 4;                   // problems whose leader-side state is kept in shared memory
 
-enum { POP_IDLE = 0, POP_FIRST = 1, POP_TRIAL = 2, POP_DOTS_FORM = 3, POP_DOTS_PLAIN = 4, POP_COMBINE = 5, POP_COMBINE_TRIAL = 6, POP_RESTORE = 7,
-       POP_MATERIALIZE = 8 };
-constexpr int kPOps = 10;   // accounting slots (ops + the "mixed" bucket 0)
+enum { POP_IDLE = 0, POP_FIRST = 1, POP_TRIAL = 2, POP_DOTS_FORM = 3, POP_DOTS_PLAIN = 4, POP_COMBINE = 5, POP_COMBINE_TRIAL = 6, POP_RESTORE = 7 };
+constexpr int kPOps = 10;   // accounting slots (ops + the "mixed" bucket 0; 8 and 9 unused, kept for the solver_profile ABI)
 constexpr int kPGramScratch = 1024;   // doubles
 
 // ---- the S/Y history of the solve: tiled layout ---------------------------------------------------------------------------------
@@ -92,12 +89,6 @@ template <class T> struct PState
     LBFGSpp::MoreThuenteCore<T> mt;
     int have_lo;
     T lo_gg, lo_xx, start_gg, start_xx;
-    // the fused first trial of a search may be "virtual": evaluated and reduced, but x1 / g1 not stored
-    int first_store;            // policy for the next COMBINE_TRIAL pass: 1 = store x1, g1
-    int adaptive_first_store;   // 1: first_store follows the fate of the last first trial (accepted -> store); 0: always store
-    int lo_virtual;             // the best-so-far point (x_lo, g_lo) is the virtual first trial: materialise it at lo_step if needed
-    T lo_step;
-    int after_materialize;      // what MATERIALIZE was for: 1 = the accepted trial, 2 = the best-so-far point
     // iteration scalars
     T fx, dg, gg, xx, gnorm, step;
     int k;
@@ -116,7 +107,7 @@ template <class T> struct alignas(128) PRound
 {
     T *x, *xp, *g, *gp, *drt;
     T step;
-    int op, c_round, head, pending, gram_cur, store_first;
+    int op, c_round, head, pending, gram_cur;
 };
 
 struct alignas(128) PCtl
@@ -154,9 +145,9 @@ template <class T> struct PArgs
     const XComm* xc;
     int64_t index_offset, n_global;
     long long wait_cycles;      // watchdog budget of a grid-barrier wait (clock64 ticks); cross-rank waits get 4x, the release wait 6x
-    int tune;                   // 4 = the trial pass stores x, g with L2 evict-first: +3 % on that pass at n = 1e7 (set by the host when the vectors cannot stay
-                                // in L2 anyway; LBFGS_B200_TUNE overrides).  Measured and dropped: unrolling the pass 4x (no change), prefetching its inputs
-                                // into L2 (-5 %), a grid-stride instead of a chunked sweep (+1 %)
+    bool evict_first_stores;    // the trial pass stores x, g with L2 evict-first: +3 % on that pass at n = 1e7 (set by the host when the vectors cannot stay
+                                // in L2 anyway).  Measured and dropped: unrolling the pass 4x (no change), prefetching its inputs into L2 (-5 %), a
+                                // grid-stride instead of a chunked sweep (+1 %)
 };
 
 template <class V> __device__ __forceinline__ V ldv(const V* p) { return *reinterpret_cast<const volatile V*>(p); }
@@ -281,47 +272,33 @@ template <int NV> __device__ __forceinline__ void block_sums(const double (&acc)
 
 // ---- FIRST / TRIAL -------------------------------------------------------------------------------------------------------------
 // MODE 0: FIRST (evaluate at x, write g and d = -g) ; MODE 1: TRIAL (x = xp + step*d, write x and g).  Operands stream through
-// registers with 128-bit loads/stores (a shared-memory staged variant measured slower for this 1:1 read/write pass).
+// registers with 128-bit loads/stores (a shared-memory staged variant measured slower for this 1:1 read/write pass).  Objectives
+// without neighbour coupling only: the coupled ones take p_trial_halo.
 template <class T, class OBJ, int MODE>
 __device__ __forceinline__ void p_trial(const OBJ& obj, const Own& own, const T* __restrict__ xp, const T* __restrict__ d, T step,
-                                        T* __restrict__ x, T* __restrict__ g, T* __restrict__ dout, PShared& sh, double* dst, int G, int tune)
+                                        T* __restrict__ x, T* __restrict__ g, T* __restrict__ dout, PShared& sh, double* dst, int G, bool evict_first)
 {
+    static_assert(!OBJ::kHalo, "neighbour-coupled objectives take p_trial_halo");
     T acc[4] = {T(0), T(0), T(0), T(0)};
     const int64_t n = own.n;
     const int64_t p1 = (own.c1 + 3) >> 2;
-    const bool evict_first = (tune & 4) != 0;
     auto body = [&](int64_t q) {
         const int64_t i0 = q << 2;
         const int cnt = (n - i0 >= 4) ? 4 : int(n - i0);
         T xv[4], dv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
-        T xl = T(0), xr = T(0);
         if (MODE == 1)
         {
             const Pack<T> px = load4<T, Hint::Stream, true>(xp, i0, cnt), pd = load4<T, Hint::Stream, true>(d, i0, cnt);
 #pragma unroll
             for (int k = 0; k < 4; k++) { dv[k] = pd.v[k]; xv[k] = px.v[k] + step * pd.v[k]; }
-            if constexpr (OBJ::kHalo)
-            {
-                if (i0 > 0) xl = __ldcg(xp + i0 - 1) + step * __ldcg(d + i0 - 1);
-                else if (obj.halo && obj.gofs > 0) xl = T(ldv(obj.halo + kHaloLeftA)) + step * T(ldv(obj.halo + kHaloLeftB));
-                if (i0 + 4 < n) xr = __ldcg(xp + i0 + 4) + step * __ldcg(d + i0 + 4);
-                else if (obj.halo && i0 + 4 == n && obj.gofs + n < obj.n_glob) xr = T(ldv(obj.halo + kHaloRightA)) + step * T(ldv(obj.halo + kHaloRightB));
-            }
         }
         else
         {
             const Pack<T> px = load4<T, Hint::Stream, true>(x, i0, cnt);
 #pragma unroll
             for (int k = 0; k < 4; k++) xv[k] = px.v[k];
-            if constexpr (OBJ::kHalo)
-            {
-                if (i0 > 0) xl = __ldcg(x + i0 - 1);
-                else if (obj.halo && obj.gofs > 0) xl = T(ldv(obj.halo + kHaloLeftA));
-                if (i0 + 4 < n) xr = __ldcg(x + i0 + 4);
-                else if (obj.halo && i0 + 4 == n && obj.gofs + n < obj.n_glob) xr = T(ldv(obj.halo + kHaloRightA));
-            }
         }
-        acc[0] += obj.eval(i0, cnt, xv, xl, xr, gv);
+        acc[0] += obj.eval(i0, cnt, xv, T(0), T(0), gv);
         Pack<T> pg, po;
 #pragma unroll
         for (int k = 0; k < 4; k++)
@@ -795,11 +772,8 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
                         ug.v[k] = gv[k];
                         uo.v[k] = xv[k];
                     }
-                    if (x1_out != nullptr)
-                    {
-                        st_unit<T>(x1_out, i0, cnt, uo);
-                        st_unit<T>(g1_out, i0, cnt, ug);
-                    }
+                    st_unit<T>(x1_out, i0, cnt, uo);
+                    st_unit<T>(g1_out, i0, cnt, ug);
                 }
             }
         }
@@ -903,11 +877,8 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
                     ug.v[k] = gv[k];
                     uo.v[k] = xv[k];
                 }
-                if (x1_out != nullptr)
-                {
-                    st_unit<T>(x1_out, i0, cnt, uo);
-                    st_unit<T>(g1_out, i0, cnt, ug);
-                }
+                st_unit<T>(x1_out, i0, cnt, uo);
+                st_unit<T>(g1_out, i0, cnt, ug);
             }
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -985,37 +956,22 @@ template <class T> __device__ __forceinline__ void after_search(PState<T>* st)
     st->c_round = st->ncorr < st->m ? st->ncorr + 1 : st->m;
 }
 
-// the trial at ls_step_ref(st) has been evaluated: {fx, dg, gg, xx}.  Sets the next op.  `is_virtual`: the fused first trial
-// whose x1 / g1 were not stored (they are x = xp + 1*d and its gradient: a MATERIALIZE pass recomputes them bit for bit if the
-// search turns out to need them).  Adaptive policy (off by default, LBFGS_B200_VIRTUAL_FIRST_TRIAL=1): store the next first trial
-// iff this one was accepted.  Measured on config 2 (3 of 21 first trials accepted): 0.25 ms saved in the combination passes,
-// 0.20 ms spent on the three MATERIALIZE rounds -- a wash at n = 1e7 and a loss at n = 1e6, hence off.
-template <class T> __device__ __forceinline__ void digest_trial(PState<T>* st, T fx, T dg, T gg, T xx, bool is_first, bool is_virtual)
+// the trial at ls_step_ref(st) has been evaluated into (x, g): {fx, dg, gg, xx}.  Sets the next op.
+template <class T> __device__ __forceinline__ void digest_trial(PState<T>* st, T fx, T dg, T gg, T xx)
 {
     record_eval(st, fx);
     bool keep = false;
-    const T step_tried = ls_step_ref(st);
     const int rc = ls_advance(st, fx, dg, keep);
-    if (is_first && st->adaptive_first_store) st->first_store = (rc == LBFGSpp::LSC_ACCEPT) ? 1 : 0;
     if (keep)
     {
-        if (is_virtual) { st->lo_virtual = 1; st->lo_step = step_tried; }
-        else
-        {
-            dswap(st->x, st->x_lo);
-            dswap(st->g, st->g_lo);
-            st->lo_virtual = 0;
-        }
+        dswap(st->x, st->x_lo);
+        dswap(st->g, st->g_lo);
         st->have_lo = 1;
         st->lo_gg = gg;
         st->lo_xx = xx;
     }
     if (rc == LBFGSpp::LSC_EVALUATE) { st->op = POP_TRIAL; st->step = ls_step_ref(st); return; }
-    if (rc == LBFGSpp::LSC_ACCEPT)
-    {
-        st->fx = fx; st->dg = dg; st->gg = gg; st->xx = xx;
-        if (is_virtual) { st->op = POP_MATERIALIZE; st->step = step_tried; st->after_materialize = 1; return; }
-    }
+    if (rc == LBFGSpp::LSC_ACCEPT) { st->fx = fx; st->dg = dg; st->gg = gg; st->xx = xx; }
     else if (rc == LBFGSpp::LSC_TAKE_BEST)
     {
         T bf, bd;
@@ -1026,7 +982,6 @@ template <class T> __device__ __forceinline__ void digest_trial(PState<T>* st, T
         {
             st->gg = st->lo_gg;
             st->xx = st->lo_xx;
-            if (st->lo_virtual) { st->op = POP_MATERIALIZE; st->step = st->lo_step; st->after_materialize = 2; return; }
             dswap(st->x, st->x_lo);
             dswap(st->g, st->g_lo);
         }
@@ -1052,7 +1007,6 @@ template <class T> __device__ __forceinline__ bool begin_search(PState<T>* st, T
     dswap(st->xp, st->x);
     dswap(st->gp, st->g);
     st->have_lo = 0;
-    st->lo_virtual = 0;
     st->start_gg = st->gg;
     st->start_xx = st->xx;
     st->op = POP_TRIAL;
@@ -1080,10 +1034,9 @@ template <class T> __device__ void advance_problem(PState<T>* st, const double* 
         return;
     }
     case POP_TRIAL:
-        digest_trial(st, (T)vals[0], (T)vals[1], (T)vals[2], (T)vals[3], false, false);
+        digest_trial(st, (T)vals[0], (T)vals[1], (T)vals[2], (T)vals[3]);
         return;
-    case POP_RESTORE:
-    case POP_MATERIALIZE:       // (x, g) now hold the search's point; its sums were digested before
+    case POP_RESTORE:           // (x, g) now hold the search's start point; its sums were restored before
         after_search(st);
         return;
     case POP_DOTS_FORM:
@@ -1110,13 +1063,12 @@ template <class T> __device__ void advance_problem(PState<T>* st, const double* 
     case POP_COMBINE_TRIAL:
     {
         const bool fused = st->op == POP_COMBINE_TRIAL;
-        const bool stored = st->first_store != 0;      // what this pass was told (the policy flag changes in digest_trial)
         if (st->pending >= 0) { st->gram_cur = 1 - st->gram_cur; st->pending = -1; }
         st->dg = (T)vals[0];                // LBFGS.h:123 for the next pass
         st->k += 1;
         if (!begin_search(st, T(1))) return;   // LBFGS.h:168
         // the pass already evaluated x + 1*d into the buffers that the rotation just made (x, g)
-        if (fused && ls_step_ref(st) == T(1)) digest_trial(st, (T)vals[1], (T)vals[2], (T)vals[3], (T)vals[4], true, !stored);
+        if (fused && ls_step_ref(st) == T(1)) digest_trial(st, (T)vals[1], (T)vals[2], (T)vals[3], (T)vals[4]);
         return;
     }
     default: return;
@@ -1124,17 +1076,17 @@ template <class T> __device__ void advance_problem(PState<T>* st, const double* 
 }
 
 // n-words a pass has to move (reads + writes of whole vectors): the roofline numerator of the persistent kernel
-__device__ __forceinline__ double words_of(int op, int c, int data_vectors, int store_first)
+__device__ __forceinline__ double words_of(int op, int c, int data_vectors)
 {
     switch (op)
     {
     case POP_FIRST: return 3.0 + data_vectors;              // R x ; W g, d
-    case POP_TRIAL: case POP_MATERIALIZE: return 4.0 + data_vectors;   // R xp, d ; W x, g
+    case POP_TRIAL: return 4.0 + data_vectors;              // R xp, d ; W x, g
     case POP_RESTORE: return 4.0;                           // R xp, gp ; W x, g
     case POP_DOTS_FORM: return 2.0 * c + 4.0;               // R x, xp, g, gp, 2(c-1) columns ; W s, y
     case POP_DOTS_PLAIN: return 2.0 * c + 1.0;              // R g, 2c columns
     case POP_COMBINE: return 2.0 * c + 2.0;                 // R g, 2c columns ; W d
-    case POP_COMBINE_TRIAL: return 2.0 * c + 3.0 + (store_first ? 2.0 : 0.0) + data_vectors;   // R g, x, 2c columns ; W d (, x1, g1)
+    case POP_COMBINE_TRIAL: return 2.0 * c + 5.0 + data_vectors;   // R g, x, 2c columns ; W d, x1, g1
     default: return 0.0;
     }
 }
@@ -1143,7 +1095,7 @@ template <class T> __device__ __forceinline__ int nvals_of(const PState<T>* st)
 {
     switch (st->op)
     {
-    case POP_FIRST: case POP_TRIAL: case POP_MATERIALIZE: return 4;
+    case POP_FIRST: case POP_TRIAL: return 4;
     case POP_DOTS_FORM: case POP_DOTS_PLAIN: return st->c_round * kGramVals;
     case POP_COMBINE: return 1;
     case POP_COMBINE_TRIAL: return 5;
@@ -1270,7 +1222,6 @@ __device__ int leader_round(const PArgs<T>& a, int G, PShared& sh, PState<T>* ca
             rd->x = st->x; rd->xp = st->xp; rd->g = st->g; rd->gp = st->gp; rd->drt = st->drt;
             rd->step = st->step;
             rd->c_round = st->c_round; rd->head = st->head; rd->pending = st->pending; rd->gram_cur = st->gram_cur;
-            rd->store_first = st->first_store;
             rd->op = st->op;
             running = st->op != POP_IDLE;
         }
@@ -1424,22 +1375,20 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
             T* const vx = ldv(&rd->x); T* const vxp = ldv(&rd->xp); T* const vg = ldv(&rd->g); T* const vgp = ldv(&rd->gp); T* const vd = ldv(&rd->drt);
             const T step = ldv(&rd->step);
             const int c_round = ldv(&rd->c_round), head = ldv(&rd->head), pending = ldv(&rd->pending), gram_cur = ldv(&rd->gram_cur);
-            const int store_first = ldv(&rd->store_first);
             if (op == POP_IDLE) continue;
             acct_bucket = (acct_bucket == -1 || acct_bucket == op) ? op : 0;
-            acct_words += words_of(op, c_round, kDataVectors, store_first);
+            acct_words += words_of(op, c_round, kDataVectors);
             double* dst = a.partials + (size_t)b * a.pstride * G + cta;
             const OBJ obj = PObjMaker<T, OBJ>::make(a, st->data0, st->data1, (HALO && a.xc != nullptr) ? st->halo : nullptr);
             switch (op)
             {
             case POP_FIRST:
                 if constexpr (HALO) p_trial_halo<T, OBJ, 0>(obj, own, nullptr, nullptr, T(0), vx, vg, vd, tiles, sh, phase_bits, dst, G);
-                else p_trial<T, OBJ, 0>(obj, own, nullptr, nullptr, T(0), vx, vg, vd, sh, dst, G, a.tune);
+                else p_trial<T, OBJ, 0>(obj, own, nullptr, nullptr, T(0), vx, vg, vd, sh, dst, G, a.evict_first_stores);
                 break;
             case POP_TRIAL:
-            case POP_MATERIALIZE:
                 if constexpr (HALO) p_trial_halo<T, OBJ, 1>(obj, own, vxp, vd, step, vx, vg, nullptr, tiles, sh, phase_bits, dst, G);
-                else p_trial<T, OBJ, 1>(obj, own, vxp, vd, step, vx, vg, nullptr, sh, dst, G, a.tune);
+                else p_trial<T, OBJ, 1>(obj, own, vxp, vd, step, vx, vg, nullptr, sh, dst, G, a.evict_first_stores);
                 break;
             case POP_RESTORE:
                 p_restore<T>(own, vxp, vgp, vx, vg);
@@ -1477,7 +1426,6 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
                 g.SY_in = st->SY[in]; g.YY_in = st->YY[in]; g.SS_in = st->SS[in];
                 g.SY_out = st->SY[out]; g.YY_out = st->YY[out]; g.SS_out = st->SS[out];
                 g.ys = st->ys; g.alpha = st->alpha; g.theta = st->theta;
-                g.ov_slot = -1; g.ov_theta_on = 0;
                 for (int age = 0; age < g.c; age++) g.slots[age] = (unsigned char)slot_by_age(head, g.M, age);
                 __syncthreads();   // the tile area / tables may still be in use by the previous problem's pass
                 // per age: packed row of the column in a staged block, and its ring slot
@@ -1502,7 +1450,7 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
                 };
                 if (!own_scratch) solve_into(tiles);   // a long history: the staging ring is the scratch, the copies start afterwards
                 auto between = [&]() { if (own_scratch) solve_into(reinterpret_cast<T*>(s_gram)); };
-                if (fuse) p_combine<T, OBJ, true, OBJ::kHalo>(obj, own, st->hist, g.c, head, tiles, vd, store_first ? vxp : nullptr, store_first ? vgp : nullptr, sh, phase_bits, dst, G, between);
+                if (fuse) p_combine<T, OBJ, true, OBJ::kHalo>(obj, own, st->hist, g.c, head, tiles, vd, vxp, vgp, sh, phase_bits, dst, G, between);
                 else p_combine<T, OBJ, false, false>(obj, own, st->hist, g.c, head, tiles, vd, nullptr, nullptr, sh, phase_bits, dst, G, between);
                 break;
             }

@@ -120,8 +120,6 @@ static lbfgs_b200_status solver_minimize(lbfgs_b200_solver* s, int objective, co
         // the first trial of every search rides on the combination pass; a neighbour-coupled objective needs its neighbours' x + d,
         // which only exist on this rank when n is not sharded
         p.fuse_first_trial = (coupled && ctx->nranks > 1) ? 0 : 1;
-        p.adaptive_first_store = (getenv("LBFGS_B200_VIRTUAL_FIRST_TRIAL") && atoi(getenv("LBFGS_B200_VIRTUAL_FIRST_TRIAL")) != 0) ? 1 : 0;
-        p.first_store = p.adaptive_first_store ? 0 : 1;
         p.ls_opt.linesearch = (ls_kind == 3) ? 3 : prm->linesearch;
         p.ls_opt.max_linesearch = prm->max_linesearch;
         p.ls_opt.min_step = (T)prm->min_step; p.ls_opt.max_step = (T)prm->max_step; p.ls_opt.ftol = (T)prm->ftol; p.ls_opt.wolfe = (T)prm->wolfe;
@@ -135,7 +133,7 @@ static lbfgs_b200_status solver_minimize(lbfgs_b200_solver* s, int objective, co
     {
         const PState<T>& p = hs[b];
         hr[b].x = p.x; hr[b].xp = p.xp; hr[b].g = p.g; hr[b].gp = p.gp; hr[b].drt = p.drt;
-        hr[b].step = T(0); hr[b].op = p.op; hr[b].c_round = 0; hr[b].head = 0; hr[b].pending = -1; hr[b].gram_cur = p.gram_cur; hr[b].store_first = p.first_store;
+        hr[b].step = T(0); hr[b].op = p.op; hr[b].c_round = 0; hr[b].head = 0; hr[b].pending = -1; hr[b].gram_cur = p.gram_cur;
     }
     // BFGSMat::reset (BFGSMat.h:61-78): no pairs, theta = 1, Gram matrices cleared
     CU(ctx, cudaMemsetAsync(s->d_small, 0, sizeof(T) * s->small_elems * (size_t)B, ctx->stream));
@@ -165,8 +163,7 @@ static lbfgs_b200_status solver_minimize(lbfgs_b200_solver* s, int objective, co
     a.index_offset = index_offset; a.n_global = n_global;
     a.wait_cycles = kPWaitCycles;
     if (const char* e = getenv("LBFGS_B200_WATCHDOG_SCALE")) { const long long k = atoll(e); if (k >= 1 && k <= 100000) a.wait_cycles *= k; }
-    a.tune = ((size_t)s->n * sizeof(T) * 4 > ((size_t)36 << 20)) ? 4 : 0;     // x, xp, g, d of one problem exceed ~3/4 of the 50 MB L2
-    if (const char* e = getenv("LBFGS_B200_TUNE")) a.tune = atoi(e);
+    a.evict_first_stores = (size_t)s->n * sizeof(T) * 4 > ((size_t)36 << 20);     // x, xp, g, d of one problem exceed ~3/4 of the 50 MB L2
     void* kargs[] = {&a};
     CU(ctx, cudaEventRecord(s->ev0, ctx->stream));
     CU(ctx, cudaLaunchCooperativeKernel(kernel, dim3((unsigned)grid), dim3(kPThreads), kargs, smem, ctx->stream));
@@ -264,9 +261,8 @@ lbfgs_b200_status lbfgs_b200_solver_create_batch(lbfgs_b200_ctx* ctx, int64_t n,
     s->M = m + 1;
     // block length of the tiled history: the largest power of two for which two stages of 2m+4 rows fit the kernel's staging ring
     {
-        int bt = 1024, want_stages = 2;
-        if (const char* e = getenv("LBFGS_B200_STAGES")) { const int v = atoi(e); if (v >= 1 && v <= lb::kPMaxStages) want_stages = v; }
-        while (bt > 32 && (size_t)want_stages * (2 * m + 4) * bt * elem_bytes > (size_t)lb::kPStageBytes) bt >>= 1;
+        int bt = 1024;
+        while (bt > 32 && (size_t)2 * (2 * m + 4) * bt * elem_bytes > (size_t)lb::kPStageBytes) bt >>= 1;
         s->bt_log = 0;
         while ((1 << s->bt_log) < bt) s->bt_log++;
     }

@@ -106,8 +106,9 @@ __device__ __forceinline__ Pack<float> lds_pack(const float* p, int)
     return r;
 }
 
-template <class T, int ROUNDS, bool FORM = false>
-__device__ __forceinline__ void gram_dots_body(const GramDotsArgs<T>& a, double* partials, unsigned* ticket, double* result, const XComm* xc, unsigned long long epoch)
+// FORM ("update + dots"): forms the newest pair from (x, xp, g, gp) while it computes [S Y]'[g s_new y_new]  (see GramDotsArgs)
+template <class T, int ROUNDS, bool FORM>
+__global__ void __launch_bounds__(kGramMaxThreads, 1) k_gram_dots(GramDotsArgs<T> a, double* partials, unsigned* ticket, double* result, const XComm* xc, unsigned long long epoch)
 {
     constexpr int NT = FORM ? 4 : 3;                             // staged vectors per tile: v, s_new, y_new (+ xp while forming)
     extern __shared__ __align__(128) unsigned char gram_smem[];
@@ -374,19 +375,6 @@ __device__ __forceinline__ void gram_dots_body(const GramDotsArgs<T>& a, double*
     }
 }
 
-template <class T, int ROUNDS>
-__global__ void __launch_bounds__(kGramMaxThreads, 1) k_gram_dots(GramDotsArgs<T> a, double* partials, unsigned* ticket, double* result, const XComm* xc, unsigned long long epoch)
-{
-    gram_dots_body<T, ROUNDS>(a, partials, ticket, result, xc, epoch);
-}
-
-// "update + dots": forms the newest pair from (x, xp, g, gp) while it computes [S Y]'[g s_new y_new]  (see GramDotsArgs)
-template <class T, int ROUNDS>
-__global__ void __launch_bounds__(kGramMaxThreads, 1) k_pair_dots(GramDotsArgs<T> a, double* partials, unsigned* ticket, double* result, const XComm* xc, unsigned long long epoch)
-{
-    gram_dots_body<T, ROUNDS, true>(a, partials, ticket, result, xc, epoch);
-}
-
 // ---- the O(c^2) recursion on coefficients ---------------------------------------------------------------------
 // Runs in shared memory in the prologue of EVERY CTA of the combine kernel (identical arithmetic everywhere, ~2 us,
 // no extra launch); CTA 0 also writes the folded Gram matrices and the alphas back for the next call.
@@ -404,11 +392,6 @@ template <class T> struct GramSolveArgs
     const T* ys;             // [M]
     T* alpha;                // [M]
     const T* theta;
-    // overrides used by the device-resident solve, where the newest pair's ys / theta are committed only after this kernel:
-    int ov_slot;             // physical slot whose ys is `ov_ys` (-1: none)
-    T ov_ys;
-    int ov_theta_on;
-    T ov_theta;
     unsigned char slots[kMaxM];
 };
 
@@ -459,9 +442,9 @@ __device__ void gram_solve_in_smem(const GramSolveArgs<T>& g, T* sm, bool writer
         {
             b0[i] = g.a * (T)__ldcg(g.raw + i * kGramVals + 0);
             b1[i] = g.a * (T)__ldcg(g.raw + i * kGramVals + 1);
-            ysv[i] = (g.slots[i] == g.ov_slot) ? g.ov_ys : __ldcg(g.ys + g.slots[i]);
+            ysv[i] = __ldcg(g.ys + g.slots[i]);
         }
-        if (tid == nt - 1) th[0] = g.ov_theta_on ? g.ov_theta : __ldcg(g.theta);
+        if (tid == nt - 1) th[0] = __ldcg(g.theta);
     }
     __syncthreads();
     if (tid < 32 && g.with_v)
@@ -535,9 +518,8 @@ template <class T> struct GramCombineArgs
     GramSolveArgs<T> solve;
 };
 
-// returns true in the last CTA (after the optional v.res reduction); the stand-alone kernel ignores it
 template <class T, bool VEC>
-__device__ __forceinline__ bool gram_combine_body(const GramCombineArgs<T>& a, const ReduceBuf& rb)
+__global__ void __launch_bounds__(kThreads) k_gram_combine(GramCombineArgs<T> a, ReduceBuf rb)
 {
     extern __shared__ __align__(16) unsigned char comb_smem[];
     T* sm = reinterpret_cast<T*>(comb_smem);
@@ -592,15 +574,8 @@ __device__ __forceinline__ bool gram_combine_body(const GramCombineArgs<T>& a, c
     if (a.want_dot)
     {
         double dacc[1] = {(double)dot};
-        return grid_reduce<1>(dacc, rb);
+        grid_reduce<1>(dacc, rb);
     }
-    return false;
-}
-
-template <class T, bool VEC>
-__global__ void __launch_bounds__(kThreads) k_gram_combine(GramCombineArgs<T> a, ReduceBuf rb)
-{
-    gram_combine_body<T, VEC>(a, rb);
 }
 
 }  // namespace lb
