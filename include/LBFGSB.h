@@ -23,6 +23,7 @@
 #include "LBFGSpp/DeviceVector.h"
 #include "LBFGSpp/LineSearchDriver.h"
 #include "LBFGSpp/LineSearchMoreThuente.h"
+#include "LBFGSpp/LoopRules.h"
 #include "LBFGSpp/Param.h"
 #include "LBFGSpp/PhaseClock.h"
 #include "LBFGSpp/SubspaceMin.h"
@@ -63,7 +64,6 @@ public:
     template <typename Foo>
     inline int minimize(Foo& f, Vector& x, Scalar& fx, const Vector& lb, const Vector& ub)
     {
-        using std::abs;
         Device& dev = x.device();
         const std::ptrdiff_t n = x.size();
         if (lb.size() != n || ub.size() != n) throw std::invalid_argument("'lb' and 'ub' must have the same size as 'x'");
@@ -85,7 +85,7 @@ public:
         fx = at.fx;
         m_projgnorm = proj_grad_norm(dev, x, m_grad, lb, ub);
         if (fpast > 0) m_fx[0] = fx;
-        if (m_projgnorm <= m_param.epsilon || m_projgnorm <= m_param.epsilon_rel * std::sqrt(at.xx)) return 1;
+        if (gradient_converged(m_projgnorm, at.xx, m_param.epsilon, m_param.epsilon_rel)) return 1;
         m_ws.gg = at.gg;
         m_ws.xx = at.xx;
 
@@ -122,19 +122,15 @@ public:
 
             {
                 PhaseClock::Scope ph(dev, "line_search");
-                run_line_search<typename LineSearch<Scalar>::Machine>(f, m_param, m_xp, m_gradp, m_drt, step_max, step, fx, dg, x, m_grad, m_ws);
+                typename LineSearch<Scalar>::Machine search(m_param, fx, dg, step, step_max);
+                run_line_search(search, f, m_xp, m_gradp, m_drt, step, fx, dg, x, m_grad, m_ws);
             }
             m_nfev += m_ws.evaluations;
 
             m_projgnorm = proj_grad_norm(dev, x, m_grad, lb, ub);                   // :206
-            if (m_projgnorm <= m_param.epsilon || m_projgnorm <= m_param.epsilon_rel * std::sqrt(m_ws.xx)) return k;
-            if (fpast > 0)
-            {
-                const Scalar fxd = m_fx[size_t(k % fpast)];
-                if (k >= fpast && abs(fxd - fx) <= m_param.delta * std::max(std::max(abs(fx), abs(fxd)), Scalar(1))) return k;
-                m_fx[size_t(k % fpast)] = fx;
-            }
-            if (m_param.max_iterations != 0 && k >= m_param.max_iterations) return k;
+            if (gradient_converged(m_projgnorm, m_ws.xx, m_param.epsilon, m_param.epsilon_rel) || stalled(m_fx.data(), fpast, k, fx, m_param.delta) ||
+                iteration_cap(k, m_param.max_iterations))
+                return k;
 
             {
                 PhaseClock::Scope ph(dev, "update+middle_matrix");

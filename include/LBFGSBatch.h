@@ -83,10 +83,7 @@ public:
             dev.check(lbfgs_b200_solver_create_batch(dev.ctx(), n, m_param.m, int(sizeof(Scalar)), B, &m_solver));
             m_dev = &dev; m_n = n; m_B = B; m_m = m_param.m;
         }
-        lbfgs_b200_param p;
-        p.m = m_param.m; p.epsilon = m_param.epsilon; p.epsilon_rel = m_param.epsilon_rel; p.past = m_param.past; p.delta = m_param.delta;
-        p.max_iterations = m_param.max_iterations; p.linesearch = m_param.linesearch; p.max_linesearch = m_param.max_linesearch;
-        p.min_step = m_param.min_step; p.max_step = m_param.max_step; p.ftol = m_param.ftol; p.wolfe = m_param.wolfe;
+        const lbfgs_b200_param p = detail::abi_param(m_param);
         std::vector<lbfgs_b200_outcome> raw((size_t)B);
         dev.check(detail::batch_abi<Scalar>::minimize(m_solver, f.builtin_kind(), f.builtin_data0(), f.builtin_data1(), 0, &p,
                                                       detail::line_search_id<LineSearch>::value, X.data(), int64_t(n), raw.data()));

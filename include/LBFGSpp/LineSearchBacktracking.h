@@ -21,14 +21,9 @@ class LineSearchBacktracking
 public:
     typedef DeviceVector<Scalar> Vector;
 
-    // The decisions live in BacktrackingCore<Scalar> (LineSearchCore.h, shared with the device-resident solve); this adapter gives
-    // them the reference's exceptions.
-    class Machine : public CoreMachine<Scalar, BacktrackingCore>
-    {
-    public:
-        Machine(const LBFGSParam<Scalar>& param, Scalar fx_init, Scalar dg_init, Scalar step0, Scalar step_max) :
-            CoreMachine<Scalar, BacktrackingCore>(CoreMachine<Scalar, BacktrackingCore>::options_of(param, param.linesearch), fx_init, dg_init, step0, step_max) {}
-    };
+    // The decisions live in BacktrackingCore<Scalar> (LineSearchCore.h, shared with the device-resident solve); Machine is that core, armed by a
+    // constructor that throws like the reference.
+    typedef CoreMachine<Scalar, BacktrackingCore> Machine;
 
     // Reference-compatible entry point.  `grad` holds the gradient at xp on entry and at x on return;
     // `dg` is an output only (the reference recomputes grad.dot(drt) itself, LineSearchBacktracking.h:60).
@@ -39,7 +34,8 @@ public:
         LineSearchWorkspace<Scalar> ws(xp.device());
         const Vector gradp(grad);
         dg = gradp.dot(drt);
-        run_line_search<Machine>(f, param, xp, gradp, drt, step_max, step, fx, dg, x, grad, ws);
+        Machine search(param, fx, dg, step, step_max);
+        run_line_search(search, f, xp, gradp, drt, step, fx, dg, x, grad, ws);
     }
 };
 

@@ -23,14 +23,9 @@ class LineSearchBracketing
 public:
     typedef DeviceVector<Scalar> Vector;
 
-    // The decisions live in BracketingCore<Scalar> (LineSearchCore.h, shared with the device-resident solve); this adapter gives
-    // them the reference's exceptions.
-    class Machine : public CoreMachine<Scalar, BracketingCore>
-    {
-    public:
-        Machine(const LBFGSParam<Scalar>& param, Scalar fx_init, Scalar dg_init, Scalar step0, Scalar step_max) :
-            CoreMachine<Scalar, BracketingCore>(CoreMachine<Scalar, BracketingCore>::options_of(param, param.linesearch), fx_init, dg_init, step0, step_max) {}
-    };
+    // The decisions live in BracketingCore<Scalar> (LineSearchCore.h, shared with the device-resident solve); Machine is that core, armed by a
+    // constructor that throws like the reference.
+    typedef CoreMachine<Scalar, BracketingCore> Machine;
 
     // Reference-compatible entry point (`dg` is an output only, LineSearchBracketing.h:60).
     template <typename Foo>
@@ -40,7 +35,8 @@ public:
         LineSearchWorkspace<Scalar> ws(xp.device());
         const Vector gradp(grad);
         dg = gradp.dot(drt);
-        run_line_search<Machine>(f, param, xp, gradp, drt, step_max, step, fx, dg, x, grad, ws);
+        Machine search(param, fx, dg, step, step_max);
+        run_line_search(search, f, xp, gradp, drt, step, fx, dg, x, grad, ws);
     }
 };
 

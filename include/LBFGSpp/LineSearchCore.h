@@ -2,10 +2,13 @@
 // the host (g++, used by the header-only front) and for the device (nvcc, used by the device-resident solve).
 //
 // A core is a resumable state machine over scalars only:
-//     int init(params, fx0, dg0, step0, step_max)    validates like the reference; returns LS_OK or an error code
-//     int advance(fx, dg, bool& keep)                digests the trial at `step`; returns LS_EVALUATE / LS_ACCEPT /
-//                                                    LS_TAKE_BEST or an error code; `keep` = remember this trial as the best
+//     int init(params, fx0, dg0, step0, step_max)    validates like the reference; returns 0 or an error code
+//     int advance(fx, dg, bool& keep)                digests the trial at `step`; returns LSC_EVALUATE / LSC_ACCEPT /
+//                                                    LSC_TAKE_BEST or an error code; `keep` = remember this trial as the best
+//     step, best_fx, best_dg                         the next trial step; f and g.d of the best trial kept so far
 // Error codes map one-to-one to the reference's exceptions (type + message, see ls_error_message / ls_error_kind).
+// The host loop runs a typed core, the device-resident solve a RunTimeCore (the same four, chosen by kind); both build the options
+// with line_search_options() and do the bookkeeping around one search with a SearchRecord.
 // Decisions follow the reference line by line in meaning:
 //   BacktrackingCore   reference include/LBFGSpp/LineSearchBacktracking.h:44-121
 //   BracketingCore     reference include/LBFGSpp/LineSearchBracketing.h:48-128
@@ -25,7 +28,7 @@
 
 namespace LBFGSpp {
 
-// actions (also defined in LineSearchDriver.h with the same values)
+// what a core asks for after a trial: evaluate at `step`, accept the trial, or (out of budget) take the best point seen so far
 enum { LSC_EVALUATE = 0, LSC_ACCEPT = 1, LSC_TAKE_BEST = 2 };
 
 // error codes: >= 16
@@ -72,6 +75,9 @@ inline const char* ls_error_message(int code)
     return "unknown line search error";
 }
 
+// which core: the same ids as LBFGS_B200_LS_* of include/lbfgs_b200.h
+enum LineSearchKind { LSK_BACKTRACKING = 0, LSK_BRACKETING = 1, LSK_NOCEDAL_WRIGHT = 2, LSK_MORE_THUENTE = 3 };
+
 // the line-search relevant fields of LBFGSParam / LBFGSBParam
 template <typename Scalar>
 struct LineSearchOptions
@@ -80,6 +86,20 @@ struct LineSearchOptions
     int max_linesearch;
     Scalar min_step, max_step, ftol, wolfe;
 };
+
+// param.linesearch; LBFGSBParam has none (L-BFGS-B runs More-Thuente)
+template <class Param> inline auto linesearch_of(const Param& p, int) -> decltype(int(p.linesearch)) { return p.linesearch; }
+template <class Param> inline int linesearch_of(const Param&, long) { return 3; }
+
+// The options of a search of the given kind from LBFGSParam, LBFGSBParam or lbfgs_b200_param.  More-Thuente always tests the strong
+// Wolfe conditions, whatever param.linesearch says.
+template <typename Scalar, class Param>
+inline LineSearchOptions<Scalar> line_search_options(const Param& p, int kind)
+{
+    const LineSearchOptions<Scalar> o = {(kind == LSK_MORE_THUENTE) ? 3 : linesearch_of(p, 0), p.max_linesearch, Scalar(p.min_step),
+                                         Scalar(p.max_step), Scalar(p.ftol), Scalar(p.wolfe)};
+    return o;
+}
 
 namespace lsdetail {
 template <typename T> LBFGS_HD inline T inf_of();
@@ -98,8 +118,10 @@ template <typename T> LBFGS_HD inline bool finite(T a) { return (a == a) && (a !
 template <typename Scalar>
 struct BacktrackingCore
 {
+    static const int kind = LSK_BACKTRACKING;
+    Scalar step, best_fx, best_dg;
     LineSearchOptions<Scalar> prm;
-    Scalar f0, slope0, armijo_slope, step, best_fx, best_dg;
+    Scalar f0, slope0, armijo_slope;
     int trials;
 
     LBFGS_HD int init(const LineSearchOptions<Scalar>& p, Scalar fx_init, Scalar dg_init, Scalar step0, Scalar /*step_max*/)
@@ -142,8 +164,10 @@ struct BacktrackingCore
 template <typename Scalar>
 struct BracketingCore
 {
+    static const int kind = LSK_BRACKETING;
+    Scalar step, best_fx, best_dg;
     LineSearchOptions<Scalar> prm;
-    Scalar f0, slope0, armijo_slope, lo, hi, step, best_fx, best_dg;
+    Scalar f0, slope0, armijo_slope, lo, hi;
     int trials;
 
     LBFGS_HD int init(const LineSearchOptions<Scalar>& p, Scalar fx_init, Scalar dg_init, Scalar step0, Scalar /*step_max*/)
@@ -185,8 +209,10 @@ struct BracketingCore
 template <typename Scalar>
 struct NocedalWrightCore
 {
+    static const int kind = LSK_NOCEDAL_WRIGHT;
+    Scalar step, best_fx, best_dg;
     LineSearchOptions<Scalar> prm;
-    Scalar f0, decrease_slope, curvature_bound, lo, hi, f_lo, f_hi, slope_lo, step, best_fx, best_dg;
+    Scalar f0, decrease_slope, curvature_bound, lo, hi, f_lo, f_hi, slope_lo;
     int zoom, budget_used;
 
     // minimiser of the parabola through (lo, f_lo) with slope slope_lo and (hi, f_hi); bisect when it is not finite,
@@ -275,7 +301,9 @@ struct MoreThuenteCore
 {
     struct Sample { Scalar at, f, g; };   // abscissa, psi value, psi slope
 
-    Scalar smin, smax, f0, decrease_slope, curvature_bound, psi_lo, width, width_before, step, best_fx, best_dg;
+    static const int kind = LSK_MORE_THUENTE;
+    Scalar step, best_fx, best_dg;
+    Scalar smin, smax, f0, decrease_slope, curvature_bound, psi_lo, width, width_before;
     Sample lo, hi;
     int bracketed, cap_next_step, stalls, trials, budget;
 
@@ -439,6 +467,83 @@ struct MoreThuenteCore
     }
 };
 
+// ---------------------------------------------------------------------------------------------------- chosen at run time
+// One of the four cores, picked by `kind` (LSK_*).  The cores begin with the same members (step, best_fx, best_dg), so those are
+// read without a dispatch.
+template <typename Scalar>
+struct RunTimeCore
+{
+    int kind;
+    union
+    {
+        BacktrackingCore<Scalar> bt;
+        BracketingCore<Scalar> br;
+        NocedalWrightCore<Scalar> nw;
+        MoreThuenteCore<Scalar> mt;
+    };
+
+    LBFGS_HD int init(const LineSearchOptions<Scalar>& p, Scalar fx_init, Scalar dg_init, Scalar step0, Scalar step_max)
+    {
+        switch (kind)
+        {
+        case LSK_BACKTRACKING: return bt.init(p, fx_init, dg_init, step0, step_max);
+        case LSK_BRACKETING: return br.init(p, fx_init, dg_init, step0, step_max);
+        case LSK_NOCEDAL_WRIGHT: return nw.init(p, fx_init, dg_init, step0, step_max);
+        default: return mt.init(p, fx_init, dg_init, step0, step_max);
+        }
+    }
+    LBFGS_HD int advance(Scalar fx, Scalar dg, bool& keep)
+    {
+        switch (kind)
+        {
+        case LSK_BACKTRACKING: return bt.advance(fx, dg, keep);
+        case LSK_BRACKETING: return br.advance(fx, dg, keep);
+        case LSK_NOCEDAL_WRIGHT: return nw.advance(fx, dg, keep);
+        default: return mt.advance(fx, dg, keep);
+        }
+    }
+    LBFGS_HD Scalar step() const { return bt.step; }
+    LBFGS_HD Scalar best_fx() const { return bt.best_fx; }
+    LBFGS_HD Scalar best_dg() const { return bt.best_dg; }
+};
+
+// ---------------------------------------------------------------------------------------------------- one search's bookkeeping
+// What a driver does after a core has digested a trial
+enum SearchStep
+{
+    SEARCH_EVALUATE = 0,     // evaluate the objective at the core's step
+    SEARCH_ACCEPT = 1,       // the trial just evaluated is the result
+    SEARCH_TAKE_KEPT = 2,    // the best trial kept so far is the result: bring x_lo, g_lo back
+    SEARCH_TAKE_START = 3    // no trial improved on the start point, which is the result: copy xp, gp back
+};
+
+// The values of the current point of the loop and their bookkeeping during one search.  Between searches {fx, dg, gg, xx} describe the
+// current point; during a search they still describe its start point, and the search's result replaces them.  A trial the core
+// keeps (`keep`) moves into the driver's x_lo / g_lo buffers; its g.g and x.x are remembered here, its f and g.d by the core.
+template <typename Scalar>
+struct SearchRecord
+{
+    Scalar fx, dg, gg, xx;   // f, g.d, g.g, x.x
+    Scalar lo_gg, lo_xx;     // g.g, x.x of the kept trial
+    int have_lo;             // a trial has been kept
+
+    LBFGS_HD void begin() { have_lo = 0; }
+    // the core's (action, keep) on the trial {tfx, tdg, tgg, txx}: returns a SearchStep, or the core's error code (then nothing is
+    // recorded and no trial is kept)
+    LBFGS_HD int digest(int action, bool keep, Scalar tfx, Scalar tdg, Scalar tgg, Scalar txx, Scalar best_fx, Scalar best_dg)
+    {
+        if (action >= LSE_STEP_NOT_POSITIVE) return action;
+        if (keep) { have_lo = 1; lo_gg = tgg; lo_xx = txx; }
+        if (action == LSC_EVALUATE) return SEARCH_EVALUATE;
+        if (action == LSC_ACCEPT) { fx = tfx; dg = tdg; gg = tgg; xx = txx; return SEARCH_ACCEPT; }
+        fx = best_fx;   // LSC_TAKE_BEST
+        dg = best_dg;
+        if (!have_lo) return SEARCH_TAKE_START;   // gg, xx are the start point's already
+        gg = lo_gg; xx = lo_xx;
+        return SEARCH_TAKE_KEPT;
+    }
+};
+
 #if !defined(__CUDACC__)
 }  // namespace LBFGSpp
 #include <stdexcept>
@@ -454,41 +559,16 @@ inline void ls_throw(int code)
     }
 }
 
-// Adapts a core to the interface LineSearchDriver.h expects from a policy's Machine: the constructor validates and throws,
-// advance() throws on failure.
+// A policy's Machine (LineSearch*.h): the core, armed by a constructor that validates the search's inputs and throws like the
+// reference.
 template <typename Scalar, template <class> class Core>
-class CoreMachine
+struct CoreMachine : Core<Scalar>
 {
-    Core<Scalar> m_core;
-
-public:
-    Scalar& step;
-    Scalar& best_fx;
-    Scalar& best_dg;
-
     template <class Param>
-    static LineSearchOptions<Scalar> options_of(const Param& p, int linesearch)
+    CoreMachine(const Param& param, Scalar fx_init, Scalar dg_init, Scalar step0, Scalar step_max)
     {
-        LineSearchOptions<Scalar> o;
-        o.linesearch = linesearch;
-        o.max_linesearch = p.max_linesearch;
-        o.min_step = p.min_step;
-        o.max_step = p.max_step;
-        o.ftol = p.ftol;
-        o.wolfe = p.wolfe;
-        return o;
-    }
-    CoreMachine(const LineSearchOptions<Scalar>& opt, Scalar fx_init, Scalar dg_init, Scalar step0, Scalar step_max) :
-        step(m_core.step), best_fx(m_core.best_fx), best_dg(m_core.best_dg)
-    {
-        const int rc = m_core.init(opt, fx_init, dg_init, step0, step_max);
+        const int rc = this->init(line_search_options<Scalar>(param, Core<Scalar>::kind), fx_init, dg_init, step0, step_max);
         if (rc != 0) ls_throw(rc);
-    }
-    int advance(Scalar fx, Scalar dg, bool& keep)
-    {
-        const int rc = m_core.advance(fx, dg, keep);
-        if (rc >= LSE_STEP_NOT_POSITIVE) ls_throw(rc);
-        return rc;
     }
 };
 #endif

@@ -2,8 +2,9 @@
 //
 // In the reference each LineSearch*.h interleaves three Eigen expressions per trial
 //     x = xp + step * drt;  fx = f(x, grad);  dg = grad.dot(drt);         (e.g. LineSearchMoreThuente.h:412-414)
-// with the scalar logic that picks the next step.  Here the scalar logic is a resumable state machine
-// (one per policy, pure host arithmetic, see LineSearch*.h) and this file owns the three expressions:
+// with the scalar logic that picks the next step.  Here the scalar logic is a resumable core and the bookkeeping
+// around one search is a SearchRecord (LineSearchCore.h, the same code the device-resident solve runs); this file
+// owns the three expressions:
 //   * for an objective that offers `fused_trial()` (the built-in device objectives) a trial is ONE kernel that
 //     also returns g.g and x.x, so the solver never launches separate norm kernels (LBFGS.h:130,137);
 //   * for any other functor it is axpy kernel -> user functor -> one 3-way reduction kernel.
@@ -18,16 +19,9 @@
 #include <utility>
 
 #include "DeviceVector.h"
+#include "LineSearchCore.h"
 
 namespace LBFGSpp {
-
-// What a machine asks the driver to do after it has digested a trial.
-enum LineSearchAction
-{
-    LS_EVALUATE = 0,   // evaluate the objective at machine.step
-    LS_ACCEPT = 1,     // the trial just evaluated is the result
-    LS_TAKE_BEST = 2   // out of budget: the best point seen so far (or the start point) is the result
-};
 
 template <typename Scalar>
 struct TrialValues
@@ -133,64 +127,41 @@ struct LineSearchWorkspace
     explicit LineSearchWorkspace(Device& dev) : x_lo(dev), grad_lo(dev), gg(0), xx(0), evaluations(0) {}
 };
 
-// Runs `Machine` to completion.
+// Runs `search` (a policy's Machine, constructed -- and so validated -- by the caller with step, fx, dg) to completion.
 //   xp, gradp : start point and its gradient (read only)
 //   x, grad   : receive the accepted point and gradient (their previous contents are irrelevant)
 //   step, fx, dg : in = initial step, f(xp), gradp.drt ; out = accepted step, f(x), grad.drt
-template <class Machine, class Foo, class Param, class Scalar>
-void run_line_search(Foo& f, const Param& param, const DeviceVector<Scalar>& xp, const DeviceVector<Scalar>& gradp,
-                     const DeviceVector<Scalar>& drt, const Scalar& step_max, Scalar& step, Scalar& fx, Scalar& dg,
+template <class Machine, class Foo, class Scalar>
+void run_line_search(Machine& search, Foo& f, const DeviceVector<Scalar>& xp, const DeviceVector<Scalar>& gradp,
+                     const DeviceVector<Scalar>& drt, Scalar& step, Scalar& fx, Scalar& dg,
                      DeviceVector<Scalar>& x, DeviceVector<Scalar>& grad, LineSearchWorkspace<Scalar>& ws)
 {
-    Machine machine(param, fx, dg, step, step_max);  // validates its inputs, throws like the reference
     const std::ptrdiff_t n = xp.size();
     x.resize(n);
     grad.resize(n);
-    bool have_lo = false;
-    Scalar lo_gg = ws.gg, lo_xx = ws.xx;
+    SearchRecord<Scalar> rec = {fx, dg, ws.gg, ws.xx, Scalar(0), Scalar(0), 0};   // the start point, nothing kept yet
     ws.evaluations = 0;
     for (;;)
     {
-        const TrialValues<Scalar> t = detail::evaluate_trial(f, xp, drt, machine.step, x, grad);
+        const TrialValues<Scalar> t = detail::evaluate_trial(f, xp, drt, search.step, x, grad);
         ws.evaluations++;
         bool keep = false;
-        const int action = machine.advance(t.fx, t.dg, keep);
-        if (keep)
-        {
-            ws.x_lo.resize(n);
-            ws.grad_lo.resize(n);
-            ws.x_lo.swap(x);
-            ws.grad_lo.swap(grad);
-            have_lo = true;
-            lo_gg = t.gg;
-            lo_xx = t.xx;
-        }
-        if (action == LS_EVALUATE) continue;
-        if (action == LS_ACCEPT)
-        {
-            step = machine.step;
-            fx = t.fx;
-            dg = t.dg;
-            ws.gg = t.gg;
-            ws.xx = t.xx;
-            return;
-        }
-        // LS_TAKE_BEST
-        if (have_lo)
+        const int action = search.advance(t.fx, t.dg, keep);
+        const int next = rec.digest(action, keep, t.fx, t.dg, t.gg, t.xx, search.best_fx, search.best_dg);
+        if (next >= LSE_STEP_NOT_POSITIVE) ls_throw(next);
+        if (keep) { ws.x_lo.resize(n); ws.grad_lo.resize(n); ws.x_lo.swap(x); ws.grad_lo.swap(grad); }
+        if (next == SEARCH_EVALUATE) continue;
+        if (next == SEARCH_TAKE_KEPT)
         {
             x.swap(ws.x_lo);
             grad.swap(ws.grad_lo);
         }
-        else
+        else if (next == SEARCH_TAKE_START)
         {
             x = xp;       // device copies; only when no trial ever improved on the start point
             grad = gradp;
         }
-        step = machine.step;
-        fx = machine.best_fx;
-        dg = machine.best_dg;
-        ws.gg = lo_gg;
-        ws.xx = lo_xx;
+        step = search.step; fx = rec.fx; dg = rec.dg; ws.gg = rec.gg; ws.xx = rec.xx;
         return;
     }
 }

@@ -29,14 +29,8 @@ public:
     typedef DeviceVector<Scalar> Vector;
 
     // The decisions (interval update, safeguarded cubic/quadratic step selection) live in MoreThuenteCore<Scalar>
-    // (LineSearchCore.h, shared with the device-resident solve); this adapter gives them the reference's exceptions.
-    class Machine : public CoreMachine<Scalar, MoreThuenteCore>
-    {
-    public:
-        template <class Param>
-        Machine(const Param& param, Scalar fx_init, Scalar dg_init, Scalar step0, Scalar step_max) :
-            CoreMachine<Scalar, MoreThuenteCore>(CoreMachine<Scalar, MoreThuenteCore>::options_of(param, 3), fx_init, dg_init, step0, step_max) {}
-    };
+    // (LineSearchCore.h, shared with the device-resident solve); Machine is that core, armed by a constructor that throws like the reference.
+    typedef CoreMachine<Scalar, MoreThuenteCore> Machine;
 
     // Reference-compatible entry point (generic over the parameter struct so that LBFGSBSolver can use it):
     // `grad`/`dg` hold the gradient / slope at xp on entry.
@@ -46,7 +40,8 @@ public:
     {
         LineSearchWorkspace<Scalar> ws(xp.device());
         const Vector gradp(grad);
-        run_line_search<Machine>(f, param, xp, gradp, drt, step_max, step, fx, dg, x, grad, ws);
+        Machine search(param, fx, dg, step, step_max);
+        run_line_search(search, f, xp, gradp, drt, step, fx, dg, x, grad, ws);
     }
 };
 

@@ -24,14 +24,9 @@ class LineSearchNocedalWright
 public:
     typedef DeviceVector<Scalar> Vector;
 
-    // The decisions live in NocedalWrightCore<Scalar> (LineSearchCore.h, shared with the device-resident solve); this adapter gives
-    // them the reference's exceptions.
-    class Machine : public CoreMachine<Scalar, NocedalWrightCore>
-    {
-    public:
-        Machine(const LBFGSParam<Scalar>& param, Scalar fx_init, Scalar dg_init, Scalar step0, Scalar step_max) :
-            CoreMachine<Scalar, NocedalWrightCore>(CoreMachine<Scalar, NocedalWrightCore>::options_of(param, param.linesearch), fx_init, dg_init, step0, step_max) {}
-    };
+    // The decisions live in NocedalWrightCore<Scalar> (LineSearchCore.h, shared with the device-resident solve); Machine is that core, armed by a
+    // constructor that throws like the reference.
+    typedef CoreMachine<Scalar, NocedalWrightCore> Machine;
 
     // Reference-compatible entry point: `grad`/`dg` hold the gradient / slope at xp on entry.
     template <typename Foo>
@@ -40,7 +35,8 @@ public:
     {
         LineSearchWorkspace<Scalar> ws(xp.device());
         const Vector gradp(grad);
-        run_line_search<Machine>(f, param, xp, gradp, drt, step_max, step, fx, dg, x, grad, ws);
+        Machine search(param, fx, dg, step, step_max);
+        run_line_search(search, f, xp, gradp, drt, step, fx, dg, x, grad, ws);
     }
 };
 

@@ -12,6 +12,7 @@
 //   (k_gram_dots, k_gram_fold, k_gram_combine live in two_loop_gram.cuh; the device-resident solve in persist.cuh)
 #include "internal.cuh"
 #include "two_loop_gram.cuh"
+#include "../../include/LBFGSpp/LoopRules.h"
 
 using namespace lb;
 
@@ -339,7 +340,7 @@ __global__ void k_commit_pair(const double* result, T eps, int gate, T* ys_slot,
                               double* mail_vals, int* mail_flag, unsigned long long* mail_word, unsigned long long mail_seq)
 {
     const T sy = (T)result[0], yy = (T)result[1];
-    const bool ok = gate ? (sy > eps * yy) : true;
+    const bool ok = gate ? LBFGSpp::curvature_ok(sy, yy, eps) : true;
     if (ok)
     {
         *ys_slot = sy;

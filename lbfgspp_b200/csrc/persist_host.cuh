@@ -115,14 +115,12 @@ static lbfgs_b200_status solver_minimize(lbfgs_b200_solver* s, int objective, co
         p.head = 0; p.ncorr = 0; p.M = s->M; p.m = s->m; p.gram_cur = 0; p.pending = -1;
         p.op = POP_FIRST; p.c_round = 0;
         p.epsilon = (T)prm->epsilon; p.epsilon_rel = (T)prm->epsilon_rel; p.delta = (T)prm->delta; p.max_step = (T)prm->max_step;
-        p.eps_gate = std::numeric_limits<T>::epsilon();
-        p.past = prm->past; p.max_iterations = prm->max_iterations; p.ls_kind = ls_kind;
+        p.past = prm->past; p.max_iterations = prm->max_iterations;
         // the first trial of every search rides on the combination pass; a neighbour-coupled objective needs its neighbours' x + d,
         // which only exist on this rank when n is not sharded
         p.fuse_first_trial = (coupled && ctx->nranks > 1) ? 0 : 1;
-        p.ls_opt.linesearch = (ls_kind == 3) ? 3 : prm->linesearch;
-        p.ls_opt.max_linesearch = prm->max_linesearch;
-        p.ls_opt.min_step = (T)prm->min_step; p.ls_opt.max_step = (T)prm->max_step; p.ls_opt.ftol = (T)prm->ftol; p.ls_opt.wolfe = (T)prm->wolfe;
+        p.ls.kind = ls_kind;
+        p.ls_opt = LBFGSpp::line_search_options<T>(*prm, ls_kind);
         p.trace = trace_host ? s->d_trace : nullptr;
         p.trace_cap = trace_host ? trace_cap : 0;
         CU(ctx, cudaMemcpyAsync(p.x, x_inout + (size_t)b * ldx, vb, cudaMemcpyDeviceToDevice, ctx->stream));
@@ -189,7 +187,7 @@ static lbfgs_b200_status solver_minimize(lbfgs_b200_solver* s, int objective, co
         outs[b].status = p.status;
         outs[b].niter = p.niter;
         outs[b].nfev = p.nfev;
-        outs[b].fx = (double)p.fx;
+        outs[b].fx = (double)p.rec.fx;
         outs[b].gnorm = (double)p.gnorm;
         outs[b].rounds = p.rounds;
     }
