@@ -53,7 +53,11 @@ def _load(name):
 
 def abi():
     """The raw C ABI (include/lbfgs_b200.h) as a ctypes library with argument types declared."""
-    lib = _load("liblbfgs_b200.so")
+    return _declare(_load("liblbfgs_b200.so"))
+
+
+def _declare(lib):
+    """Declare the argument and result types of every lbfgs_b200_* entry point on `lib` (any library exporting the ABI)."""
     if getattr(lib, "_typed", False):
         return lib
     vp, i64, ci, sz = C.c_void_p, C.c_int64, C.c_int, C.c_size_t
@@ -108,6 +112,28 @@ def abi():
         getattr(lib, "lbfgs_b200_hist_apply_Hv_" + suf).argtypes = [vp, vp, ct, vp, ci, pt]
         getattr(lib, "lbfgs_b200_hist_update_apply_Hv_" + suf).argtypes = [vp, vp, vp, vp, vp, ct, ct, vp, ci, C.POINTER(ci), pt]
         getattr(lib, "lbfgs_b200_hist_scalars_" + suf).argtypes = [vp, pt, pt, pt]
+    # bound-constrained path
+    lib.lbfgs_b200_box_create.argtypes = [vp, C.POINTER(vp)]
+    lib.lbfgs_b200_box_destroy.argtypes = [vp]
+    lib.lbfgs_b200_box_destroy.restype = None
+    for name in ("lbfgs_b200_box_xcp", "lbfgs_b200_box_classes"):
+        getattr(lib, name).restype = vp
+        getattr(lib, name).argtypes = [vp]
+    lib.lbfgs_b200_box_vector.restype = vp
+    lib.lbfgs_b200_box_vector.argtypes = [vp, ci]
+    for suf, ct in (("f64", C.c_double), ("f32", C.c_float)):
+        pt = C.POINTER(ct)
+        getattr(lib, "lbfgs_b200_box_clamp_" + suf).argtypes = [vp, i64, vp, vp, vp]
+        getattr(lib, "lbfgs_b200_box_proj_grad_norm_" + suf).argtypes = [vp, i64, vp, vp, vp, vp, pt]
+        getattr(lib, "lbfgs_b200_box_dir_info_" + suf).argtypes = [vp, i64, vp, vp, vp, vp, vp, pt]
+        getattr(lib, "lbfgs_b200_hist_wt_dot_" + suf).argtypes = [vp, vp, pt]
+        getattr(lib, "lbfgs_b200_hist_gram_" + suf).argtypes = [vp, pt, pt, pt, pt, pt]
+        getattr(lib, "lbfgs_b200_hist_lincomb_" + suf).argtypes = [vp, vp, ct, vp, pt, vp, ci, vp]
+        getattr(lib, "lbfgs_b200_hist_masked_gram_" + suf).argtypes = [vp, vp, vp, ci, pt]
+        getattr(lib, "lbfgs_b200_box_cauchy_breaks_" + suf).argtypes = [vp, vp, vp, vp, vp, pt]
+        getattr(lib, "lbfgs_b200_box_cauchy_sweep_" + suf).argtypes = [vp, vp, pt, pt, ct, ct, i64, i64, pt]
+        getattr(lib, "lbfgs_b200_box_cauchy_build_" + suf).argtypes = [vp, vp, vp, vp, ct, ct, pt]
+        getattr(lib, "lbfgs_b200_box_sub_step_" + suf).argtypes = [vp, ci, ci, vp, vp, vp, vp, vp, ct, pt]
     # device-resident solve (persistent kernel; single problem or batch)
     lib.lbfgs_b200_solver_create.argtypes = [vp, i64, ci, ci, C.POINTER(vp)]
     lib.lbfgs_b200_solver_create_batch.argtypes = [vp, i64, ci, ci, ci, C.POINTER(vp)]
@@ -158,8 +184,6 @@ def driver():
                                             C.c_int, fp, fp, dp, C.c_long, C.POINTER(_DrvResult)]
     lib.lbfgsb200_drv_ctx.restype = C.c_void_p
     lib.lbfgsb200_drv_ctx.argtypes = [C.c_int]
-    lib.lbfgsb200_drv_lbfgsb_f64.argtypes = [C.c_int, C.c_int, dp, dp, C.c_long, C.POINTER(_DrvParam), dp, dp, dp, dp, dp, C.c_long,
-                                             C.POINTER(_DrvResult)]
     lib.lbfgsb200_drv_session_create.restype = C.c_void_p
     lib.lbfgsb200_drv_session_create.argtypes = [C.c_int, C.c_int, dp, dp, C.c_long, C.c_int, C.POINTER(_DrvParam), C.c_int, dp,
                                                  C.c_char_p, C.c_int, C.c_int]
@@ -283,28 +307,34 @@ class LBFGSSolver:
 
 
 class LBFGSBSolver:
-    """LBFGSpp::LBFGSBSolver<double> (More-Thuente line search) on the GPU, host buffers in and out."""
+    """LBFGSpp::LBFGSBSolver<Scalar> (More-Thuente line search) on the GPU, host buffers in and out; Scalar from `dtype`."""
 
-    def __init__(self, param=None, device=0):
+    def __init__(self, param=None, device=0, dtype=np.float64):
         self.param = param if param is not None else LBFGSBParam()
         self.device = device
+        self.dtype = np.dtype(dtype)
 
-    def minimize(self, objective, x0, lb, ub, data0=None, data1=None, trace_cap=100000, raise_errors=False):
-        drv = driver()
-        x = np.array(x0, dtype=np.float64, order="C").copy()
+    def minimize(self, objective, x0, lb, ub, data0=None, data1=None, trace_cap=100000, raise_errors=False, lib=None):
+        """lib: a library exporting the driver's entry points to use instead of liblbfgs_b200_driver.so."""
+        drv = driver() if lib is None else lib
+        dt = self.dtype
+        ct = C.c_double if dt == np.float64 else C.c_float
+        x = np.array(x0, dtype=dt, order="C").copy()
         n = x.size
-        lbv = np.ascontiguousarray(np.broadcast_to(lb, n), dtype=np.float64)
-        ubv = np.ascontiguousarray(np.broadcast_to(ub, n), dtype=np.float64)
-        grad = np.zeros(n)
+        lbv = np.ascontiguousarray(np.broadcast_to(lb, n), dtype=dt)
+        ubv = np.ascontiguousarray(np.broadcast_to(ub, n), dtype=dt)
+        grad = np.zeros(n, dtype=dt)
         trace = np.zeros(trace_cap)
-        d0 = None if data0 is None else np.ascontiguousarray(data0, dtype=np.float64)
-        d1 = None if data1 is None else np.ascontiguousarray(data1, dtype=np.float64)
-        dp = C.POINTER(C.c_double)
-        ptr = lambda a: a.ctypes.data_as(dp) if a is not None else None
+        d0 = None if data0 is None else np.ascontiguousarray(data0, dtype=dt)
+        d1 = None if data1 is None else np.ascontiguousarray(data1, dtype=dt)
+        ptr = lambda a, t=ct: a.ctypes.data_as(C.POINTER(t)) if a is not None else None
         res = _DrvResult()
         p = self.param._c()
-        drv.lbfgsb200_drv_lbfgsb_f64(self.device, objective, ptr(d0), ptr(d1), n, C.byref(p), ptr(x), ptr(lbv), ptr(ubv),
-                                     ptr(grad), ptr(trace), trace_cap, C.byref(res))
+        fn = drv.lbfgsb200_drv_lbfgsb_f64 if dt == np.float64 else drv.lbfgsb200_drv_lbfgsb_f32
+        fn.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_long, C.POINTER(_DrvParam)] + [C.c_void_p] * 5 + [C.c_long,
+                                                                                                                     C.POINTER(_DrvResult)]
+        fn(self.device, objective, ptr(d0), ptr(d1), n, C.byref(p), ptr(x), ptr(lbv), ptr(ubv), ptr(grad),
+           ptr(trace, C.c_double), trace_cap, C.byref(res))
         if res.status and raise_errors:
             raise _EXC.get(res.status, RuntimeError)(res.msg.decode())
         return dict(status=STATUS_NAMES[res.status], msg=res.msg.decode(), niter=res.niter, nfev=res.nfev, fx=res.fx,
@@ -316,8 +346,10 @@ class LBFGSBSolver:
 # thin object wrappers over the raw C ABI (kernel-level tests, microbenchmarks)
 # ------------------------------------------------------------------------------------------------------
 class Context:
-    def __init__(self, device=0, stream=None):
-        self.lib = abi()
+    """lib: a ctypes library exporting the C ABI to use instead of liblbfgs_b200.so (its types are declared on first use)."""
+
+    def __init__(self, device=0, stream=None, lib=None):
+        self.lib = abi() if lib is None else _declare(lib)
         self.h = C.c_void_p()
         st = self.lib.lbfgs_b200_ctx_create(C.byref(self.h), device, stream)
         if st:
@@ -448,6 +480,7 @@ class History:
         try:
             if self.h and self.ctx.h:
                 self.ctx.lib.lbfgs_b200_hist_destroy(self.h)
+            self.h = None   # a Box on this history checks it: finalisers of garbage cycles run in no particular order
         except Exception:
             pass
 
@@ -498,6 +531,46 @@ class History:
         out = np.empty(self.n, dtype=self.dtype)
         self.ctx.check(self.ctx.lib.lbfgs_b200_memcpy_d2h(self.ctx.h, out.ctypes.data_as(C.c_void_p), p, out.nbytes))
         return out
+
+
+BOXV_VECC, BOXV_VECY, BOXV_LAMBDA, BOXV_MU, BOXV_TMP, BOXV_TMP2, BOXV_YFB, BOXV_DVEC, BOXV_BRK, BOXV_XCP = range(10)
+CLS_FIXED, CLS_ACT, CLS_FREE, SUB_L, SUB_U, SUB_P = 1, 2, 4, 8, 16, 32
+
+
+class Box:
+    """The workspace of the bound-constrained path (lbfgs_b200_box) on a History: its n-vectors (BOXV_*) and class bytes."""
+
+    def __init__(self, hist):
+        self.hist, self.ctx, self.n, self.dtype = hist, hist.ctx, hist.n, hist.dtype
+        self.h = C.c_void_p()
+        self.ctx.check(self.ctx.lib.lbfgs_b200_box_create(hist.h, C.byref(self.h)))
+
+    def __del__(self):
+        try:
+            if self.h and self.hist.h and self.ctx.h:   # lbfgs_b200_box_destroy reads its history
+                self.ctx.lib.lbfgs_b200_box_destroy(self.h)
+        except Exception:
+            pass
+
+    def _ptr(self, which):
+        return self.ctx.lib.lbfgs_b200_box_classes(self.h) if which == "cls" else self.ctx.lib.lbfgs_b200_box_vector(self.h, which)
+
+    def _spec(self, which):
+        return (np.uint8, self.n) if which == "cls" else (self.dtype, self.n)
+
+    def get(self, which):
+        """Download BOXV_* vector `which`, or the class bytes for which = "cls"."""
+        dt, n = self._spec(which)
+        out = np.empty(n, dtype=dt)
+        self.ctx.check(self.ctx.lib.lbfgs_b200_memcpy_d2h(self.ctx.h, out.ctypes.data_as(C.c_void_p), self._ptr(which), out.nbytes))
+        return out
+
+    def set(self, which, host):
+        dt, n = self._spec(which)
+        host = np.ascontiguousarray(host, dtype=dt)
+        assert host.size == n
+        self.ctx.check(self.ctx.lib.lbfgs_b200_memcpy_h2d(self.ctx.h, self._ptr(which), host.ctypes.data_as(C.c_void_p), host.nbytes))
+        self.ctx.sync()
 
 
 class Session:

@@ -517,29 +517,33 @@ extern "C" int lbfgsb200_drv_set_global_extent(int device_ordinal, long long ind
 }
 
 
-// LBFGSBSolver<double>::minimize with host buffers (More-Thuente line search, built-in objective, fused trials)
-extern "C" int lbfgsb200_drv_lbfgsb_f64(int device_ordinal, int objective, const double* data0_host, const double* data1_host, long n,
-                                        const drv_param* q, double* x_host, const double* lb_host, const double* ub_host,
-                                        double* grad_host, double* fx_trace, long trace_cap, drv_result* out)
+namespace {
+
+// LBFGSBSolver<Scalar>::minimize with host buffers (More-Thuente line search, built-in objective, fused trials)
+template <class Scalar>
+int lbfgsb_any(int device_ordinal, int objective, const Scalar* data0_host, const Scalar* data1_host, long n, const drv_param* q,
+               Scalar* x_host, const Scalar* lb_host, const Scalar* ub_host, Scalar* grad_host, double* fx_trace, long trace_cap,
+               drv_result* out)
 {
     return guarded(out, [&]() {
         const double t_begin = now();
         Device& dev = device(device_ordinal);
-        typedef DeviceVector<double> Vector;
+        typedef DeviceVector<Scalar> Vector;
         Vector d0(dev), d1(dev), x(dev), lb(dev), ub(dev);
         if (data0_host) d0.copy_from_host(data0_host, n);
         if (data1_host) d1.copy_from_host(data1_host, n);
         x.copy_from_host(x_host, n);
         lb.copy_from_host(lb_host, n);
         ub.copy_from_host(ub_host, n);
-        LBFGSBParam<double> prm;
-        prm.m = q->m; prm.epsilon = q->epsilon; prm.epsilon_rel = q->epsilon_rel; prm.past = q->past; prm.delta = q->delta;
-        prm.max_iterations = q->max_iterations; prm.max_submin = q->max_submin; prm.max_linesearch = q->max_linesearch;
-        prm.min_step = q->min_step; prm.max_step = q->max_step; prm.ftol = q->ftol; prm.wolfe = q->wolfe;
-        LBFGSBSolver<double> solver(prm);
-        BuiltinObjective<double> obj(objective, d0.data(), d1.data());
-        Traced<BuiltinObjective<double>, double, true> f(obj, fx_trace, trace_cap);
-        double fx = 0;
+        LBFGSBParam<Scalar> prm;
+        prm.m = q->m; prm.epsilon = Scalar(q->epsilon); prm.epsilon_rel = Scalar(q->epsilon_rel); prm.past = q->past;
+        prm.delta = Scalar(q->delta); prm.max_iterations = q->max_iterations; prm.max_submin = q->max_submin;
+        prm.max_linesearch = q->max_linesearch; prm.min_step = Scalar(q->min_step); prm.max_step = Scalar(q->max_step);
+        prm.ftol = Scalar(q->ftol); prm.wolfe = Scalar(q->wolfe);
+        LBFGSBSolver<Scalar> solver(prm);
+        BuiltinObjective<Scalar> obj(objective, d0.data(), d1.data());
+        Traced<BuiltinObjective<Scalar>, Scalar, true> f(obj, fx_trace, trace_cap);
+        Scalar fx = 0;
         const unsigned long long launches0 = lbfgs_b200_launch_count(dev.ctx());
         const double t0 = now();
         int niter = 0;
@@ -555,16 +559,33 @@ extern "C" int lbfgsb200_drv_lbfgsb_f64(int device_ordinal, int objective, const
         x.copy_to_host(x_host);
         if (grad_host) solver.final_grad().copy_to_host(grad_host);
         out->niter = niter;
-        out->fx = fx;
-        out->gnorm = solver.final_grad_norm();
+        out->fx = double(fx);
+        out->gnorm = double(solver.final_grad_norm());
         out->nfev = f.count;
         out->trace_len = f.count < trace_cap ? f.count : trace_cap;
         out->seconds = t1 - t0;
         out->seconds_e2e = now() - t_begin;
         out->launches = lbfgs_b200_launch_count(dev.ctx()) - launches0;
-        out->h2d_bytes = 8L * n * 3;
-        out->d2h_bytes = 8L * n * (grad_host ? 2 : 1);
+        out->h2d_bytes = long(sizeof(Scalar)) * n * 3;
+        out->d2h_bytes = long(sizeof(Scalar)) * n * (grad_host ? 2 : 1);
     });
+}
+
+}  // namespace
+
+extern "C" int lbfgsb200_drv_lbfgsb_f64(int device_ordinal, int objective, const double* data0_host, const double* data1_host, long n,
+                                        const drv_param* q, double* x_host, const double* lb_host, const double* ub_host,
+                                        double* grad_host, double* fx_trace, long trace_cap, drv_result* out)
+{
+    return lbfgsb_any<double>(device_ordinal, objective, data0_host, data1_host, n, q, x_host, lb_host, ub_host, grad_host, fx_trace,
+                              trace_cap, out);
+}
+extern "C" int lbfgsb200_drv_lbfgsb_f32(int device_ordinal, int objective, const float* data0_host, const float* data1_host, long n,
+                                        const drv_param* q, float* x_host, const float* lb_host, const float* ub_host,
+                                        float* grad_host, double* fx_trace, long trace_cap, drv_result* out)
+{
+    return lbfgsb_any<float>(device_ordinal, objective, data0_host, data1_host, n, q, x_host, lb_host, ub_host, grad_host, fx_trace,
+                             trace_cap, out);
 }
 
 // Cauchy point on an explicit history (kernel-level test hook): pairs are appended with add_correction, then

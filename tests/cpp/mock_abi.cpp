@@ -206,6 +206,7 @@ lbfgs_b200_status do_lincomb(lbfgs_b200_hist* h, T a0, const T* v0, const T* coe
     if (auto st = check_hist<T>(h)) return st;
     orc::History<T>& H = h->get<T>();
     const int c = H.ncorr;
+    if (!out || (c > 0 && !coef)) return fail(h->ctx, LBFGS_B200_ERR_INVALID, "hist_lincomb: NULL argument");
     for (long i = 0; i < H.n; i++)
     {
         if (cls && !(cls[i] & mask)) continue;
@@ -243,8 +244,8 @@ lbfgs_b200_status do_cauchy_breaks(lbfgs_b200_box* b, const T* x, const T* g, co
     T* brk = b->vec<T>(V_BRK);
     T* dvec = b->vec<T>(V_DVEC);
     const T inf = std::numeric_limits<T>::infinity();
-    double nfixed = 0, ninf = 0, nord = 0;
-    T dd = T(0), tmin = inf;
+    double nfixed = 0, ninf = 0, nord = 0, dd = 0;   // d.d accumulated in double, as k_cauchy_breaks does
+    T tmin = inf;
     for (int64_t i = 0; i < b->n; i++)
     {
         T t;
@@ -256,12 +257,12 @@ lbfgs_b200_status do_cauchy_breaks(lbfgs_b200_box* b, const T* x, const T* g, co
         const T di = zero ? T(0) : -g[i];
         brk[i] = t;
         dvec[i] = di;
-        dd += di * di;
+        dd += double(di * di);
         if (t == inf) { ninf += 1; b->cls[i] = CLS_FREE; }
         else if (!zero) { nord += 1; tmin = std::min(tmin, t); b->cls[i] = 0; }
         else { nfixed += 1; b->cls[i] = CLS_FIXED; }
     }
-    out5[0] = T(nfixed); out5[1] = T(ninf); out5[2] = T(nord); out5[3] = dd; out5[4] = tmin;
+    out5[0] = T(nfixed); out5[1] = T(ninf); out5[2] = T(nord); out5[3] = T(dd); out5[4] = tmin;
     return LBFGS_B200_OK;
 }
 
