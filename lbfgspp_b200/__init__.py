@@ -172,38 +172,74 @@ class _DrvResult(C.Structure):
                 ("d2h_bytes", C.c_long)]
 
 
-def driver():
+def driver(lib=None):
+    """liblbfgs_b200_driver.so, or `lib` (a library exporting the same entry points, e.g. built on a test double), typed."""
+    if lib is not None:
+        return _declare_driver(lib)
     abi()  # the driver links against the kernel library: load it first, globally
-    lib = _load("liblbfgs_b200_driver.so")
-    if getattr(lib, "_typed", False):
+    return _declare_driver(_load("liblbfgs_b200_driver.so"))
+
+
+def _declare_driver(lib):
+    """Declare the argument and result types of every lbfgsb200_drv_* entry point on `lib` (any library exporting the driver)."""
+    if getattr(lib, "_drv_typed", False):
         return lib
+    vp, ci, cl, err, errlen = C.c_void_p, C.c_int, C.c_long, C.c_char_p, C.c_int
     dp, fp = C.POINTER(C.c_double), C.POINTER(C.c_float)
-    lib.lbfgsb200_drv_lbfgs_f64.argtypes = [C.c_int, C.c_int, dp, dp, C.c_long, C.c_int, C.POINTER(_DrvParam), C.c_int,
-                                            C.c_int, dp, dp, dp, C.c_long, C.POINTER(_DrvResult)]
-    lib.lbfgsb200_drv_lbfgs_f32.argtypes = [C.c_int, C.c_int, fp, fp, C.c_long, C.c_int, C.POINTER(_DrvParam), C.c_int,
-                                            C.c_int, fp, fp, dp, C.c_long, C.POINTER(_DrvResult)]
-    lib.lbfgsb200_drv_ctx.restype = C.c_void_p
-    lib.lbfgsb200_drv_ctx.argtypes = [C.c_int]
-    lib.lbfgsb200_drv_session_create.restype = C.c_void_p
-    lib.lbfgsb200_drv_session_create.argtypes = [C.c_int, C.c_int, dp, dp, C.c_long, C.c_int, C.POINTER(_DrvParam), C.c_int, dp,
-                                                 C.c_char_p, C.c_int, C.c_int]
-    lib.lbfgsb200_drv_session_destroy.argtypes = [C.c_void_p]
-    lib.lbfgsb200_drv_session_destroy.restype = None
-    lib.lbfgsb200_drv_session_solve.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(_DrvResult)]
+    prm, res, item = C.POINTER(_DrvParam), C.POINTER(_DrvResult), C.POINTER(_BatchItem)
+    for suf, pt in (("f64", dp), ("f32", fp)):
+        getattr(lib, "lbfgsb200_drv_lbfgs_" + suf).argtypes = [ci, ci, pt, pt, cl, ci, prm, ci, ci, pt, pt, dp, cl, res]
+        getattr(lib, "lbfgsb200_drv_lbfgsb_" + suf).argtypes = [ci, ci, pt, pt, cl, prm, pt, pt, pt, pt, dp, cl, res]
+    for name in ("ctx", "session_create", "batch_session_create"):
+        getattr(lib, "lbfgsb200_drv_" + name).restype = vp
+    for name in ("shutdown", "session_destroy", "batch_session_destroy", "phase_enable"):
+        getattr(lib, "lbfgsb200_drv_" + name).restype = None
+    lib.lbfgsb200_drv_ctx.argtypes = [ci]
+    lib.lbfgsb200_drv_shutdown.argtypes = []
+    lib.lbfgsb200_drv_session_create.argtypes = [ci, ci, dp, dp, cl, ci, prm, ci, dp, err, errlen, ci]
+    lib.lbfgsb200_drv_session_destroy.argtypes = [vp]
+    lib.lbfgsb200_drv_session_solve.argtypes = [vp, ci, ci, res]
     lib.lbfgsb200_drv_session_result.restype = dp
-    lib.lbfgsb200_drv_session_result.argtypes = [C.c_void_p]
-    lib.lbfgsb200_drv_session_download.argtypes = [C.c_void_p, dp]
-    lib.lbfgsb200_drv_batch_session_download.argtypes = [C.c_void_p, dp]
-    lib.lbfgsb200_drv_batch_session_create.restype = C.c_void_p
-    lib.lbfgsb200_drv_batch_session_create.argtypes = [C.c_int, C.c_int, C.c_long, C.c_int, dp, C.c_int, C.POINTER(_DrvParam), C.c_char_p, C.c_int]
-    lib.lbfgsb200_drv_batch_session_destroy.argtypes = [C.c_void_p]
-    lib.lbfgsb200_drv_batch_session_destroy.restype = None
-    lib.lbfgsb200_drv_batch_session_solve.argtypes = [C.c_void_p, C.POINTER(_BatchItem), C.POINTER(C.c_long), dp, dp, C.c_char_p, C.c_int]
-    lib.lbfgsb200_drv_comm_init.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_char_p, C.c_int]
-    lib.lbfgsb200_drv_p2p_export.argtypes = [C.c_int, C.c_void_p, C.c_char_p, C.c_int]
-    lib.lbfgsb200_drv_p2p_attach.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_char_p, C.c_int]
-    lib._typed = True
+    lib.lbfgsb200_drv_session_result.argtypes = [vp]
+    lib.lbfgsb200_drv_session_download.argtypes = [vp, dp]
+    lib.lbfgsb200_drv_comm_init.argtypes = [ci, vp, ci, ci, C.c_longlong, err, errlen]
+    lib.lbfgsb200_drv_p2p_export.argtypes = [ci, vp, err, errlen]
+    lib.lbfgsb200_drv_p2p_attach.argtypes = [ci, vp, ci, ci, C.c_longlong, err, errlen]
+    lib.lbfgsb200_drv_set_global_extent.argtypes = [ci, C.c_longlong, C.c_longlong, err, errlen]
+    lib.lbfgsb200_drv_cauchy_f64.argtypes = [ci, cl, ci, ci, dp, dp, dp, dp, dp, dp, dp, C.POINTER(C.c_ubyte), dp, C.POINTER(cl), dp, err, errlen]
+    lib.lbfgsb200_drv_batch_f64.argtypes = [ci, ci, cl, ci, dp, ci, prm, ci, ci, ci, item, dp, dp]
+    lib.lbfgsb200_drv_batch_session_create.argtypes = [ci, ci, cl, ci, dp, ci, prm, err, errlen]
+    lib.lbfgsb200_drv_batch_session_destroy.argtypes = [vp]
+    lib.lbfgsb200_drv_batch_session_download.argtypes = [vp, dp]
+    lib.lbfgsb200_drv_batch_session_upload.argtypes = [vp, dp, err, errlen]
+    lib.lbfgsb200_drv_batch_session_solve.argtypes = [vp, item, C.POINTER(cl), dp, dp, err, errlen]
+    for name in ("lbfgsb200_drv_session_profile", "lbfgsb200_drv_batch_session_profile"):
+        getattr(lib, name).argtypes = [vp, dp, dp, C.POINTER(C.c_ulonglong), dp, dp]
+    lib.lbfgsb200_drv_solve_dense_f64.argtypes = [ci, ci, cl, ci, prm, ci, dp, dp, dp, C.POINTER(ci), err, errlen]
+    lib.lbfgsb200_drv_phase_enable.argtypes = [ci]
+    lib.lbfgsb200_drv_phase_report.argtypes = [C.c_char_p, ci]
+    lib.lbfgsb200_drv_dense_f64.argtypes = [ci, cl, ci, ci, dp, dp, ci, dp, err, errlen]
+    lib._drv_typed = True
     return lib
+
+
+def _checked(what, call, failed=bool):
+    """call(err, errlen) runs an entry point that reports failure as text in (err, errlen): its result, or
+    RuntimeError("<what> failed: <text>") when failed(result)."""
+    err = C.create_string_buffer(256)
+    r = call(err, len(err))
+    if failed(r):
+        raise RuntimeError("%s failed: %s" % (what, err.value.decode()))
+    return r
+
+
+def _ls_id(linesearch):
+    return LINE_SEARCHES[linesearch] if isinstance(linesearch, str) else int(linesearch)
+
+
+def _ptr(a):
+    """A pointer to the data of a float64 / float32 array, None for None."""
+    return None if a is None else a.ctypes.data_as(C.POINTER(C.c_float if a.dtype == np.float32 else C.c_double))
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -265,45 +301,48 @@ _EXC = {1: ValueError, 2: ArithmeticError, 3: RuntimeError, 4: RuntimeError}
 STATUS_NAMES = {0: "ok", 1: "invalid_argument", 2: "logic_error", 3: "runtime_error", 4: "other"}
 
 
+def _solve_result(res, x, grad, trace, raise_errors):
+    """The dict a host-buffer minimize() returns for its _DrvResult, or the reference's exception when raise_errors."""
+    if res.status and raise_errors:
+        raise _EXC.get(res.status, RuntimeError)(res.msg.decode())
+    return dict(status=STATUS_NAMES[res.status], msg=res.msg.decode(), niter=res.niter, nfev=res.nfev, fx=res.fx,
+                gnorm=res.gnorm, x=x, grad=grad, trace=trace[:res.trace_len].copy(), seconds=res.seconds,
+                seconds_e2e=res.seconds_e2e, launches=res.launches)
+
+
 class LBFGSSolver:
     """LBFGSpp::LBFGSSolver<Scalar, LineSearch> on the GPU, host buffers in and out.
 
     minimize(objective, x0) returns a dict(niter, nfev, fx, gnorm, x, grad, trace, status, msg, seconds, ...);
     with raise_errors=True the reference's exceptions come back as ValueError (std::invalid_argument),
     ArithmeticError (std::logic_error) or RuntimeError (std::runtime_error).
+    lib: a library exporting the driver's entry points to use instead of liblbfgs_b200_driver.so.
     """
 
     def __init__(self, param=None, linesearch="NocedalWright", dtype=np.float64, device=0, hv_algo=HV_AUTO,
-                 fused=True, resident=False):
+                 fused=True, resident=False, lib=None):
         self.param = param if param is not None else LBFGSParam()
-        self.ls = LINE_SEARCHES[linesearch] if isinstance(linesearch, str) else int(linesearch)
+        self.ls = _ls_id(linesearch)
         self.dtype = np.dtype(dtype)
         self.device = device
         self.hv_algo = hv_algo
         self.fused = 2 if resident else fused   # 2: device-resident solve (one persistent kernel launch per minimize)
+        self.lib = lib
 
     def minimize(self, objective, x0, data0=None, data1=None, trace_cap=100000, raise_errors=False, want_grad=True):
-        drv = driver()
+        drv = driver(self.lib)
         dt = self.dtype
-        ct = C.c_double if dt == np.float64 else C.c_float
         x = np.array(x0, dtype=dt, order="C").copy()
         n = x.size
         grad = np.zeros(n, dtype=dt) if want_grad else None
         trace = np.zeros(trace_cap, dtype=np.float64)
-        d0 = None if data0 is None else np.ascontiguousarray(data0, dtype=dt)
-        d1 = None if data1 is None else np.ascontiguousarray(data1, dtype=dt)
-        ptr = lambda a, t=ct: a.ctypes.data_as(C.POINTER(t)) if a is not None else None
+        d0, d1 = (None if a is None else np.ascontiguousarray(a, dtype=dt) for a in (data0, data1))
         res = _DrvResult()
         p = self.param._c()
         fn = drv.lbfgsb200_drv_lbfgs_f64 if dt == np.float64 else drv.lbfgsb200_drv_lbfgs_f32
-        fn(self.device, objective, ptr(d0), ptr(d1), n, self.ls, C.byref(p), self.hv_algo, int(self.fused), ptr(x),
-           ptr(grad), ptr(trace, C.c_double), trace_cap, C.byref(res))
-        if res.status and raise_errors:
-            raise _EXC.get(res.status, RuntimeError)(res.msg.decode())
-        return dict(status=STATUS_NAMES[res.status], msg=res.msg.decode(), niter=res.niter, nfev=res.nfev, fx=res.fx,
-                    gnorm=res.gnorm, x=x, grad=grad, trace=trace[:res.trace_len].copy(), seconds=res.seconds,
-                    seconds_e2e=res.seconds_e2e, launches=res.launches, h2d_bytes=res.h2d_bytes,
-                    d2h_bytes=res.d2h_bytes)
+        fn(self.device, objective, _ptr(d0), _ptr(d1), n, self.ls, C.byref(p), self.hv_algo, int(self.fused), _ptr(x), _ptr(grad),
+           _ptr(trace), trace_cap, C.byref(res))
+        return dict(_solve_result(res, x, grad, trace, raise_errors), h2d_bytes=res.h2d_bytes, d2h_bytes=res.d2h_bytes)
 
 
 class LBFGSBSolver:
@@ -316,30 +355,21 @@ class LBFGSBSolver:
 
     def minimize(self, objective, x0, lb, ub, data0=None, data1=None, trace_cap=100000, raise_errors=False, lib=None):
         """lib: a library exporting the driver's entry points to use instead of liblbfgs_b200_driver.so."""
-        drv = driver() if lib is None else lib
+        drv = driver(lib)
         dt = self.dtype
-        ct = C.c_double if dt == np.float64 else C.c_float
         x = np.array(x0, dtype=dt, order="C").copy()
         n = x.size
         lbv = np.ascontiguousarray(np.broadcast_to(lb, n), dtype=dt)
         ubv = np.ascontiguousarray(np.broadcast_to(ub, n), dtype=dt)
         grad = np.zeros(n, dtype=dt)
         trace = np.zeros(trace_cap)
-        d0 = None if data0 is None else np.ascontiguousarray(data0, dtype=dt)
-        d1 = None if data1 is None else np.ascontiguousarray(data1, dtype=dt)
-        ptr = lambda a, t=ct: a.ctypes.data_as(C.POINTER(t)) if a is not None else None
+        d0, d1 = (None if a is None else np.ascontiguousarray(a, dtype=dt) for a in (data0, data1))
         res = _DrvResult()
         p = self.param._c()
         fn = drv.lbfgsb200_drv_lbfgsb_f64 if dt == np.float64 else drv.lbfgsb200_drv_lbfgsb_f32
-        fn.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_long, C.POINTER(_DrvParam)] + [C.c_void_p] * 5 + [C.c_long,
-                                                                                                                     C.POINTER(_DrvResult)]
-        fn(self.device, objective, ptr(d0), ptr(d1), n, C.byref(p), ptr(x), ptr(lbv), ptr(ubv), ptr(grad),
-           ptr(trace, C.c_double), trace_cap, C.byref(res))
-        if res.status and raise_errors:
-            raise _EXC.get(res.status, RuntimeError)(res.msg.decode())
-        return dict(status=STATUS_NAMES[res.status], msg=res.msg.decode(), niter=res.niter, nfev=res.nfev, fx=res.fx,
-                    gnorm=res.gnorm, x=x, grad=grad, trace=trace[:res.trace_len].copy(), seconds=res.seconds,
-                    seconds_e2e=res.seconds_e2e, launches=res.launches)
+        fn(self.device, objective, _ptr(d0), _ptr(d1), n, C.byref(p), _ptr(x), _ptr(lbv), _ptr(ubv), _ptr(grad), _ptr(trace), trace_cap,
+           C.byref(res))
+        return _solve_result(res, x, grad, trace, raise_errors)
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -574,24 +604,19 @@ class Box:
 
 
 class Session:
-    """A solver and its vectors kept resident on one GPU (bench.py): solve() repeats the same problem."""
+    """A solver and its vectors kept resident on one GPU (bench.py): solve() repeats the same problem.
+    lib: a library exporting the driver's entry points to use instead of liblbfgs_b200_driver.so."""
 
     def __init__(self, objective, x0, param, linesearch="MoreThuente", device=0, hv_algo=HV_AUTO, data0=None, data1=None,
-                 resident=True):
-        self.drv = driver()
+                 resident=True, lib=None):
+        self.drv = driver(lib)
         x0 = np.ascontiguousarray(x0, dtype=np.float64)
         self.n = x0.size
-        dp = C.POINTER(C.c_double)
-        ptr = lambda a: a.ctypes.data_as(dp) if a is not None else None
-        d0 = None if data0 is None else np.ascontiguousarray(data0, dtype=np.float64)
-        d1 = None if data1 is None else np.ascontiguousarray(data1, dtype=np.float64)
-        err = C.create_string_buffer(256)
+        d0, d1 = (None if a is None else np.ascontiguousarray(a, dtype=np.float64) for a in (data0, data1))
         p = param._c()
-        ls = LINE_SEARCHES[linesearch] if isinstance(linesearch, str) else int(linesearch)
-        self.h = self.drv.lbfgsb200_drv_session_create(device, objective, ptr(d0), ptr(d1), self.n, ls, C.byref(p), hv_algo,
-                                                       ptr(x0), err, 256, int(resident))
-        if not self.h:
-            raise RuntimeError("session_create failed: " + err.value.decode())
+        self.h = _checked("session_create", lambda *err: self.drv.lbfgsb200_drv_session_create(
+            device, objective, _ptr(d0), _ptr(d1), self.n, _ls_id(linesearch), C.byref(p), hv_algo, _ptr(x0), *err, int(resident)),
+            failed=lambda h: not h)
 
     def solve(self, from_host=False, to_host=False):
         res = _DrvResult()
@@ -606,13 +631,7 @@ class Session:
     def profile(self):
         """Accounting of the last device-resident solve: dict(kernel_ms, sync_ms, ops={name: dict(ms, rounds, alg_bytes)}); None for
         the host-driven loop."""
-        ms, rounds, nbytes = (C.c_double * 10)(), (C.c_ulonglong * 10)(), (C.c_double * 10)()
-        kms, sync = C.c_double(0), (C.c_double * 3)()
-        self.drv.lbfgsb200_drv_session_profile.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        if self.drv.lbfgsb200_drv_session_profile(self.h, C.byref(kms), ms, rounds, nbytes, sync):
-            return None
-        return dict(kernel_ms=kms.value, sync_ms=sync[0], wait_last_cta_ms=sync[1], exchange_ms=sync[2],
-                    ops={self.OPS[k]: dict(ms=ms[k], rounds=int(rounds[k]), alg_bytes=nbytes[k]) for k in range(10) if rounds[k]})
+        return _profile(self.drv.lbfgsb200_drv_session_profile, self.h)
 
     def result(self):
         p = self.drv.lbfgsb200_drv_session_result(self.h)
@@ -621,7 +640,7 @@ class Session:
     def solution(self):
         """x of the last solve(), copied from the device (the solve itself need not have asked for to_host)."""
         x = np.empty(self.n)
-        if self.drv.lbfgsb200_drv_session_download(self.h, x.ctypes.data_as(C.POINTER(C.c_double))):
+        if self.drv.lbfgsb200_drv_session_download(self.h, _ptr(x)):
             raise RuntimeError("session download failed")
         return x
 
@@ -631,25 +650,31 @@ class Session:
             self.h = None
 
 
+def _profile(fn, h):
+    """The profile dict of Session.profile() from a *_profile entry point, or None when the solve ran no device-resident solver."""
+    ms, rounds, nbytes = (C.c_double * 10)(), (C.c_ulonglong * 10)(), (C.c_double * 10)()
+    kms, sync = C.c_double(0), (C.c_double * 3)()
+    if fn(h, C.byref(kms), ms, rounds, nbytes, sync):
+        return None
+    return dict(kernel_ms=kms.value, sync_ms=sync[0], wait_last_cta_ms=sync[1], exchange_ms=sync[2],
+                ops={Session.OPS[k]: dict(ms=ms[k], rounds=int(rounds[k]), alg_bytes=nbytes[k]) for k in range(10) if rounds[k]})
+
+
 def solve_batch(objective, X0, param=None, linesearch="MoreThuente", device=0, hv_algo=HV_AUTO, threads=4, sharded=False,
-                return_x=True):
+                return_x=True, lib=None):
     """B independent problems (rows of X0) on one GPU: LBFGSSolver::minimize per problem, `threads` host threads each with
     its own context/stream.  sharded=True: run on the driver's communicator-attached context (n-sharded over ranks), one
     thread.  Returns (list of dicts, X, seconds)."""
-    drv = driver()
+    drv = driver(lib)
     X0 = np.ascontiguousarray(X0, dtype=np.float64)
     B, n = X0.shape
     param = param if param is not None else LBFGSParam()
     items = (_BatchItem * B)()
     X = np.empty_like(X0) if return_x else None
     secs = C.c_double(0)
-    dp = C.POINTER(C.c_double)
-    drv.lbfgsb200_drv_batch_f64.argtypes = [C.c_int, C.c_int, C.c_long, C.c_int, dp, C.c_int, C.POINTER(_DrvParam), C.c_int, C.c_int,
-                                            C.c_int, C.POINTER(_BatchItem), dp, dp]
     p = param._c()
-    ls = LINE_SEARCHES[linesearch] if isinstance(linesearch, str) else int(linesearch)
-    drv.lbfgsb200_drv_batch_f64(device, objective, n, B, X0.ctypes.data_as(dp), ls, C.byref(p), hv_algo, threads, int(sharded), items,
-                                X.ctypes.data_as(dp) if return_x else None, C.byref(secs))
+    drv.lbfgsb200_drv_batch_f64(device, objective, n, B, _ptr(X0), _ls_id(linesearch), C.byref(p), hv_algo, threads, int(sharded), items,
+                                _ptr(X), C.byref(secs))
     res = [dict(status=STATUS_NAMES[it.status], niter=it.niter, nfev=it.nfev, fx=it.fx, gnorm=it.gnorm) for it in items]
     return res, X, secs.value
 
@@ -659,29 +684,22 @@ class BatchSession:
     include/LBFGSBatch.h).  The start points stay resident; with a communicator attached to the device's driver context the rows
     are this rank's blocks of n-sharded problems."""
 
-    def __init__(self, objective, X0, param=None, linesearch="MoreThuente", device=0):
-        self.drv = driver()
+    def __init__(self, objective, X0, param=None, linesearch="MoreThuente", device=0, lib=None):
+        self.drv = driver(lib)
         X0 = np.ascontiguousarray(X0, dtype=np.float64)
         self.B, self.n = X0.shape
         param = param if param is not None else LBFGSParam()
         p = param._c()
-        ls = LINE_SEARCHES[linesearch] if isinstance(linesearch, str) else int(linesearch)
-        err = C.create_string_buffer(256)
-        self.h = self.drv.lbfgsb200_drv_batch_session_create(device, objective, self.n, self.B, X0.ctypes.data_as(C.POINTER(C.c_double)), ls,
-                                                             C.byref(p), err, 256)
-        if not self.h:
-            raise RuntimeError("batch_session_create failed: " + err.value.decode())
+        self.h = _checked("batch_session_create", lambda *err: self.drv.lbfgsb200_drv_batch_session_create(
+            device, objective, self.n, self.B, _ptr(X0), _ls_id(linesearch), C.byref(p), *err), failed=lambda h: not h)
 
     def solve(self, return_x=True):
         items = (_BatchItem * self.B)()
         rounds = (C.c_long * self.B)()
         X = np.empty((self.B, self.n)) if return_x else None
         secs = C.c_double(0)
-        err = C.create_string_buffer(256)
-        bad = self.drv.lbfgsb200_drv_batch_session_solve(self.h, items, rounds, X.ctypes.data_as(C.POINTER(C.c_double)) if return_x else None,
-                                                         C.byref(secs), err, 256)
-        if bad < 0:
-            raise RuntimeError("batch solve failed: " + err.value.decode())
+        _checked("batch solve", lambda *err: self.drv.lbfgsb200_drv_batch_session_solve(self.h, items, rounds, _ptr(X), C.byref(secs), *err),
+                 failed=lambda bad: bad < 0)
         res = [dict(status=STATUS_NAMES[it.status], niter=it.niter, nfev=it.nfev, fx=it.fx, gnorm=it.gnorm, rounds=int(r))
                for it, r in zip(items, rounds)]
         return res, X, secs.value
@@ -690,28 +708,19 @@ class BatchSession:
         """New start points (host array, B x n) for the following solves: the host -> device leg of the end-to-end path."""
         X0 = np.ascontiguousarray(X0, dtype=np.float64)
         assert X0.shape == (self.B, self.n)
-        err = C.create_string_buffer(256)
-        self.drv.lbfgsb200_drv_batch_session_upload.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.c_char_p, C.c_int]
-        if self.drv.lbfgsb200_drv_batch_session_upload(self.h, X0.ctypes.data_as(C.POINTER(C.c_double)), err, 256):
-            raise RuntimeError("batch upload failed: " + err.value.decode())
+        _checked("batch upload", lambda *err: self.drv.lbfgsb200_drv_batch_session_upload(self.h, _ptr(X0), *err))
         return X0.nbytes
 
     def solution(self):
         """X (B x n) of the last solve(), copied from the device (also after solve(return_x=False))."""
         X = np.empty((self.B, self.n))
-        if self.drv.lbfgsb200_drv_batch_session_download(self.h, X.ctypes.data_as(C.POINTER(C.c_double))):
+        if self.drv.lbfgsb200_drv_batch_session_download(self.h, _ptr(X)):
             raise RuntimeError("batch session download failed")
         return X
 
     def profile(self):
         """Accounting of the last batched solve (one kernel launch for the whole batch): same dict as Session.profile()."""
-        ms, rounds, nbytes = (C.c_double * 10)(), (C.c_ulonglong * 10)(), (C.c_double * 10)()
-        kms, sync = C.c_double(0), (C.c_double * 3)()
-        self.drv.lbfgsb200_drv_batch_session_profile.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        if self.drv.lbfgsb200_drv_batch_session_profile(self.h, C.byref(kms), ms, rounds, nbytes, sync):
-            return None
-        return dict(kernel_ms=kms.value, sync_ms=sync[0], wait_last_cta_ms=sync[1], exchange_ms=sync[2],
-                    ops={Session.OPS[k]: dict(ms=ms[k], rounds=int(rounds[k]), alg_bytes=nbytes[k]) for k in range(10) if rounds[k]})
+        return _profile(self.drv.lbfgsb200_drv_batch_session_profile, self.h)
 
     def close(self):
         if self.h:
@@ -719,23 +728,17 @@ class BatchSession:
             self.h = None
 
 
-def solve_dense(objective, x0, param=None, linesearch="NocedalWright", resident=True, device=0):
+def solve_dense(objective, x0, param=None, linesearch="NocedalWright", resident=True, device=0, lib=None):
     """minimize() then final_approx_hessian() / final_approx_inverse_hessian() (small n).  Returns (niter, x, B, H)."""
-    drv = driver()
+    drv = driver(lib)
     x = np.array(x0, dtype=np.float64, order="C").copy()
     n = x.size
     param = param if param is not None else LBFGSParam()
     p = param._c()
-    ls = LINE_SEARCHES[linesearch] if isinstance(linesearch, str) else int(linesearch)
     Bm, Hm = np.zeros((n, n)), np.zeros((n, n))
     niter = C.c_int(0)
-    err = C.create_string_buffer(256)
-    dp = C.POINTER(C.c_double)
-    drv.lbfgsb200_drv_solve_dense_f64.argtypes = [C.c_int, C.c_int, C.c_long, C.c_int, C.POINTER(_DrvParam), C.c_int, dp, dp, dp,
-                                                  C.POINTER(C.c_int), C.c_char_p, C.c_int]
-    if drv.lbfgsb200_drv_solve_dense_f64(device, objective, n, ls, C.byref(p), int(resident), x.ctypes.data_as(dp), Bm.ctypes.data_as(dp),
-                                         Hm.ctypes.data_as(dp), C.byref(niter), err, 256):
-        raise RuntimeError("solve_dense failed: " + err.value.decode())
+    _checked("solve_dense", lambda *err: drv.lbfgsb200_drv_solve_dense_f64(device, objective, n, _ls_id(linesearch), C.byref(p), int(resident),
+                                                                          _ptr(x), _ptr(Bm), _ptr(Hm), C.byref(niter), *err))
     return niter.value, x, Bm, Hm
 
 
@@ -758,36 +761,27 @@ def driver_ctx(device=0):
 
 def comm_init(device, unique_id_bytes, rank, nranks, index_offset=0):
     """Attach an NCCL communicator to the driver's context of `device`: n is sharded over `nranks` GPUs."""
-    err = C.create_string_buffer(256)
     buf = C.create_string_buffer(bytes(unique_id_bytes), 128)
-    st = driver().lbfgsb200_drv_comm_init(device, buf, rank, nranks, index_offset, err, 256)
-    if st:
-        raise RuntimeError("comm_init failed: " + err.value.decode())
+    _checked("comm_init", lambda *err: driver().lbfgsb200_drv_comm_init(device, buf, rank, nranks, index_offset, *err))
 
 
 def p2p_export(device):
     """64-byte cudaIpc handle of this rank's inbox for the in-kernel NVLink all-reduce."""
-    err = C.create_string_buffer(256)
     buf = C.create_string_buffer(64)
-    if driver().lbfgsb200_drv_p2p_export(device, buf, err, 256):
-        raise RuntimeError("p2p_export failed: " + err.value.decode())
+    _checked("p2p_export", lambda *err: driver().lbfgsb200_drv_p2p_export(device, buf, *err))
     return buf.raw
 
 
 def p2p_attach(device, all_handles, rank, nranks, index_offset=0):
     """all_handles: the nranks 64-byte handles concatenated in rank order."""
-    err = C.create_string_buffer(256)
     buf = C.create_string_buffer(bytes(all_handles), 64 * nranks)
-    if driver().lbfgsb200_drv_p2p_attach(device, buf, rank, nranks, index_offset, err, 256):
-        raise RuntimeError("p2p_attach failed: " + err.value.decode())
+    _checked("p2p_attach", lambda *err: driver().lbfgsb200_drv_p2p_attach(device, buf, rank, nranks, index_offset, *err))
 
 
 def set_global_extent(device, index_offset, n_global):
     """Declare this rank's block of the global vector (needed by the chained-Rosenbrock / tridiagonal objectives when sharded:
     they exchange one boundary coordinate per side with the neighbouring ranks before every evaluation)."""
-    err = C.create_string_buffer(256)
-    if driver().lbfgsb200_drv_set_global_extent(device, C.c_longlong(index_offset), C.c_longlong(n_global), err, 256):
-        raise RuntimeError("set_global_extent failed: " + err.value.decode())
+    _checked("set_global_extent", lambda *err: driver().lbfgsb200_drv_set_global_extent(device, index_offset, n_global, *err))
 
 
 def comm_unique_id():

@@ -67,6 +67,28 @@ Device& device(int ordinal)
     return *d;
 }
 
+// The solver types of one line-search policy; with_line_search() hands one of these to its callback.
+template <template <class> class LS>
+struct LineSearchTag
+{
+    template <class Scalar> using Solver = LBFGSSolver<Scalar, LS>;
+    template <class Scalar> using BatchSolver = LBFGSBatchSolver<Scalar, LS>;
+};
+
+// f(LineSearchTag<LS>()) for the policy of a DRV_LS_* id: the one place a line-search id becomes a type.
+template <class F>
+auto with_line_search(int ls, F f) -> decltype(f(LineSearchTag<LineSearchMoreThuente>()))
+{
+    switch (ls)
+    {
+    case DRV_LS_BACKTRACKING: return f(LineSearchTag<LineSearchBacktracking>());
+    case DRV_LS_BRACKETING: return f(LineSearchTag<LineSearchBracketing>());
+    case DRV_LS_NOCEDAL_WRIGHT: return f(LineSearchTag<LineSearchNocedalWright>());
+    case DRV_LS_MORE_THUENTE: return f(LineSearchTag<LineSearchMoreThuente>());
+    default: throw std::invalid_argument("unknown line search id");
+    }
+}
+
 // Records f of every evaluation (the reference offers the functor as its only observation point,
 // examples/example-rosenbrock-comparison.cpp:14-41) while forwarding the fused hooks when Base has them.
 template <class Base, class Scalar, bool Fused>
@@ -121,6 +143,19 @@ int guarded(drv_result* out, Body body)
     return out->status;
 }
 
+// The entry points that report through a caller's text buffer: body()'s result, or `failed` with the exception's message in
+// err (errlen bytes, NUL-terminated).
+template <class R, class Body>
+R reported(char* err, int errlen, R failed, Body body)
+{
+    try { return body(); }
+    catch (const std::exception& e)
+    {
+        if (err && errlen > 0) { std::strncpy(err, e.what(), size_t(errlen) - 1); err[errlen - 1] = 0; }
+        return failed;
+    }
+}
+
 template <class Scalar>
 LBFGSParam<Scalar> to_param(const drv_param* q)
 {
@@ -140,83 +175,45 @@ LBFGSParam<Scalar> to_param(const drv_param* q)
     return p;
 }
 
+template <class Scalar>
+LBFGSBParam<Scalar> to_box_param(const drv_param* q)
+{
+    LBFGSBParam<Scalar> p;
+    p.m = q->m;
+    p.epsilon = Scalar(q->epsilon);
+    p.epsilon_rel = Scalar(q->epsilon_rel);
+    p.past = q->past;
+    p.delta = Scalar(q->delta);
+    p.max_iterations = q->max_iterations;
+    p.max_submin = q->max_submin;
+    p.max_linesearch = q->max_linesearch;
+    p.min_step = Scalar(q->min_step);
+    p.max_step = Scalar(q->max_step);
+    p.ftol = Scalar(q->ftol);
+    p.wolfe = Scalar(q->wolfe);
+    return p;
+}
+
 double now() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 
-template <class Scalar, template <class> class LS, class Objective, bool Fused>
-void solve_with(Device& dev, Objective& obj, const drv_param* q, int hv_algo, long n, Scalar* x_host, Scalar* grad_host,
-                double* trace, long cap, drv_result* out, double t_begin, long h2d_extra)
+// One minimize() on x (already uploaded) with its outcome written to `out`.  minimize(fx) runs the solve and returns the
+// iterations; nfev() counts the evaluations, also after a throw.  x_host receives the solution, and on a throw the last
+// iterate when x_on_error; grad_host (optional) the final gradient.  h2d_bytes: everything uploaded for this call.
+template <class Scalar, class Solver, class Minimize, class Nfev>
+void run_and_record(Device& dev, const Solver& solver, DeviceVector<Scalar>& x, Minimize minimize, Nfev nfev, bool x_on_error,
+                    Scalar* x_host, Scalar* grad_host, long cap, long h2d_bytes, double t_begin, drv_result* out)
 {
-    typedef DeviceVector<Scalar> Vector;
-    const LBFGSParam<Scalar> prm = to_param<Scalar>(q);
-    LBFGSSolver<Scalar, LS> solver(prm);
-    solver.set_hv_algorithm(hv_algo);
-    Traced<Objective, Scalar, Fused> f(obj, trace, cap);
-    Vector x(dev);
-    x.copy_from_host(x_host, n);
+    const long n = long(x.size());
     Scalar fx = Scalar(0);
     const unsigned long long launches0 = lbfgs_b200_launch_count(dev.ctx());
     const double t0 = now();
     int niter = 0;
-    try { niter = solver.minimize(f, x, fx); }
+    try { niter = minimize(fx); }
     catch (...)
     {
-        out->nfev = f.count;
-        out->trace_len = f.count < cap ? f.count : cap;
-        x.copy_to_host(x_host);
-        throw;
-    }
-    dev.synchronize();
-    const double t1 = now();
-    x.copy_to_host(x_host);
-    if (grad_host) solver.final_grad().copy_to_host(grad_host);
-    const double t2 = now();
-    out->niter = niter;
-    out->fx = double(fx);
-    out->gnorm = double(solver.final_grad_norm());
-    out->nfev = f.count;
-    out->trace_len = f.count < cap ? f.count : cap;
-    out->seconds = t1 - t0;
-    out->seconds_e2e = t2 - t_begin;
-    out->launches = lbfgs_b200_launch_count(dev.ctx()) - launches0;
-    out->h2d_bytes = long(sizeof(Scalar)) * n + h2d_extra;
-    out->d2h_bytes = long(sizeof(Scalar)) * n * (grad_host ? 2 : 1);
-}
-
-template <class Scalar, class Objective, bool Fused>
-void solve_ls(int ls, Device& dev, Objective& obj, const drv_param* q, int hv_algo, long n, Scalar* x_host, Scalar* grad_host,
-              double* trace, long cap, drv_result* out, double t_begin, long h2d_extra)
-{
-    switch (ls)
-    {
-    case DRV_LS_BACKTRACKING: solve_with<Scalar, LineSearchBacktracking, Objective, Fused>(dev, obj, q, hv_algo, n, x_host, grad_host, trace, cap, out, t_begin, h2d_extra); break;
-    case DRV_LS_BRACKETING: solve_with<Scalar, LineSearchBracketing, Objective, Fused>(dev, obj, q, hv_algo, n, x_host, grad_host, trace, cap, out, t_begin, h2d_extra); break;
-    case DRV_LS_NOCEDAL_WRIGHT: solve_with<Scalar, LineSearchNocedalWright, Objective, Fused>(dev, obj, q, hv_algo, n, x_host, grad_host, trace, cap, out, t_begin, h2d_extra); break;
-    case DRV_LS_MORE_THUENTE: solve_with<Scalar, LineSearchMoreThuente, Objective, Fused>(dev, obj, q, hv_algo, n, x_host, grad_host, trace, cap, out, t_begin, h2d_extra); break;
-    default: throw std::invalid_argument("unknown line search id");
-    }
-}
-
-template <class Scalar, template <class> class LS>
-void solve_resident_with(Device& dev, BuiltinObjective<Scalar>& obj, const drv_param* q, long n, Scalar* x_host, Scalar* grad_host,
-                         double* trace, long cap, drv_result* out, double t_begin, long h2d_extra)
-{
-    typedef DeviceVector<Scalar> Vector;
-    const LBFGSParam<Scalar> prm = to_param<Scalar>(q);
-    LBFGSSolver<Scalar, LS> solver(prm);
-    solver.set_device_resident(true);
-    solver.set_trace_buffer(trace, cap);
-    Vector x(dev);
-    x.copy_from_host(x_host, n);
-    Scalar fx = Scalar(0);
-    const unsigned long long launches0 = lbfgs_b200_launch_count(dev.ctx());
-    const double t0 = now();
-    int niter = 0;
-    try { niter = solver.minimize(obj, x, fx); }
-    catch (...)
-    {
-        out->nfev = solver.num_evaluations();
+        out->nfev = nfev();
         out->trace_len = out->nfev < cap ? out->nfev : cap;
-        x.copy_to_host(x_host);
+        if (x_on_error) x.copy_to_host(x_host);
         throw;
     }
     dev.synchronize();
@@ -226,27 +223,13 @@ void solve_resident_with(Device& dev, BuiltinObjective<Scalar>& obj, const drv_p
     out->niter = niter;
     out->fx = double(fx);
     out->gnorm = double(solver.final_grad_norm());
-    out->nfev = solver.num_evaluations();
+    out->nfev = nfev();
     out->trace_len = out->nfev < cap ? out->nfev : cap;
     out->seconds = t1 - t0;
     out->seconds_e2e = now() - t_begin;
     out->launches = lbfgs_b200_launch_count(dev.ctx()) - launches0;
-    out->h2d_bytes = long(sizeof(Scalar)) * n + h2d_extra;
+    out->h2d_bytes = h2d_bytes;
     out->d2h_bytes = long(sizeof(Scalar)) * n * (grad_host ? 2 : 1);
-}
-
-template <class Scalar>
-void solve_resident(int ls, Device& dev, BuiltinObjective<Scalar>& obj, const drv_param* q, long n, Scalar* x_host, Scalar* grad_host,
-                    double* trace, long cap, drv_result* out, double t_begin, long h2d_extra)
-{
-    switch (ls)
-    {
-    case DRV_LS_BACKTRACKING: solve_resident_with<Scalar, LineSearchBacktracking>(dev, obj, q, n, x_host, grad_host, trace, cap, out, t_begin, h2d_extra); break;
-    case DRV_LS_BRACKETING: solve_resident_with<Scalar, LineSearchBracketing>(dev, obj, q, n, x_host, grad_host, trace, cap, out, t_begin, h2d_extra); break;
-    case DRV_LS_NOCEDAL_WRIGHT: solve_resident_with<Scalar, LineSearchNocedalWright>(dev, obj, q, n, x_host, grad_host, trace, cap, out, t_begin, h2d_extra); break;
-    case DRV_LS_MORE_THUENTE: solve_resident_with<Scalar, LineSearchMoreThuente>(dev, obj, q, n, x_host, grad_host, trace, cap, out, t_begin, h2d_extra); break;
-    default: throw std::invalid_argument("unknown line search id");
-    }
 }
 
 template <class Scalar>
@@ -258,24 +241,39 @@ int lbfgs_any(int dev_ordinal, int objective, const Scalar* data0_host, const Sc
         const double t_begin = now();
         Device& dev = device(dev_ordinal);
         DeviceVector<Scalar> d0(dev), d1(dev);
-        long extra = 0;
-        if (data0_host) { d0.copy_from_host(data0_host, n); extra += long(sizeof(Scalar)) * n; }
-        if (data1_host) { d1.copy_from_host(data1_host, n); extra += long(sizeof(Scalar)) * n; }
-        if (fused == 2)   // device-resident solve: the objective must stay visible as a built-in (no tracing wrapper)
-        {
-            BuiltinObjective<Scalar> obj(objective, d0.data(), d1.data());
-            solve_resident<Scalar>(ls, dev, obj, q, n, x_host, grad_host, trace, cap, out, t_begin, extra);
-        }
-        else if (fused)
-        {
-            BuiltinObjective<Scalar> obj(objective, d0.data(), d1.data());
-            solve_ls<Scalar, BuiltinObjective<Scalar>, true>(ls, dev, obj, q, hv_algo, n, x_host, grad_host, trace, cap, out, t_begin, extra);
-        }
-        else
-        {
-            PlainObjective<Scalar> obj(objective, d0.data(), d1.data());
-            solve_ls<Scalar, PlainObjective<Scalar>, false>(ls, dev, obj, q, hv_algo, n, x_host, grad_host, trace, cap, out, t_begin, extra);
-        }
+        long h2d = long(sizeof(Scalar)) * n;
+        if (data0_host) { d0.copy_from_host(data0_host, n); h2d += long(sizeof(Scalar)) * n; }
+        if (data1_host) { d1.copy_from_host(data1_host, n); h2d += long(sizeof(Scalar)) * n; }
+        const LBFGSParam<Scalar> prm = to_param<Scalar>(q);
+        with_line_search(ls, [&](auto tag) {
+            typename decltype(tag)::template Solver<Scalar> solver(prm);
+            DeviceVector<Scalar> x(dev);
+            x.copy_from_host(x_host, n);
+            auto record = [&](auto minimize, auto nfev) {
+                run_and_record(dev, solver, x, minimize, nfev, true, x_host, grad_host, cap, h2d, t_begin, out);
+            };
+            if (fused == 2)   // device-resident solve: the objective must stay visible as a built-in (no tracing wrapper)
+            {
+                solver.set_device_resident(true);
+                solver.set_trace_buffer(trace, cap);
+                BuiltinObjective<Scalar> obj(objective, d0.data(), d1.data());
+                record([&](Scalar& fx) { return solver.minimize(obj, x, fx); }, [&]() { return solver.num_evaluations(); });
+                return;
+            }
+            solver.set_hv_algorithm(hv_algo);
+            if (fused)
+            {
+                BuiltinObjective<Scalar> obj(objective, d0.data(), d1.data());
+                Traced<BuiltinObjective<Scalar>, Scalar, true> f(obj, trace, cap);
+                record([&](Scalar& fx) { return solver.minimize(f, x, fx); }, [&]() { return f.count; });
+            }
+            else
+            {
+                PlainObjective<Scalar> obj(objective, d0.data(), d1.data());
+                Traced<PlainObjective<Scalar>, Scalar, false> f(obj, trace, cap);
+                record([&](Scalar& fx) { return solver.minimize(f, x, fx); }, [&]() { return f.count; });
+            }
+        });
     });
 }
 
@@ -315,24 +313,52 @@ void lbfgsb200_drv_shutdown(void) { devices().clear(); }
 // ----------------------------------------------------------------------------------------------------------
 namespace {
 
+// accounting of a device-resident solver's last solve (lbfgs_b200_solver_profile; sync_ms has 3 slots): 0 on success, 1 when
+// there is no such solver, 2 when the query fails
+int profile_of(const lbfgs_b200_solver* r, double* kernel_ms, double* ms_by_op10, unsigned long long* rounds_by_op10,
+               double* alg_bytes_by_op10, double* sync_ms)
+{
+    if (!r) return 1;
+    return lbfgs_b200_solver_profile(r, kernel_ms, ms_by_op10, rounds_by_op10, alg_bytes_by_op10, sync_ms) == LBFGS_B200_OK ? 0 : 2;
+}
+
 struct Session
 {
     Device* dev;
     long n;
-    int ls;
-    LBFGSParam<double> prm;
     DeviceVector<double> x0, x, d0, d1;
     BuiltinObjective<double> obj;
-    // one solver per line-search policy (only the selected one is used)
-    LBFGSSolver<double, LineSearchBacktracking> s_bt;
-    LBFGSSolver<double, LineSearchBracketing> s_br;
-    LBFGSSolver<double, LineSearchNocedalWright> s_nw;
-    LBFGSSolver<double, LineSearchMoreThuente> s_mt;
     double* pinned_in;   // host staging (pinned): x0 for the end-to-end path
     double* pinned_out;  // host staging (pinned): result x
-    Session(Device& d, long n_, int ls_, const drv_param* q, int objective) :
-        dev(&d), n(n_), ls(ls_), prm(to_param<double>(q)), x0(d), x(d), d0(d), d1(d), obj(objective),
-        s_bt(prm), s_br(prm), s_nw(prm), s_mt(prm), pinned_in(nullptr), pinned_out(nullptr) {}
+    Session(Device& d, long n_, int objective) :
+        dev(&d), n(n_), x0(d), x(d), d0(d), d1(d), obj(objective), pinned_in(nullptr), pinned_out(nullptr) {}
+    virtual ~Session() {}
+    // minimize() from x: niter, nfev, fx and gnorm into out
+    virtual void minimize(drv_result* out) = 0;
+    virtual const lbfgs_b200_solver* resident_handle() const = 0;
+};
+
+// a session's solver, for the one line search it was created with
+template <class Tag>
+struct SessionOf : Session
+{
+    const LBFGSParam<double> prm;   // the solver holds it by reference
+    typename Tag::template Solver<double> solver;
+    SessionOf(Device& d, long n_, const drv_param* q, int objective, int hv_algo, bool resident) :
+        Session(d, n_, objective), prm(to_param<double>(q)), solver(prm)
+    {
+        solver.set_hv_algorithm(hv_algo);
+        solver.set_device_resident(resident);
+    }
+    void minimize(drv_result* out) override
+    {
+        double fx = 0;
+        out->niter = solver.minimize(obj, x, fx);
+        out->nfev = solver.num_evaluations();
+        out->fx = fx;
+        out->gnorm = solver.final_grad_norm();
+    }
+    const lbfgs_b200_solver* resident_handle() const override { return solver.resident_handle(); }
 };
 
 }  // namespace
@@ -344,10 +370,11 @@ void* lbfgsb200_drv_session_create(int device_ordinal, int objective, const doub
                                    long n, int ls, const drv_param* prm, int hv_algo, const double* x0_host, char* err, int errlen,
                                    int resident)
 {
-    try
-    {
+    return reported<void*>(err, errlen, nullptr, [&]() {
         Device& dev = device(device_ordinal);
-        std::unique_ptr<Session> s(new Session(dev, n, ls, prm, objective));
+        std::unique_ptr<Session> s(with_line_search(ls, [&](auto tag) -> Session* {
+            return new SessionOf<decltype(tag)>(dev, n, prm, objective, hv_algo, resident != 0);
+        }));
         s->x0.copy_from_host(x0_host, n);
         s->x.resize(n);
         if (data0_host) s->d0.copy_from_host(data0_host, n);
@@ -359,21 +386,8 @@ void* lbfgsb200_drv_session_create(int device_ordinal, int objective, const doub
         dev.check(lbfgs_b200_malloc_host(dev.ctx(), &p, sizeof(double) * size_t(n)));
         s->pinned_out = static_cast<double*>(p);
         std::memcpy(s->pinned_in, x0_host, sizeof(double) * size_t(n));
-        s->s_bt.set_hv_algorithm(hv_algo);
-        s->s_br.set_hv_algorithm(hv_algo);
-        s->s_nw.set_hv_algorithm(hv_algo);
-        s->s_mt.set_hv_algorithm(hv_algo);
-        s->s_bt.set_device_resident(resident != 0);
-        s->s_br.set_device_resident(resident != 0);
-        s->s_nw.set_device_resident(resident != 0);
-        s->s_mt.set_device_resident(resident != 0);
-        return s.release();
-    }
-    catch (const std::exception& e)
-    {
-        if (err && errlen > 0) { std::strncpy(err, e.what(), size_t(errlen) - 1); err[errlen - 1] = 0; }
-        return nullptr;
-    }
+        return static_cast<void*>(s.release());
+    });
 }
 
 void lbfgsb200_drv_session_destroy(void* handle)
@@ -398,22 +412,8 @@ int lbfgsb200_drv_session_solve(void* handle, int from_host, int to_host, drv_re
         if (from_host) dev.check(lbfgs_b200_memcpy_h2d(dev.ctx(), s->x.data(), s->pinned_in, bytes));
         else dev.check(lbfgs_b200_memcpy_d2d(dev.ctx(), s->x.data(), s->x0.data(), bytes));
         const unsigned long long launches0 = lbfgs_b200_launch_count(dev.ctx());
-        double fx = 0;
-        int niter = 0;
-        long nfev = 0;
-        double gnorm = 0;
-        switch (s->ls)
-        {
-        case DRV_LS_BACKTRACKING: niter = s->s_bt.minimize(s->obj, s->x, fx); nfev = s->s_bt.num_evaluations(); gnorm = s->s_bt.final_grad_norm(); break;
-        case DRV_LS_BRACKETING: niter = s->s_br.minimize(s->obj, s->x, fx); nfev = s->s_br.num_evaluations(); gnorm = s->s_br.final_grad_norm(); break;
-        case DRV_LS_NOCEDAL_WRIGHT: niter = s->s_nw.minimize(s->obj, s->x, fx); nfev = s->s_nw.num_evaluations(); gnorm = s->s_nw.final_grad_norm(); break;
-        default: niter = s->s_mt.minimize(s->obj, s->x, fx); nfev = s->s_mt.num_evaluations(); gnorm = s->s_mt.final_grad_norm(); break;
-        }
+        s->minimize(out);
         if (to_host) dev.check(lbfgs_b200_memcpy_d2h(dev.ctx(), s->pinned_out, s->x.data(), bytes));
-        out->niter = niter;
-        out->nfev = nfev;
-        out->fx = fx;
-        out->gnorm = gnorm;
         out->launches = lbfgs_b200_launch_count(dev.ctx()) - launches0;
         out->h2d_bytes = from_host ? long(bytes) : 0;
         out->d2h_bytes = to_host ? long(bytes) : 0;
@@ -435,17 +435,7 @@ int lbfgsb200_drv_session_download(void* handle, double* x_out_host)
 int lbfgsb200_drv_session_profile(void* handle, double* kernel_ms, double* ms_by_op10, unsigned long long* rounds_by_op10, double* alg_bytes_by_op10,
                                   double* sync_ms)
 {
-    Session* s = static_cast<Session*>(handle);
-    lbfgs_b200_solver* r = nullptr;
-    switch (s->ls)
-    {
-    case DRV_LS_BACKTRACKING: r = s->s_bt.resident_handle(); break;
-    case DRV_LS_BRACKETING: r = s->s_br.resident_handle(); break;
-    case DRV_LS_NOCEDAL_WRIGHT: r = s->s_nw.resident_handle(); break;
-    default: r = s->s_mt.resident_handle(); break;
-    }
-    if (!r) return 1;
-    return lbfgs_b200_solver_profile(r, kernel_ms, ms_by_op10, rounds_by_op10, alg_bytes_by_op10, sync_ms) == LBFGS_B200_OK ? 0 : 2;
+    return profile_of(static_cast<Session*>(handle)->resident_handle(), kernel_ms, ms_by_op10, rounds_by_op10, alg_bytes_by_op10, sync_ms);
 }
 
 }  // extern "C"
@@ -453,67 +443,43 @@ int lbfgsb200_drv_session_profile(void* handle, double* kernel_ms, double* ms_by
 extern "C" int lbfgsb200_drv_comm_init(int device_ordinal, const void* unique_id_128, int rank, int nranks, long long index_offset,
                                        char* err, int errlen)
 {
-    try
-    {
+    return reported(err, errlen, 1, [&]() {
         Device& dev = device(device_ordinal);
         dev.check(lbfgs_b200_comm_init(dev.ctx(), unique_id_128, rank, nranks));
         dev.check(lbfgs_b200_set_index_offset(dev.ctx(), index_offset));
         return 0;
-    }
-    catch (const std::exception& e)
-    {
-        if (err && errlen > 0) { std::strncpy(err, e.what(), size_t(errlen) - 1); err[errlen - 1] = 0; }
-        return 1;
-    }
+    });
 }
 
 extern "C" int lbfgsb200_drv_p2p_export(int device_ordinal, void* handle64, char* err, int errlen)
 {
-    try
-    {
+    return reported(err, errlen, 1, [&]() {
         Device& dev = device(device_ordinal);
         dev.check(lbfgs_b200_comm_p2p_export(dev.ctx(), handle64));
         return 0;
-    }
-    catch (const std::exception& e)
-    {
-        if (err && errlen > 0) { std::strncpy(err, e.what(), size_t(errlen) - 1); err[errlen - 1] = 0; }
-        return 1;
-    }
+    });
 }
 
 extern "C" int lbfgsb200_drv_p2p_attach(int device_ordinal, const void* handles, int rank, int nranks, long long index_offset,
                                         char* err, int errlen)
 {
-    try
-    {
+    return reported(err, errlen, 1, [&]() {
         Device& dev = device(device_ordinal);
         dev.check(lbfgs_b200_comm_p2p_attach(dev.ctx(), handles, rank, nranks));
         dev.check(lbfgs_b200_set_index_offset(dev.ctx(), index_offset));
         return 0;
-    }
-    catch (const std::exception& e)
-    {
-        if (err && errlen > 0) { std::strncpy(err, e.what(), size_t(errlen) - 1); err[errlen - 1] = 0; }
-        return 1;
-    }
+    });
 }
 
 // n-sharding: declare this rank's block [index_offset, index_offset + n_local) of a global vector of n_global coordinates
 // (needed by the neighbour-coupled built-in objectives, which exchange halos; see lbfgs_b200_set_global_extent)
 extern "C" int lbfgsb200_drv_set_global_extent(int device_ordinal, long long index_offset, long long n_global, char* err, int errlen)
 {
-    try
-    {
+    return reported(err, errlen, 1, [&]() {
         Device& dev = device(device_ordinal);
         dev.check(lbfgs_b200_set_global_extent(dev.ctx(), index_offset, n_global));
         return 0;
-    }
-    catch (const std::exception& e)
-    {
-        if (err && errlen > 0) { std::strncpy(err, e.what(), size_t(errlen) - 1); err[errlen - 1] = 0; }
-        return 1;
-    }
+    });
 }
 
 
@@ -535,39 +501,12 @@ int lbfgsb_any(int device_ordinal, int objective, const Scalar* data0_host, cons
         x.copy_from_host(x_host, n);
         lb.copy_from_host(lb_host, n);
         ub.copy_from_host(ub_host, n);
-        LBFGSBParam<Scalar> prm;
-        prm.m = q->m; prm.epsilon = Scalar(q->epsilon); prm.epsilon_rel = Scalar(q->epsilon_rel); prm.past = q->past;
-        prm.delta = Scalar(q->delta); prm.max_iterations = q->max_iterations; prm.max_submin = q->max_submin;
-        prm.max_linesearch = q->max_linesearch; prm.min_step = Scalar(q->min_step); prm.max_step = Scalar(q->max_step);
-        prm.ftol = Scalar(q->ftol); prm.wolfe = Scalar(q->wolfe);
+        const LBFGSBParam<Scalar> prm = to_box_param<Scalar>(q);
         LBFGSBSolver<Scalar> solver(prm);
         BuiltinObjective<Scalar> obj(objective, d0.data(), d1.data());
         Traced<BuiltinObjective<Scalar>, Scalar, true> f(obj, fx_trace, trace_cap);
-        Scalar fx = 0;
-        const unsigned long long launches0 = lbfgs_b200_launch_count(dev.ctx());
-        const double t0 = now();
-        int niter = 0;
-        try { niter = solver.minimize(f, x, fx, lb, ub); }
-        catch (...)
-        {
-            out->nfev = f.count;
-            out->trace_len = f.count < trace_cap ? f.count : trace_cap;
-            throw;
-        }
-        dev.synchronize();
-        const double t1 = now();
-        x.copy_to_host(x_host);
-        if (grad_host) solver.final_grad().copy_to_host(grad_host);
-        out->niter = niter;
-        out->fx = double(fx);
-        out->gnorm = double(solver.final_grad_norm());
-        out->nfev = f.count;
-        out->trace_len = f.count < trace_cap ? f.count : trace_cap;
-        out->seconds = t1 - t0;
-        out->seconds_e2e = now() - t_begin;
-        out->launches = lbfgs_b200_launch_count(dev.ctx()) - launches0;
-        out->h2d_bytes = long(sizeof(Scalar)) * n * 3;
-        out->d2h_bytes = long(sizeof(Scalar)) * n * (grad_host ? 2 : 1);
+        run_and_record(dev, solver, x, [&](Scalar& fx) { return solver.minimize(f, x, fx, lb, ub); }, [&]() { return f.count; }, false,
+                       x_host, grad_host, trace_cap, long(sizeof(Scalar)) * n * 3, t_begin, out);
     });
 }
 
@@ -595,8 +534,7 @@ extern "C" int lbfgsb200_drv_cauchy_f64(int device_ordinal, long n, int m, int n
                                         double* xcp_host, unsigned char* cls_host, double* vecc_host, long* counts2, double* theta_out,
                                         char* err, int errlen)
 {
-    try
-    {
+    return reported(err, errlen, 1, [&]() {
         Device& dev = device(device_ordinal);
         typedef DeviceVector<double> Vector;
         BFGSMat<double, true> mat;
@@ -622,12 +560,7 @@ extern "C" int lbfgsb200_drv_cauchy_f64(int device_ordinal, long n, int m, int n
         counts2[1] = cp.nfree;
         *theta_out = mat.theta();
         return 0;
-    }
-    catch (const std::exception& e)
-    {
-        if (err && errlen > 0) { std::strncpy(err, e.what(), size_t(errlen) - 1); err[errlen - 1] = 0; }
-        return 1;
-    }
+    });
 }
 
 // ----------------------------------------------------------------------------------------------------------
@@ -650,7 +583,7 @@ typedef struct
 
 namespace {
 
-template <template <class> class LS>
+template <class Solver>
 void batch_worker(int dev_ordinal, bool use_shared_device, int objective, long n, int B, int first, int stride, const double* x0s,
                   const drv_param* q, int hv_algo, drv_batch_item* items, double* xs_out)
 {
@@ -663,7 +596,7 @@ void batch_worker(int dev_ordinal, bool use_shared_device, int objective, long n
         if (use_shared_device) dev = &device(dev_ordinal);
         else { own.reset(new Device(dev_ordinal)); dev = own.get(); }
         const LBFGSParam<double> prm = to_param<double>(q);
-        LBFGSSolver<double, LS> solver(prm);
+        Solver solver(prm);
         solver.set_hv_algorithm(hv_algo);
         BuiltinObjective<double> obj(objective);
         Vector x(*dev);
@@ -704,22 +637,27 @@ extern "C" int lbfgsb200_drv_batch_f64(int device_ordinal, int objective, long n
     if (shared_device) nthreads = 1;
     for (int b = 0; b < B; b++) items[b] = drv_batch_item{4, 0, 0, 0.0, 0.0};
     const double t0 = now();
-    std::vector<std::thread> pool;
-    for (int t = 0; t < nthreads; t++)
+    // the line search is resolved here, before any worker starts: an exception inside a worker thread would terminate the process
+    try
     {
-        auto fn = [=]() {
-            switch (ls)
+        with_line_search(ls, [&](auto tag) {
+            typedef typename decltype(tag)::template Solver<double> Solver;
+            std::vector<std::thread> pool;
+            for (int t = 0; t < nthreads; t++)
             {
-            case DRV_LS_BACKTRACKING: batch_worker<LineSearchBacktracking>(device_ordinal, shared_device != 0, objective, n, B, t, nthreads, x0s_host, prm, hv_algo, items, xs_out_host); break;
-            case DRV_LS_BRACKETING: batch_worker<LineSearchBracketing>(device_ordinal, shared_device != 0, objective, n, B, t, nthreads, x0s_host, prm, hv_algo, items, xs_out_host); break;
-            case DRV_LS_NOCEDAL_WRIGHT: batch_worker<LineSearchNocedalWright>(device_ordinal, shared_device != 0, objective, n, B, t, nthreads, x0s_host, prm, hv_algo, items, xs_out_host); break;
-            default: batch_worker<LineSearchMoreThuente>(device_ordinal, shared_device != 0, objective, n, B, t, nthreads, x0s_host, prm, hv_algo, items, xs_out_host); break;
+                auto fn = [=]() {
+                    batch_worker<Solver>(device_ordinal, shared_device != 0, objective, n, B, t, nthreads, x0s_host, prm, hv_algo, items, xs_out_host);
+                };
+                if (nthreads == 1) fn();
+                else pool.emplace_back(fn);
             }
-        };
-        if (nthreads == 1) fn();
-        else pool.emplace_back(fn);
+            for (auto& th : pool) th.join();
+        });
     }
-    for (auto& th : pool) th.join();
+    catch (const std::invalid_argument&)   // unknown line search id: no problem was started
+    {
+        for (int b = 0; b < B; b++) items[b].status = 1;
+    }
     if (seconds_out) *seconds_out = now() - t0;
     int bad = 0;
     for (int b = 0; b < B; b++) bad += items[b].status != 0;
@@ -731,39 +669,46 @@ extern "C" int lbfgsb200_drv_batch_f64(int device_ordinal, int objective, long n
 // resident, solve() can be repeated (bench.py --config c5), every problem bit-identical to a lone resident solve.
 // ----------------------------------------------------------------------------------------------------------
 namespace {
+
 struct BatchSession
 {
     Device* dev;
     long n;
-    int B, ls;
-    LBFGSParam<double> prm;
+    int B;
     DeviceVector<double> X0, X;
     BuiltinObjective<double> obj;
-    LBFGSBatchSolver<double, LineSearchBacktracking> s_bt;
-    LBFGSBatchSolver<double, LineSearchBracketing> s_br;
-    LBFGSBatchSolver<double, LineSearchNocedalWright> s_nw;
-    LBFGSBatchSolver<double, LineSearchMoreThuente> s_mt;
-    BatchSession(Device& d, long n_, int B_, int ls_, const drv_param* q, int objective) :
-        dev(&d), n(n_), B(B_), ls(ls_), prm(to_param<double>(q)), X0(d), X(d), obj(objective), s_bt(prm), s_br(prm), s_nw(prm), s_mt(prm) {}
+    BatchSession(Device& d, long n_, int B_, int objective) : dev(&d), n(n_), B(B_), X0(d), X(d), obj(objective) {}
+    virtual ~BatchSession() {}
+    virtual std::vector<BatchOutcome<double> > minimize() = 0;
+    virtual const lbfgs_b200_solver* solver_handle() const = 0;
 };
+
+// a batch session's solver, for the one line search it was created with
+template <class Tag>
+struct BatchSessionOf : BatchSession
+{
+    const LBFGSParam<double> prm;   // the solver holds it by reference
+    typename Tag::template BatchSolver<double> solver;
+    BatchSessionOf(Device& d, long n_, int B_, const drv_param* q, int objective) :
+        BatchSession(d, n_, B_, objective), prm(to_param<double>(q)), solver(prm) {}
+    std::vector<BatchOutcome<double> > minimize() override { return solver.minimize(obj, X, B); }
+    const lbfgs_b200_solver* solver_handle() const override { return solver.solver_handle(); }
+};
+
 }  // namespace
 
 extern "C" void* lbfgsb200_drv_batch_session_create(int device_ordinal, int objective, long n, int B, const double* x0s_host, int ls,
                                                     const drv_param* prm, char* err, int errlen)
 {
-    try
-    {
+    return reported<void*>(err, errlen, nullptr, [&]() {
         Device& dev = device(device_ordinal);
-        std::unique_ptr<BatchSession> s(new BatchSession(dev, n, B, ls, prm, objective));
+        std::unique_ptr<BatchSession> s(with_line_search(ls, [&](auto tag) -> BatchSession* {
+            return new BatchSessionOf<decltype(tag)>(dev, n, B, prm, objective);
+        }));
         s->X0.copy_from_host(x0s_host, std::ptrdiff_t(n) * B);
         s->X.resize(std::ptrdiff_t(n) * B);
-        return s.release();
-    }
-    catch (const std::exception& e)
-    {
-        if (err && errlen > 0) { std::strncpy(err, e.what(), size_t(errlen) - 1); err[errlen - 1] = 0; }
-        return nullptr;
-    }
+        return static_cast<void*>(s.release());
+    });
 }
 extern "C" void lbfgsb200_drv_batch_session_destroy(void* handle) { delete static_cast<BatchSession*>(handle); }
 
@@ -779,16 +724,10 @@ extern "C" int lbfgsb200_drv_batch_session_download(void* handle, double* xs_out
 extern "C" int lbfgsb200_drv_batch_session_upload(void* handle, const double* x0s_host, char* err, int errlen)
 {
     BatchSession* s = static_cast<BatchSession*>(handle);
-    try
-    {
+    return reported(err, errlen, -1, [&]() {
         s->X0.copy_from_host(x0s_host, std::ptrdiff_t(s->n) * s->B);
         return 0;
-    }
-    catch (const std::exception& e)
-    {
-        if (err && errlen > 0) { std::strncpy(err, e.what(), size_t(errlen) - 1); err[errlen - 1] = 0; }
-        return -1;
-    }
+    });
 }
 
 // One batched solve from the resident start points.  items[B]; rounds_out[B] (optional); seconds_out: host wall clock around the
@@ -797,20 +736,12 @@ extern "C" int lbfgsb200_drv_batch_session_solve(void* handle, drv_batch_item* i
                                                  char* err, int errlen)
 {
     BatchSession* s = static_cast<BatchSession*>(handle);
-    try
-    {
+    return reported(err, errlen, -1, [&]() {
         Device& dev = *s->dev;
         dev.check(lbfgs_b200_memcpy_d2d(dev.ctx(), s->X.data(), s->X0.data(), sizeof(double) * size_t(s->n) * size_t(s->B)));
         dev.synchronize();
         const double t0 = now();
-        std::vector<BatchOutcome<double> > out;
-        switch (s->ls)
-        {
-        case DRV_LS_BACKTRACKING: out = s->s_bt.minimize(s->obj, s->X, s->B); break;
-        case DRV_LS_BRACKETING: out = s->s_br.minimize(s->obj, s->X, s->B); break;
-        case DRV_LS_NOCEDAL_WRIGHT: out = s->s_nw.minimize(s->obj, s->X, s->B); break;
-        default: out = s->s_mt.minimize(s->obj, s->X, s->B); break;
-        }
+        const std::vector<BatchOutcome<double> > out = s->minimize();
         dev.synchronize();
         if (seconds_out) *seconds_out = now() - t0;
         int bad = 0;
@@ -824,29 +755,14 @@ extern "C" int lbfgsb200_drv_batch_session_solve(void* handle, drv_batch_item* i
         }
         if (xs_out_host) s->X.copy_to_host(xs_out_host);
         return bad;
-    }
-    catch (const std::exception& e)
-    {
-        if (err && errlen > 0) { std::strncpy(err, e.what(), size_t(errlen) - 1); err[errlen - 1] = 0; }
-        return -1;
-    }
+    });
 }
 
 // accounting of the batch session's last solve (the whole batch is one kernel launch: lbfgs_b200_solver_profile)
 extern "C" int lbfgsb200_drv_batch_session_profile(void* handle, double* kernel_ms, double* ms_by_op10, unsigned long long* rounds_by_op10,
                                                    double* alg_bytes_by_op10, double* sync_ms)
 {
-    BatchSession* s = static_cast<BatchSession*>(handle);
-    lbfgs_b200_solver* r = nullptr;
-    switch (s->ls)
-    {
-    case DRV_LS_BACKTRACKING: r = s->s_bt.solver_handle(); break;
-    case DRV_LS_BRACKETING: r = s->s_br.solver_handle(); break;
-    case DRV_LS_NOCEDAL_WRIGHT: r = s->s_nw.solver_handle(); break;
-    default: r = s->s_mt.solver_handle(); break;
-    }
-    if (!r) return 1;
-    return lbfgs_b200_solver_profile(r, kernel_ms, ms_by_op10, rounds_by_op10, alg_bytes_by_op10, sync_ms) == LBFGS_B200_OK ? 0 : 2;
+    return profile_of(static_cast<BatchSession*>(handle)->solver_handle(), kernel_ms, ms_by_op10, rounds_by_op10, alg_bytes_by_op10, sync_ms);
 }
 
 // minimize() followed by final_approx_hessian() / final_approx_inverse_hessian() (reference LBFGS.h:192-197) on a built-in objective;
@@ -854,8 +770,7 @@ extern "C" int lbfgsb200_drv_batch_session_profile(void* handle, double* kernel_
 extern "C" int lbfgsb200_drv_solve_dense_f64(int device_ordinal, int objective, long n, int ls, const drv_param* q, int resident, double* x_host,
                                              double* B_out /* n*n */, double* H_out /* n*n */, int* niter_out, char* err, int errlen)
 {
-    try
-    {
+    return reported(err, errlen, 1, [&]() {
         Device& dev = device(device_ordinal);
         const LBFGSParam<double> prm = to_param<double>(q);
         BuiltinObjective<double> obj(objective);
@@ -864,29 +779,18 @@ extern "C" int lbfgsb200_drv_solve_dense_f64(int device_ordinal, int objective, 
         double fx = 0;
         SmallMatrix<double> Bm, Hm;
         int niter = 0;
-        auto run = [&](auto& solver) {
+        with_line_search(ls, [&](auto tag) {
+            typename decltype(tag)::template Solver<double> solver(prm);
             solver.set_device_resident(resident != 0);
             niter = solver.minimize(obj, x, fx);
             Bm = solver.final_approx_hessian();
             Hm = solver.final_approx_inverse_hessian();
-        };
-        switch (ls)
-        {
-        case DRV_LS_BACKTRACKING: { LBFGSSolver<double, LineSearchBacktracking> s(prm); run(s); break; }
-        case DRV_LS_BRACKETING: { LBFGSSolver<double, LineSearchBracketing> s(prm); run(s); break; }
-        case DRV_LS_NOCEDAL_WRIGHT: { LBFGSSolver<double, LineSearchNocedalWright> s(prm); run(s); break; }
-        default: { LBFGSSolver<double, LineSearchMoreThuente> s(prm); run(s); break; }
-        }
+        });
         x.copy_to_host(x_host);
         for (long i = 0; i < n * n; i++) { B_out[i] = Bm.data()[i]; H_out[i] = Hm.data()[i]; }
         if (niter_out) *niter_out = niter;
         return 0;
-    }
-    catch (const std::exception& e)
-    {
-        if (err && errlen > 0) { std::strncpy(err, e.what(), size_t(errlen) - 1); err[errlen - 1] = 0; }
-        return 1;
-    }
+    });
 }
 
 // PhaseClock (include/LBFGSpp/PhaseClock.h): wall-clock accounting of the host-driven L-BFGS-B loop's phases for bench.py / profiles
@@ -916,8 +820,7 @@ extern "C" int lbfgsb200_drv_phase_report(char* buf, int len)
 extern "C" int lbfgsb200_drv_dense_f64(int device_ordinal, long n, int m, int npairs, const double* S_host, const double* Y_host,
                                        int inverse, double* out_host /* n*n row-major */, char* err, int errlen)
 {
-    try
-    {
+    return reported(err, errlen, 1, [&]() {
         Device& dev = device(device_ordinal);
         BFGSMat<double> mat;
         mat.reset(dev, n, m);
@@ -931,12 +834,7 @@ extern "C" int lbfgsb200_drv_dense_f64(int device_ordinal, long n, int m, int np
         const SmallMatrix<double> D = mat.dense(inverse != 0);
         for (long i = 0; i < n * n; i++) out_host[i] = D.data()[i];
         return 0;
-    }
-    catch (const std::exception& e)
-    {
-        if (err && errlen > 0) { std::strncpy(err, e.what(), size_t(errlen) - 1); err[errlen - 1] = 0; }
-        return 1;
-    }
+    });
 }
 
 #pragma GCC visibility pop

@@ -17,7 +17,6 @@ from util import LS, golden_cases, unhex
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SO = os.path.join(ROOT, "tests", "cpp", "front_on_mock.so")
-STATUS = ["ok", "invalid_argument", "logic_error", "runtime_error", "other"]
 
 
 @pytest.fixture(scope="module")
@@ -26,30 +25,7 @@ def front():
                     "-Wno-unknown-pragmas", "-fvisibility=hidden", "-fvisibility-inlines-hidden", "-Wl,-Bsymbolic", "-o", SO,
                     os.path.join(ROOT, "lbfgspp_b200", "csrc", "driver.cpp"), os.path.join(ROOT, "tests", "cpp", "mock_abi.cpp"),
                     "-pthread"], check=True)
-    lib = C.CDLL(SO)
-    dp, fp = C.POINTER(C.c_double), C.POINTER(C.c_float)
-    lib.lbfgsb200_drv_lbfgs_f64.argtypes = [C.c_int, C.c_int, dp, dp, C.c_long, C.c_int, C.POINTER(lb._DrvParam), C.c_int, C.c_int,
-                                            dp, dp, dp, C.c_long, C.POINTER(lb._DrvResult)]
-    lib.lbfgsb200_drv_lbfgs_f32.argtypes = [C.c_int, C.c_int, fp, fp, C.c_long, C.c_int, C.POINTER(lb._DrvParam), C.c_int, C.c_int,
-                                            fp, fp, dp, C.c_long, C.POINTER(lb._DrvResult)]
-    return lib
-
-
-def run_front(lib, objective, x0, ls, prm, fused=1, dtype=np.float64, data0=None, data1=None, cap=100000):
-    ct = C.c_double if dtype == np.float64 else C.c_float
-    ptr = lambda a, t=ct: a.ctypes.data_as(C.POINTER(t)) if a is not None else None
-    x = np.array(x0, dtype=dtype).copy()
-    grad = np.zeros(x.size, dtype=dtype)
-    trace = np.zeros(cap)
-    d0 = None if data0 is None else np.ascontiguousarray(data0, dtype=dtype)
-    d1 = None if data1 is None else np.ascontiguousarray(data1, dtype=dtype)
-    res = lb._DrvResult()
-    p = prm._c()
-    fn = lib.lbfgsb200_drv_lbfgs_f64 if dtype == np.float64 else lib.lbfgsb200_drv_lbfgs_f32
-    fn(0, objective, ptr(d0), ptr(d1), x.size, ls, C.byref(p), lb.HV_AUTO, fused, ptr(x), ptr(grad), ptr(trace, C.c_double), cap,
-       C.byref(res))
-    return dict(status=STATUS[res.status], msg=res.msg.decode(), niter=res.niter, nfev=res.nfev, fx=res.fx, gnorm=res.gnorm, x=x,
-                grad=grad, trace=trace[:res.trace_len].copy())
+    return C.CDLL(SO)
 
 
 def cpu_param(orc, prm):
@@ -73,7 +49,7 @@ def test_front_reproduces_golden_vectors_bit_for_bit(front, orc, case, fused):
     dtype = np.float64 if case["dtype"] == "f64" else np.float32
     prm = lb.LBFGSParam(**case["param"])
     d0, d1 = (unhex(case["data"][0]), unhex(case["data"][1])) if case["data"] else (None, None)
-    f = run_front(front, case["objective"], unhex(case["x0"]), LS[case["ls"]], prm, fused=fused, dtype=dtype, data0=d0, data1=d1)
+    f = lb.LBFGSSolver(prm, LS[case["ls"]], dtype=dtype, fused=fused, lib=front).minimize(case["objective"], unhex(case["x0"]), data0=d0, data1=d1)
     assert f["status"] == case["status"] and f["msg"].replace("lbfgs_b200: ", "") == case["msg"]
     assert (f["niter"], f["nfev"]) == (case["niter"], case["nfev"])
     assert np.array_equal(f["trace"], unhex(case["trace"]))
@@ -93,15 +69,15 @@ def test_front_equals_checker_on_random_problems(front, orc, ls):
                                 delta=1e-9, linesearch=int(rng.choice([1, 2, 3])) if ls != "NocedalWright" and ls != "MoreThuente" else 3)
             c = orc.lbfgs(po.OBJ_ROSENBROCK_PAIRED, x0, LS[ls], cpu_param(orc, prm))
             for fused in (1, 0):
-                assert_same(run_front(front, lb.OBJ_ROSENBROCK_PAIRED, x0, LS[ls], prm, fused=fused), c, (ls, n, t, fused))
+                assert_same(lb.LBFGSSolver(prm, LS[ls], fused=fused, lib=front).minimize(lb.OBJ_ROSENBROCK_PAIRED, x0), c, (ls, n, t, fused))
     n = 3000
     d, b, _ = po.quad_tridiag_data(n)
     prm = lb.LBFGSParam(m=20)
     c = orc.lbfgs(po.OBJ_QUAD_TRIDIAG, np.zeros(n), LS[ls], cpu_param(orc, prm), data0=d, data1=b)
-    assert_same(run_front(front, lb.OBJ_QUAD_TRIDIAG, np.zeros(n), LS[ls], prm, data0=d, data1=b), c, (ls, "tridiag"))
+    assert_same(lb.LBFGSSolver(prm, LS[ls], lib=front).minimize(lb.OBJ_QUAD_TRIDIAG, np.zeros(n), data0=d, data1=b), c, (ls, "tridiag"))
     x0 = np.full(300, 1.3)
     c = orc.lbfgs(po.OBJ_ROSENBROCK_CHAINED, x0, LS[ls], cpu_param(orc, lb.LBFGSParam()))
-    assert_same(run_front(front, lb.OBJ_ROSENBROCK_CHAINED, x0, LS[ls], lb.LBFGSParam()), c, (ls, "chained"))
+    assert_same(lb.LBFGSSolver(lb.LBFGSParam(), LS[ls], lib=front).minimize(lb.OBJ_ROSENBROCK_CHAINED, x0), c, (ls, "chained"))
 
 
 def test_front_error_paths_equal_the_checker(front, orc):
@@ -115,14 +91,70 @@ def test_front_error_paths_equal_the_checker(front, orc):
     for prm, ls, x0 in cases:
         c = orc.lbfgs(po.OBJ_ROSENBROCK_PAIRED, x0, LS[ls], cpu_param(orc, prm))
         for fused in (1, 0):
-            assert_same(run_front(front, lb.OBJ_ROSENBROCK_PAIRED, x0, LS[ls], prm, fused=fused), c, (ls, fused, c["status"], c["msg"]))
+            assert_same(lb.LBFGSSolver(prm, LS[ls], fused=fused, lib=front).minimize(lb.OBJ_ROSENBROCK_PAIRED, x0), c, (ls, fused, c["status"], c["msg"]))
 
 
 def test_front_float32_equals_checker(front, orc):
     for ls in ("Backtracking", "Bracketing", "NocedalWright", "MoreThuente"):
         prm = lb.LBFGSParam()
         c = orc.lbfgs(po.OBJ_ROSENBROCK_PAIRED, np.zeros(10), LS[ls], cpu_param(orc, prm), dtype=np.float32)
-        assert_same(run_front(front, lb.OBJ_ROSENBROCK_PAIRED, np.zeros(10), LS[ls], prm, dtype=np.float32), c, ls)
+        assert_same(lb.LBFGSSolver(prm, LS[ls], dtype=np.float32, lib=front).minimize(lb.OBJ_ROSENBROCK_PAIRED, np.zeros(10)), c, ls)
+
+
+@pytest.mark.parametrize("ls", ["Backtracking", "Bracketing", "NocedalWright", "MoreThuente"])
+def test_session_solve_equals_one_shot_minimize(front, ls):
+    """A host-driven Session keeps one solver for its line search across solves: every solve, from the resident start point or from
+    the host, reproduces a one-shot minimize() bit for bit."""
+    n = 300
+    d, b, _ = po.quad_tridiag_data(n)
+    for objective, x0, data in ((lb.OBJ_ROSENBROCK_PAIRED, np.zeros(n), {}), (lb.OBJ_QUAD_TRIDIAG, np.zeros(n), dict(data0=d, data1=b))):
+        prm = lb.LBFGSParam(m=8)
+        c = lb.LBFGSSolver(prm, ls, fused=True, lib=front).minimize(objective, x0, **data)
+        assert c["status"] == "ok", c["msg"]
+        s = lb.Session(objective, x0, prm, ls, resident=False, lib=front, **data)
+        try:
+            for from_host in (False, True):
+                r = s.solve(from_host=from_host, to_host=from_host)
+                assert (r["niter"], r["nfev"], r["fx"], r["gnorm"]) == (c["niter"], c["nfev"], c["fx"], c["gnorm"]), (ls, objective, from_host)
+                assert np.array_equal(s.solution(), c["x"])
+                if from_host:
+                    assert np.array_equal(s.result(), c["x"])
+            assert s.profile() is None   # the host-driven loop has no device-resident accounting
+        finally:
+            s.close()
+
+
+def test_thread_batch_equals_lone_solves(front):
+    """The thread-pool batch (host-driven loop: the two-loop recursion keeps built-in objectives off the device-resident solve) gives
+    every problem exactly its lone solve, whichever worker thread ran it."""
+    rng = np.random.default_rng(3)
+    X0 = rng.uniform(-1, 1, (5, 40))
+    prm = lb.LBFGSParam(m=5)
+    for ls in ("Bracketing", "MoreThuente"):
+        res, X, _ = lb.solve_batch(lb.OBJ_ROSENBROCK_PAIRED, X0, prm, ls, hv_algo=lb.HV_TWO_LOOP, threads=2, lib=front)
+        for b in range(len(X0)):
+            c = lb.LBFGSSolver(prm, ls, hv_algo=lb.HV_TWO_LOOP, lib=front).minimize(lb.OBJ_ROSENBROCK_PAIRED, X0[b])
+            assert res[b] == {k: c[k] for k in ("status", "niter", "nfev", "fx", "gnorm")}, (ls, b)
+            assert np.array_equal(X[b], c["x"]), (ls, b)
+
+
+@pytest.mark.parametrize("bad", [4, -1])
+def test_every_entry_point_rejects_an_unknown_line_search(front, bad):
+    """No entry point that takes a line-search id falls back to a default search on an id it does not know."""
+    x0, prm = np.zeros(8), lb.LBFGSParam()
+    f = lb.LBFGSSolver(prm, bad, lib=front).minimize(lb.OBJ_ROSENBROCK_PAIRED, x0)
+    assert (f["status"], f["msg"]) == ("invalid_argument", "unknown line search id")
+    with pytest.raises(RuntimeError, match="^session_create failed: unknown line search id$"):
+        lb.Session(lb.OBJ_ROSENBROCK_PAIRED, x0, prm, bad, resident=False, lib=front)
+    with pytest.raises(RuntimeError, match="^batch_session_create failed: unknown line search id$"):
+        lb.BatchSession(lb.OBJ_ROSENBROCK_PAIRED, np.zeros((2, 8)), prm, bad, lib=front)
+    with pytest.raises(RuntimeError, match="^solve_dense failed: unknown line search id$"):
+        lb.solve_dense(lb.OBJ_ROSENBROCK_PAIRED, x0, prm, bad, resident=False, lib=front)
+    # the thread-pool batch on the host-driven loop (the test double has no device-resident solve): the same call solves every problem
+    # with a known id, so "invalid_argument" can only come from the id
+    for ls, status in (("MoreThuente", "ok"), (bad, "invalid_argument")):
+        res, _, _ = lb.solve_batch(lb.OBJ_ROSENBROCK_PAIRED, np.zeros((5, 8)), prm, ls, hv_algo=lb.HV_TWO_LOOP, threads=2, lib=front)
+        assert [r["status"] for r in res] == [status] * 5, ls
 
 
 # ---- the reference's example programs (examples/*.cpp) against the test double: host-functor compatibility mode, dense B / H ----
@@ -152,25 +184,6 @@ def test_examples_run_on_the_test_double(example_bins):
 
 
 # ---- the bound-constrained front (include/LBFGSB.h, LBFGSpp/{Cauchy,SubspaceMin,BFGSMat,BKLDLT}.h) on the test double -------------
-def run_front_box(lib, objective, x0, lbv, ubv, prm, data0=None, data1=None, cap=100000):
-    dp = C.POINTER(C.c_double)
-    lib.lbfgsb200_drv_lbfgsb_f64.argtypes = [C.c_int, C.c_int, dp, dp, C.c_long, C.POINTER(lb._DrvParam), dp, dp, dp, dp, dp, C.c_long,
-                                             C.POINTER(lb._DrvResult)]
-    ptr = lambda a: a.ctypes.data_as(dp) if a is not None else None
-    x = np.array(x0, dtype=np.float64).copy()
-    n = x.size
-    lbv = np.ascontiguousarray(np.broadcast_to(lbv, n), dtype=np.float64)
-    ubv = np.ascontiguousarray(np.broadcast_to(ubv, n), dtype=np.float64)
-    grad, trace, res = np.zeros(n), np.zeros(cap), lb._DrvResult()
-    d0 = None if data0 is None else np.ascontiguousarray(data0, dtype=np.float64)
-    d1 = None if data1 is None else np.ascontiguousarray(data1, dtype=np.float64)
-    p = prm._c()
-    lib.lbfgsb200_drv_lbfgsb_f64(0, objective, ptr(d0), ptr(d1), n, C.byref(p), ptr(x), ptr(lbv), ptr(ubv), ptr(grad), ptr(trace), cap,
-                                 C.byref(res))
-    return dict(status=STATUS[res.status], msg=res.msg.decode(), niter=res.niter, nfev=res.nfev, fx=res.fx, gnorm=res.gnorm, x=x,
-                grad=grad, trace=trace[:res.trace_len].copy())
-
-
 def check_box(f, c, lbv, ubv, iter_slack=0):
     """The product's Cauchy sweep (prefix sums over sorted breakpoints) and BOXCQP algebra re-associate sums, so this is parity
     to rounding, not bit for bit: same iterations, evaluations within one, fx to 1e-9, x to 1e-6 (the bar of the GPU tests)."""
@@ -193,7 +206,7 @@ def check_box(f, c, lbv, ubv, iter_slack=0):
 def test_box_front_on_golden_vectors(front, case):
     prm = lb.LBFGSBParam(**case["param"])
     lbv, ubv = unhex(case["lb"]), unhex(case["ub"])
-    f = run_front_box(front, case["objective"], unhex(case["x0"]), lbv, ubv, prm)
+    f = lb.LBFGSBSolver(prm).minimize(case["objective"], unhex(case["x0"]), lbv, ubv, lib=front)
     c = dict(status=case["status"], msg=case["msg"], niter=case["niter"], nfev=case["nfev"], fx=float.fromhex(case["fx"]), x=unhex(case["x"]))
     check_box(f, c, lbv, ubv, iter_slack=0 if case["niter"] < 20 else 2)
 
@@ -217,13 +230,13 @@ def test_box_front_equals_checker_on_random_boxes(front, orc):
                 d0, d1 = po.quad_tridiag_data(n, seed=trial)[:2] if obj == po.OBJ_QUAD_TRIDIAG else (None, None)
                 kw = dict(m=int(rng.choice([1, 3, 6, 10])), max_iterations=12, max_submin=int(rng.choice([0, 1, 10])))
                 c = orc.lbfgsb(obj, x0, lo, hi, orc.default_param(lbfgsb=True, **kw), data0=d0, data1=d1)
-                f = run_front_box(front, obj, x0, lo, hi, lb.LBFGSBParam(**kw), data0=d0, data1=d1)
+                f = lb.LBFGSBSolver(lb.LBFGSBParam(**kw)).minimize(obj, x0, lo, hi, data0=d0, data1=d1, lib=front)
                 # short runs (<= 12 iterations) keep the comparison in the regime where rounding has not yet moved the path
                 check_box(f, c, lo, hi)
 
 
 def test_box_front_parameter_and_size_errors(front, orc):
-    f = run_front_box(front, po.OBJ_QUAD_SHIFT, np.zeros(4), 0.0, 1.0, lb.LBFGSBParam(m=0))
+    f = lb.LBFGSBSolver(lb.LBFGSBParam(m=0)).minimize(po.OBJ_QUAD_SHIFT, np.zeros(4), 0.0, 1.0, lib=front)
     c = orc.lbfgsb(po.OBJ_QUAD_SHIFT, np.zeros(4), 0.0, 1.0, orc.default_param(lbfgsb=True, m=0))
     assert f["status"] == c["status"] == "invalid_argument" and f["msg"].replace("lbfgs_b200: ", "") == c["msg"]
 

@@ -210,7 +210,6 @@ def test_dense_hessian_approximations(n, m, npairs):
         B = B - np.outer(Bs, Bs) / (s @ Bs) + np.outer(y, y) / (y @ s)
     drv = lb.driver()
     dp = C.POINTER(C.c_double)
-    drv.lbfgsb200_drv_dense_f64.argtypes = [C.c_int, C.c_long, C.c_int, C.c_int, dp, dp, C.c_int, dp, C.c_char_p, C.c_int]
     err = C.create_string_buffer(256)
     for inverse, ref in ((0, B), (1, np.linalg.inv(B))):
         out = np.zeros((n, n))

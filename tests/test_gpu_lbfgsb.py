@@ -158,8 +158,6 @@ def test_cauchy_point_against_sequential_sweep(n, m, npairs, seed):
     theta = C.c_double(0)
     err = C.create_string_buffer(256)
     Sc, Yc = np.ascontiguousarray(S), np.ascontiguousarray(Y)
-    drv.lbfgsb200_drv_cauchy_f64.argtypes = [C.c_int, C.c_long, C.c_int, C.c_int, dp, dp, dp, dp, dp, dp, dp, C.POINTER(C.c_ubyte),
-                                             dp, C.POINTER(C.c_long), dp, C.c_char_p, C.c_int]
     st = drv.lbfgsb200_drv_cauchy_f64(0, n, m, npairs, P(Sc) if npairs else None, P(Yc) if npairs else None, P(x0), P(g), P(lbv),
                                       P(ubv), P(xcp), cls.ctypes.data_as(C.POINTER(C.c_ubyte)), P(vecc), counts, C.byref(theta),
                                       err, 256)
