@@ -188,6 +188,7 @@ __device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long
     asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
     return v;
 }
+template <class V> __device__ __forceinline__ V ldv(const V* p) { return *reinterpret_cast<const volatile V*>(p); }
 __device__ __forceinline__ double ld_volatile_f64(const double* p)
 {
     double v;

@@ -15,6 +15,7 @@
 #include <map>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 
@@ -211,4 +212,39 @@ struct lbfgs_b200_hist
     template <class T> T* s_col(int phys) const { return static_cast<T*>(S) + (int64_t)phys * ld; }
     template <class T> T* y_col(int phys) const { return static_cast<T*>(Y) + (int64_t)phys * ld; }
 };
+
+// ---- the built-in objectives (objectives.cuh): the id -> type dispatch, and the argument checks both solver loops run before
+// they launch anything
+// with_objective<T>(ctx, id, f) calls f(OBJ{}) for the functor type of objective `id`.
+template <class T, class F> lbfgs_b200_status with_objective(lbfgs_b200_ctx* ctx, int id, F f)
+{
+    switch (id)
+    {
+    case LBFGS_B200_OBJ_ROSENBROCK_PAIRED: return f(lb::RosenbrockPaired<T>{});
+    case LBFGS_B200_OBJ_QUAD_SHIFT: return f(lb::QuadShift<T>{});
+    case LBFGS_B200_OBJ_ROSENBROCK_CHAINED: return f(lb::RosenbrockChained<T>{});
+    case LBFGS_B200_OBJ_QUAD_TRIDIAG: return f(lb::QuadTridiag<T>{});
+    }
+    return fail(ctx, LBFGS_B200_ERR_INVALID, "unknown objective id %d", id);
+}
+
+// The geometry of this rank's block of objective OBJ (halo left for the caller).  A neighbour-coupled objective on a single GPU
+// sees the whole vector: offset 0 and n_glob = n, whatever index offset the context holds.
+template <class OBJ, class T>
+lbfgs_b200_status objective_geometry(lbfgs_b200_ctx* ctx, int64_t n, const T* data0, const T* data1, lb::ObjGeom<T>& geo)
+{
+    const bool sharded = OBJ::kHalo && ctx->nranks > 1;
+    geo = lb::ObjGeom<T>{n, (OBJ::kHalo && !sharded) ? 0 : ctx->index_offset, sharded ? ctx->n_global : n, nullptr, data0, data1};
+    if constexpr (std::is_same_v<OBJ, lb::RosenbrockPaired<T>>) REQUIRE(ctx, n % 2 == 0, "paired Rosenbrock needs an even n (got %lld)", (long long)n);
+    if constexpr (OBJ::kDataVectors == 2) REQUIRE(ctx, data0 && data1, "quad_tridiag needs data0 = diag, data1 = rhs");
+    if (sharded)
+    {
+        REQUIRE(ctx, ctx->n_global > 0, "a neighbour-coupled objective under n-sharding needs lbfgs_b200_set_global_extent()");
+        REQUIRE(ctx, ctx->index_offset + n <= ctx->n_global, "the local block [%lld, %lld) exceeds the global extent %lld",
+                (long long)ctx->index_offset, (long long)(ctx->index_offset + n), (long long)ctx->n_global);
+        REQUIRE(ctx, ctx->rank == ctx->nranks - 1 || n % 4 == 0, "every block but the last must hold a multiple of 4 coordinates (got %lld)", (long long)n);
+    }
+    if constexpr (std::is_same_v<OBJ, lb::RosenbrockChained<T>>) REQUIRE(ctx, geo.n_glob >= 2, "chained Rosenbrock needs n >= 2 (got %lld)", (long long)geo.n_glob);
+    return LBFGS_B200_OK;
+}
 

@@ -9,7 +9,8 @@
 //   k_axpy_out, k_scale_out                                                      [R 2 W 1 / R 1 W 1]
 //   k_update          s = x-xp, y = g-gp -> ring slot ; {s.y, y.y}               [R 4 + W 2]
 //   k_hv_stage<KIND>  one fused AXPY+dot stage of the two-loop recursion         [R 3 + W 1]
-//   (k_gram_dots, k_gram_fold, k_gram_combine live in two_loop_gram.cuh; the device-resident solve in persist.cuh)
+//   (k_gram_dots, k_gram_fold, k_gram_combine live in two_loop_gram.cuh; the device-resident solve in persist.cuh; the built-in
+//   objectives and the steps k_trial shares with the resident solve in objectives.cuh, their id dispatch and checks in internal.cuh)
 #include "internal.cuh"
 #include "two_loop_gram.cuh"
 #include "../../include/LBFGSpp/LoopRules.h"
@@ -231,35 +232,16 @@ __global__ void __launch_bounds__(kThreads) k_trial(OBJ obj, int64_t n, const T*
             const Pack<T> px = load4<T, Hint::Stream, VEC>(xp, i0, cnt), pd = load4<T, Hint::Stream, VEC>(d, i0, cnt);
 #pragma unroll
             for (int k = 0; k < 4; k++) { dv[k] = pd.v[k]; xv[k] = px.v[k] + step * pd.v[k]; }
-            if constexpr (OBJ::kHalo)
-            {
-                if (i0 > 0) xl = xp[i0 - 1] + step * d[i0 - 1];
-                else if (obj.halo && obj.gofs > 0) xl = T(obj.halo[kHaloLeftA]) + step * T(obj.halo[kHaloLeftB]);
-                if (i0 + 4 < n) xr = xp[i0 + 4] + step * d[i0 + 4];
-                else if (obj.halo && i0 + 4 == n && obj.gofs + n < obj.n_glob) xr = T(obj.halo[kHaloRightA]) + step * T(obj.halo[kHaloRightB]);
-            }
+            if constexpr (OBJ::kHalo) pack_neighbours<true>(obj, i0, n, step, [&](int j) { return xp[i0 + j] + step * d[i0 + j]; }, xl, xr);
         }
         else
         {
             const Pack<T> px = load4<T, Hint::Stream, VEC>(x, i0, cnt);
 #pragma unroll
             for (int k = 0; k < 4; k++) xv[k] = px.v[k];
-            if constexpr (OBJ::kHalo)
-            {
-                if (i0 > 0) xl = x[i0 - 1];
-                else if (obj.halo && obj.gofs > 0) xl = T(obj.halo[kHaloLeftA]);
-                if (i0 + 4 < n) xr = x[i0 + 4];
-                else if (obj.halo && i0 + 4 == n && obj.gofs + n < obj.n_glob) xr = T(obj.halo[kHaloRightA]);
-            }
+            if constexpr (OBJ::kHalo) pack_neighbours<false>(obj, i0, n, step, [&](int j) { return x[i0 + j]; }, xl, xr);
         }
-        acc[0] += obj.eval(i0, cnt, xv, xl, xr, gv);
-#pragma unroll
-        for (int k = 0; k < 4; k++)
-        {
-            acc[1] += gv[k] * dv[k];
-            acc[2] += gv[k] * gv[k];
-            acc[3] += (k < cnt) ? xv[k] * xv[k] : T(0);
-        }
+        eval_pack(obj, i0, cnt, xv, xl, xr, dv, gv, acc);
         Pack<T> pg, pxo;
 #pragma unroll
         for (int k = 0; k < 4; k++) { pg.v[k] = gv[k]; pxo.v[k] = xv[k]; }
@@ -788,10 +770,6 @@ static lbfgs_b200_status do_scale_out(lbfgs_b200_ctx* ctx, int64_t n, T s, const
 template <class T>
 static lbfgs_b200_status exchange_halo(lbfgs_b200_ctx* ctx, int64_t n, const T* a, const T* b)
 {
-    REQUIRE(ctx, ctx->n_global > 0, "a neighbour-coupled objective under n-sharding needs lbfgs_b200_set_global_extent()");
-    REQUIRE(ctx, n >= 1 && ctx->index_offset + n <= ctx->n_global, "halo exchange: local block [%lld, %lld) exceeds the global extent %lld",
-            (long long)ctx->index_offset, (long long)(ctx->index_offset + n), (long long)ctx->n_global);
-    REQUIRE(ctx, ctx->rank == ctx->nranks - 1 || n % 4 == 0, "halo exchange: every block but the last must hold a multiple of 4 coordinates (got %lld)", (long long)n);
     if (ctx->x_active)
     {
         k_halo_exchange<T><<<1, 32, 0, ctx->stream>>>(n, a, b, ctx->d_halo, ctx->x_comm, ++ctx->x_epoch);
@@ -833,57 +811,24 @@ static lbfgs_b200_status do_trial(lbfgs_b200_ctx* ctx, int objective, const T* d
 {
     REQUIRE(ctx, ctx && x && g && out_host && n >= 1, "trial/objective: bad arguments");
     if (TRIAL) REQUIRE(ctx, xp && d, "trial: xp/d are NULL");
-    const bool coupled = objective == LBFGS_B200_OBJ_ROSENBROCK_CHAINED || objective == LBFGS_B200_OBJ_QUAD_TRIDIAG;
-    const double* halo = nullptr;
-    int64_t gofs = 0, n_glob = n;
-    if (coupled && ctx->nranks > 1)
-    {
-        if (auto sh = exchange_halo<T>(ctx, n, TRIAL ? xp : x, TRIAL ? d : nullptr)) return sh;
-        halo = ctx->d_halo;
-        gofs = ctx->index_offset;
-        n_glob = ctx->n_global;
-    }
-    const bool vec = all_aligned<T>({xp, d, x, g});
-    lbfgs_b200_status st = LBFGS_B200_OK;
-    ProfSpan span(ctx, PH_TRIAL, double(sizeof(T)) * double(n) * ((TRIAL ? 4.0 : 2.0) + (objective == LBFGS_B200_OBJ_QUAD_TRIDIAG ? 2.0 : 0.0)));
-    switch (objective)
-    {
-    case LBFGS_B200_OBJ_ROSENBROCK_PAIRED:
-    {
-        REQUIRE(ctx, n % 2 == 0, "paired Rosenbrock needs an even n (got %lld)", (long long)n);
-        RosenbrockPaired<T> o{n};
-        st = launch_trial<T, RosenbrockPaired<T>, TRIAL>(ctx, o, n, xp, d, step, x, g, vec);
-        break;
-    }
-    case LBFGS_B200_OBJ_QUAD_SHIFT:
-    {
-        QuadShift<T> o{n, ctx->index_offset};
-        st = launch_trial<T, QuadShift<T>, TRIAL>(ctx, o, n, xp, d, step, x, g, vec);
-        break;
-    }
-    case LBFGS_B200_OBJ_ROSENBROCK_CHAINED:
-    {
-        REQUIRE(ctx, n_glob >= 2, "chained Rosenbrock needs n >= 2");
-        RosenbrockChained<T> o{n, gofs, n_glob, halo};
-        st = launch_trial<T, RosenbrockChained<T>, TRIAL>(ctx, o, n, xp, d, step, x, g, vec);
-        break;
-    }
-    case LBFGS_B200_OBJ_QUAD_TRIDIAG:
-    {
-        REQUIRE(ctx, data0 && data1, "quad_tridiag needs data0 = diag, data1 = rhs");
-        QuadTridiag<T> o{n, data0, data1, gofs, n_glob, halo};
-        st = launch_trial<T, QuadTridiag<T>, TRIAL>(ctx, o, n, xp, d, step, x, g, vec);
-        break;
-    }
-    default: return fail(ctx, LBFGS_B200_ERR_INVALID, "unknown objective id %d", objective);
-    }
-    if (st) return st;
-    if (auto s2 = allreduce_result(ctx, 4)) return s2;
-    span.stop();
-    if (auto s2 = receive(ctx, 4)) return s2;
-    for (int k = 0; k < 4; k++) out_host[k] = (T)ctx->h_result[k];
-    if (!TRIAL) out_host[1] = T(0);
-    return LBFGS_B200_OK;
+    return with_objective<T>(ctx, objective, [&](auto tag) -> lbfgs_b200_status {
+        using OBJ = decltype(tag);
+        ObjGeom<T> geo;
+        if (auto st = objective_geometry<OBJ>(ctx, n, data0, data1, geo)) return st;
+        if (OBJ::kHalo && ctx->nranks > 1)
+        {
+            if (auto st = exchange_halo<T>(ctx, n, TRIAL ? xp : x, TRIAL ? d : nullptr)) return st;
+            geo.halo = ctx->d_halo;
+        }
+        ProfSpan span(ctx, PH_TRIAL, double(sizeof(T)) * double(n) * ((TRIAL ? 4.0 : 2.0) + OBJ::kDataVectors));
+        if (auto st = launch_trial<T, OBJ, TRIAL>(ctx, OBJ{geo}, n, xp, d, step, x, g, all_aligned<T>({xp, d, x, g}))) return st;
+        if (auto st = allreduce_result(ctx, 4)) return st;
+        span.stop();
+        if (auto st = receive(ctx, 4)) return st;
+        for (int k = 0; k < 4; k++) out_host[k] = (T)ctx->h_result[k];
+        if (!TRIAL) out_host[1] = T(0);
+        return LBFGS_B200_OK;
+    });
 }
 
 // ----------------------------------------------------------------------------- history

@@ -1,11 +1,15 @@
-// objectives.cuh -- device versions of the benchmark objective functions (SURVEY.md 8a row A12).
+// objectives.cuh -- the built-in objective functions (SURVEY.md 8a row A12) as both solver loops use them: the functors, the record
+// they are built from and the device steps that evaluate one pack.  Their id -> type dispatch and argument checks are the host side
+// (with_objective, objective_geometry in internal.cuh).
 //
-// Each functor evaluates 4 consecutive coordinates at once ("pack") so that it can sit inside the fused
-// line-search trial kernel between the wide loads of xp/d and the wide stores of x/g.
-//   eval(i0, cnt, x[4], xl, xr, g[4]) -> this pack's contribution to f
+// Each functor evaluates 4 consecutive coordinates at once ("pack") so that it can sit inside the fused line-search trial pass
+// between the wide loads of xp/d and the wide stores of x/g.
+//   eval(i0, cnt, x[4], xl, xr, g[4]) -> this pack's contribution to f; g = 0 in the lanes past cnt (RosenbrockPaired works on
+//   pairs of lanes, so this holds for it because its n is even, which makes cnt even)
 //     i0   local index of x[0];  cnt valid lanes (ragged tail);  xl = x_{i0-1}, xr = x_{i0+4} (0 outside the GLOBAL vector)
-// n-sharding: a functor whose coordinates couple to their neighbours (kHalo) also carries the global position of its block
-// (gofs, n_glob) and a pointer to the halo record that the exchange kernel fills before every evaluation:
+// Every functor is an ObjGeom: the host-driven loop (k_trial) and the device-resident solve (k_persist) build it from the same record.
+// n-sharding: a functor whose coordinates couple to their neighbours (kHalo) reads the global position of its block (gofs, n_glob)
+// and, at the two ends of the block, the halo record that the exchange fills before every evaluation (pack_neighbours):
 //     halo[kHaloLeftA] + step*halo[kHaloLeftB]   = the left neighbour's last  coordinate of the trial point
 //     halo[kHaloRightA] + step*halo[kHaloRightB] = the right neighbour's first coordinate
 // (halo == nullptr on a single GPU).
@@ -17,6 +21,8 @@
 #pragma once
 #include <stdint.h>
 
+#include "device_utils.cuh"
+
 namespace lb {
 
 // layout of the 12-double halo record: [0..3] own {a_first, b_first, a_last, b_last}, [4..7] the left neighbour's four,
@@ -24,11 +30,19 @@ namespace lb {
 constexpr int kHaloDoubles = 12;
 constexpr int kHaloLeftA = 6, kHaloLeftB = 7, kHaloRightA = 8, kHaloRightB = 9;
 
-template <class T> struct RosenbrockPaired
+// where this rank's block of the objective lies, and its data
+template <class T> struct ObjGeom
+{
+    int64_t n;               // local length
+    int64_t gofs, n_glob;    // global index of local element 0, global length
+    const double* halo;      // the halo record (neighbour-coupled objectives under n-sharding), else nullptr
+    const T *data0, *data1;  // per-coordinate data vectors of this block (kDataVectors of them)
+};
+
+template <class T> struct RosenbrockPaired : ObjGeom<T>
 {
     static constexpr bool kHalo = false;
     static constexpr int kDataVectors = 0;   // per-coordinate data vectors read by every evaluation
-    int64_t n;
     __device__ __forceinline__ T eval(int64_t, int cnt, const T (&x)[4], T, T, T (&g)[4]) const
     {
         T f = T(0);
@@ -50,19 +64,17 @@ template <class T> struct RosenbrockPaired
     }
 };
 
-template <class T> struct QuadShift
+template <class T> struct QuadShift : ObjGeom<T>
 {
     static constexpr bool kHalo = false;
     static constexpr int kDataVectors = 0;
-    int64_t n;
-    int64_t index_offset;  // global index of local element 0 (n-sharding)
     __device__ __forceinline__ T eval(int64_t i0, int cnt, const T (&x)[4], T, T, T (&g)[4]) const
     {
         T f = T(0);
 #pragma unroll
         for (int k = 0; k < 4; k++)
         {
-            const T r = x[k] - T(i0 + index_offset + k);
+            const T r = x[k] - T(i0 + this->gofs + k);
             g[k] = (k < cnt) ? T(2) * r : T(0);
             f += (k < cnt) ? r * r : T(0);
         }
@@ -70,21 +82,18 @@ template <class T> struct QuadShift
     }
 };
 
-template <class T> struct RosenbrockChained
+template <class T> struct RosenbrockChained : ObjGeom<T>
 {
     static constexpr bool kHalo = true;
     static constexpr int kDataVectors = 0;
     __device__ __forceinline__ RosenbrockChained staged(const T*, const T*, int64_t) const { return *this; }
-    int64_t n;             // local length
-    int64_t gofs, n_glob;  // global index of local element 0, global length (gofs = 0, n_glob = n unsharded)
-    const double* halo;
     __device__ __forceinline__ T eval(int64_t i0, int cnt, const T (&x)[4], T xl, T xr, T (&g)[4]) const
     {
         T f = T(0);
 #pragma unroll
         for (int k = 0; k < 4; k++)
         {
-            const int64_t i = gofs + i0 + k;
+            const int64_t i = this->gofs + i0 + k;
             const T xm = (k == 0) ? xl : x[k > 0 ? k - 1 : 0];
             const T xn = (k == 3) ? xr : x[k < 3 ? k + 1 : 3];
             T gi, fi;
@@ -97,7 +106,7 @@ template <class T> struct RosenbrockChained
             {
                 const T u = x[k] - xm * xm;
                 fi = T(4) * u * u;
-                gi = (i == n_glob - 1) ? T(8) * u : T(8) * u + T(16) * (x[k] * x[k] - xn) * x[k];
+                gi = (i == this->n_glob - 1) ? T(8) * u : T(8) * u + T(16) * (x[k] * x[k] - xn) * x[k];
             }
             g[k] = (k < cnt) ? gi : T(0);
             f += (k < cnt) ? fi : T(0);
@@ -106,21 +115,17 @@ template <class T> struct RosenbrockChained
     }
 };
 
-template <class T> struct QuadTridiag
+// data0 = d, data1 = b
+template <class T> struct QuadTridiag : ObjGeom<T>
 {
     static constexpr bool kHalo = true;
     static constexpr int kDataVectors = 2;
-    int64_t n;
-    const T* diag;  // d (this rank's block)
-    const T* rhs;   // b
-    int64_t gofs, n_glob;
-    const double* halo;
     // the same objective reading its two data vectors from a staged tile: `d_tile[0]` / `b_tile[0]` hold element `e0`
     __device__ __forceinline__ QuadTridiag staged(const T* d_tile, const T* b_tile, int64_t e0) const
     {
         QuadTridiag o = *this;
-        o.diag = d_tile - e0;
-        o.rhs = b_tile - e0;
+        o.data0 = d_tile - e0;
+        o.data1 = b_tile - e0;
         return o;
     }
     __device__ __forceinline__ T eval(int64_t i0, int cnt, const T (&x)[4], T xl, T xr, T (&g)[4]) const
@@ -133,7 +138,7 @@ template <class T> struct QuadTridiag
             {
                 const T xm = (k == 0) ? xl : x[k > 0 ? k - 1 : 0];
                 const T xn = (k == 3) ? xr : x[k < 3 ? k + 1 : 3];
-                const T dk = diag[i0 + k], bk = rhs[i0 + k];
+                const T dk = this->data0[i0 + k], bk = this->data1[i0 + k];
                 const T ax = (dk + T(1)) * x[k] - T(0.5) * (xm + xn);
                 g[k] = ax - bk;
                 f += x[k] * (T(0.5) * ax - bk);
@@ -144,5 +149,41 @@ template <class T> struct QuadTridiag
         return f;
     }
 };
+
+// ---- device: the steps every pass that evaluates an objective shares ----------------------------------------------------------
+// xl = x_{i0-1}, xr = x_{i0+4} of the pack at local index i0 of a block of n: inside the block `at(j)` gives
+// x_{i0+j}; at a rank boundary the halo record gives the neighbour's coordinate (TRIAL: a + step*b, else a); beyond the ends of the
+// global vector 0.  The record is read with volatile loads: the resident solve's leader rewrites it between rounds.
+template <bool TRIAL, class T, class OBJ, class At>
+__device__ __forceinline__ void pack_neighbours(const OBJ& obj, int64_t i0, int64_t n, T step, At at, T& xl, T& xr)
+{
+    auto from_halo = [&](int a, int b) {
+        T v = T(ldv(obj.halo + a));
+        if (TRIAL) v = v + step * T(ldv(obj.halo + b));
+        return v;
+    };
+    xl = xr = T(0);
+    if (i0 > 0) xl = at(-1);
+    else if (obj.halo && obj.gofs > 0) xl = from_halo(kHaloLeftA, kHaloLeftB);
+    if (i0 + 4 < n) xr = at(4);
+    else if (obj.halo && i0 + 4 == n && obj.gofs + n < obj.n_glob) xr = from_halo(kHaloRightA, kHaloRightB);
+}
+
+// one pack at x with direction d (L = 4, or the lanes of a 16-byte unit): g of the pack into g, and its {f, g.d, g.g, x.x} over the
+// cnt valid lanes added to acc[0..3].  The lanes past cnt add nothing: g is 0 there (eval), the caller passes d = 0 there, and x.x
+// is masked.
+template <class T, class OBJ, int L>
+__device__ __forceinline__ void eval_pack(const OBJ& obj, int64_t i0, int cnt, const T (&x)[4], T xl, T xr, const T (&d)[L], T (&g)[4], T* acc)
+{
+    static_assert(L <= 4, "a pack has 4 lanes");
+    acc[0] += obj.eval(i0, cnt, x, xl, xr, g);
+#pragma unroll
+    for (int k = 0; k < L; k++)
+    {
+        acc[1] += g[k] * d[k];
+        acc[2] += g[k] * g[k];
+        acc[3] += (k < cnt) ? x[k] * x[k] : T(0);
+    }
+}
 
 }  // namespace lb

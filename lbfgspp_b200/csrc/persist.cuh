@@ -1,6 +1,7 @@
 // persist.cuh -- the device-resident L-BFGS solve: LBFGSSolver::minimize() (reference LBFGS.h:78-173) for built-in objectives as
 // ONE persistent cooperative kernel launch, for one problem or for a batch of B independent problems (BASELINE config 5).
-// Included by persist_f64.cu / persist_f32.cu.
+// Included by persist_f64.cu / persist_f32.cu.  The objective comes from objectives.cuh: built from the same geometry record as the
+// host-driven loop's, checked by the same rules before the launch, and every pass evaluates it with the same pack steps.
 //
 // The kernel is a "phase machine".  One CTA per SM (768 threads), all co-resident (cooperative launch).  Work proceeds in ROUNDS;
 // in a round every problem that is still running executes the ONE streaming pass its state asks for:
@@ -146,23 +147,8 @@ template <class T> struct PArgs
                                 // grid-stride instead of a chunked sweep (+1 %)
 };
 
-template <class V> __device__ __forceinline__ V ldv(const V* p) { return *reinterpret_cast<const volatile V*>(p); }
-
 template <class P> __device__ __forceinline__ void dswap(P& a, P& b) { P t = a; a = b; b = t; }
 __device__ __forceinline__ int slot_by_age(int head, int M, int age) { return ((head - 1 - age) % M + M) % M; }
-
-// ---- objectives as the persistent kernel builds them ------------------------------------------------------------------------
-template <class T, class OBJ> struct PObjMaker;
-template <class T> struct PObjMaker<T, RosenbrockPaired<T> >
-{ static __device__ RosenbrockPaired<T> make(const PArgs<T>& a, const T*, const T*, const double*) { return RosenbrockPaired<T>{a.n}; } };
-template <class T> struct PObjMaker<T, QuadShift<T> >
-{ static __device__ QuadShift<T> make(const PArgs<T>& a, const T*, const T*, const double*) { return QuadShift<T>{a.n, a.index_offset}; } };
-template <class T> struct PObjMaker<T, RosenbrockChained<T> >
-{ static __device__ RosenbrockChained<T> make(const PArgs<T>& a, const T*, const T*, const double* halo)
-  { return RosenbrockChained<T>{a.n, a.index_offset, a.n_global, halo}; } };
-template <class T> struct PObjMaker<T, QuadTridiag<T> >
-{ static __device__ QuadTridiag<T> make(const PArgs<T>& a, const T* d0, const T* d1, const double* halo)
-  { return QuadTridiag<T>{a.n, d0, d1, a.index_offset, a.n_global, halo}; } };
 
 // ---- shared memory of the kernel ----------------------------------------------------------------------------------------------
 struct PShared
@@ -254,17 +240,10 @@ __device__ __forceinline__ void p_trial(const OBJ& obj, const Own& own, const T*
 #pragma unroll
             for (int k = 0; k < 4; k++) xv[k] = px.v[k];
         }
-        acc[0] += obj.eval(i0, cnt, xv, T(0), T(0), gv);
+        eval_pack(obj, i0, cnt, xv, T(0), T(0), dv, gv, acc);
         Pack<T> pg, po;
 #pragma unroll
-        for (int k = 0; k < 4; k++)
-        {
-            acc[1] += gv[k] * dv[k];
-            acc[2] += gv[k] * gv[k];
-            acc[3] += (k < cnt) ? xv[k] * xv[k] : T(0);
-            pg.v[k] = gv[k];
-            po.v[k] = (MODE == 1) ? xv[k] : T(-1) * gv[k];
-        }
+        for (int k = 0; k < 4; k++) { pg.v[k] = gv[k]; po.v[k] = (MODE == 1) ? xv[k] : T(-1) * gv[k]; }
         T* const out0 = (MODE == 1) ? x : dout;
         if (evict_first) { store4<T, Hint::Stream, true>(out0, i0, cnt, po); store4<T, Hint::Stream, true>(g, i0, cnt, pg); }
         else { store4<T, Hint::Plain, true>(out0, i0, cnt, po); store4<T, Hint::Plain, true>(g, i0, cnt, pg); }
@@ -315,8 +294,8 @@ __device__ __forceinline__ void p_trial_halo(const OBJ& obj, const Own& own, con
         if (MODE == 1) tma_load_1d(dstt + TS + shift, d + lo, bytes, &full_bar[stage]);
         if constexpr (DV == 2)
         {
-            tma_load_1d(dstt + (size_t)NIN * TS + shift, obj.diag + lo, bytes, &full_bar[stage]);
-            tma_load_1d(dstt + (size_t)(NIN + 1) * TS + shift, obj.rhs + lo, bytes, &full_bar[stage]);
+            tma_load_1d(dstt + (size_t)NIN * TS + shift, obj.data0 + lo, bytes, &full_bar[stage]);
+            tma_load_1d(dstt + (size_t)(NIN + 1) * TS + shift, obj.data1 + lo, bytes, &full_bar[stage]);
         }
     };
 
@@ -338,40 +317,26 @@ __device__ __forceinline__ void p_trial_halo(const OBJ& obj, const Own& own, con
         {
             const int64_t i0 = e0 + off;
             const int cnt = (len - off >= 4) ? 4 : (len - off);
-            T xv[4], dv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
-            T xl = T(0), xr = T(0);
+            T xv[4], dv[4] = {T(0), T(0), T(0), T(0)};
+            T xl, xr;
             const Pack<T> pa = lds_pack(ta + off, lane);
             if (MODE == 1)
             {
                 const Pack<T> pb = lds_pack(tb + off, lane);
 #pragma unroll
                 for (int k = 0; k < 4; k++) { dv[k] = (k < cnt) ? pb.v[k] : T(0); xv[k] = (k < cnt) ? pa.v[k] + step * pb.v[k] : T(0); }
-                if (i0 > 0) xl = ta[off - 1] + step * tb[off - 1];
-                else if (obj.halo && obj.gofs > 0) xl = T(ldv(obj.halo + kHaloLeftA)) + step * T(ldv(obj.halo + kHaloLeftB));
-                if (i0 + 4 < n) xr = ta[off + 4] + step * tb[off + 4];
-                else if (obj.halo && i0 + 4 == n && obj.gofs + n < obj.n_glob) xr = T(ldv(obj.halo + kHaloRightA)) + step * T(ldv(obj.halo + kHaloRightB));
+                pack_neighbours<true>(obj, i0, n, step, [&](int j) { return ta[off + j] + step * tb[off + j]; }, xl, xr);
             }
             else
             {
 #pragma unroll
                 for (int k = 0; k < 4; k++) xv[k] = (k < cnt) ? pa.v[k] : T(0);
-                if (i0 > 0) xl = ta[off - 1];
-                else if (obj.halo && obj.gofs > 0) xl = T(ldv(obj.halo + kHaloLeftA));
-                if (i0 + 4 < n) xr = ta[off + 4];
-                else if (obj.halo && i0 + 4 == n && obj.gofs + n < obj.n_glob) xr = T(ldv(obj.halo + kHaloRightA));
+                pack_neighbours<false>(obj, i0, n, step, [&](int j) { return ta[off + j]; }, xl, xr);
             }
-            if constexpr (DV == 2) acc[0] += obj.staged(ta + (size_t)NIN * TS, ta + (size_t)(NIN + 1) * TS, e0).eval(i0, cnt, xv, xl, xr, gv);
-            else acc[0] += obj.eval(i0, cnt, xv, xl, xr, gv);
             Pack<T> pg, po;
+            eval_pack(obj.staged(ta + (size_t)NIN * TS, ta + (size_t)(NIN + 1) * TS, e0), i0, cnt, xv, xl, xr, dv, pg.v, acc);
 #pragma unroll
-            for (int k = 0; k < 4; k++)
-            {
-                acc[1] += gv[k] * dv[k];
-                acc[2] += gv[k] * gv[k];
-                acc[3] += (k < cnt) ? xv[k] * xv[k] : T(0);
-                pg.v[k] = gv[k];
-                po.v[k] = (MODE == 1) ? xv[k] : T(-1) * gv[k];
-            }
+            for (int k = 0; k < 4; k++) po.v[k] = (MODE == 1) ? xv[k] : T(-1) * pg.v[k];
             if (MODE == 1) store4<T, Hint::Plain, true>(x, i0, cnt, po);
             else store4<T, Hint::Plain, true>(dout, i0, cnt, po);
             store4<T, Hint::Plain, true>(g, i0, cnt, pg);
@@ -656,6 +621,18 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
 
     T acc[5] = {T(0), T(0), T(0), T(0), T(0)};
     T pre[5] = {T(0), T(0), T(0), T(0), T(0)};   // HALO, right-margin warp: operands of the element after the current tile
+    // FUSE: the trial of one unit at x1 = xv (lanes past EPT: 0, or x1 of the right neighbour) -> acc[1..4], x1 and g1 stored
+    auto first_trial = [&](const OBJ& o, int64_t i0, int cnt, const T (&xv)[4], T xl, T xr, const T (&r)[EPT]) {
+        T dv[EPT], gv[4];
+#pragma unroll
+        for (int k = 0; k < EPT; k++) dv[k] = (k < cnt) ? r[k] : T(0);   // (past cnt, d comes from whatever the vectors' padding holds)
+        eval_pack(o, i0, cnt, xv, xl, xr, dv, gv, acc + 1);
+        Unit<T> ug, uo;
+#pragma unroll
+        for (int k = 0; k < EPT; k++) { ug.v[k] = gv[k]; uo.v[k] = xv[k]; }
+        st_unit<T>(x1_out, i0, cnt, uo);
+        st_unit<T>(g1_out, i0, cnt, ug);
+    };
     __syncthreads();   // sh.vecs / sh.slots are in place and the staging ring is free
     int64_t next_tile = 0;
     for (int s = 0; s < stages; s++, next_tile++)
@@ -714,22 +691,10 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
                 if constexpr (FUSE)
                 {
                     const Unit<T> ux = lds_unit<T>(xrow + off);
-                    T xv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
+                    T xv[4] = {T(0), T(0), T(0), T(0)};
 #pragma unroll
                     for (int k = 0; k < EPT; k++) xv[k] = (k < cnt) ? ux.v[k] + T(1) * r[k] : T(0);
-                    acc[1] += obj.eval(i0, cnt, xv, T(0), T(0), gv);
-                    Unit<T> ug, uo;
-#pragma unroll
-                    for (int k = 0; k < EPT; k++)
-                    {
-                        acc[2] += (k < cnt) ? gv[k] * r[k] : T(0);
-                        acc[3] += (k < cnt) ? gv[k] * gv[k] : T(0);
-                        acc[4] += (k < cnt) ? xv[k] * xv[k] : T(0);
-                        ug.v[k] = gv[k];
-                        uo.v[k] = xv[k];
-                    }
-                    st_unit<T>(x1_out, i0, cnt, uo);
-                    st_unit<T>(g1_out, i0, cnt, ug);
+                    first_trial(obj, i0, cnt, xv, T(0), T(0), r);
                 }
             }
         }
@@ -813,7 +778,7 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
             // ---- phase 2: the objective at x1 with its neighbours from shared memory ----
             if (mine)
             {
-                T xv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
+                T xv[4] = {T(0), T(0), T(0), T(0)};
                 const Unit<T> u1 = lds_unit<T>(xrow + off);
 #pragma unroll
                 for (int k = 0; k < EPT; k++) xv[k] = u1.v[k];
@@ -821,20 +786,7 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
                 const T right = (i0 + EPT < n) ? xrow[off + EPT] : T(0);
                 T xr = T(0);
                 if (EPT < 4) xv[EPT < 4 ? EPT : 3] = right; else xr = right;
-                if constexpr (DV == 2) acc[1] += obj.staged(base + 2 * (size_t)TE + 2 * PAD, base + 3 * (size_t)TE + 2 * PAD, e0).eval(i0, cnt, xv, xl, xr, gv);
-                else acc[1] += obj.eval(i0, cnt, xv, xl, xr, gv);
-                Unit<T> ug, uo;
-#pragma unroll
-                for (int k = 0; k < EPT; k++)
-                {
-                    acc[2] += (k < cnt) ? gv[k] * r[k] : T(0);
-                    acc[3] += (k < cnt) ? gv[k] * gv[k] : T(0);
-                    acc[4] += (k < cnt) ? xv[k] * xv[k] : T(0);
-                    ug.v[k] = gv[k];
-                    uo.v[k] = xv[k];
-                }
-                st_unit<T>(x1_out, i0, cnt, uo);
-                st_unit<T>(g1_out, i0, cnt, ug);
+                first_trial(obj.staged(base + 2 * (size_t)TE + 2 * PAD, base + 3 * (size_t)TE + 2 * PAD, e0), i0, cnt, xv, xl, xr, r);
             }
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -1297,7 +1249,7 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
             acct_bucket = (acct_bucket == -1 || acct_bucket == op) ? op : 0;
             acct_words += words_of(op, c_round, kDataVectors);
             double* dst = a.partials + (size_t)b * a.pstride * G + cta;
-            const OBJ obj = PObjMaker<T, OBJ>::make(a, st->data0, st->data1, (HALO && a.xc != nullptr) ? st->halo : nullptr);
+            const OBJ obj{ObjGeom<T>{a.n, a.index_offset, a.n_global, (HALO && a.xc != nullptr) ? st->halo : nullptr, st->data0, st->data1}};
             switch (op)
             {
             case POP_FIRST:

@@ -35,19 +35,10 @@ struct lbfgs_b200_solver
     lb::PCtl last_ctl{};                  // its accounting
 };
 
-template <class T> static void* persist_kernel_for(int objective, int rounds)
+template <class T, class OBJ> static void* persist_kernel_for(int rounds)
 {
-    using namespace lb;
-#define LB_PK(OBJ) (rounds <= 1 ? (void*)k_persist<T, OBJ, 1> : rounds == 2 ? (void*)k_persist<T, OBJ, 2> : (void*)k_persist<T, OBJ, 3>)
-    switch (objective)
-    {
-    case LBFGS_B200_OBJ_ROSENBROCK_PAIRED: return LB_PK(RosenbrockPaired<T>);
-    case LBFGS_B200_OBJ_QUAD_SHIFT: return LB_PK(QuadShift<T>);
-    case LBFGS_B200_OBJ_ROSENBROCK_CHAINED: return LB_PK(RosenbrockChained<T>);
-    case LBFGS_B200_OBJ_QUAD_TRIDIAG: return LB_PK(QuadTridiag<T>);
-    }
-#undef LB_PK
-    return nullptr;
+    using lb::k_persist;
+    return rounds <= 1 ? (void*)k_persist<T, OBJ, 1> : rounds == 2 ? (void*)k_persist<T, OBJ, 2> : (void*)k_persist<T, OBJ, 3>;
 }
 
 // x_inout: B vectors of n elements, `ldx` elements apart (device).  data0/data1: nullptr, or per-problem vectors `ldd` apart (ldd = 0:
@@ -67,22 +58,20 @@ static lbfgs_b200_status solver_minimize(lbfgs_b200_solver* s, int objective, co
     REQUIRE(ctx, ctx->nranks == 1 || ctx->x_active, "the device-resident solve needs the in-kernel exchange (comm_p2p) when sharded");
     REQUIRE(ctx, B == 1 || ldx >= s->n, "solver_minimize: the batch stride of x is shorter than n");
     REQUIRE(ctx, trace_host == nullptr || B == 1, "solver_minimize: traces are recorded for single problems only");
-    const bool coupled = objective == LBFGS_B200_OBJ_ROSENBROCK_CHAINED || objective == LBFGS_B200_OBJ_QUAD_TRIDIAG;
-    if (objective == LBFGS_B200_OBJ_ROSENBROCK_PAIRED) REQUIRE(ctx, s->n % 2 == 0, "paired Rosenbrock needs an even n");
-    if (objective == LBFGS_B200_OBJ_QUAD_TRIDIAG) REQUIRE(ctx, data0 && data1, "quad_tridiag needs data0 = diag, data1 = rhs");
-    int64_t n_global = s->n, index_offset = ctx->index_offset;
-    if (ctx->nranks > 1 && coupled)
-    {
-        REQUIRE(ctx, ctx->n_global > 0, "a neighbour-coupled objective under n-sharding needs lbfgs_b200_set_global_extent()");
-        REQUIRE(ctx, ctx->index_offset + s->n <= ctx->n_global, "local block exceeds the global extent");
-        REQUIRE(ctx, ctx->rank == ctx->nranks - 1 || s->n % 4 == 0, "every block but the last must hold a multiple of 4 coordinates");
-        n_global = ctx->n_global;
-    }
-    else if (coupled) index_offset = 0;
     if (ctx->x_active) REQUIRE(ctx, (size_t)B * (s->pstride + 4) <= (size_t)kXMaxVals, "batch of %d problems with m = %d exceeds the exchange buffer", B, s->m);
     const int rounds = (s->m + kGramMaxWarps - 1) / kGramMaxWarps;   // column pairs per round of the dots pass: at most one per warp
-    void* kernel = persist_kernel_for<T>(objective, rounds);
-    if (!kernel) return fail(ctx, LBFGS_B200_ERR_INVALID, "unknown objective id %d", objective);
+    ObjGeom<T> geo;
+    void* kernel = nullptr;
+    // the first trial of every search rides on the combination pass; a neighbour-coupled objective needs its neighbours' x + d,
+    // which only exist on this rank when n is not sharded
+    bool fuse_first_trial = true;
+    if (auto st = with_objective<T>(ctx, objective, [&](auto tag) {
+            using OBJ = decltype(tag);
+            kernel = persist_kernel_for<T, OBJ>(rounds);
+            fuse_first_trial = !(OBJ::kHalo && ctx->nranks > 1);
+            return objective_geometry<OBJ>(ctx, s->n, data0, data1, geo);
+        }))
+        return st;
 
     if (trace_host && trace_cap > s->trace_cap)
     {
@@ -116,9 +105,7 @@ static lbfgs_b200_status solver_minimize(lbfgs_b200_solver* s, int objective, co
         p.op = POP_FIRST; p.c_round = 0;
         p.epsilon = (T)prm->epsilon; p.epsilon_rel = (T)prm->epsilon_rel; p.delta = (T)prm->delta; p.max_step = (T)prm->max_step;
         p.past = prm->past; p.max_iterations = prm->max_iterations;
-        // the first trial of every search rides on the combination pass; a neighbour-coupled objective needs its neighbours' x + d,
-        // which only exist on this rank when n is not sharded
-        p.fuse_first_trial = (coupled && ctx->nranks > 1) ? 0 : 1;
+        p.fuse_first_trial = fuse_first_trial;
         p.ls.kind = ls_kind;
         p.ls_opt = LBFGSpp::line_search_options<T>(*prm, ls_kind);
         p.trace = trace_host ? s->d_trace : nullptr;
@@ -158,7 +145,7 @@ static lbfgs_b200_status solver_minimize(lbfgs_b200_solver* s, int objective, co
     PArgs<T> a{};
     a.probs = static_cast<PState<T>*>(s->d_state); a.rounds = static_cast<PRound<T>*>(s->d_rounds); a.B = B; a.ctl = s->d_ctl; a.partials = s->d_partials; a.pstride = s->pstride;
     a.n = s->n; a.grain = 1 << s->bt_log; a.xc = ctx->x_active ? ctx->x_comm : nullptr;
-    a.index_offset = index_offset; a.n_global = n_global;
+    a.index_offset = geo.gofs; a.n_global = geo.n_glob;
     a.wait_cycles = kPWaitCycles;
     if (const char* e = getenv("LBFGS_B200_WATCHDOG_SCALE")) { const long long k = atoll(e); if (k >= 1 && k <= 100000) a.wait_cycles *= k; }
     a.evict_first_stores = (size_t)s->n * sizeof(T) * 4 > ((size_t)36 << 20);     // x, xp, g, d of one problem exceed ~3/4 of the 50 MB L2
