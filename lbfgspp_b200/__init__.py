@@ -626,7 +626,7 @@ class Session:
         return dict(niter=res.niter, nfev=res.nfev, fx=res.fx, gnorm=res.gnorm, launches=res.launches,
                     h2d_bytes=res.h2d_bytes, d2h_bytes=res.d2h_bytes)
 
-    OPS = ("mixed", "first", "trial", "dots_form", "dots_plain", "combine", "combine_trial", "restore", "-", "-")   # slots 8, 9 unused
+    OPS = ("mixed", "first", "trial", "dots_form", "dots_plain", "combine", "combine_trial", "restore", "materialize", "-")   # slot 9 unused
 
     def profile(self):
         """Accounting of the last device-resident solve: dict(kernel_ms, sync_ms, ops={name: dict(ms, rounds, alg_bytes)}); None for

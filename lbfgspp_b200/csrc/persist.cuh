@@ -13,6 +13,14 @@
 //     COMBINE_TRIAL  COMBINE + the first trial of the next line search in the same pass: the reference restarts every search
 //                    at step = 1 (LBFGS.h:168), so x1 = x + d, g1 = grad f(x1) ; {g.d, f1, g1.d, g1.g1, x1.x1}
 //     RESTORE        x = xp, g = gp (a search that never improved on its start point; LineSearchMoreThuente.h:602-614)
+//     MATERIALIZE    x = xp + step*d, g = grad f(x) (or x = xp, g = gp): writes the point a finished problem stopped at
+// Trials on the ray.  For objectives without neighbour coupling g = grad f(x) is a per-element function of x, and every trial point
+// is x = xp + step*d, so a trial stores nothing: its point is IMPLIED by {step, at_start} (the start point xp, gp when at_start).
+// The pass after the search -- DOTS_FORM, which reads x and g anyway -- rebuilds the accepted point from xp, d (or xp, gp) with the
+// trial's own arithmetic, bit for bit, writes x and g, and forms the pair from them; a problem that stops while its point is still
+// implied takes one MATERIALIZE round.  The kept best trial of a search is its step, so there is no x_lo/g_lo and no RESTORE pass.
+// Neighbour-coupled objectives (kHalo) store every trial's x, g and keep the best one by pointer swap with x_lo/g_lo, as the
+// reference's search does (LineSearchMoreThuente.h:534,553), and restore the start point with RESTORE.
 // Every CTA owns the same contiguous chunk (granularity: the block length of the tiled history) of EVERY vector in EVERY pass, so a CTA only ever reads vector
 // elements it wrote itself (halo coordinates excepted, those are read through L2) and streams long contiguous runs.  Between rounds there is one
 // grid-wide synchronisation: CTAs deposit their partial sums in fixed slots, CTA 0 adds them in a fixed order (deterministic: no
@@ -43,8 +51,9 @@ constexpr int kPStageBytes = kGramStages * 4 * kGramTE * 8;   // dynamic shared 
 constexpr int kPMaxStages = 4;
 constexpr int kPCache = 4;                   // problems whose leader-side state is kept in shared memory
 
-enum { POP_IDLE = 0, POP_FIRST = 1, POP_TRIAL = 2, POP_DOTS_FORM = 3, POP_DOTS_PLAIN = 4, POP_COMBINE = 5, POP_COMBINE_TRIAL = 6, POP_RESTORE = 7 };
-constexpr int kPOps = 10;   // accounting slots (ops + the "mixed" bucket 0; 8 and 9 unused, kept for the solver_profile ABI)
+enum { POP_IDLE = 0, POP_FIRST = 1, POP_TRIAL = 2, POP_DOTS_FORM = 3, POP_DOTS_PLAIN = 4, POP_COMBINE = 5, POP_COMBINE_TRIAL = 6, POP_RESTORE = 7,
+       POP_MATERIALIZE = 8 };
+constexpr int kPOps = 10;   // accounting slots (ops + the "mixed" bucket 0; 9 unused, kept for the solver_profile ABI)
 constexpr int kPGramScratch = 1024;   // doubles
 
 // ---- the S/Y history of the solve: tiled layout ---------------------------------------------------------------------------------
@@ -66,7 +75,7 @@ template <class T> struct PHist
 // ---- per-problem state (device memory; the leader CTA's working copy) ----------------------------------------------------------
 template <class T> struct PState
 {
-    // vectors (rotate by pointer swap)
+    // vectors (rotate by pointer swap); x_lo, g_lo: neighbour-coupled objectives only (nullptr otherwise)
     T *x, *xp, *g, *gp, *drt, *x_lo, *g_lo;
     // history storage (fixed for the duration of the kernel: other CTAs read these fields with ordinary loads)
     PHist<T> hist;              // the S/Y ring, tiled (see PHist)
@@ -86,8 +95,10 @@ template <class T> struct PState
     // line-search state
     LBFGSpp::RunTimeCore<T> ls;
     LBFGSpp::SearchRecord<T> rec;   // fx, dg, gg, xx of the current point
-    // iteration scalars
-    T gnorm, step;
+    // iteration scalars.  step: the trial to evaluate, or (objectives without neighbour coupling) the step of the point (x, g)
+    // stand for while they are implied; step_kept: the step of the search's kept trial; at_start: the point is the search's start
+    T gnorm, step, step_kept;
+    int at_start;
     int k;
     long long nfev;
     int status;     // 0 ok, otherwise a LineSearchError code
@@ -103,9 +114,11 @@ template <class T> struct PState
 template <class T> struct alignas(128) PRound
 {
     T *x, *xp, *g, *gp, *drt;
-    T step;
+    T step;                     // TRIAL: the trial's step; DOTS_FORM / MATERIALIZE of an implied point: the step of that point
     int op, c_round, head, pending, gram_cur;
+    int at_start;               // DOTS_FORM / MATERIALIZE of an implied point: the point is (xp, gp)
 };
+static_assert(sizeof(PRound<double>) == 128 && sizeof(PRound<float>) == 128, "a round descriptor is one 128-byte line");
 
 struct alignas(128) PCtl
 {
@@ -142,7 +155,7 @@ template <class T> struct PArgs
     const XComm* xc;
     int64_t index_offset, n_global;
     long long wait_cycles;      // watchdog budget of a grid-barrier wait (clock64 ticks); cross-rank waits get 4x, the release wait 6x
-    bool evict_first_stores;    // the trial pass stores x, g with L2 evict-first: +3 % on that pass at n = 1e7 (set by the host when the vectors cannot stay
+    bool evict_first_stores;    // the streaming passes (FIRST, MATERIALIZE) store with L2 evict-first: +3 % on the trial pass when it stored x, g at n = 1e7 (set by the host when the vectors cannot stay
                                 // in L2 anyway).  Measured and dropped: unrolling the pass 4x (no change), prefetching its inputs into L2 (-5 %), a
                                 // grid-stride instead of a chunked sweep (+1 %)
 };
@@ -213,7 +226,8 @@ template <int NV> __device__ __forceinline__ void block_sums(const double (&acc)
 }
 
 // ---- FIRST / TRIAL -------------------------------------------------------------------------------------------------------------
-// MODE 0: FIRST (evaluate at x, write g and d = -g) ; MODE 1: TRIAL (x = xp + step*d, write x and g).  Operands stream through
+// MODE 0: FIRST (evaluate at x, write g and d = -g) ; MODE 1: TRIAL (evaluate at x = xp + step*d, store nothing: the point is
+// rebuilt by the pass that needs it) ; MODE 2: MATERIALIZE (x = xp + step*d, write x and g; no sums).  Operands stream through
 // registers with 128-bit loads/stores (a shared-memory staged variant measured slower for this 1:1 read/write pass).  Objectives
 // without neighbour coupling only: the coupled ones take p_trial_halo.
 template <class T, class OBJ, int MODE>
@@ -228,7 +242,7 @@ __device__ __forceinline__ void p_trial(const OBJ& obj, const Own& own, const T*
         const int64_t i0 = q << 2;
         const int cnt = (n - i0 >= 4) ? 4 : int(n - i0);
         T xv[4], dv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
-        if (MODE == 1)
+        if (MODE != 0)
         {
             const Pack<T> px = load4<T, Hint::Stream, true>(xp, i0, cnt), pd = load4<T, Hint::Stream, true>(d, i0, cnt);
 #pragma unroll
@@ -241,17 +255,23 @@ __device__ __forceinline__ void p_trial(const OBJ& obj, const Own& own, const T*
             for (int k = 0; k < 4; k++) xv[k] = px.v[k];
         }
         eval_pack(obj, i0, cnt, xv, T(0), T(0), dv, gv, acc);
-        Pack<T> pg, po;
+        if constexpr (MODE != 1)
+        {
+            Pack<T> pg, po;
 #pragma unroll
-        for (int k = 0; k < 4; k++) { pg.v[k] = gv[k]; po.v[k] = (MODE == 1) ? xv[k] : T(-1) * gv[k]; }
-        T* const out0 = (MODE == 1) ? x : dout;
-        if (evict_first) { store4<T, Hint::Stream, true>(out0, i0, cnt, po); store4<T, Hint::Stream, true>(g, i0, cnt, pg); }
-        else { store4<T, Hint::Plain, true>(out0, i0, cnt, po); store4<T, Hint::Plain, true>(g, i0, cnt, pg); }
+            for (int k = 0; k < 4; k++) { pg.v[k] = gv[k]; po.v[k] = (MODE == 2) ? xv[k] : T(-1) * gv[k]; }
+            T* const out0 = (MODE == 2) ? x : dout;
+            if (evict_first) { store4<T, Hint::Stream, true>(out0, i0, cnt, po); store4<T, Hint::Stream, true>(g, i0, cnt, pg); }
+            else { store4<T, Hint::Plain, true>(out0, i0, cnt, po); store4<T, Hint::Plain, true>(g, i0, cnt, pg); }
+        }
     };
 #pragma unroll 2
     for (int64_t q = (own.c0 >> 2) + threadIdx.x; q < p1; q += kPThreads) body(q);
-    const double dacc[4] = {(double)acc[0], (double)acc[1], (double)acc[2], (double)acc[3]};
-    block_sums<4>(dacc, sh, dst, G);
+    if constexpr (MODE != 2)
+    {
+        const double dacc[4] = {(double)acc[0], (double)acc[1], (double)acc[2], (double)acc[3]};
+        block_sums<4>(dacc, sh, dst, G);
+    }
 }
 
 // Neighbour-coupled objectives (chained Rosenbrock, tridiagonal quadratic): the same pass with its inputs staged tile by tile through
@@ -351,7 +371,7 @@ __device__ __forceinline__ void p_trial_halo(const OBJ& obj, const Own& own, con
     block_sums<4>(dacc, sh, dst, G);
 }
 
-// ---- RESTORE --------------------------------------------------------------------------------------------------------------------
+// ---- RESTORE (and MATERIALIZE of a search's start point) ----------------------------------------------------------------------
 template <class T>
 __device__ __forceinline__ void p_restore(const Own& own, const T* __restrict__ xp, const T* __restrict__ gp, T* __restrict__ x, T* __restrict__ g)
 {
@@ -425,9 +445,12 @@ __device__ __forceinline__ void stage_tiled(T* dstt, int TE, int nrhs, int64_t e
 
 // ---- DOTS -----------------------------------------------------------------------------------------------------------------------
 // [S Y]'[v s_new y_new] over this CTA's chunk, one block (tile) at a time, everything staged by bulk copies.  FORM: the newest pair
-// is formed on the fly from (x, xp, v = g, gp) -- s = x - xp, y = g - gp, identical in every warp that needs them -- takes part as
-// column 0 and is written to ring slot `new_slot` by the warps that own column 0.  Column j (by age) belongs to warp group j, whose
-// `split` warps share the tile's units.  PLAIN: s.v and y.v over the old history only.
+// s = x - xp, y = g - gp is formed on the fly, identically in every warp that needs it, takes part as column 0 and is written to ring
+// slot `new_slot` by the warps that own column 0.  The point (x, g) comes from the staged rows {g, x, gp, xp} (neighbour-coupled
+// objectives: the trials stored it) or is rebuilt from the staged rows {d, xp, gp} -- x = xp + step*d, g = grad f(x) with the trial's
+// own arithmetic, or x = xp, g = gp when the search ended on its start point -- and then also written to (x, g) by the column-0 warps.
+// (Forming it once per tile into the staged rows, behind one more barrier per tile, measured 21 % slower per pass on config 2.)
+// Column j (by age) belongs to warp group j, whose `split` warps share the tile's units.  PLAIN: s.v and y.v over the old history only.
 template <class T> struct PDots
 {
     int64_t n;
@@ -435,13 +458,17 @@ template <class T> struct PDots
     int c;               // columns taking part (FORM: including the new pair)
     int end, cnt_old;    // the old columns: the cnt_old slots below `end`
     int new_slot, split, cols_per_round;
+    T step;              // FORM of an implied point: its step, or (at_start) the start point
+    int at_start;
+    T *x, *g;            // FORM of an implied point: where it is written
 };
 
-template <class T, int ROUNDS, bool FORM>
-__device__ __forceinline__ void p_dots(const PDots<T>& a, const Own& own, T* tiles, PShared& sh, unsigned& phase_bits, double* dst, int G)
+template <class T, class OBJ, int ROUNDS, bool FORM>
+__device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const Own& own, T* tiles, PShared& sh, unsigned& phase_bits, double* dst, int G)
 {
     constexpr int EPT = 16 / (int)sizeof(T);
-    constexpr int NRHS = FORM ? 4 : 1;                           // staged right-hand vectors: g (, x, gp, xp)
+    constexpr bool IMPLIED = !OBJ::kHalo;
+    constexpr int NRHS = FORM ? (IMPLIED ? 3 : 4) : 1;           // staged right-hand vectors: g / g, x, gp, xp / d, xp, gp
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int TE = a.h.BT();
     const int my_col = warp / a.split, my_part = warp % a.split;
@@ -487,14 +514,40 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const Own& own, T* til
                     const int off = u * EPT;
                     const int cnt = len - off;
                     if (cnt <= 0) break;
-                    Unit<T> ug = lds_unit<T>(base + off), us, uy, usn, uyn;
+                    Unit<T> ug, us, uy, usn, uyn, ux;
                     if constexpr (FORM)
                     {
-                        const Unit<T> ux = lds_unit<T>(base + TE + off), ugp = lds_unit<T>(base + 2 * TE + off), uxp = lds_unit<T>(base + 3 * TE + off);
+                        Unit<T> ugp, uxp;
+                        if constexpr (IMPLIED)
+                        {
+                            const Unit<T> ud = lds_unit<T>(base + off);
+                            uxp = lds_unit<T>(base + TE + off);
+                            ugp = lds_unit<T>(base + 2 * TE + off);
+                            if (a.at_start) { ux = uxp; ug = ugp; }
+                            else
+                            {
+                                // the trial's arithmetic (p_trial, and p_combine's first trial with step 1 on the stored d)
+                                const int c4 = cnt < EPT ? cnt : EPT;
+                                T xv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
+#pragma unroll
+                                for (int k = 0; k < EPT; k++) xv[k] = (k < c4) ? uxp.v[k] + a.step * ud.v[k] : T(0);
+                                obj.eval(e0 + off, c4, xv, T(0), T(0), gv);
+#pragma unroll
+                                for (int k = 0; k < EPT; k++) { ux.v[k] = xv[k]; ug.v[k] = gv[k]; }
+                            }
+                        }
+                        else
+                        {
+                            ug = lds_unit<T>(base + off);
+                            ux = lds_unit<T>(base + TE + off);
+                            ugp = lds_unit<T>(base + 2 * TE + off);
+                            uxp = lds_unit<T>(base + 3 * TE + off);
+                        }
 #pragma unroll
                         for (int k = 0; k < EPT; k++) { usn.v[k] = ux.v[k] - uxp.v[k]; uyn.v[k] = ug.v[k] - ugp.v[k]; }
                         if (cnt < EPT) { mask_unit(usn, cnt); mask_unit(uyn, cnt); }
                     }
+                    else ug = lds_unit<T>(base + off);
                     bool loaded = false;
                     if constexpr (FORM)
                     {
@@ -503,6 +556,7 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const Own& own, T* til
                             us = usn; uy = uyn;
                             st_unit<T>(s_new, off, cnt, usn);
                             st_unit<T>(s_new + TE, off, cnt, uyn);
+                            if (IMPLIED) { st_unit<T>(a.x, e0 + off, cnt, ux); st_unit<T>(a.g, e0 + off, cnt, ug); }
                             loaded = true;
                         }
                     }
@@ -565,7 +619,8 @@ __device__ __forceinline__ void dots_geometry(int c, int units, int& split, int&
 }
 
 // ---- COMBINE (+ first trial) ---------------------------------------------------------------------------------------------------
-// d = cv*v + sum_j cy_j*y_j + cs_j*s_j ; FUSE: x1 = xc + d, g1 = grad f(x1) written to (x1_out, g1_out) and the four trial sums.
+// d = cv*v + sum_j cy_j*y_j + cs_j*s_j ; FUSE: x1 = xc + d, g1 = grad f(x1) and the four trial sums (neighbour-coupled objectives:
+// x1, g1 written to (x1_out, g1_out)).
 // Staged rows of a tile: v, (xc,) then the history block's live slots; sh.slots[j] = packed row of the pair of age j.  A thread owns
 // one 16-byte unit of the tile and adds the terms in the order the recursion would (y newest -> oldest, then s oldest -> newest), with
 // the operand loads of 8 columns in flight before their multiply-adds retire (the pass is bound by shared-memory latency otherwise).
@@ -621,17 +676,21 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
 
     T acc[5] = {T(0), T(0), T(0), T(0), T(0)};
     T pre[5] = {T(0), T(0), T(0), T(0), T(0)};   // HALO, right-margin warp: operands of the element after the current tile
-    // FUSE: the trial of one unit at x1 = xv (lanes past EPT: 0, or x1 of the right neighbour) -> acc[1..4], x1 and g1 stored
+    // FUSE: the trial of one unit at x1 = xv (lanes past EPT: 0, or x1 of the right neighbour) -> acc[1..4]; x1 and g1 stored for a
+    // neighbour-coupled objective only (otherwise the pair-forming pass rebuilds the point if the search accepts it)
     auto first_trial = [&](const OBJ& o, int64_t i0, int cnt, const T (&xv)[4], T xl, T xr, const T (&r)[EPT]) {
         T dv[EPT], gv[4];
 #pragma unroll
         for (int k = 0; k < EPT; k++) dv[k] = (k < cnt) ? r[k] : T(0);   // (past cnt, d comes from whatever the vectors' padding holds)
         eval_pack(o, i0, cnt, xv, xl, xr, dv, gv, acc + 1);
-        Unit<T> ug, uo;
+        if constexpr (OBJ::kHalo)
+        {
+            Unit<T> ug, uo;
 #pragma unroll
-        for (int k = 0; k < EPT; k++) { ug.v[k] = gv[k]; uo.v[k] = xv[k]; }
-        st_unit<T>(x1_out, i0, cnt, uo);
-        st_unit<T>(g1_out, i0, cnt, ug);
+            for (int k = 0; k < EPT; k++) { ug.v[k] = gv[k]; uo.v[k] = xv[k]; }
+            st_unit<T>(x1_out, i0, cnt, uo);
+            st_unit<T>(g1_out, i0, cnt, ug);
+        }
     };
     __syncthreads();   // sh.vecs / sh.slots are in place and the staging ring is free
     int64_t next_tile = 0;
@@ -827,16 +886,18 @@ template <class T> __device__ __forceinline__ void record_eval(PState<T>* st, T 
     if (st->trace && st->nfev < st->trace_cap) st->trace[st->nfev] = (double)fx;
     st->nfev++;
 }
-template <class T> __device__ __forceinline__ void finish(PState<T>* st, int niter, int status = 0)
+// the problem stops; `implied`: (x, g) do not hold its point yet, one MATERIALIZE round writes them (step, at_start) first
+template <class T> __device__ __forceinline__ void finish(PState<T>* st, int niter, int status = 0, bool implied = false)
 {
     st->finished = 1;
     st->niter = niter;
     if (status) st->status = status;
-    st->op = POP_IDLE;
+    st->op = implied ? POP_MATERIALIZE : POP_IDLE;
 }
 
-// after a search has produced its point in (x, g): the stopping rules (LBFGS.h:137-154), then on to the pair-forming dots
-template <class T> __device__ __forceinline__ void after_search(PState<T>* st)
+// after a search has produced its point -- in (x, g) when STORED, else implied by (step, at_start): the stopping rules
+// (LBFGS.h:137-154), then on to the pair-forming dots
+template <class T, bool STORED> __device__ __forceinline__ void after_search(PState<T>* st)
 {
     using namespace LBFGSpp;
     const int k = st->k;
@@ -844,47 +905,59 @@ template <class T> __device__ __forceinline__ void after_search(PState<T>* st)
     if (gradient_converged(st->gnorm, st->rec.xx, st->epsilon, st->epsilon_rel) || stalled(st->fx_hist, st->past, k, st->rec.fx, st->delta) ||
         iteration_cap(k, st->max_iterations))
     {
-        finish(st, k);
+        finish(st, k, 0, !STORED);
         return;
     }
     st->op = POP_DOTS_FORM;
     st->c_round = st->ncorr < st->m ? st->ncorr + 1 : st->m;
 }
 
-// the trial at st->ls.step() has been evaluated into (x, g): {fx, dg, gg, xx}.  Sets the next op.
-template <class T> __device__ __forceinline__ void digest_trial(PState<T>* st, T fx, T dg, T gg, T xx)
+// the trial at st->step has been evaluated: {fx, dg, gg, xx}.  Sets the next op.  STORED: the trial is in (x, g), a kept trial
+// moves to (x_lo, g_lo) by pointer swap; otherwise a trial is its step, and the kept one is st->step_kept.
+template <class T, bool STORED> __device__ __forceinline__ void digest_trial(PState<T>* st, T fx, T dg, T gg, T xx)
 {
     record_eval(st, fx);
     bool keep = false;
     const int action = st->ls.advance(fx, dg, keep);
     const int next = st->rec.digest(action, keep, fx, dg, gg, xx, st->ls.best_fx(), st->ls.best_dg());
-    if (next >= LBFGSpp::LSE_STEP_NOT_POSITIVE) { finish(st, st->k, next); return; }
-    if (keep) { dswap(st->x, st->x_lo); dswap(st->g, st->g_lo); }
+    if (next >= LBFGSpp::LSE_STEP_NOT_POSITIVE) { finish(st, st->k, next, !STORED); return; }   // (x, g): this trial
+    if (keep)
+    {
+        if (STORED) { dswap(st->x, st->x_lo); dswap(st->g, st->g_lo); }
+        else st->step_kept = st->step;
+    }
     switch (next)
     {
     case LBFGSpp::SEARCH_EVALUATE: st->op = POP_TRIAL; st->step = st->ls.step(); return;
-    case LBFGSpp::SEARCH_TAKE_KEPT: dswap(st->x, st->x_lo); dswap(st->g, st->g_lo); break;
-    case LBFGSpp::SEARCH_TAKE_START: st->op = POP_RESTORE; return;   // copy xp/gp back, then carry on
+    case LBFGSpp::SEARCH_TAKE_KEPT:
+        if (STORED) { dswap(st->x, st->x_lo); dswap(st->g, st->g_lo); }
+        else st->step = st->step_kept;
+        break;
+    case LBFGSpp::SEARCH_TAKE_START:
+        if (STORED) { st->op = POP_RESTORE; return; }   // copy xp/gp back, then carry on
+        st->at_start = 1;
+        break;
     }
-    after_search(st);
+    after_search<T, STORED>(st);
 }
 
 // top of an iteration (LBFGS.h:121-127): the search is armed, the current point becomes the previous one
 template <class T> __device__ __forceinline__ bool begin_search(PState<T>* st, T step)
 {
     // the search validates its inputs before anything moves (the reference throws before touching x): on failure x stays the
-    // current point
+    // current point (it is in (x, g): FIRST or the pair-forming pass wrote it)
     const int rc = st->ls.init(st->ls_opt, st->rec.fx, st->rec.dg, step, st->max_step);
     if (rc != 0) { finish(st, st->k, rc); return false; }
     dswap(st->xp, st->x);
     dswap(st->gp, st->g);
     st->rec.begin();
+    st->at_start = 0;
     st->op = POP_TRIAL;
     st->step = st->ls.step();
     return true;
 }
 
-template <class T> __device__ void advance_problem(PState<T>* st, const double* vals)
+template <class T, bool STORED> __device__ void advance_problem(PState<T>* st, const double* vals)
 {
     st->rounds++;
     switch (st->op)
@@ -904,10 +977,13 @@ template <class T> __device__ void advance_problem(PState<T>* st, const double* 
         return;
     }
     case POP_TRIAL:
-        digest_trial(st, (T)vals[0], (T)vals[1], (T)vals[2], (T)vals[3]);
+        digest_trial<T, STORED>(st, (T)vals[0], (T)vals[1], (T)vals[2], (T)vals[3]);
         return;
     case POP_RESTORE:           // (x, g) now hold the search's start point; its sums were restored before
-        after_search(st);
+        after_search<T, STORED>(st);
+        return;
+    case POP_MATERIALIZE:       // (x, g) now hold the point the problem stopped at
+        st->op = POP_IDLE;
         return;
     case POP_DOTS_FORM:
     {
@@ -937,26 +1013,28 @@ template <class T> __device__ void advance_problem(PState<T>* st, const double* 
         st->rec.dg = (T)vals[0];            // LBFGS.h:123 for the next pass
         st->k += 1;
         if (!begin_search(st, T(1))) return;   // LBFGS.h:168
-        // the pass already evaluated x + 1*d into the buffers that the rotation just made (x, g)
-        if (fused && st->ls.step() == T(1)) digest_trial(st, (T)vals[1], (T)vals[2], (T)vals[3], (T)vals[4]);
+        // the pass already evaluated xp + 1*d (STORED: into the buffers that the rotation just made (x, g))
+        if (fused && st->ls.step() == T(1)) digest_trial<T, STORED>(st, (T)vals[1], (T)vals[2], (T)vals[3], (T)vals[4]);
         return;
     }
     default: return;
     }
 }
 
-// n-words a pass has to move (reads + writes of whole vectors): the roofline numerator of the persistent kernel
-__device__ __forceinline__ double words_of(int op, int c, int data_vectors)
+// n-words a pass has to move (reads + writes of whole vectors): the roofline numerator of the persistent kernel.  stored: the
+// trials store their points (neighbour-coupled objectives)
+__device__ __forceinline__ double words_of(int op, int c, int data_vectors, bool stored)
 {
     switch (op)
     {
     case POP_FIRST: return 3.0 + data_vectors;              // R x ; W g, d
-    case POP_TRIAL: return 4.0 + data_vectors;              // R xp, d ; W x, g
+    case POP_TRIAL: return (stored ? 4.0 : 2.0) + data_vectors;   // R xp, d (; W x, g)
     case POP_RESTORE: return 4.0;                           // R xp, gp ; W x, g
-    case POP_DOTS_FORM: return 2.0 * c + 4.0;               // R x, xp, g, gp, 2(c-1) columns ; W s, y
+    case POP_MATERIALIZE: return 4.0;                       // R xp, d (or gp) ; W x, g
+    case POP_DOTS_FORM: return 2.0 * c + (stored ? 4.0 : 5.0);   // R x, xp, g, gp / xp, d, gp, 2(c-1) columns ; (W x, g,) W s, y
     case POP_DOTS_PLAIN: return 2.0 * c + 1.0;              // R g, 2c columns
     case POP_COMBINE: return 2.0 * c + 2.0;                 // R g, 2c columns ; W d
-    case POP_COMBINE_TRIAL: return 2.0 * c + 5.0 + data_vectors;   // R g, x, 2c columns ; W d, x1, g1
+    case POP_COMBINE_TRIAL: return 2.0 * c + (stored ? 5.0 : 3.0) + data_vectors;   // R g, x, 2c columns ; W d (, x1, g1)
     default: return 0.0;
     }
 }
@@ -1087,10 +1165,10 @@ __device__ int leader_round(const PArgs<T>& a, int G, PShared& sh, PState<T>* ca
         if (b < a.B && state_of(b)->op != POP_IDLE)
         {
             PState<T>* st = state_of(b);
-            advance_problem(st, st->raw);
+            advance_problem<T, HALO>(st, st->raw);
             PRound<T>* rd = a.rounds + b;
             rd->x = st->x; rd->xp = st->xp; rd->g = st->g; rd->gp = st->gp; rd->drt = st->drt;
-            rd->step = st->step;
+            rd->step = st->step; rd->at_start = st->at_start;
             rd->c_round = st->c_round; rd->head = st->head; rd->pending = st->pending; rd->gram_cur = st->gram_cur;
             rd->op = st->op;
             running = st->op != POP_IDLE;
@@ -1245,9 +1323,10 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
             T* const vx = ldv(&rd->x); T* const vxp = ldv(&rd->xp); T* const vg = ldv(&rd->g); T* const vgp = ldv(&rd->gp); T* const vd = ldv(&rd->drt);
             const T step = ldv(&rd->step);
             const int c_round = ldv(&rd->c_round), head = ldv(&rd->head), pending = ldv(&rd->pending), gram_cur = ldv(&rd->gram_cur);
+            const int at_start = ldv(&rd->at_start);
             if (op == POP_IDLE) continue;
             acct_bucket = (acct_bucket == -1 || acct_bucket == op) ? op : 0;
-            acct_words += words_of(op, c_round, kDataVectors);
+            acct_words += words_of(op, c_round, kDataVectors, HALO);
             double* dst = a.partials + (size_t)b * a.pstride * G + cta;
             const OBJ obj{ObjGeom<T>{a.n, a.index_offset, a.n_global, (HALO && a.xc != nullptr) ? st->halo : nullptr, st->data0, st->data1}};
             switch (op)
@@ -1258,10 +1337,17 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
                 break;
             case POP_TRIAL:
                 if constexpr (HALO) p_trial_halo<T, OBJ, 1>(obj, own, vxp, vd, step, vx, vg, nullptr, tiles, sh, phase_bits, dst, G);
-                else p_trial<T, OBJ, 1>(obj, own, vxp, vd, step, vx, vg, nullptr, sh, dst, G, a.evict_first_stores);
+                else p_trial<T, OBJ, 1>(obj, own, vxp, vd, step, nullptr, nullptr, nullptr, sh, dst, G, a.evict_first_stores);
                 break;
             case POP_RESTORE:
                 p_restore<T>(own, vxp, vgp, vx, vg);
+                break;
+            case POP_MATERIALIZE:
+                if constexpr (!HALO)
+                {
+                    if (at_start) p_restore<T>(own, vxp, vgp, vx, vg);
+                    else p_trial<T, OBJ, 2>(obj, own, vxp, vd, step, vx, vg, nullptr, sh, dst, G, a.evict_first_stores);
+                }
                 break;
             case POP_DOTS_FORM:
             case POP_DOTS_PLAIN:
@@ -1272,6 +1358,7 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
                 d.end = head;                                   // the old columns: the slots below the free slot `head`
                 d.cnt_old = form ? c_round - 1 : c_round;
                 d.new_slot = form ? head : -1;
+                d.step = step; d.at_start = at_start; d.x = vx; d.g = vg;
                 dots_geometry(d.c, d.h.BT() / (16 / (int)sizeof(T)), d.split, d.cols_per_round);
                 __syncthreads();   // sh.slots / sh.vecs may still be read by the previous problem's pass
                 {
@@ -1279,10 +1366,14 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
                     // age j (FORM: j >= 1) -> packed row of its slot in the staged block
                     if (tid < d.c && !(form && tid == 0))
                         sh.slots[tid] = (unsigned char)runs.row_of(slot_by_age(head, d.h.M, form ? tid - 1 : tid));
-                    if (tid == 0) { sh.vecs[0] = vg; sh.vecs[1] = vx; sh.vecs[2] = vgp; sh.vecs[3] = vxp; }
+                    if (tid == 0)
+                    {
+                        if (form && !HALO) { sh.vecs[0] = vd; sh.vecs[1] = vxp; sh.vecs[2] = vgp; }   // the point is rebuilt from them
+                        else { sh.vecs[0] = vg; sh.vecs[1] = vx; sh.vecs[2] = vgp; sh.vecs[3] = vxp; }
+                    }
                 }
-                if (form) p_dots<T, ROUNDS, true>(d, own, tiles, sh, phase_bits, dst, G);
-                else p_dots<T, ROUNDS, false>(d, own, tiles, sh, phase_bits, dst, G);
+                if (form) p_dots<T, OBJ, ROUNDS, true>(d, obj, own, tiles, sh, phase_bits, dst, G);
+                else p_dots<T, OBJ, ROUNDS, false>(d, obj, own, tiles, sh, phase_bits, dst, G);
                 break;
             }
             case POP_COMBINE:

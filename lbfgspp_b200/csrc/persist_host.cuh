@@ -16,7 +16,8 @@ struct lbfgs_b200_solver
     std::vector<int> ring_head, ring_ncorr, ring_gram_cur;   // ring state after the last solve (for the export below)
     std::vector<lbfgs_b200_hist*> exported;                   // column-major copies made on request (lbfgs_b200_solver_history_of)
     std::vector<char> export_fresh;
-    void* vec_slab = nullptr;             // [B][7][vec_elems] : x, xp, g, gp, drt, x_lo, g_lo
+    void* vec_slab = nullptr;             // [B][5][vec_elems] : x, xp, g, gp, drt
+    void* lo_slab = nullptr;              // [B][2][vec_elems] : x_lo, g_lo (made on the first solve of a neighbour-coupled objective)
     size_t vec_elems = 0;                 // n rounded up to a whole number of 256-byte lines
     void* d_state = nullptr;              // PState<T>[B]
     void* d_rounds = nullptr;             // PRound<T>[B]
@@ -65,13 +66,16 @@ static lbfgs_b200_status solver_minimize(lbfgs_b200_solver* s, int objective, co
     // the first trial of every search rides on the combination pass; a neighbour-coupled objective needs its neighbours' x + d,
     // which only exist on this rank when n is not sharded
     bool fuse_first_trial = true;
+    bool stored_trials = false;   // the trials store their points and the search keeps its best one in (x_lo, g_lo)
     if (auto st = with_objective<T>(ctx, objective, [&](auto tag) {
             using OBJ = decltype(tag);
             kernel = persist_kernel_for<T, OBJ>(rounds);
             fuse_first_trial = !(OBJ::kHalo && ctx->nranks > 1);
+            stored_trials = OBJ::kHalo;
             return objective_geometry<OBJ>(ctx, s->n, data0, data1, geo);
         }))
         return st;
+    if (stored_trials && !s->lo_slab) CU(ctx, pool_alloc(ctx, &s->lo_slab, (size_t)B * 2 * s->vec_elems * sizeof(T)));
 
     if (trace_host && trace_cap > s->trace_cap)
     {
@@ -88,9 +92,11 @@ static lbfgs_b200_status solver_minimize(lbfgs_b200_solver* s, int objective, co
     for (int b = 0; b < B; b++)
     {
         PState<T>& p = hs[b];
-        T* base = static_cast<T*>(s->vec_slab) + (size_t)b * 7 * s->vec_elems;
+        T* base = static_cast<T*>(s->vec_slab) + (size_t)b * 5 * s->vec_elems;
         p.x = base; p.xp = base + s->vec_elems; p.g = base + 2 * s->vec_elems; p.gp = base + 3 * s->vec_elems;
-        p.drt = base + 4 * s->vec_elems; p.x_lo = base + 5 * s->vec_elems; p.g_lo = base + 6 * s->vec_elems;
+        p.drt = base + 4 * s->vec_elems;
+        T* lo = stored_trials ? static_cast<T*>(s->lo_slab) + (size_t)b * 2 * s->vec_elems : nullptr;
+        p.x_lo = lo; p.g_lo = lo ? lo + s->vec_elems : nullptr;
         p.hist.H = static_cast<T*>(s->d_hist) + (size_t)b * s->hist_elems;
         p.hist.bt_log = s->bt_log; p.hist.M = s->M; p.hist.bstride = (int64_t)s->M * 2 * ((int64_t)1 << s->bt_log);
         T* small = static_cast<T*>(s->d_small) + (size_t)b * s->small_elems;
@@ -260,7 +266,7 @@ lbfgs_b200_status lbfgs_b200_solver_create_batch(lbfgs_b200_ctx* ctx, int64_t n,
     s->vec_elems = (((size_t)n * elem_bytes + 255) & ~size_t(255)) / elem_bytes;
     s->pstride = ((m * lb::kGramVals > 8 ? m * lb::kGramVals : 8) + 7) & ~7;
     const size_t state_bytes = (elem_bytes == 8 ? sizeof(lb::PState<double>) : sizeof(lb::PState<float>)) * (size_t)batch;
-    if (e == cudaSuccess) e = pool_alloc(ctx, (void**)&s->vec_slab, (size_t)batch * 7 * s->vec_elems * elem_bytes);
+    if (e == cudaSuccess) e = pool_alloc(ctx, (void**)&s->vec_slab, (size_t)batch * 5 * s->vec_elems * elem_bytes);
     if (e == cudaSuccess) e = pool_alloc(ctx, (void**)&s->d_hist, (size_t)batch * s->hist_elems * elem_bytes);
     if (e == cudaSuccess) e = pool_alloc(ctx, (void**)&s->d_small, (size_t)batch * s->small_elems * elem_bytes);
     if (e == cudaSuccess) e = pool_alloc(ctx, (void**)&s->d_state, state_bytes);
@@ -289,7 +295,7 @@ void lbfgs_b200_solver_destroy(lbfgs_b200_solver* s)
 {
     if (!s) return;
     if (s->ctx && s->ctx->stream) cudaStreamSynchronize(s->ctx->stream);   // the events below must not be in use
-    for (void* p : {(void*)s->vec_slab, (void*)s->d_state, (void*)s->d_rounds, (void*)s->d_ctl, (void*)s->d_partials, (void*)s->d_raw, (void*)s->d_halo,
+    for (void* p : {(void*)s->vec_slab, (void*)s->lo_slab, (void*)s->d_state, (void*)s->d_rounds, (void*)s->d_ctl, (void*)s->d_partials, (void*)s->d_raw, (void*)s->d_halo,
                     (void*)s->d_trace, (void*)s->d_hist, (void*)s->d_small})
         pool_free(s->ctx, p);
     if (s->ev0) cudaEventDestroy(s->ev0);
