@@ -297,8 +297,23 @@ public:
     // n x n matrices, only sensible for small n; returned row-major on the host.
     SmallMatrix<Scalar> final_approx_hessian() { sync_history(); return m_bfgs.dense(false); }
     SmallMatrix<Scalar> final_approx_inverse_hessian() { sync_history(); return m_bfgs.dense(true); }
+    // The same approximations as operators, at any n (preconditioning, Newton-Krylov warm starts, covariance products): OUT = B V or
+    // H V, where V holds k = V.size()/n vectors back to back (the LBFGSBatchSolver convention) and OUT receives as many.  Every pass
+    // over the S/Y history serves up to 16 vectors (BFGSMat::hessian_times).  Valid after minimize() in either loop; std::logic_error
+    // before the first one, std::invalid_argument when V.size() is not a positive multiple of n.
+    void final_approx_hessian_times(const Vector& V, Vector& OUT) { approx_times(V, OUT, false); }
+    void final_approx_inverse_hessian_times(const Vector& V, Vector& OUT) { approx_times(V, OUT, true); }
 
 private:
+    void approx_times(const Vector& V, Vector& OUT, bool inverse)
+    {
+        sync_history();
+        m_bfgs.require_history();
+        const int k = BFGSMat<Scalar>::block_count(V.size(), m_bfgs.dim());
+        if (inverse) m_bfgs.inverse_hessian_times(V, k, OUT);
+        else m_bfgs.hessian_times(V, k, OUT);
+    }
+
     // after a device-resident solve the S/Y ring lives in the solver (tiled layout): fetch a column-major copy and let m_bfgs look at it
     void sync_history()
     {

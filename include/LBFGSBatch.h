@@ -100,6 +100,25 @@ public:
     const Scalar* final_grad(int b) const { return static_cast<const Scalar*>(lbfgs_b200_solver_final_grad_of(m_solver, b)); }
     // the solver object behind the last minimize() (nullptr before the first one): accounting via lbfgs_b200_solver_profile()
     lbfgs_b200_solver* solver_handle() const { return m_solver; }
+
+    // LBFGSSolver::final_approx_hessian_times / final_approx_inverse_hessian_times for problem b of the last minimize(): OUT = B_b V
+    // or H_b V, V holding k = V.size()/n vectors back to back.  The products are those of the same problem solved alone.
+    void final_approx_hessian_times(int b, const Vector& V, Vector& OUT) { approx_times(b, V, OUT, false); }
+    void final_approx_inverse_hessian_times(int b, const Vector& V, Vector& OUT) { approx_times(b, V, OUT, true); }
+
+private:
+    void approx_times(int b, const Vector& V, Vector& OUT, bool inverse)
+    {
+        if (!m_solver) throw std::logic_error("LBFGSBatchSolver: no history yet (minimize() has not run)");
+        if (b < 0 || b >= m_B) throw std::invalid_argument("LBFGSBatchSolver: problem index out of range");
+        const int k = BFGSMat<Scalar>::block_count(V.size(), m_n);
+        lbfgs_b200_hist* h = lbfgs_b200_solver_history_of(m_solver, b);   // column-major copy of problem b's ring
+        if (!h) m_dev->check(LBFGS_B200_ERR_CUDA);
+        BFGSMat<Scalar> mat;
+        mat.borrow(*m_dev, h, m_n, m_m);
+        if (inverse) mat.inverse_hessian_times(V, k, OUT);
+        else mat.hessian_times(V, k, OUT);
+    }
 };
 
 }  // namespace LBFGSpp

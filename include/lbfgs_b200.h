@@ -220,6 +220,17 @@ void* lbfgs_b200_box_vector(lbfgs_b200_box* b, int which);               /* LBFG
     /* G[(2c)x(2c)] = sum over rows with (cls & mask) of r r', r = (y_0[i]..,s_0[i]..) by age.  WP'WP, BFGSMat.h:529-565 */ \
     lbfgs_b200_status lbfgs_b200_hist_masked_gram_##SUF(lbfgs_b200_hist*, lbfgs_b200_box*,                     \
                                                         const unsigned char* cls, int mask, T* G_host);        \
+    /* Products of the final quasi-Newton approximation with blocks of vectors (LBFGSSolver::final_approx_hessian_times /     \
+     * final_approx_inverse_hessian_times, the operator form of final_approx_hessian(), LBFGS.h:192-197 / BFGSMat.h:150-271): \
+     * V and OUT hold k column vectors (1 <= k <= 16) with leading dimensions ldv, ldo >= n; every history column and every     \
+     * column of V is read once per call.  No box workspace, any m; replicas only (a context with more than one rank is refused).     \
+     * R_host[2c][k] = [Y S]'V, rows y by age then s by age, summed in fp64 in an order that does not depend on k.           */ \
+    lbfgs_b200_status lbfgs_b200_hist_wt_dot_multi_##SUF(lbfgs_b200_hist* h, int k, const T* V, int64_t ldv,   \
+                                                         T* R_host);                                           \
+    /* OUT[:,j] = a0*V[:,j] + sum_a C[a][j]*y_a + C[c+a][j]*s_a, C_host row-major [2c][k] (y by age, then s by age); per       \
+     * element the terms are added in that order (with k = 1 the arithmetic of hist_lincomb).  OUT may be V when ldo == ldv. */ \
+    lbfgs_b200_status lbfgs_b200_hist_lincomb_multi_##SUF(lbfgs_b200_hist* h, T a0, int k, const T* V,         \
+                                                          int64_t ldv, const T* C_host, T* OUT, int64_t ldo);  \
     /* Cauchy.h:111-129: breakpoints, d = -g on movable coordinates, class bytes.                                      \
      * out5 = { #fixed, #never-bounded, #with a finite breakpoint, d.d, smallest breakpoint } */                       \
     lbfgs_b200_status lbfgs_b200_box_cauchy_breaks_##SUF(lbfgs_b200_box*, const T* x, const T* g, const T* lb, \

@@ -130,6 +130,9 @@ def _declare(lib):
         getattr(lib, "lbfgs_b200_hist_gram_" + suf).argtypes = [vp, pt, pt, pt, pt, pt]
         getattr(lib, "lbfgs_b200_hist_lincomb_" + suf).argtypes = [vp, vp, ct, vp, pt, vp, ci, vp]
         getattr(lib, "lbfgs_b200_hist_masked_gram_" + suf).argtypes = [vp, vp, vp, ci, pt]
+        if hasattr(lib, "lbfgs_b200_hist_wt_dot_multi_" + suf):   # the k-vector passes (a test double of the ABI may lack them)
+            getattr(lib, "lbfgs_b200_hist_wt_dot_multi_" + suf).argtypes = [vp, ci, vp, i64, pt]
+            getattr(lib, "lbfgs_b200_hist_lincomb_multi_" + suf).argtypes = [vp, ct, ci, vp, i64, pt, vp, i64]
         getattr(lib, "lbfgs_b200_box_cauchy_breaks_" + suf).argtypes = [vp, vp, vp, vp, vp, pt]
         getattr(lib, "lbfgs_b200_box_cauchy_sweep_" + suf).argtypes = [vp, vp, pt, pt, ct, ct, i64, i64, pt]
         getattr(lib, "lbfgs_b200_box_cauchy_build_" + suf).argtypes = [vp, vp, vp, vp, ct, ct, pt]
@@ -219,6 +222,11 @@ def _declare_driver(lib):
     lib.lbfgsb200_drv_phase_enable.argtypes = [ci]
     lib.lbfgsb200_drv_phase_report.argtypes = [C.c_char_p, ci]
     lib.lbfgsb200_drv_dense_f64.argtypes = [ci, cl, ci, ci, dp, dp, ci, dp, err, errlen]
+    # the operator form of the final approximation (csrc/driver_hessian_ops.cpp): a library built from driver.cpp alone lacks it
+    if hasattr(lib, "lbfgsb200_drv_solve_hessian_times_f64"):
+        lib.lbfgsb200_drv_solve_hessian_times_f64.argtypes = [ci, ci, cl, ci, prm, ci, dp, dp, cl, dp, dp, dp, C.POINTER(ci), err, errlen]
+        lib.lbfgsb200_drv_batch_hessian_times_f64.argtypes = [ci, ci, cl, ci, dp, ci, prm, ci, dp, cl, dp, dp, dp, err, errlen]
+        lib.lbfgsb200_drv_hist_times_f64.argtypes = [ci, cl, ci, ci, dp, dp, dp, cl, dp, dp, err, errlen]
     lib._drv_typed = True
     return lib
 
@@ -555,6 +563,19 @@ class History:
         c = self.ncorr
         return theta[0], np.array(ys[:c]), np.array(al[:c])
 
+    def wt_dot_multi(self, V, k, ldv):
+        """[Y S]'V for the k columns of the DeviceArray V (leading dimension ldv): a (2c, k) array, rows y by age then s by age."""
+        c = self.ncorr
+        R = (self.ct * max(1, 2 * c * k))()
+        self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_hist_wt_dot_multi_" + self.suf)(self.h, k, V.ptr, ldv, R))
+        return np.array(R[:2 * c * k], dtype=self.dtype).reshape(2 * c, k)
+
+    def lincomb_multi(self, a0, V, k, ldv, C_coef, OUT, ldo):
+        """OUT[:, j] = a0 V[:, j] + sum_a C[a, j] y_a + C[c + a, j] s_a (C: (2c, k), y by age then s by age)."""
+        coef = np.ascontiguousarray(C_coef, dtype=self.dtype).reshape(-1)
+        self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_hist_lincomb_multi_" + self.suf)(
+            self.h, a0, k, V.ptr, ldv, coef.ctypes.data_as(C.POINTER(self.ct)) if coef.size else None, OUT.ptr, ldo))
+
     def column(self, which, age):
         fn = self.ctx.lib.lbfgs_b200_hist_s_col if which == "s" else self.ctx.lib.lbfgs_b200_hist_y_col
         p = fn(self.h, age)
@@ -740,6 +761,40 @@ def solve_dense(objective, x0, param=None, linesearch="NocedalWright", resident=
     _checked("solve_dense", lambda *err: drv.lbfgsb200_drv_solve_dense_f64(device, objective, n, _ls_id(linesearch), C.byref(p), int(resident),
                                                                           _ptr(x), _ptr(Bm), _ptr(Hm), C.byref(niter), *err))
     return niter.value, x, Bm, Hm
+
+
+def _hessian_products(call, V, n):
+    """call(V, v_len, BV, HV, HBV, *err) runs a *_hessian_times entry point; V is (k, n) or a flat block of k n-vectors."""
+    V = np.ascontiguousarray(V, dtype=np.float64).reshape(-1)
+    shape = (V.size // n, n) if n and V.size % n == 0 else (V.size,)
+    BV, HV, HBV = (np.zeros(V.size) for _ in range(3))
+    call(V, V.size, BV, HV, HBV)
+    return BV.reshape(shape), HV.reshape(shape), HBV.reshape(shape)
+
+
+def solve_hessian_times(objective, x0, V, param=None, linesearch="NocedalWright", resident=True, device=0, lib=None):
+    """minimize(), then the final approximation as an operator (LBFGSSolver::final_approx_hessian_times /
+    final_approx_inverse_hessian_times) on the rows of V (k x n).  Returns (niter, x, B V, H V, H (B V))."""
+    drv = driver(lib)
+    x = np.array(x0, dtype=np.float64, order="C").copy()
+    n = x.size
+    p = (param if param is not None else LBFGSParam())._c()
+    niter = C.c_int(0)
+    BV, HV, HBV = _hessian_products(lambda v, vlen, bv, hv, hbv: _checked("solve_hessian_times", lambda *err: drv.lbfgsb200_drv_solve_hessian_times_f64(
+        device, objective, n, _ls_id(linesearch), C.byref(p), int(resident), _ptr(x), _ptr(v), vlen, _ptr(bv), _ptr(hv), _ptr(hbv),
+        C.byref(niter), *err)), V, n)
+    return niter.value, x, BV, HV, HBV
+
+
+def batch_hessian_times(objective, X0, b, V, param=None, linesearch="MoreThuente", device=0, lib=None):
+    """A batch (rows of X0) minimised by LBFGSBatchSolver, then problem b's final approximation as an operator on the rows of V.
+    Returns (B V, H V, H (B V))."""
+    drv = driver(lib)
+    X0 = np.ascontiguousarray(X0, dtype=np.float64)
+    B, n = X0.shape
+    p = (param if param is not None else LBFGSParam())._c()
+    return _hessian_products(lambda v, vlen, bv, hv, hbv: _checked("batch_hessian_times", lambda *err: drv.lbfgsb200_drv_batch_hessian_times_f64(
+        device, objective, n, B, _ptr(X0), _ls_id(linesearch), C.byref(p), b, _ptr(v), vlen, _ptr(bv), _ptr(hv), _ptr(hbv), *err)), V, n)
 
 
 def phase_clock(on=True):

@@ -63,12 +63,15 @@ def build_kernels(force=False, verbose=False):
     return LIB
 
 
+DRIVER_UNITS = ["driver.cpp", "driver_hessian_ops.cpp"]   # g++ units of the driver library
+
+
 def build_driver(force=False):
     srcs = _sources(CSRC, os.path.join(ROOT, "include"))
     if not force and _newer(DRV, srcs + [LIB]):
         return DRV
     cmd = [CXX, "-std=c++17", "-O2", "-fPIC", "-shared", "-Wall", "-fvisibility=hidden", "-fvisibility-inlines-hidden",
-           "-Wl,-Bsymbolic", "-o", DRV, os.path.join(CSRC, "driver.cpp"),
+           "-Wl,-Bsymbolic", "-o", DRV] + [os.path.join(CSRC, unit) for unit in DRIVER_UNITS] + [
            "-L", PKG, "-l:liblbfgs_b200.so", "-Wl,-rpath,$ORIGIN", "-pthread"]
     subprocess.run(cmd, check=True)
     return DRV

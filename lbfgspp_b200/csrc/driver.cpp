@@ -11,28 +11,15 @@
 #include <memory>
 #include <stdexcept>
 
-#include "../../include/LBFGS.h"
 #include "../../include/LBFGSB.h"
-#include "../../include/LBFGSBatch.h"
 #include "../../include/LBFGSpp/DeviceObjectives.h"
+#include "driver_common.h"
 
 using namespace LBFGSpp;
+using namespace lbfgsb200_drv;
 
 #pragma GCC visibility push(default)
 extern "C" {
-
-typedef struct
-{
-    int m;
-    double epsilon, epsilon_rel;
-    int past;
-    double delta;
-    int max_iterations;
-    int linesearch;
-    int max_submin;
-    int max_linesearch;
-    double min_step, max_step, ftol, wolfe;
-} drv_param;
 
 typedef struct
 {
@@ -49,45 +36,9 @@ typedef struct
     long h2d_bytes, d2h_bytes;
 } drv_result;
 
-enum { DRV_LS_BACKTRACKING = 0, DRV_LS_BRACKETING = 1, DRV_LS_NOCEDAL_WRIGHT = 2, DRV_LS_MORE_THUENTE = 3 };
-
 }  // extern "C"
 
 namespace {
-
-std::map<int, std::shared_ptr<Device> >& devices()
-{
-    static std::map<int, std::shared_ptr<Device> > m;
-    return m;
-}
-Device& device(int ordinal)
-{
-    std::shared_ptr<Device>& d = devices()[ordinal];
-    if (!d) d = std::make_shared<Device>(ordinal);
-    return *d;
-}
-
-// The solver types of one line-search policy; with_line_search() hands one of these to its callback.
-template <template <class> class LS>
-struct LineSearchTag
-{
-    template <class Scalar> using Solver = LBFGSSolver<Scalar, LS>;
-    template <class Scalar> using BatchSolver = LBFGSBatchSolver<Scalar, LS>;
-};
-
-// f(LineSearchTag<LS>()) for the policy of a DRV_LS_* id: the one place a line-search id becomes a type.
-template <class F>
-auto with_line_search(int ls, F f) -> decltype(f(LineSearchTag<LineSearchMoreThuente>()))
-{
-    switch (ls)
-    {
-    case DRV_LS_BACKTRACKING: return f(LineSearchTag<LineSearchBacktracking>());
-    case DRV_LS_BRACKETING: return f(LineSearchTag<LineSearchBracketing>());
-    case DRV_LS_NOCEDAL_WRIGHT: return f(LineSearchTag<LineSearchNocedalWright>());
-    case DRV_LS_MORE_THUENTE: return f(LineSearchTag<LineSearchMoreThuente>());
-    default: throw std::invalid_argument("unknown line search id");
-    }
-}
 
 // Records f of every evaluation (the reference offers the functor as its only observation point,
 // examples/example-rosenbrock-comparison.cpp:14-41) while forwarding the fused hooks when Base has them.
@@ -141,38 +92,6 @@ int guarded(drv_result* out, Body body)
     catch (const std::runtime_error& e) { set_error(out, 3, e.what()); }
     catch (const std::exception& e) { set_error(out, 4, e.what()); }
     return out->status;
-}
-
-// The entry points that report through a caller's text buffer: body()'s result, or `failed` with the exception's message in
-// err (errlen bytes, NUL-terminated).
-template <class R, class Body>
-R reported(char* err, int errlen, R failed, Body body)
-{
-    try { return body(); }
-    catch (const std::exception& e)
-    {
-        if (err && errlen > 0) { std::strncpy(err, e.what(), size_t(errlen) - 1); err[errlen - 1] = 0; }
-        return failed;
-    }
-}
-
-template <class Scalar>
-LBFGSParam<Scalar> to_param(const drv_param* q)
-{
-    LBFGSParam<Scalar> p;
-    p.m = q->m;
-    p.epsilon = Scalar(q->epsilon);
-    p.epsilon_rel = Scalar(q->epsilon_rel);
-    p.past = q->past;
-    p.delta = Scalar(q->delta);
-    p.max_iterations = q->max_iterations;
-    p.linesearch = q->linesearch;
-    p.max_linesearch = q->max_linesearch;
-    p.min_step = Scalar(q->min_step);
-    p.max_step = Scalar(q->max_step);
-    p.ftol = Scalar(q->ftol);
-    p.wolfe = Scalar(q->wolfe);
-    return p;
 }
 
 template <class Scalar>

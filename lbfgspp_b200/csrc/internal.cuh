@@ -207,6 +207,7 @@ struct lbfgs_b200_hist
     int pending = -1;  // physical slot of the newest pair whose Gram row/column has not been folded in yet
     int head = 0;   // physical slot the next pair is written to
     int ncorr = 0;  // valid pairs (<= m)
+    void* multi = nullptr;  // scratch of the k-vector passes (hist_wt_dot_multi / hist_lincomb_multi), made on first use
     // physical slot of the pair with the given age (0 = newest)
     int slot(int age) const { return ((head - 1 - age) % M + M) % M; }
     template <class T> T* s_col(int phys) const { return static_cast<T*>(S) + (int64_t)phys * ld; }

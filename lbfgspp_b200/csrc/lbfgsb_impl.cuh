@@ -86,6 +86,21 @@ template <class T> static lbfgs_b200_status do_hist_gram(lbfgs_b200_hist* h, T* 
     return LBFGS_B200_OK;
 }
 
+// OUT[:,j] = a0*V[:,j] + sum_a C[a][j]*y_a + C[c+a][j]*s_a on the rows of (cls, mask); coef_dev: device [2c][k] (see k_hist_lincomb)
+template <class T>
+static lbfgs_b200_status launch_lincomb(lbfgs_b200_hist* h, T a0, int k, const T* V, int64_t ldv, const T* coef_dev, const unsigned char* cls,
+                                        int mask, T* out, int64_t ldo)
+{
+    lbfgs_b200_ctx* ctx = h->ctx;
+    LincombArgs<T> a{};
+    a.n = h->n; a.ld = h->ld; a.ldv = ldv; a.ldo = ldo; a.S = static_cast<const T*>(h->S); a.Y = static_cast<const T*>(h->Y);
+    a.V = V; a.a0 = a0; a.coef = coef_dev; a.cls = cls; a.mask = (unsigned char)mask; a.out = out; a.c = h->ncorr; a.k = k;
+    fill_slots<T>(h, a.slots);
+    if (k == 1) k_hist_lincomb<T, 1><<<grid_for(ctx, h->n * 4, 4), kThreads, 0, ctx->stream>>>(a);
+    else k_hist_lincomb<T, kMaxK><<<grid_for(ctx, h->n * 4, 4), kThreads, 0, ctx->stream>>>(a);
+    return post_launch(ctx, "k_hist_lincomb");
+}
+
 template <class T>
 static lbfgs_b200_status do_hist_lincomb(lbfgs_b200_hist* h, lbfgs_b200_box* b, T a0, const T* v0, const T* coef_host,
                                          const unsigned char* cls, int mask, T* out)
@@ -101,12 +116,90 @@ static lbfgs_b200_status do_hist_lincomb(lbfgs_b200_hist* h, lbfgs_b200_box* b, 
         CU(ctx, cudaMemcpyAsync(coef_dev, coef_host, sizeof(T) * 2 * c, cudaMemcpyHostToDevice, ctx->stream));
         CU(ctx, cudaStreamSynchronize(ctx->stream));   // coef_host may be a stack array of the caller
     }
-    LincombArgs<T> a{};
-    a.n = h->n; a.ld = h->ld; a.S = static_cast<const T*>(h->S); a.Y = static_cast<const T*>(h->Y);
-    a.v0 = v0; a.a0 = a0; a.coef = coef_dev; a.cls = cls; a.mask = (unsigned char)mask; a.out = out; a.c = c;
+    return launch_lincomb<T>(h, a0, 1, v0, h->n, coef_dev, cls, mask, out, h->n);
+}
+
+// ------------------------------------------------------------------------------------------------ k-vector passes (compact B / H products)
+// Grid of k_hist_wt_dot_multi: a function of n and the device only, so that a dot's summation order does not depend on k.
+static int wt_multi_grid(const lbfgs_b200_hist* h)
+{
+    const int64_t nstrips = (h->n + kWtRows - 1) / kWtRows;
+    return (int)(nstrips < 4 * h->ctx->sm_count ? nstrips : 4 * h->ctx->sm_count);
+}
+
+// The history's scratch for the k-vector passes, made on first use: partials [grid][2m*kMaxK] | result [2m*kMaxK] |
+// coefficients [2m*kMaxK] (doubles; the coefficients are stored as T)
+static lbfgs_b200_status multi_scratch(lbfgs_b200_hist* h, double** partials, double** result, void** coef)
+{
+    lbfgs_b200_ctx* ctx = h->ctx;
+    const size_t vals = (size_t)2 * h->m * kMaxK;
+    if (!h->multi)
+    {
+        const cudaError_t e = pool_alloc(ctx, &h->multi, sizeof(double) * vals * (wt_multi_grid(h) + 2));
+        if (e != cudaSuccess)
+            return fail(ctx, e == cudaErrorMemoryAllocation ? LBFGS_B200_ERR_ALLOC : LBFGS_B200_ERR_CUDA, "history scratch: %s", cudaGetErrorString(e));
+    }
+    double* base = static_cast<double*>(h->multi);
+    *partials = base;
+    *result = base + vals * wt_multi_grid(h);
+    *coef = base + vals * (wt_multi_grid(h) + 1);
+    return LBFGS_B200_OK;
+}
+
+template <class T> static lbfgs_b200_status multi_check(lbfgs_b200_hist* h, int k, int64_t ldv, const char* what)
+{
+    if (auto st = hist_check<T>(h)) return st;
+    lbfgs_b200_ctx* ctx = h->ctx;
+    REQUIRE(ctx, k >= 1 && k <= kMaxK, "%s: k must be in 1..%d (got %d)", what, kMaxK, k);
+    REQUIRE(ctx, ldv >= h->n, "%s: leading dimension %lld is smaller than n = %lld", what, (long long)ldv, (long long)h->n);
+    REQUIRE(ctx, ctx->nranks == 1, "%s: replicas only, not for a context with %d ranks", what, ctx->nranks);
+    return LBFGS_B200_OK;
+}
+
+// R_host[2c][k] = [Y S]' V  (rows: y by age, then s by age)
+template <class T> static lbfgs_b200_status do_hist_wt_dot_multi(lbfgs_b200_hist* h, int k, const T* V, int64_t ldv, T* R_host)
+{
+    if (auto st = multi_check<T>(h, k, ldv, "hist_wt_dot_multi")) return st;
+    lbfgs_b200_ctx* ctx = h->ctx;
+    REQUIRE(ctx, V && R_host, "hist_wt_dot_multi: NULL argument");
+    const int c = h->ncorr, w = 2 * c;
+    if (c == 0) return LBFGS_B200_OK;
+    double *partials, *result;
+    void* coef;
+    if (auto st = multi_scratch(h, &partials, &result, &coef)) return st;
+    WtDotMultiArgs<T> a{};
+    a.n = h->n; a.ld = h->ld; a.ldv = ldv; a.S = static_cast<const T*>(h->S); a.Y = static_cast<const T*>(h->Y); a.V = V;
+    a.c = c; a.k = k; a.partials = partials; a.ticket = ctx->rb.ticket; a.result = result;
     fill_slots<T>(h, a.slots);
-    k_hist_lincomb<T><<<grid_for(ctx, h->n * 4, 4), kThreads, 0, ctx->stream>>>(a);
-    return post_launch(ctx, "k_hist_lincomb");
+    const size_t smem = (size_t)(w + k) * kWtPitch * sizeof(T);
+    if (smem > 48 * 1024) CU(ctx, cudaFuncSetAttribute(k_hist_wt_dot_multi<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_hist_wt_dot_multi<T><<<wt_multi_grid(h), kThreads, smem, ctx->stream>>>(a);
+    if (auto st = post_launch(ctx, "k_hist_wt_dot_multi")) return st;
+    std::vector<double> tmp((size_t)w * k);
+    CU(ctx, cudaMemcpyAsync(tmp.data(), result, sizeof(double) * w * k, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(ctx, cudaStreamSynchronize(ctx->stream));
+    for (int e = 0; e < w * k; e++) R_host[e] = (T)tmp[(size_t)e];
+    return LBFGS_B200_OK;
+}
+
+template <class T>
+static lbfgs_b200_status do_hist_lincomb_multi(lbfgs_b200_hist* h, T a0, int k, const T* V, int64_t ldv, const T* C_host, T* OUT, int64_t ldo)
+{
+    if (auto st = multi_check<T>(h, k, ldv, "hist_lincomb_multi")) return st;
+    lbfgs_b200_ctx* ctx = h->ctx;
+    REQUIRE(ctx, V && OUT, "hist_lincomb_multi: NULL argument");
+    REQUIRE(ctx, ldo >= h->n, "hist_lincomb_multi: leading dimension %lld is smaller than n = %lld", (long long)ldo, (long long)h->n);
+    const int c = h->ncorr;
+    double *partials, *result;
+    void* coef;
+    if (auto st = multi_scratch(h, &partials, &result, &coef)) return st;
+    if (c > 0)
+    {
+        REQUIRE(ctx, C_host != nullptr, "hist_lincomb_multi: NULL argument");
+        CU(ctx, cudaMemcpyAsync(coef, C_host, sizeof(T) * 2 * c * k, cudaMemcpyHostToDevice, ctx->stream));
+        CU(ctx, cudaStreamSynchronize(ctx->stream));   // C_host may be a stack array of the caller
+    }
+    return launch_lincomb<T>(h, a0, k, V, ldv, static_cast<const T*>(coef), nullptr, 0, OUT, ldo);
 }
 
 // G[(2c)x(2c)] over rows with (cls & mask) != 0, ordering [Y by age, S by age]   (WP'WP of BFGSMat.h:529-565)
@@ -404,6 +497,11 @@ void* lbfgs_b200_box_vector(lbfgs_b200_box* b, int which)
     lbfgs_b200_status lbfgs_b200_hist_masked_gram_##SUF(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls,    \
                                                         int mask, T* G_host)                                                \
     { return do_hist_masked_gram<T>(h, b, cls, mask, G_host); }                                                             \
+    lbfgs_b200_status lbfgs_b200_hist_wt_dot_multi_##SUF(lbfgs_b200_hist* h, int k, const T* V, int64_t ldv, T* R_host)     \
+    { return do_hist_wt_dot_multi<T>(h, k, V, ldv, R_host); }                                                               \
+    lbfgs_b200_status lbfgs_b200_hist_lincomb_multi_##SUF(lbfgs_b200_hist* h, T a0, int k, const T* V, int64_t ldv,         \
+                                                          const T* C_host, T* OUT, int64_t ldo)                             \
+    { return do_hist_lincomb_multi<T>(h, a0, k, V, ldv, C_host, OUT, ldo); }                                                \
     lbfgs_b200_status lbfgs_b200_box_cauchy_breaks_##SUF(lbfgs_b200_box* b, const T* x, const T* g, const T* lb,            \
                                                          const T* ub, T* out5_host)                                         \
     { return do_box_cauchy_breaks<T>(b, x, g, lb, ub, out5_host); }                                                         \

@@ -6,6 +6,7 @@
 //   W'(mask o v)       -> k_gram_dots on the masked vector            (apply_WtPv, compute_FtBAb; BFGSMat.h:382-433,486-522)
 //   (W_P)'(W_P)        -> k_masked_gram                                (solve_PtBP; BFGSMat.h:529-565)
 //   W_P * coef         -> k_hist_lincomb                               (apply_PtWMv, apply_PtBQv; BFGSMat.h:435-478,570-615)
+// (k_hist_lincomb and k_hist_wt_dot_multi also serve blocks of up to 16 vectors: the operator form of the final approximation)
 // The generalized Cauchy point (Cauchy.h:86-284) is sort + prefix sums: after sorting the breakpoints, the state of the
 // reference's sequential sweep just after crossing sorted position k is a function of prefix sums over positions <= k
 // (sum g^2, sum g*w, sum t*g*w with w = row of W), so all segments are examined in parallel and the first one whose
@@ -473,30 +474,37 @@ template <class T> __global__ void __launch_bounds__(kThreads) k_cauchy_build(in
     grid_reduce_mixed<2>(acc, rb, 0u);
 }
 
-// ---------------------------------------------------------------- history primitives on masked rows
-// out_i = a0*v0_i + sum_j cy_j*y_j[i] + cs_j*s_j[i]   for rows with (cls_i & mask) != 0 (cls == nullptr: all rows);
-// rows outside the mask are left untouched.
+// ---------------------------------------------------------------- history primitives on blocks of k vectors
+// Both passes read every history column once per call, whatever k (1 <= k <= kMaxK): one product with the compact form of B or H
+// moves w*n*(4c + 3k) bytes instead of w*n*(4c + 3)*k for k single-vector passes.
+constexpr int kMaxK = 16;
+
+// OUT[:,j] = a0*V[:,j] + sum_a C[a][j]*y_a + C[c+a][j]*s_a   (C row-major [2c][k], y then s by age; V == nullptr: no a0 term)
+// for rows with (cls_i & mask) != 0 (cls == nullptr: all rows); rows outside the mask are left untouched.  Per element the terms are
+// added in the order a0*v, y by age, s by age; with k = 1 this is the L-BFGS-B combination (apply_PtWMv / apply_PtBQv / solve_PtBP).
 template <class T> struct LincombArgs
 {
-    int64_t n, ld;
+    int64_t n, ld, ldv, ldo;
     const T* S;
     const T* Y;
-    const T* v0;       // may be nullptr
+    const T* V;        // may be nullptr
     T a0;
-    const T* coef;     // device [2c]: cy (by age) then cs
+    const T* coef;     // device [2c][k]
     const unsigned char* cls;
     unsigned char mask;
     T* out;
-    int c;
+    int c, k;
     unsigned char slots[kMaxM];
 };
 
-template <class T> __global__ void __launch_bounds__(kThreads) k_hist_lincomb(LincombArgs<T> a)
+// KMAX: 1 (the L-BFGS-B pass) or kMaxK; the k running sums of an element stay in registers
+template <class T, int KMAX> __global__ void __launch_bounds__(kThreads) k_hist_lincomb(LincombArgs<T> a)
 {
-    __shared__ T s_coef[kMaxW];
+    __shared__ T s_coef[kMaxW * KMAX];
     __shared__ const T* s_y[kMaxM];
     __shared__ const T* s_s[kMaxM];
-    for (int j = threadIdx.x; j < 2 * a.c; j += kThreads) s_coef[j] = a.coef[j];
+    const int k = KMAX == 1 ? 1 : a.k;
+    for (int e = threadIdx.x; e < 2 * a.c * k; e += kThreads) s_coef[e] = a.coef[e];
     for (int j = threadIdx.x; j < a.c; j += kThreads)
     {
         s_y[j] = a.Y + (int64_t)a.slots[j] * a.ld;
@@ -506,11 +514,116 @@ template <class T> __global__ void __launch_bounds__(kThreads) k_hist_lincomb(Li
     for (int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x; i < a.n; i += (int64_t)gridDim.x * kThreads)
     {
         if (a.cls && !(a.cls[i] & a.mask)) continue;
-        T r = a.v0 ? a.a0 * a.v0[i] : T(0);
-        for (int j = 0; j < a.c; j++) r += s_coef[j] * s_y[j][i];
-        for (int j = 0; j < a.c; j++) r += s_coef[a.c + j] * s_s[j][i];
-        a.out[i] = r;
+        T r[KMAX];
+#pragma unroll
+        for (int j = 0; j < KMAX; j++)
+            if (j < k) r[j] = a.V ? a.a0 * a.V[j * a.ldv + i] : T(0);
+        for (int q = 0; q < a.c; q++)
+        {
+            const T yq = s_y[q][i];
+#pragma unroll
+            for (int j = 0; j < KMAX; j++)
+                if (j < k) r[j] += s_coef[q * k + j] * yq;
+        }
+        for (int q = 0; q < a.c; q++)
+        {
+            const T sq = s_s[q][i];
+#pragma unroll
+            for (int j = 0; j < KMAX; j++)
+                if (j < k) r[j] += s_coef[(a.c + q) * k + j] * sq;
+        }
+#pragma unroll
+        for (int j = 0; j < KMAX; j++)
+            if (j < k) a.out[j * a.ldo + i] = r[j];
     }
+}
+
+// R[2c][k] = [Y S]' V  (y then s by age), summed in fp64.  A CTA stages a strip of kWtRows rows of the 2c history columns and of the
+// k vectors in shared memory (every element read once from HBM) and thread (g, j) accumulates the dots of vector j = tid % k with
+// columns g, g + G, ... (G = kThreads / k groups).  Strips go to CTAs round robin and the grid depends on n only, so a dot's sum
+// (over a CTA's strips in order, then over CTAs in order by the last CTA) does not depend on k: column j of a k = 16 call is
+// bit-identical to the k = 1 call on that column alone.
+constexpr int kWtRows = 128;
+constexpr int kWtPitch = kWtRows + 1;   // row pitch of the staged strip: the k threads reading one row index hit k different banks
+template <class T> struct WtDotMultiArgs
+{
+    int64_t n, ld, ldv;
+    const T* S;
+    const T* Y;
+    const T* V;
+    int c, k;
+    double* partials;   // [grid][2c*k]
+    unsigned* ticket;
+    double* result;     // [2c*k]
+    unsigned char slots[kMaxM];
+};
+
+template <class T> __global__ void __launch_bounds__(kThreads) k_hist_wt_dot_multi(WtDotMultiArgs<T> a)
+{
+    extern __shared__ __align__(16) unsigned char wt_smem[];
+    T* rows = reinterpret_cast<T*>(wt_smem);   // [2c + k][kWtPitch]: y by age, s by age, then the k vectors
+    __shared__ const T* s_col[kMaxW + kMaxK];
+    __shared__ bool s_last;
+    const int w = 2 * a.c, k = a.k, nrows = w + k, tid = threadIdx.x;
+    for (int q = tid; q < nrows; q += kThreads)
+        s_col[q] = q < a.c ? a.Y + (int64_t)a.slots[q] * a.ld : q < w ? a.S + (int64_t)a.slots[q - a.c] * a.ld : a.V + (int64_t)(q - w) * a.ldv;
+    const int groups = kThreads / k, j = tid % k, g = tid / k;
+    const bool active = g < groups;
+    constexpr int kMaxOwn = kMaxW / (kThreads / kMaxK);   // columns per thread: ceil(2c / G) <= 8 with G >= 16
+    double acc[kMaxOwn];
+#pragma unroll
+    for (int q = 0; q < kMaxOwn; q++) acc[q] = 0.0;
+    __syncthreads();
+    const int64_t nstrips = (a.n + kWtRows - 1) / kWtRows;
+    for (int64_t strip = blockIdx.x; strip < nstrips; strip += gridDim.x)
+    {
+        const int64_t r0 = strip * kWtRows;
+        for (int t = tid; t < nrows * kWtRows; t += kThreads)
+        {
+            const int q = t / kWtRows, r = t % kWtRows;
+            const int64_t i = r0 + r;
+            rows[q * kWtPitch + r] = i < a.n ? __ldcs(s_col[q] + i) : T(0);
+        }
+        __syncthreads();
+        if (active)
+        {
+            // one running sum per owned column over the strip's rows in order; the vector's element is read once per row
+            const T* vr = rows + (w + j) * kWtPitch;
+            double s[kMaxOwn];
+#pragma unroll
+            for (int q = 0; q < kMaxOwn; q++) s[q] = 0.0;
+            for (int r = 0; r < kWtRows; r++)
+            {
+                const double v = (double)vr[r];
+#pragma unroll
+                for (int q = 0; q < kMaxOwn; q++)
+                    if (g + q * groups < w) s[q] += (double)rows[(g + q * groups) * kWtPitch + r] * v;
+            }
+#pragma unroll
+            for (int q = 0; q < kMaxOwn; q++) acc[q] += s[q];
+        }
+        __syncthreads();
+    }
+    if (active)
+#pragma unroll
+        for (int q = 0; q < kMaxOwn; q++)
+        {
+            const int col = g + q * groups;
+            if (col < w) a.partials[(size_t)blockIdx.x * (w * k) + col * k + j] = acc[q];
+        }
+    __threadfence();
+    __syncthreads();
+    if (tid == 0) s_last = (atomicAdd(a.ticket, 1u) == gridDim.x - 1);
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    for (int e = tid; e < w * k; e += kThreads)
+    {
+        double t = 0.0;
+        for (unsigned b = 0; b < gridDim.x; b++) t += __ldcg(&a.partials[(size_t)b * (w * k) + e]);
+        a.result[e] = t;
+    }
+    if (tid == 0) *a.ticket = 0u;
 }
 
 // G[a][b] = sum over masked rows of r_i[a]*r_i[b],  r_i = (y_0[i]..y_{c-1}[i], s_0[i]..s_{c-1}[i]) by age.
