@@ -320,6 +320,33 @@ lbfgs_b200_status lbfgs_b200_solver_minimize_batch_f32(lbfgs_b200_solver* s, int
                                                        int64_t ldd, const lbfgs_b200_param* prm, int line_search, float* x_inout,
                                                        int64_t ldx, lbfgs_b200_outcome* outs);
 
+/* ---------------------------------------------------------------- small-batch solve (built-in objectives)
+ * Many independent small problems in ONE ordinary launch: one thread block per problem runs that problem's whole minimize()
+ * (reference LBFGS.h:78-173) in its own shared memory, with the device-resident solve's per-problem state machine (same line
+ * searches, stopping rules, curvature gate and outcomes).  No grid-wide synchronisation: B is limited only by device memory for
+ * X (and G).  Every problem's sums are taken in an order that depends on n only (32 threads per block up to n = 128, 128 above), so
+ * a problem's result is bit-identical whatever B is and wherever it sits in the batch; it equals LBFGSSolver's result to rounding
+ * (the sums are associated differently), not bit for bit.  One rank only.
+ * Shared memory of one block, with M = m + 1, p = round_up(max(6m, 8), 8), e = elem_bytes and N = round_up(n, 4):
+ *     e*N*(5 + 2M + 2*[chained Rosenbrock, tridiagonal quadratic: stored trials] + 2*[tridiagonal quadratic: data])
+ *   + 2048 (problem state) + 8*5p (sums) + a16(e*(2M + 4 + 6M^2)) (ys, alpha, theta, Gram matrices) + a16(e*(2m^2 + 6m + 2)) (recursion)
+ * where a16 rounds up to a multiple of 16; it must not exceed 232448 bytes (227 KB, the per-block limit of sm_90).  For fp64 paired
+ * Rosenbrock that is 152 bytes per coordinate at m = 6 (n <= 1480) and 216 at m = 10 (n <= 1016); at large m the Gram matrices
+ * alone exceed the limit. */
+/* largest n that fits one block's shared memory for (m, precision, objective): a multiple of 4, 0 if none.  Pure host function. */
+int64_t lbfgs_b200_small_max_n(int m, int elem_bytes, int objective);
+/* B independent problems of n coordinates, one block each.  X: B device vectors ldx >= n elements apart (start points in,
+ * solutions out); G (nullable): the final gradients, same layout; data0/data1 (as the objective needs): problem b's at data + b*ldd
+ * (ldd = 0: shared by all problems); outs_host[B]: status / niter / nfev / fx / gnorm / rounds exactly as
+ * lbfgs_b200_solver_minimize_batch reports them.  LBFGS_B200_ERR_INVALID for n > lbfgs_b200_small_max_n, B < 1, ldx < n,
+ * past > 64 or a context with more than one rank.  Synchronises. */
+lbfgs_b200_status lbfgs_b200_small_minimize_f64(lbfgs_b200_ctx* ctx, int objective, const double* data0, const double* data1, int64_t ldd,
+                                                int64_t n, int64_t B, const lbfgs_b200_param* prm, int line_search,
+                                                double* X, int64_t ldx, double* G, lbfgs_b200_outcome* outs_host);
+lbfgs_b200_status lbfgs_b200_small_minimize_f32(lbfgs_b200_ctx* ctx, int objective, const float* data0, const float* data1, int64_t ldd,
+                                                int64_t n, int64_t B, const lbfgs_b200_param* prm, int line_search,
+                                                float* X, int64_t ldx, float* G, lbfgs_b200_outcome* outs_host);
+
 #ifdef __cplusplus
 }
 #endif

@@ -153,6 +153,12 @@ def _declare(lib):
     for suf in ("f64", "f32"):
         getattr(lib, "lbfgs_b200_solver_minimize_" + suf).argtypes = [vp, ci, vp, vp, vp, ci, vp, vp, C.c_longlong, vp]
         getattr(lib, "lbfgs_b200_solver_minimize_batch_" + suf).argtypes = [vp, ci, vp, vp, i64, vp, ci, vp, i64, vp]
+    # small-batch solve (one thread block per problem; a test double of the ABI may lack it)
+    if hasattr(lib, "lbfgs_b200_small_max_n"):
+        lib.lbfgs_b200_small_max_n.restype = i64
+        lib.lbfgs_b200_small_max_n.argtypes = [ci, ci, ci]
+        for suf in ("f64", "f32"):
+            getattr(lib, "lbfgs_b200_small_minimize_" + suf).argtypes = [vp, ci, vp, vp, i64, i64, i64, vp, ci, vp, i64, vp, vp]
     lib._typed = True
     return lib
 
@@ -166,6 +172,11 @@ class _DrvParam(C.Structure):
 
 class _BatchItem(C.Structure):
     _fields_ = [("status", C.c_int), ("niter", C.c_int), ("nfev", C.c_long), ("fx", C.c_double), ("gnorm", C.c_double)]
+
+
+class _SmallItem(C.Structure):
+    _fields_ = [("code", C.c_int), ("kind", C.c_int), ("niter", C.c_int), ("nfev", C.c_long), ("fx", C.c_double), ("gnorm", C.c_double),
+                ("rounds", C.c_long)]
 
 
 class _DrvResult(C.Structure):
@@ -227,6 +238,11 @@ def _declare_driver(lib):
         lib.lbfgsb200_drv_solve_hessian_times_f64.argtypes = [ci, ci, cl, ci, prm, ci, dp, dp, cl, dp, dp, dp, C.POINTER(ci), err, errlen]
         lib.lbfgsb200_drv_batch_hessian_times_f64.argtypes = [ci, ci, cl, ci, dp, ci, prm, ci, dp, cl, dp, dp, dp, err, errlen]
         lib.lbfgsb200_drv_hist_times_f64.argtypes = [ci, cl, ci, ci, dp, dp, dp, cl, dp, dp, err, errlen]
+    # the small-batch solve (csrc/driver_small_batch.cpp)
+    if hasattr(lib, "lbfgsb200_drv_small_batch_f64"):
+        for suf, pt in (("f64", dp), ("f32", fp)):
+            getattr(lib, "lbfgsb200_drv_small_batch_" + suf).argtypes = [ci, ci, cl, cl, pt, pt, pt, cl, ci, prm, pt, pt,
+                                                                         C.POINTER(_SmallItem), err, errlen]
     lib._drv_typed = True
     return lib
 
@@ -795,6 +811,36 @@ def batch_hessian_times(objective, X0, b, V, param=None, linesearch="MoreThuente
     p = (param if param is not None else LBFGSParam())._c()
     return _hessian_products(lambda v, vlen, bv, hv, hbv: _checked("batch_hessian_times", lambda *err: drv.lbfgsb200_drv_batch_hessian_times_f64(
         device, objective, n, B, _ptr(X0), _ls_id(linesearch), C.byref(p), b, _ptr(v), vlen, _ptr(bv), _ptr(hv), _ptr(hbv), *err)), V, n)
+
+
+def small_max_n(m, objective, dtype=np.float64):
+    """Largest n of a problem the small-batch solve takes for history size m and built-in objective `objective` (0 if none)."""
+    return int(abi().lbfgs_b200_small_max_n(int(m), np.dtype(dtype).itemsize, int(objective)))
+
+
+def solve_small_batch(objective, X0, param=None, linesearch="MoreThuente", dtype=np.float64, data0=None, data1=None, ldd=0,
+                      want_grad=False, device=0, lib=None):
+    """B independent small problems (rows of X0) minimised by LBFGSSmallBatchSolver (include/LBFGSSmallBatch.h): one launch, one
+    thread block per problem.  data0/data1: one vector shared by all problems (ldd = 0) or problem b's at offset b*ldd of a flat
+    array.  Returns (list of dicts with status / msg-free outcome, X, G or None).  A refused call (n above small_max_n, odd n for
+    paired Rosenbrock, ...) raises ValueError; other failures RuntimeError."""
+    drv = driver(lib)
+    X0 = np.ascontiguousarray(X0, dtype=dtype)
+    B, n = X0.shape
+    p = (param if param is not None else LBFGSParam())._c()
+    d0 = None if data0 is None else np.ascontiguousarray(data0, dtype=dtype).reshape(-1)
+    d1 = None if data1 is None else np.ascontiguousarray(data1, dtype=dtype).reshape(-1)
+    X = np.empty_like(X0)
+    G = np.empty_like(X0) if want_grad else None
+    items = (_SmallItem * B)()
+    fn = drv.lbfgsb200_drv_small_batch_f32 if np.dtype(dtype) == np.float32 else drv.lbfgsb200_drv_small_batch_f64
+    err = C.create_string_buffer(256)
+    r = fn(device, objective, n, B, _ptr(X0), _ptr(d0), _ptr(d1), int(ldd), _ls_id(linesearch), C.byref(p), _ptr(X), _ptr(G), items, err, len(err))
+    if r < 0:
+        raise (ValueError if r == -1 else RuntimeError)("solve_small_batch failed: %s" % err.value.decode())
+    res = [dict(status=STATUS_NAMES[it.kind], code=it.code, niter=it.niter, nfev=it.nfev, fx=it.fx, gnorm=it.gnorm, rounds=it.rounds)
+           for it in items]
+    return res, X, G
 
 
 def phase_clock(on=True):

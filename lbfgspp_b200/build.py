@@ -40,7 +40,7 @@ def _sources(*dirs, exts=(".cu", ".cuh", ".h", ".cpp", ".hpp")):
     return out
 
 
-KERNEL_UNITS = ["lbfgs_b200.cu", "persist_f64.cu", "persist_f32.cu"]   # compiled in parallel, linked into one library
+KERNEL_UNITS = ["lbfgs_b200.cu", "persist_f64.cu", "persist_f32.cu", "small_batch.cu"]   # compiled in parallel, linked into one library
 
 
 def build_kernels(force=False, verbose=False):
@@ -63,7 +63,7 @@ def build_kernels(force=False, verbose=False):
     return LIB
 
 
-DRIVER_UNITS = ["driver.cpp", "driver_hessian_ops.cpp"]   # g++ units of the driver library
+DRIVER_UNITS = ["driver.cpp", "driver_hessian_ops.cpp", "driver_small_batch.cpp"]   # g++ units of the driver library
 
 
 def build_driver(force=False):

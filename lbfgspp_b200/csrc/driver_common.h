@@ -10,6 +10,7 @@
 
 #include "../../include/LBFGS.h"
 #include "../../include/LBFGSBatch.h"
+#include "../../include/LBFGSSmallBatch.h"
 
 extern "C" {
 
@@ -53,6 +54,7 @@ struct LineSearchTag
 {
     template <class Scalar> using Solver = LBFGSSolver<Scalar, LS>;
     template <class Scalar> using BatchSolver = LBFGSBatchSolver<Scalar, LS>;
+    template <class Scalar> using SmallBatchSolver = LBFGSSmallBatchSolver<Scalar, LS>;
 };
 
 // f(LineSearchTag<LS>()) for the policy of a DRV_LS_* id: the one place a line-search id becomes a type.

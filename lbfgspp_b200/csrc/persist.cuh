@@ -40,75 +40,18 @@
 // are in flight.  DESIGN.md section 10 has what was measured about the limits of this arrangement.
 #pragma once
 
-#include "../../include/LBFGSpp/LoopRules.h"
+#include "problem_machine.cuh"
 
 namespace lb {
 
-constexpr int kMaxPast = 64;
 constexpr int kPThreads = kGramMaxThreads;   // 768: one CTA per SM
 constexpr int kPWarps = kPThreads / 32;
 constexpr int kPStageBytes = kGramStages * 4 * kGramTE * 8;   // dynamic shared memory of the kernel: 196608 bytes
 constexpr int kPMaxStages = 4;
 constexpr int kPCache = 4;                   // problems whose leader-side state is kept in shared memory
 
-enum { POP_IDLE = 0, POP_FIRST = 1, POP_TRIAL = 2, POP_DOTS_FORM = 3, POP_DOTS_PLAIN = 4, POP_COMBINE = 5, POP_COMBINE_TRIAL = 6, POP_RESTORE = 7,
-       POP_MATERIALIZE = 8 };
 constexpr int kPOps = 10;   // accounting slots (ops + the "mixed" bucket 0; 9 unused, kept for the solver_profile ABI)
 constexpr int kPGramScratch = 1024;   // doubles
-
-// ---- the S/Y history of the solve: tiled layout ---------------------------------------------------------------------------------
-// H[block][slot][S|Y][BT]: all ring slots of one block of BT coordinates lie next to each other (BT = the largest power of two for
-// which two stages of 2m+4 rows fit the kernel's shared memory: 512 for fp64 m = 10).  A pass over a tile then needs the right-hand
-// vectors plus ONE or TWO bulk copies of 8..90 KB for all history columns (the live slots form a cyclic range of the ring), instead
-// of one 4 KB copy per column: measured, the per-copy cost of 22 separate copies was ~15 % of the combination pass, and 42 copies of
-// 2 KB at m = 20 made it 2.8x slower per byte.  The new pair of an iteration is written as one 2*BT run per block.
-template <class T> struct PHist
-{
-    T* H;
-    int bt_log, M;
-    int64_t bstride;      // elements per block: M * 2 * BT
-    __device__ __forceinline__ int BT() const { return 1 << bt_log; }
-    __device__ __forceinline__ T* s_at(int slot, int64_t i) const { return H + (i >> bt_log) * bstride + ((int64_t)slot << (bt_log + 1)) + (i & (BT() - 1)); }
-    __device__ __forceinline__ T* y_at(int slot, int64_t i) const { return s_at(slot, i) + BT(); }
-};
-
-// ---- per-problem state (device memory; the leader CTA's working copy) ----------------------------------------------------------
-template <class T> struct PState
-{
-    // vectors (rotate by pointer swap); x_lo, g_lo: neighbour-coupled objectives only (nullptr otherwise)
-    T *x, *xp, *g, *gp, *drt, *x_lo, *g_lo;
-    // history storage (fixed for the duration of the kernel: other CTAs read these fields with ordinary loads)
-    PHist<T> hist;              // the S/Y ring, tiled (see PHist)
-    T *ys, *alpha, *theta;
-    T *SY[2], *YY[2], *SS[2];
-    const T *data0, *data1;
-    double* raw;               // [pstride] reduced values of the last round
-    double* halo;              // kHaloDoubles (neighbour-coupled objectives under n-sharding)
-    // ring geometry
-    int head, ncorr, M, m, gram_cur, pending;
-    // what the next round does
-    int op, c_round;
-    // options (LBFGSParam)
-    T epsilon, epsilon_rel, delta, max_step;
-    int past, max_iterations, fuse_first_trial;
-    LBFGSpp::LineSearchOptions<T> ls_opt;
-    // line-search state
-    LBFGSpp::RunTimeCore<T> ls;
-    LBFGSpp::SearchRecord<T> rec;   // fx, dg, gg, xx of the current point
-    // iteration scalars.  step: the trial to evaluate, or (objectives without neighbour coupling) the step of the point (x, g)
-    // stand for while they are implied; step_kept: the step of the search's kept trial; at_start: the point is the search's start
-    T gnorm, step, step_kept;
-    int at_start;
-    int k;
-    long long nfev;
-    int status;     // 0 ok, otherwise a LineSearchError code
-    int finished;
-    int niter;      // return value of minimize()
-    T fx_hist[kMaxPast];
-    double* trace;              // optional: f of every evaluation
-    long long trace_cap;
-    long long rounds;           // rounds this problem took part in
-};
 
 // what every CTA needs to know about a problem's next round: one 128-byte line, written by the leader, read through L2
 template <class T> struct alignas(128) PRound
@@ -159,9 +102,6 @@ template <class T> struct PArgs
                                 // in L2 anyway).  Measured and dropped: unrolling the pass 4x (no change), prefetching its inputs into L2 (-5 %), a
                                 // grid-stride instead of a chunked sweep (+1 %)
 };
-
-template <class P> __device__ __forceinline__ void dswap(P& a, P& b) { P t = a; a = b; b = t; }
-__device__ __forceinline__ int slot_by_age(int head, int M, int age) { return ((head - 1 - age) % M + M) % M; }
 
 // ---- shared memory of the kernel ----------------------------------------------------------------------------------------------
 struct PShared
@@ -880,147 +820,6 @@ __device__ __forceinline__ void st_release_gpu_u32(unsigned* p, unsigned v)
     asm volatile("st.release.gpu.global.u32 [%0], %1;" :: "l"(p), "r"(v) : "memory");
 }
 
-// ---- the leader's work between two rounds ------------------------------------------------------------------------------------
-template <class T> __device__ __forceinline__ void record_eval(PState<T>* st, T fx)
-{
-    if (st->trace && st->nfev < st->trace_cap) st->trace[st->nfev] = (double)fx;
-    st->nfev++;
-}
-// the problem stops; `implied`: (x, g) do not hold its point yet, one MATERIALIZE round writes them (step, at_start) first
-template <class T> __device__ __forceinline__ void finish(PState<T>* st, int niter, int status = 0, bool implied = false)
-{
-    st->finished = 1;
-    st->niter = niter;
-    if (status) st->status = status;
-    st->op = implied ? POP_MATERIALIZE : POP_IDLE;
-}
-
-// after a search has produced its point -- in (x, g) when STORED, else implied by (step, at_start): the stopping rules
-// (LBFGS.h:137-154), then on to the pair-forming dots
-template <class T, bool STORED> __device__ __forceinline__ void after_search(PState<T>* st)
-{
-    using namespace LBFGSpp;
-    const int k = st->k;
-    st->gnorm = std::sqrt(st->rec.gg);
-    if (gradient_converged(st->gnorm, st->rec.xx, st->epsilon, st->epsilon_rel) || stalled(st->fx_hist, st->past, k, st->rec.fx, st->delta) ||
-        iteration_cap(k, st->max_iterations))
-    {
-        finish(st, k, 0, !STORED);
-        return;
-    }
-    st->op = POP_DOTS_FORM;
-    st->c_round = st->ncorr < st->m ? st->ncorr + 1 : st->m;
-}
-
-// the trial at st->step has been evaluated: {fx, dg, gg, xx}.  Sets the next op.  STORED: the trial is in (x, g), a kept trial
-// moves to (x_lo, g_lo) by pointer swap; otherwise a trial is its step, and the kept one is st->step_kept.
-template <class T, bool STORED> __device__ __forceinline__ void digest_trial(PState<T>* st, T fx, T dg, T gg, T xx)
-{
-    record_eval(st, fx);
-    bool keep = false;
-    const int action = st->ls.advance(fx, dg, keep);
-    const int next = st->rec.digest(action, keep, fx, dg, gg, xx, st->ls.best_fx(), st->ls.best_dg());
-    if (next >= LBFGSpp::LSE_STEP_NOT_POSITIVE) { finish(st, st->k, next, !STORED); return; }   // (x, g): this trial
-    if (keep)
-    {
-        if (STORED) { dswap(st->x, st->x_lo); dswap(st->g, st->g_lo); }
-        else st->step_kept = st->step;
-    }
-    switch (next)
-    {
-    case LBFGSpp::SEARCH_EVALUATE: st->op = POP_TRIAL; st->step = st->ls.step(); return;
-    case LBFGSpp::SEARCH_TAKE_KEPT:
-        if (STORED) { dswap(st->x, st->x_lo); dswap(st->g, st->g_lo); }
-        else st->step = st->step_kept;
-        break;
-    case LBFGSpp::SEARCH_TAKE_START:
-        if (STORED) { st->op = POP_RESTORE; return; }   // copy xp/gp back, then carry on
-        st->at_start = 1;
-        break;
-    }
-    after_search<T, STORED>(st);
-}
-
-// top of an iteration (LBFGS.h:121-127): the search is armed, the current point becomes the previous one
-template <class T> __device__ __forceinline__ bool begin_search(PState<T>* st, T step)
-{
-    // the search validates its inputs before anything moves (the reference throws before touching x): on failure x stays the
-    // current point (it is in (x, g): FIRST or the pair-forming pass wrote it)
-    const int rc = st->ls.init(st->ls_opt, st->rec.fx, st->rec.dg, step, st->max_step);
-    if (rc != 0) { finish(st, st->k, rc); return false; }
-    dswap(st->xp, st->x);
-    dswap(st->gp, st->g);
-    st->rec.begin();
-    st->at_start = 0;
-    st->op = POP_TRIAL;
-    st->step = st->ls.step();
-    return true;
-}
-
-template <class T, bool STORED> __device__ void advance_problem(PState<T>* st, const double* vals)
-{
-    st->rounds++;
-    switch (st->op)
-    {
-    case POP_FIRST:
-    {
-        const T fx = (T)vals[0], gg = (T)vals[2], xx = (T)vals[3];
-        st->nfev = 0;
-        record_eval(st, fx);
-        st->rec.fx = fx; st->rec.gg = gg; st->rec.xx = xx;
-        st->k = 1;
-        if (st->past > 0) st->fx_hist[0] = fx;
-        st->gnorm = std::sqrt(gg);
-        if (LBFGSpp::gradient_converged(st->gnorm, xx, st->epsilon, st->epsilon_rel)) { finish(st, 1); return; }
-        st->rec.dg = -gg;                   // grad . (-grad)
-        begin_search(st, T(1) / st->gnorm); // LBFGS.h:108
-        return;
-    }
-    case POP_TRIAL:
-        digest_trial<T, STORED>(st, (T)vals[0], (T)vals[1], (T)vals[2], (T)vals[3]);
-        return;
-    case POP_RESTORE:           // (x, g) now hold the search's start point; its sums were restored before
-        after_search<T, STORED>(st);
-        return;
-    case POP_MATERIALIZE:       // (x, g) now hold the point the problem stopped at
-        st->op = POP_IDLE;
-        return;
-    case POP_DOTS_FORM:
-    {
-        // curvature gate on the pair's own dots (age-0 column: [2] = s'y, [3] = y'y), LBFGS.h:161; commit = BFGSMat.h:89-97
-        const T sy = (T)vals[2], yy = (T)vals[3];
-        if (LBFGSpp::curvature_ok(sy, yy, LBFGSpp::lsdetail::eps_of<T>()))
-        {
-            st->ys[st->head] = sy;
-            *st->theta = yy / sy;
-            st->pending = st->head;
-            st->head = (st->head + 1) % st->M;
-            st->ncorr = st->c_round;
-            st->op = st->fuse_first_trial ? POP_COMBINE_TRIAL : POP_COMBINE;
-        }
-        else if (st->ncorr > 0) { st->op = POP_DOTS_PLAIN; st->c_round = st->ncorr; }
-        else { st->op = st->fuse_first_trial ? POP_COMBINE_TRIAL : POP_COMBINE; st->c_round = 0; }
-        return;
-    }
-    case POP_DOTS_PLAIN:
-        st->op = st->fuse_first_trial ? POP_COMBINE_TRIAL : POP_COMBINE;
-        return;
-    case POP_COMBINE:
-    case POP_COMBINE_TRIAL:
-    {
-        const bool fused = st->op == POP_COMBINE_TRIAL;
-        if (st->pending >= 0) { st->gram_cur = 1 - st->gram_cur; st->pending = -1; }
-        st->rec.dg = (T)vals[0];            // LBFGS.h:123 for the next pass
-        st->k += 1;
-        if (!begin_search(st, T(1))) return;   // LBFGS.h:168
-        // the pass already evaluated xp + 1*d (STORED: into the buffers that the rotation just made (x, g))
-        if (fused && st->ls.step() == T(1)) digest_trial<T, STORED>(st, (T)vals[1], (T)vals[2], (T)vals[3], (T)vals[4]);
-        return;
-    }
-    default: return;
-    }
-}
-
 // n-words a pass has to move (reads + writes of whole vectors): the roofline numerator of the persistent kernel.  stored: the
 // trials store their points (neighbour-coupled objectives)
 __device__ __forceinline__ double words_of(int op, int c, int data_vectors, bool stored)
@@ -1036,18 +835,6 @@ __device__ __forceinline__ double words_of(int op, int c, int data_vectors, bool
     case POP_COMBINE: return 2.0 * c + 2.0;                 // R g, 2c columns ; W d
     case POP_COMBINE_TRIAL: return 2.0 * c + (stored ? 5.0 : 3.0) + data_vectors;   // R g, x, 2c columns ; W d (, x1, g1)
     default: return 0.0;
-    }
-}
-
-template <class T> __device__ __forceinline__ int nvals_of(const PState<T>* st)
-{
-    switch (st->op)
-    {
-    case POP_FIRST: case POP_TRIAL: return 4;
-    case POP_DOTS_FORM: case POP_DOTS_PLAIN: return st->c_round * kGramVals;
-    case POP_COMBINE: return 1;
-    case POP_COMBINE_TRIAL: return 5;
-    default: return 0;
     }
 }
 

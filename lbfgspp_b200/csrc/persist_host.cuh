@@ -107,13 +107,7 @@ static lbfgs_b200_status solver_minimize(lbfgs_b200_solver* s, int objective, co
         p.data1 = data1 ? data1 + (size_t)b * ldd : nullptr;
         p.raw = s->d_raw + (size_t)b * s->pstride;
         p.halo = s->d_halo + (size_t)b * kHaloDoubles;
-        p.head = 0; p.ncorr = 0; p.M = s->M; p.m = s->m; p.gram_cur = 0; p.pending = -1;
-        p.op = POP_FIRST; p.c_round = 0;
-        p.epsilon = (T)prm->epsilon; p.epsilon_rel = (T)prm->epsilon_rel; p.delta = (T)prm->delta; p.max_step = (T)prm->max_step;
-        p.past = prm->past; p.max_iterations = prm->max_iterations;
-        p.fuse_first_trial = fuse_first_trial;
-        p.ls.kind = ls_kind;
-        p.ls_opt = LBFGSpp::line_search_options<T>(*prm, ls_kind);
+        init_problem_state<T>(p, *prm, ls_kind, fuse_first_trial);   // (prm->m == s->m: p.M == s->M)
         p.trace = trace_host ? s->d_trace : nullptr;
         p.trace_cap = trace_host ? trace_cap : 0;
         CU(ctx, cudaMemcpyAsync(p.x, x_inout + (size_t)b * ldx, vb, cudaMemcpyDeviceToDevice, ctx->stream));

@@ -1,0 +1,419 @@
+// small_batch.cuh -- many small L-BFGS problems in one launch: LBFGSSolver::minimize() (reference LBFGS.h:78-173) for B independent
+// problems of a built-in objective, one thread block (CTA) per problem, the whole solve in that CTA's shared memory.
+// Included by small_batch.cu.
+//
+// The device-resident solve (persist.cuh) spreads one pass of a problem over every SM and separates rounds by grid-wide barriers;
+// below a few thousand coordinates it has nothing to spread, and a batch of such problems runs one after another on one SM.  Here a
+// CTA runs one problem's whole minimize() with nobody to wait for: an ordinary launch of B CTAs (they run in waves), no grid
+// barrier, no atomics, no watchdog.  HBM is read once (x0 and the problem's data vectors) and written once (x and, optionally, g).
+//
+// The scalar side is the resident solve's own: PState, the POP_* ops and advance_problem of problem_machine.cuh.  The CTA loops
+//     run the pass for st->op over the vectors in shared memory -> reduce its nvals_of(st) values into raw[] -> thread 0 calls
+//     advance_problem -> __syncthreads
+// until the op is POP_IDLE.  The passes are the resident ones restated for one CTA over on-chip vectors: FIRST, TRIAL and
+// MATERIALIZE with the resident solve's implied-point rule (a trial of an objective without neighbour coupling stores nothing; the
+// pair-forming pass rebuilds the accepted point with the trial's arithmetic), DOTS_FORM / DOTS_PLAIN in k_gram_dots' layout
+// (kGramVals values per column pair), COMBINE(_TRIAL) with the coefficient recursion of gram_solve_in_smem, RESTORE for the
+// neighbour-coupled objectives, whose trials store their points and keep the best one in x_lo / g_lo.  The first trial of every
+// search always rides on the combination pass.
+//
+// Determinism.  A CTA has small_threads(n) threads: one warp up to n = 128, four warps above.  A thread owns the packs of 4
+// coordinates q = tid, tid + nt, ... and accumulates them in index order (in T, as the resident passes do); the block sum is a fixed
+// shuffle tree per warp and the warp totals added in warp order, in double for both precisions.  So a problem's result depends on n
+// (and the precision) only -- not on B, nor on where the problem sits in the batch.  It is not bit-identical to LBFGSSolver's resident
+// solve or to LBFGSBatchSolver, whose sums are associated across CTAs; the decisions follow the same code, the sums differ by rounding.
+//
+// Shared memory of one CTA (byte offsets: small_layout; the budget in include/lbfgs_b200.h):
+//     [ PState + slot table: kSStateBytes ][ raw: p doubles ][ red: kSMaxWarps x p doubles ][ ys M | alpha M | theta (4) | SY,YY,SS x2:
+//     6 M^2 ][ recursion scratch: gram_solve_smem_elems(m) ][ vectors, ld = round_up(n, 4) elements each: x xp g gp d, S/Y of slot 0..M-1,
+//     (x_lo g_lo), (data0 data1) ]          with M = m + 1 ring slots and p = round_up(max(6m, 8), 8)
+#pragma once
+
+#include "problem_machine.cuh"
+
+namespace lb {
+
+constexpr int kSMaxThreads = 128;
+constexpr int kSMaxWarps = kSMaxThreads / 32;
+constexpr size_t kSStateBytes = 2048;          // the problem's PState and its slot table
+constexpr size_t kSSmemLimit = 232448;         // largest dynamic shared memory of one CTA on sm_90 (227 KB)
+static_assert(sizeof(PState<double>) + kMaxM <= kSStateBytes && sizeof(PState<float>) + kMaxM <= kSStateBytes, "state region");
+
+// threads per CTA: a fixed function of n, so that a problem's sums never depend on anything else
+__host__ __device__ inline int small_threads(int64_t n) { return n <= 128 ? 32 : kSMaxThreads; }
+
+struct SmallLayout
+{
+    size_t raw, red, small, gram, vecs, total;   // byte offsets (the state is at 0)
+    int64_t ld;                                   // elements per vector
+    int pstride, nvec;
+};
+inline size_t small_align16(size_t b) { return (b + 15) & ~size_t(15); }
+inline SmallLayout small_layout(int64_t n, int m, int elem, bool stored, int data_vectors)
+{
+    SmallLayout L;
+    const size_t M = (size_t)m + 1;
+    L.ld = (n + 3) & ~int64_t(3);
+    L.pstride = ((m * kGramVals > 8 ? m * kGramVals : 8) + 7) & ~7;
+    L.nvec = 5 + 2 * (int)M + (stored ? 2 : 0) + data_vectors;
+    L.raw = kSStateBytes;
+    L.red = L.raw + sizeof(double) * (size_t)L.pstride;
+    L.small = L.red + sizeof(double) * (size_t)kSMaxWarps * L.pstride;
+    L.gram = L.small + small_align16((size_t)elem * (2 * M + 4 + 6 * M * M));
+    L.vecs = L.gram + small_align16((size_t)elem * gram_solve_smem_elems(m));
+    L.total = L.vecs + (size_t)elem * (size_t)L.nvec * (size_t)L.ld;
+    return L;
+}
+
+template <class T> struct SmallArgs
+{
+    const PState<T>* proto;     // options and initial ring / op (init_problem_state), the same for every problem (device memory)
+    int M;                      // ring slots: m + 1
+    SmallLayout L;
+    int64_t n;
+    const T *data0, *data1;     // problem b's data at data + b*ldd (ldd = 0: shared)
+    int64_t ldd;
+    T* X;                       // problem b: X + b*ldx (start point in, solution out)
+    int64_t ldx;
+    T* G;                       // optional: final gradients, same layout as X
+    lbfgs_b200_outcome* outs;   // [B]
+};
+
+// block sums of NV per-thread values -> raw[0..NV): a fixed shuffle tree per warp, warp totals in warp order.  All threads call.
+template <int NV> __device__ __forceinline__ void small_sums(const double (&v)[NV], double* red, int ps, double* raw)
+{
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+#pragma unroll
+    for (int k = 0; k < NV; k++)
+    {
+        const double w = warp_sum(v[k]);
+        if (lane == 0) red[warp * ps + k] = w;
+    }
+    __syncthreads();
+    if (threadIdx.x < NV)
+    {
+        double t = 0.0;
+        for (int w = 0; w < nw; w++) t += red[w * ps + threadIdx.x];
+        raw[threadIdx.x] = t;
+    }
+}
+
+template <class T, class OBJ>
+__global__ void __launch_bounds__(kSMaxThreads) k_small_batch(const SmallArgs<T> a)
+{
+    extern __shared__ __align__(16) unsigned char s_smem[];
+    constexpr bool STORED = OBJ::kHalo;          // neighbour-coupled objectives: trials store their points
+    constexpr int DV = OBJ::kDataVectors;
+    const int tid = threadIdx.x, nt = blockDim.x;
+    const int64_t b = blockIdx.x, n = a.n, ld = a.L.ld;
+    const int64_t npacks = (n + 3) >> 2;
+    const int M = a.M, ps = a.L.pstride;
+    PState<T>* st = reinterpret_cast<PState<T>*>(s_smem);
+    unsigned char* s_slot = s_smem + sizeof(PState<T>);   // by age: physical ring slot (combination pass)
+    double* raw = reinterpret_cast<double*>(s_smem + a.L.raw);
+    double* red = reinterpret_cast<double*>(s_smem + a.L.red);
+    T* small = reinterpret_cast<T*>(s_smem + a.L.small);
+    T* gram = reinterpret_cast<T*>(s_smem + a.L.gram);
+    T* vec = reinterpret_cast<T*>(s_smem + a.L.vecs);
+    T* const ring = vec + 5 * ld;                            // S of slot k at ring + 2k*ld, Y of slot k right after it
+    T* const sdata = ring + (2 * M + (STORED ? 2 : 0)) * ld;
+    auto s_col = [&](int slot) { return ring + 2 * (int64_t)slot * ld; };
+
+    // ---- the problem's state, history and vectors ----
+    {
+        const unsigned* src = reinterpret_cast<const unsigned*>(a.proto);
+        unsigned* dst = reinterpret_cast<unsigned*>(st);
+        for (int w = tid; w < (int)(sizeof(PState<T>) / 4); w += nt) dst[w] = src[w];
+    }
+    const size_t small_elems = (size_t)2 * M + 4 + 6 * (size_t)M * M;
+    for (size_t i = tid; i < small_elems; i += nt) small[i] = T(0);   // BFGSMat::reset (BFGSMat.h:61-78): no pairs, Gram cleared
+    for (int64_t i = tid; i < (int64_t)a.L.nvec * ld; i += nt) vec[i] = T(0);   // (lanes past n stay 0 in every vector)
+    __syncthreads();
+    if (tid == 0)
+    {
+        const size_t mm = (size_t)M * M;
+        st->x = vec; st->xp = vec + ld; st->g = vec + 2 * ld; st->gp = vec + 3 * ld; st->drt = vec + 4 * ld;
+        st->x_lo = STORED ? ring + 2 * M * ld : nullptr;
+        st->g_lo = STORED ? ring + (2 * M + 1) * ld : nullptr;
+        st->hist.H = ring; st->hist.M = M; st->hist.bt_log = 0; st->hist.bstride = 0;   // (the ring is addressed through s_col)
+        st->ys = small; st->alpha = small + M; st->theta = small + 2 * M;
+        for (int k = 0; k < 2; k++) { st->SY[k] = small + 2 * M + 4 + (3 * k + 0) * mm; st->YY[k] = small + 2 * M + 4 + (3 * k + 1) * mm; st->SS[k] = small + 2 * M + 4 + (3 * k + 2) * mm; }
+        st->data0 = DV ? sdata : nullptr;
+        st->data1 = DV ? sdata + ld : nullptr;
+        st->raw = raw; st->halo = nullptr; st->trace = nullptr; st->trace_cap = 0;
+        *st->theta = T(1);
+    }
+    {
+        const T* x0 = a.X + b * a.ldx;
+        for (int64_t i = tid; i < n; i += nt) vec[i] = x0[i];
+        if constexpr (DV == 2)
+        {
+            const T* d0 = a.data0 + b * a.ldd;
+            const T* d1 = a.data1 + b * a.ldd;
+            for (int64_t i = tid; i < n; i += nt) { sdata[i] = d0[i]; sdata[ld + i] = d1[i]; }
+        }
+    }
+    // neighbours straight from shared memory: no index offset, the whole vector, no halo
+    const OBJ obj{ObjGeom<T>{n, 0, n, nullptr, DV ? sdata : nullptr, DV ? sdata + ld : nullptr}};
+
+    for (;;)
+    {
+        __syncthreads();   // the state thread 0 left, and every vector of the last pass
+        const int op = st->op;
+        if (op == POP_IDLE) break;
+        T* const x = st->x; T* const xp = st->xp; T* const g = st->g; T* const gp = st->gp; T* const d = st->drt;
+        const T step = st->step;
+        const int at_start = st->at_start, c = st->c_round, head = st->head;
+        switch (op)
+        {
+        // FIRST: g = grad f(x), d = -g ; {f, g.d (= 0), g.g, x.x}.  TRIAL: x = xp + step*d, g = grad f(x) ; {f, g.d, g.g, x.x}, stored
+        // only by the neighbour-coupled objectives.  MATERIALIZE: x = xp + step*d, g = grad f(x), stored; no sums.
+        case POP_FIRST:
+        case POP_TRIAL:
+        case POP_MATERIALIZE:
+        {
+            if (op == POP_MATERIALIZE && at_start)
+            {
+                for (int64_t i = tid; i < n; i += nt) { x[i] = xp[i]; g[i] = gp[i]; }
+                break;
+            }
+            const bool first = op == POP_FIRST;
+            const bool store = first || STORED || op == POP_MATERIALIZE;
+            T acc[4] = {T(0), T(0), T(0), T(0)};
+            for (int64_t q = tid; q < npacks; q += nt)
+            {
+                const int64_t i0 = q << 2;
+                const int cnt = (n - i0 >= 4) ? 4 : int(n - i0);
+                T xv[4], dv[4], gv[4], xl = T(0), xr = T(0);
+#pragma unroll
+                for (int k = 0; k < 4; k++)
+                {
+                    dv[k] = (!first && k < cnt) ? d[i0 + k] : T(0);
+                    xv[k] = (k < cnt) ? (first ? x[i0 + k] : xp[i0 + k] + step * d[i0 + k]) : T(0);
+                }
+                if constexpr (OBJ::kHalo)
+                {
+                    if (first) pack_neighbours<false>(obj, i0, n, step, [&](int j) { return x[i0 + j]; }, xl, xr);
+                    else pack_neighbours<true>(obj, i0, n, step, [&](int j) { return xp[i0 + j] + step * d[i0 + j]; }, xl, xr);
+                }
+                eval_pack(obj, i0, cnt, xv, xl, xr, dv, gv, acc);
+                if (store)
+                {
+#pragma unroll
+                    for (int k = 0; k < 4; k++)
+                        if (k < cnt)
+                        {
+                            g[i0 + k] = gv[k];
+                            if (first) d[i0 + k] = T(-1) * gv[k];
+                            else x[i0 + k] = xv[k];
+                        }
+                }
+            }
+            if (op == POP_MATERIALIZE) break;
+            const double dacc[4] = {(double)acc[0], (double)acc[1], (double)acc[2], (double)acc[3]};
+            small_sums<4>(dacc, red, ps, raw);
+            break;
+        }
+        case POP_RESTORE:
+            for (int64_t i = tid; i < n; i += nt) { x[i] = xp[i]; g[i] = gp[i]; }
+            break;
+        // [S Y]'[g s_new y_new], kGramVals values per column pair, by age.  FORM: the new pair s = x - xp, y = g - gp goes into ring slot
+        // `head` and takes part as column 0; an implied point is rebuilt first (the trial's arithmetic) and written to (x, g).
+        // PLAIN: s.g and y.g of the old columns only.  A thread only touches its own packs, so no barrier is needed in between.
+        case POP_DOTS_FORM:
+        case POP_DOTS_PLAIN:
+        {
+            const bool form = op == POP_DOTS_FORM;
+            T* const sn = s_col(head);
+            T* const yn = sn + ld;
+            if (form)
+                for (int64_t q = tid; q < npacks; q += nt)
+                {
+                    const int64_t i0 = q << 2;
+                    const int cnt = (n - i0 >= 4) ? 4 : int(n - i0);
+                    if (!STORED)
+                    {
+                        T xv[4], gv[4];
+                        if (at_start)
+                        {
+#pragma unroll
+                            for (int k = 0; k < 4; k++) { xv[k] = (k < cnt) ? xp[i0 + k] : T(0); gv[k] = (k < cnt) ? gp[i0 + k] : T(0); }
+                        }
+                        else
+                        {
+#pragma unroll
+                            for (int k = 0; k < 4; k++) xv[k] = (k < cnt) ? xp[i0 + k] + step * d[i0 + k] : T(0);
+                            obj.eval(i0, cnt, xv, T(0), T(0), gv);
+                        }
+#pragma unroll
+                        for (int k = 0; k < 4; k++)
+                            if (k < cnt) { x[i0 + k] = xv[k]; g[i0 + k] = gv[k]; }
+                    }
+#pragma unroll
+                    for (int k = 0; k < 4; k++)
+                        if (k < cnt) { sn[i0 + k] = x[i0 + k] - xp[i0 + k]; yn[i0 + k] = g[i0 + k] - gp[i0 + k]; }
+                }
+            for (int j = 0; j < c; j++)
+            {
+                const int slot = form ? (j == 0 ? head : slot_by_age(head, M, j - 1)) : slot_by_age(head, M, j);
+                const T* sj = s_col(slot);
+                const T* yj = sj + ld;
+                T acc[kGramVals] = {T(0), T(0), T(0), T(0), T(0), T(0)};
+                for (int64_t q = tid; q < npacks; q += nt)
+                {
+                    const int64_t i0 = q << 2;
+                    const int cnt = (n - i0 >= 4) ? 4 : int(n - i0);
+#pragma unroll
+                    for (int k = 0; k < 4; k++)
+                        if (k < cnt)
+                        {
+                            const int64_t i = i0 + k;
+                            const T s = sj[i], y = yj[i], v = g[i];
+                            acc[0] += s * v;
+                            acc[1] += y * v;
+                            if (form)
+                            {
+                                const T ynew = yn[i], snew = sn[i];
+                                acc[2] += s * ynew;
+                                acc[3] += y * ynew;
+                                acc[4] += y * snew;
+                                acc[5] += s * snew;
+                            }
+                        }
+                }
+                const int lane = tid & 31, warp = tid >> 5;
+#pragma unroll
+                for (int k = 0; k < kGramVals; k++)
+                {
+                    const double w = warp_sum((double)acc[k]);
+                    if (lane == 0) red[warp * ps + j * kGramVals + k] = w;
+                }
+            }
+            __syncthreads();
+            for (int idx = tid; idx < c * kGramVals; idx += nt)
+            {
+                double t = 0.0;
+                for (int w = 0; w < (nt >> 5); w++) t += red[w * ps + idx];
+                raw[idx] = t;
+            }
+            break;
+        }
+        // d = -H g by the coefficient recursion (gram_solve_in_smem, which also folds the new pair into the Gram matrices) and one
+        // combination d = cv*g + sum_j cy_j y_j + cs_j s_j (y newest -> oldest, then s oldest -> newest) ; {g.d}.  COMBINE_TRIAL: the
+        // first trial of the next search, x1 = x + d, in the same pass ; {g.d, f1, g1.d, g1.g1, x1.x1}; the neighbour-coupled objectives
+        // write x1, g1 to (xp, gp), which the rotation of begin_search turns into (x, g).
+        case POP_COMBINE:
+        case POP_COMBINE_TRIAL:
+        {
+            const bool fuse = op == POP_COMBINE_TRIAL;
+            GramSolveArgs<T> ga;
+            ga.c = c; ga.M = M; ga.new_slot = st->pending; ga.with_v = 1; ga.a = T(-1);
+            ga.raw = raw;
+            const int in = st->gram_cur, out = (ga.new_slot >= 0) ? 1 - in : in;
+            ga.SY_in = st->SY[in]; ga.YY_in = st->YY[in]; ga.SS_in = st->SS[in];
+            ga.SY_out = st->SY[out]; ga.YY_out = st->YY[out]; ga.SS_out = st->SS[out];
+            ga.ys = st->ys; ga.alpha = st->alpha; ga.theta = st->theta;
+            for (int age = 0; age < c; age++) ga.slots[age] = (unsigned char)slot_by_age(head, M, age);
+            for (int age = tid; age < c; age += nt) s_slot[age] = ga.slots[age];
+            gram_solve_in_smem<T, false>(ga, gram, true);   // (ends with a barrier: the coefficients and s_slot are in place)
+            const T* coef = gram + 2 * c * c;
+            const T cv = coef[0];
+            T acc[5] = {T(0), T(0), T(0), T(0), T(0)};
+            for (int64_t q = tid; q < npacks; q += nt)
+            {
+                const int64_t i0 = q << 2;
+                const int cnt = (n - i0 >= 4) ? 4 : int(n - i0);
+                T r[4], xv[4] = {T(0), T(0), T(0), T(0)};
+#pragma unroll
+                for (int k = 0; k < 4; k++) r[k] = (k < cnt) ? cv * g[i0 + k] : T(0);
+                for (int j = 0; j < c; j++)
+                {
+                    const T* yj = s_col(s_slot[j]) + ld;
+                    const T cy = coef[1 + j];
+#pragma unroll
+                    for (int k = 0; k < 4; k++) r[k] += (k < cnt) ? cy * yj[i0 + k] : T(0);
+                }
+                for (int j = c - 1; j >= 0; j--)
+                {
+                    const T* sj = s_col(s_slot[j]);
+                    const T cs = coef[1 + c + j];
+#pragma unroll
+                    for (int k = 0; k < 4; k++) r[k] += (k < cnt) ? cs * sj[i0 + k] : T(0);
+                }
+#pragma unroll
+                for (int k = 0; k < 4; k++)
+                    if (k < cnt)
+                    {
+                        d[i0 + k] = r[k];
+                        acc[0] += g[i0 + k] * r[k];
+                        xv[k] = x[i0 + k] + T(1) * r[k];
+                    }
+                if (fuse && !STORED)
+                {
+                    T gv[4];
+                    eval_pack(obj, i0, cnt, xv, T(0), T(0), r, gv, acc + 1);
+                }
+                else if (fuse)
+                {
+#pragma unroll
+                    for (int k = 0; k < 4; k++)
+                        if (k < cnt) xp[i0 + k] = xv[k];
+                }
+            }
+            if (fuse && STORED)
+            {
+                __syncthreads();   // x1 of every coordinate is in xp: the objective takes its neighbours from there
+                for (int64_t q = tid; q < npacks; q += nt)
+                {
+                    const int64_t i0 = q << 2;
+                    const int cnt = (n - i0 >= 4) ? 4 : int(n - i0);
+                    T xv[4], dv[4], gv[4], xl, xr;
+#pragma unroll
+                    for (int k = 0; k < 4; k++) { xv[k] = (k < cnt) ? xp[i0 + k] : T(0); dv[k] = (k < cnt) ? d[i0 + k] : T(0); }
+                    pack_neighbours<false>(obj, i0, n, T(0), [&](int j) { return xp[i0 + j]; }, xl, xr);
+                    eval_pack(obj, i0, cnt, xv, xl, xr, dv, gv, acc + 1);
+#pragma unroll
+                    for (int k = 0; k < 4; k++)
+                        if (k < cnt) gp[i0 + k] = gv[k];
+                }
+            }
+            if (fuse)
+            {
+                const double dacc[5] = {(double)acc[0], (double)acc[1], (double)acc[2], (double)acc[3], (double)acc[4]};
+                small_sums<5>(dacc, red, ps, raw);
+            }
+            else
+            {
+                const double dacc[1] = {(double)acc[0]};
+                small_sums<1>(dacc, red, ps, raw);
+            }
+            break;
+        }
+        default: break;
+        }
+        __syncthreads();   // raw[] and the pass's vectors are complete
+        if (tid == 0) advance_problem<T, STORED>(st, raw);
+    }
+
+    // ---- results: the point (and gradient) the problem stopped at, and its outcome ----
+    {
+        T* const xo = a.X + b * a.ldx;
+        const T* xs = st->x;
+        const T* gs = st->g;
+        for (int64_t i = tid; i < n; i += nt) xo[i] = xs[i];
+        if (a.G)
+        {
+            T* const go = a.G + b * a.ldx;
+            for (int64_t i = tid; i < n; i += nt) go[i] = gs[i];
+        }
+        if (tid == 0)
+        {
+            lbfgs_b200_outcome o;
+            o.status = st->status; o.niter = st->niter; o.nfev = st->nfev;
+            o.fx = (double)st->rec.fx; o.gnorm = (double)st->gnorm; o.rounds = st->rounds;
+            a.outs[b] = o;
+        }
+    }
+}
+
+}  // namespace lb

@@ -399,9 +399,12 @@ template <class T> struct GramSolveArgs
 __host__ __device__ inline size_t gram_solve_smem_elems(int c) { return (size_t)2 * c * c + 6 * c + 2; }
 
 // All global reads go through L2 (__ldcg): inside the persistent solve these scalars are rewritten by another CTA between rounds.
-template <class T>
+// GLOBAL = false: the operands (raw, Gram matrices, ys, theta) live in this CTA's shared memory (the small-batch solve) and are read
+// with ordinary loads.
+template <class T, bool GLOBAL = true>
 __device__ void gram_solve_in_smem(const GramSolveArgs<T>& g, T* sm, bool writer)
 {
+    auto ld = [](const auto* p) { if constexpr (GLOBAL) return __ldcg(p); else return *p; };
     const int c = g.c, M = g.M, tid = threadIdx.x, nt = blockDim.x;
     T* sSY = sm;
     T* sYY = sm + c * c;
@@ -412,19 +415,19 @@ __device__ void gram_solve_in_smem(const GramSolveArgs<T>& g, T* sm, bool writer
     {
         const int i = idx / c, j = idx % c;
         const int pi = g.slots[i], pj = g.slots[j];
-        T sy = __ldcg(g.SY_in + pi * M + pj), yy = __ldcg(g.YY_in + pi * M + pj);
+        T sy = ld(g.SY_in + pi * M + pj), yy = ld(g.YY_in + pi * M + pj);
         if (g.new_slot >= 0)
         {
-            if (j == 0) { sy = (T)__ldcg(g.raw + i * kGramVals + 2); yy = (T)__ldcg(g.raw + i * kGramVals + 3); }       // s_i'y_new, y_i'y_new
-            else if (i == 0) { sy = (T)__ldcg(g.raw + j * kGramVals + 4); yy = (T)__ldcg(g.raw + j * kGramVals + 3); }  // s_new'y_j, y_new'y_j
+            if (j == 0) { sy = (T)ld(g.raw + i * kGramVals + 2); yy = (T)ld(g.raw + i * kGramVals + 3); }       // s_i'y_new, y_i'y_new
+            else if (i == 0) { sy = (T)ld(g.raw + j * kGramVals + 4); yy = (T)ld(g.raw + j * kGramVals + 3); }  // s_new'y_j, y_new'y_j
         }
         sSY[idx] = sy;
         sYY[idx] = yy;
         if (writer && g.new_slot >= 0)
         {
-            T ss = __ldcg(g.SS_in + pi * M + pj);
-            if (j == 0) ss = (T)__ldcg(g.raw + i * kGramVals + 5);        // s_i's_new
-            else if (i == 0) ss = (T)__ldcg(g.raw + j * kGramVals + 5);   // s_new's_j
+            T ss = ld(g.SS_in + pi * M + pj);
+            if (j == 0) ss = (T)ld(g.raw + i * kGramVals + 5);        // s_i's_new
+            else if (i == 0) ss = (T)ld(g.raw + j * kGramVals + 5);   // s_new's_j
             g.SY_out[pi * M + pj] = sy;
             g.YY_out[pi * M + pj] = yy;
             g.SS_out[pi * M + pj] = ss;
@@ -440,11 +443,11 @@ __device__ void gram_solve_in_smem(const GramSolveArgs<T>& g, T* sm, bool writer
     {
         for (int i = nt - 1 - tid; i < c; i += nt)
         {
-            b0[i] = g.a * (T)__ldcg(g.raw + i * kGramVals + 0);
-            b1[i] = g.a * (T)__ldcg(g.raw + i * kGramVals + 1);
-            ysv[i] = __ldcg(g.ys + g.slots[i]);
+            b0[i] = g.a * (T)ld(g.raw + i * kGramVals + 0);
+            b1[i] = g.a * (T)ld(g.raw + i * kGramVals + 1);
+            ysv[i] = ld(g.ys + g.slots[i]);
         }
-        if (tid == nt - 1) th[0] = __ldcg(g.theta);
+        if (tid == nt - 1) th[0] = ld(g.theta);
     }
     __syncthreads();
     if (tid < 32 && g.with_v)
