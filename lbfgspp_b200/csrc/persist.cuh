@@ -384,12 +384,10 @@ __device__ __forceinline__ void stage_tiled(T* dstt, int TE, int nrhs, int64_t e
 }
 
 // ---- DOTS -----------------------------------------------------------------------------------------------------------------------
-// [S Y]'[v s_new y_new] over this CTA's chunk, one block (tile) at a time, everything staged by bulk copies.  FORM: the newest pair
-// s = x - xp, y = g - gp is formed on the fly, identically in every warp that needs it, takes part as column 0 and is written to ring
-// slot `new_slot` by the warps that own column 0.  The point (x, g) comes from the staged rows {g, x, gp, xp} (neighbour-coupled
-// objectives: the trials stored it) or is rebuilt from the staged rows {d, xp, gp} -- x = xp + step*d, g = grad f(x) with the trial's
-// own arithmetic, or x = xp, g = gp when the search ended on its start point -- and then also written to (x, g) by the column-0 warps.
-// (Forming it once per tile into the staged rows, behind one more barrier per tile, measured 21 % slower per pass on config 2.)
+// [S Y]'[v s_new y_new] over this CTA's chunk, one block (tile) at a time, everything staged by bulk copies.  FORM (p_dots: a stored
+// point, neighbour-coupled objectives): the newest pair s = x - xp, y = g - gp is formed on the fly from the staged rows {g, x, gp, xp},
+// identically in every warp that needs it, takes part as column 0 and is written to ring slot `new_slot` by the warps that own
+// column 0.  An implied point (p_dots_implied) is formed once per element instead, see there.
 // Column j (by age) belongs to warp group j, whose `split` warps share the tile's units.  PLAIN: s.v and y.v over the old history only.
 template <class T> struct PDots
 {
@@ -403,12 +401,11 @@ template <class T> struct PDots
     T *x, *g;            // FORM of an implied point: where it is written
 };
 
-template <class T, class OBJ, int ROUNDS, bool FORM>
-__device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const Own& own, T* tiles, PShared& sh, unsigned& phase_bits, double* dst, int G)
+template <class T, int ROUNDS, bool FORM>
+__device__ __forceinline__ void p_dots(const PDots<T>& a, const Own& own, T* tiles, PShared& sh, unsigned& phase_bits, double* dst, int G)
 {
     constexpr int EPT = 16 / (int)sizeof(T);
-    constexpr bool IMPLIED = !OBJ::kHalo;
-    constexpr int NRHS = FORM ? (IMPLIED ? 3 : 4) : 1;           // staged right-hand vectors: g / g, x, gp, xp / d, xp, gp
+    constexpr int NRHS = FORM ? 4 : 1;                           // staged right-hand vectors: g, x, gp, xp / g
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int TE = a.h.BT();
     const int my_col = warp / a.split, my_part = warp % a.split;
@@ -458,31 +455,10 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const 
                     if constexpr (FORM)
                     {
                         Unit<T> ugp, uxp;
-                        if constexpr (IMPLIED)
-                        {
-                            const Unit<T> ud = lds_unit<T>(base + off);
-                            uxp = lds_unit<T>(base + TE + off);
-                            ugp = lds_unit<T>(base + 2 * TE + off);
-                            if (a.at_start) { ux = uxp; ug = ugp; }
-                            else
-                            {
-                                // the trial's arithmetic (p_trial, and p_combine's first trial with step 1 on the stored d)
-                                const int c4 = cnt < EPT ? cnt : EPT;
-                                T xv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
-#pragma unroll
-                                for (int k = 0; k < EPT; k++) xv[k] = (k < c4) ? uxp.v[k] + a.step * ud.v[k] : T(0);
-                                obj.eval(e0 + off, c4, xv, T(0), T(0), gv);
-#pragma unroll
-                                for (int k = 0; k < EPT; k++) { ux.v[k] = xv[k]; ug.v[k] = gv[k]; }
-                            }
-                        }
-                        else
-                        {
-                            ug = lds_unit<T>(base + off);
-                            ux = lds_unit<T>(base + TE + off);
-                            ugp = lds_unit<T>(base + 2 * TE + off);
-                            uxp = lds_unit<T>(base + 3 * TE + off);
-                        }
+                        ug = lds_unit<T>(base + off);
+                        ux = lds_unit<T>(base + TE + off);
+                        ugp = lds_unit<T>(base + 2 * TE + off);
+                        uxp = lds_unit<T>(base + 3 * TE + off);
 #pragma unroll
                         for (int k = 0; k < EPT; k++) { usn.v[k] = ux.v[k] - uxp.v[k]; uyn.v[k] = ug.v[k] - ugp.v[k]; }
                         if (cnt < EPT) { mask_unit(usn, cnt); mask_unit(uyn, cnt); }
@@ -496,7 +472,6 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const 
                             us = usn; uy = uyn;
                             st_unit<T>(s_new, off, cnt, usn);
                             st_unit<T>(s_new + TE, off, cnt, uyn);
-                            if (IMPLIED) { st_unit<T>(a.x, e0 + off, cnt, ux); st_unit<T>(a.g, e0 + off, cnt, ug); }
                             loaded = true;
                         }
                     }
@@ -539,6 +514,179 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const 
             if (lane == 0) sh.red[warp][r * kGramVals + k] = w;
         }
     __syncthreads();
+    const int nvals = a.c * kGramVals;
+    for (int idx = tid; idx < nvals; idx += kPThreads)
+    {
+        const int j = idx / kGramVals, k = idx % kGramVals;
+        const int r = j / a.cols_per_round, col = j % a.cols_per_round;
+        double t = 0.0;
+        for (int p = 0; p < a.split; p++) t += sh.red[col * a.split + p][r * kGramVals + k];
+        dst[(size_t)idx * G] = t;
+    }
+}
+
+// DOTS_FORM of an implied point (objectives without neighbour coupling): the sums of p_dots<FORM>, with the point rebuilt from the
+// staged rows {d, xp, gp} ONCE per element.  The forming warps take every unit of a staged tile: x = xp + step*d, g = grad f(x) with
+// the trial's own arithmetic (or x = xp, g = gp when the search ended on its start point), s = x - xp, y = g - gp; they write x, g and
+// the pair to HBM and g, s, y over d, xp, gp in the stage.  The column groups then read those rows.  The forming warps are the ones
+// dots_geometry leaves without a column (c = 10: 4 of 24) or, when every warp has a column (c = 3, 6, 12, ...), the warps of
+// column 0, which form a tile before taking their own dots of it.  Split, columns and the unit-to-lane mapping are p_dots', and so is
+// every accumulator: the sums are bit-identical to forming the point in every column group.
+// No CTA-wide barrier per tile: every stage has three mbarriers -- full (the bulk copies; parity in phase_bits), formed (arrivals of
+// the forming warps) and empty (arrivals of the column warps), the latter two initialised by the pass -- and warp 0, after its own
+// dots of a tile, waits for the stage's empty barrier and re-arms it.  So a column group starts a tile as soon as it is formed.
+template <class T, class OBJ, int ROUNDS>
+__device__ __forceinline__ void p_dots_implied(const PDots<T>& a, const OBJ& obj, const Own& own, T* tiles, PShared& sh, unsigned& phase_bits,
+                                               double* dst, int G)
+{
+    static_assert(!OBJ::kHalo, "neighbour-coupled objectives store their trial points: p_dots<FORM>");
+    constexpr int EPT = 16 / (int)sizeof(T);
+    constexpr int NRHS = 3;                                      // staged right-hand vectors: d, xp, gp, formed into g, s_new, y_new
+    __shared__ uint64_t formed_bar[kPMaxStages], empty_bar[kPMaxStages];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int TE = a.h.BT();
+    const int units = TE / EPT;
+    const int my_col = warp / a.split, my_part = warp % a.split;
+    const int upp = units / a.split;                             // units of a tile per warp of a column group
+    const SlotRuns runs(a.end, a.cnt_old, a.h.M);
+    const int nrows = NRHS + 2 * a.cnt_old;
+    int stages = (int)((size_t)kPStageBytes / ((size_t)nrows * TE * sizeof(T)));
+    stages = stages > kPMaxStages ? kPMaxStages : stages;
+    const int64_t ntl = own.ntiles(TE);
+    uint64_t* full_bar = sh.full_bar;
+    const int col_warps = (a.c < a.cols_per_round ? a.c : a.cols_per_round) * a.split;   // warps with a column
+    const bool spare = col_warps < kPWarps;
+    const int nform = spare ? kPWarps - col_warps : a.split;
+    const int fw = spare ? warp - col_warps : warp;              // index among the forming warps
+    const bool former = fw >= 0 && fw < nform;
+
+    T acc[ROUNDS][kGramVals];
+#pragma unroll
+    for (int r = 0; r < ROUNDS; r++)
+#pragma unroll
+        for (int k = 0; k < kGramVals; k++) acc[r][k] = T(0);
+
+    if (tid == 0)
+        for (int s = 0; s < stages; s++) { mbar_init(&formed_bar[s], nform); mbar_init(&empty_bar[s], col_warps); }
+    __syncthreads();   // sh.vecs / sh.slots and the barriers are in place, the staging ring is free
+    int64_t next_tile = 0;
+    for (int s = 0; s < stages; s++, next_tile++)
+        if (next_tile < ntl) stage_tiled<T>(tiles + (size_t)s * nrows * TE, TE, NRHS, own.start(next_tile, TE), own.len(next_tile, TE), a.h, runs, sh, &full_bar[s]);
+    const unsigned full_phase = phase_bits;
+    int stage = 0;
+    unsigned lap = 0;                                            // parity of the current use of `stage` in this pass
+    for (int64_t t = 0; t < ntl; t++)
+    {
+        T* base = tiles + (size_t)stage * nrows * TE;
+        const T* hist = base + (size_t)NRHS * TE;
+        const int64_t e0 = own.start(t, TE);
+        const int len = own.len(t, TE);
+        if (former)
+        {
+            mbar_wait(&full_bar[stage], ((full_phase >> stage) & 1u) ^ lap);
+            T* s_new = a.h.s_at(a.new_slot, e0);
+            for (int u = fw * 32 + lane; u < units; u += nform * 32)
+            {
+                const int off = u * EPT;
+                const int cnt = len - off;
+                if (cnt <= 0) break;
+                const Unit<T> ud = lds_unit<T>(base + off);
+                const Unit<T> uxp = lds_unit<T>(base + TE + off);
+                const Unit<T> ugp = lds_unit<T>(base + 2 * TE + off);
+                Unit<T> ux, ug, usn, uyn;
+                if (a.at_start) { ux = uxp; ug = ugp; }
+                else
+                {
+                    // the trial's arithmetic (p_trial, and p_combine's first trial with step 1 on the stored d)
+                    const int c4 = cnt < EPT ? cnt : EPT;
+                    T xv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
+#pragma unroll
+                    for (int k = 0; k < EPT; k++) xv[k] = (k < c4) ? uxp.v[k] + a.step * ud.v[k] : T(0);
+                    obj.eval(e0 + off, c4, xv, T(0), T(0), gv);
+#pragma unroll
+                    for (int k = 0; k < EPT; k++) { ux.v[k] = xv[k]; ug.v[k] = gv[k]; }
+                }
+#pragma unroll
+                for (int k = 0; k < EPT; k++) { usn.v[k] = ux.v[k] - uxp.v[k]; uyn.v[k] = ug.v[k] - ugp.v[k]; }
+                if (cnt < EPT) { mask_unit(usn, cnt); mask_unit(uyn, cnt); }
+                st_unit<T>(s_new, off, cnt, usn);
+                st_unit<T>(s_new + TE, off, cnt, uyn);
+                st_unit<T>(a.x, e0 + off, cnt, ux);
+                st_unit<T>(a.g, e0 + off, cnt, ug);
+                *reinterpret_cast<float4*>(base + off) = *reinterpret_cast<const float4*>(ug.v);
+                *reinterpret_cast<float4*>(base + TE + off) = *reinterpret_cast<const float4*>(usn.v);
+                *reinterpret_cast<float4*>(base + 2 * TE + off) = *reinterpret_cast<const float4*>(uyn.v);
+            }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // these writes before the bulk copies that re-arm the stage
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&formed_bar[stage]);
+        }
+        if (warp < col_warps)
+        {
+            mbar_wait(&formed_bar[stage], lap);
+#pragma unroll
+            for (int r = 0; r < ROUNDS; r++)
+            {
+                const int j = r * a.cols_per_round + my_col;
+                if (my_col < a.cols_per_round && j < a.c)
+                {
+                    const T* srow = hist + (size_t)2 * (j == 0 ? 0 : sh.slots[j]) * TE;     // sh.slots[j]: packed row of the column of age j
+                    const T* yrow = srow + TE;
+                    for (int u = my_part * upp + lane; u < (my_part + 1) * upp; u += 32)
+                    {
+                        const int off = u * EPT;
+                        const int cnt = len - off;
+                        if (cnt <= 0) break;
+                        Unit<T> ug = lds_unit<T>(base + off), us, uy;
+                        const Unit<T> usn = lds_unit<T>(base + TE + off), uyn = lds_unit<T>(base + 2 * TE + off);
+                        if (j == 0) { us = usn; uy = uyn; }
+                        else { us = lds_unit<T>(srow + off); uy = lds_unit<T>(yrow + off); }
+                        if (cnt < EPT) { mask_unit(ug, cnt); mask_unit(us, cnt); mask_unit(uy, cnt); }
+#pragma unroll
+                        for (int k = 0; k < EPT; k++)
+                        {
+                            acc[r][0] += us.v[k] * ug.v[k];
+                            acc[r][1] += uy.v[k] * ug.v[k];
+                        }
+#pragma unroll
+                        for (int k = 0; k < EPT; k++)
+                        {
+                            acc[r][2] += us.v[k] * uyn.v[k];
+                            acc[r][3] += uy.v[k] * uyn.v[k];
+                            acc[r][4] += uy.v[k] * usn.v[k];
+                            acc[r][5] += us.v[k] * usn.v[k];
+                        }
+                    }
+                }
+            }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // these reads before the bulk copies that re-arm the stage
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[stage]);
+        }
+        if (warp == 0 && next_tile < ntl)
+        {
+            mbar_wait(&empty_bar[stage], lap);
+            stage_tiled<T>(base, TE, NRHS, own.start(next_tile, TE), own.len(next_tile, TE), a.h, runs, sh, &full_bar[stage]);
+        }
+        next_tile++;
+        if (++stage == stages) { stage = 0; lap ^= 1u; }
+    }
+    // the full barriers: one completed phase per tile a stage carried (every thread keeps the same parities, waiting or not)
+    for (int s = 0; s < stages; s++)
+        if (s < ntl) phase_bits ^= (unsigned)(((ntl - 1 - s) / stages + 1) & 1) << s;
+
+    // block reduction: as p_dots (the forming warps without a column contribute zeros that nobody reads)
+#pragma unroll
+    for (int r = 0; r < ROUNDS; r++)
+#pragma unroll
+        for (int k = 0; k < kGramVals; k++)
+        {
+            const double w = warp_sum((double)acc[r][k]);
+            if (lane == 0) sh.red[warp][r * kGramVals + k] = w;
+        }
+    __syncthreads();   // (also: every arrival on and wait for the formed / empty barriers is done)
+    if (tid == 0)
+        for (int s = 0; s < stages; s++) { mbar_inval(&formed_bar[s]); mbar_inval(&empty_bar[s]); }
     const int nvals = a.c * kGramVals;
     for (int idx = tid; idx < nvals; idx += kPThreads)
     {
@@ -1159,8 +1307,12 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
                         else { sh.vecs[0] = vg; sh.vecs[1] = vx; sh.vecs[2] = vgp; sh.vecs[3] = vxp; }
                     }
                 }
-                if (form) p_dots<T, OBJ, ROUNDS, true>(d, obj, own, tiles, sh, phase_bits, dst, G);
-                else p_dots<T, OBJ, ROUNDS, false>(d, obj, own, tiles, sh, phase_bits, dst, G);
+                if (form)
+                {
+                    if constexpr (HALO) p_dots<T, ROUNDS, true>(d, own, tiles, sh, phase_bits, dst, G);
+                    else p_dots_implied<T, OBJ, ROUNDS>(d, obj, own, tiles, sh, phase_bits, dst, G);
+                }
+                else p_dots<T, ROUNDS, false>(d, own, tiles, sh, phase_bits, dst, G);
                 break;
             }
             case POP_COMBINE:

@@ -63,6 +63,14 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, unsigned bytes)
 {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void mbar_inval(uint64_t* bar)    // before the barrier's memory is initialised again
+{
+    asm volatile("mbarrier.inval.shared::cta.b64 [%0];" :: "r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar)   // one arrival, release semantics (the default of mbarrier.arrive)
+{
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(bar)) : "memory");
+}
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, unsigned parity)
 {
     unsigned ok;
