@@ -13,12 +13,16 @@
 //     COMBINE_TRIAL  COMBINE + the first trial of the next line search in the same pass: the reference restarts every search
 //                    at step = 1 (LBFGS.h:168), so x1 = x + d, g1 = grad f(x1) ; {g.d, f1, g1.d, g1.g1, x1.x1}
 //     RESTORE        x = xp, g = gp (a search that never improved on its start point; LineSearchMoreThuente.h:602-614)
-//     MATERIALIZE    x = xp + step*d, g = grad f(x) (or x = xp, g = gp): writes the point a finished problem stopped at
+//     MATERIALIZE    x = xp + step*d (or x = xp, or x as stored), g = grad f(x): writes the point a finished problem stopped at
 // Trials on the ray.  For objectives without neighbour coupling g = grad f(x) is a per-element function of x, and every trial point
-// is x = xp + step*d, so a trial stores nothing: its point is IMPLIED by {step, at_start} (the start point xp, gp when at_start).
-// The pass after the search -- DOTS_FORM, which reads x and g anyway -- rebuilds the accepted point from xp, d (or xp, gp) with the
-// trial's own arithmetic, bit for bit, writes x and g, and forms the pair from them; a problem that stops while its point is still
-// implied takes one MATERIALIZE round.  The kept best trial of a search is its step, so there is no x_lo/g_lo and no RESTORE pass.
+// is x = xp + step*d, so a trial stores nothing: its point is IMPLIED by {step, at_start} (PT_START: the start point xp).
+// The pass after the search -- DOTS_FORM, which reads the point anyway -- rebuilds the accepted point from xp, d with the trial's own
+// arithmetic, bit for bit, writes x, and forms the pair from it.  Nor is g itself stored between passes: the passes that need the
+// gradient of a stored point (gp = grad f(xp) in DOTS_FORM, g = grad f(x) in DOTS_PLAIN and COMBINE) evaluate it from that point
+// with the same arithmetic, bit for bit the g a pass would have stored; that spares DOTS_FORM the read of gp and the write of g and
+// COMBINE the read of g.  Only FIRST and MATERIALIZE write g: a problem that stops anywhere but at FIRST takes one MATERIALIZE round
+// for the point it stopped at -- on the ray, its search's start point, or the point in x (arming the next search failed).  The kept
+// best trial of a search is its step, so there is no x_lo/g_lo and no RESTORE pass.
 // Neighbour-coupled objectives (kHalo) store every trial's x, g and keep the best one by pointer swap with x_lo/g_lo, as the
 // reference's search does (LineSearchMoreThuente.h:534,553), and restore the start point with RESTORE.
 // Every CTA owns the same contiguous chunk (granularity: the block length of the tiled history) of EVERY vector in EVERY pass, so a CTA only ever reads vector
@@ -59,7 +63,7 @@ template <class T> struct alignas(128) PRound
     T *x, *xp, *g, *gp, *drt;
     T step;                     // TRIAL: the trial's step; DOTS_FORM / MATERIALIZE of an implied point: the step of that point
     int op, c_round, head, pending, gram_cur;
-    int at_start;               // DOTS_FORM / MATERIALIZE of an implied point: the point is (xp, gp)
+    int at_start;               // DOTS_FORM / MATERIALIZE of an implied point: which point (PT_RAY, PT_START, PT_X)
 };
 static_assert(sizeof(PRound<double>) == 128 && sizeof(PRound<float>) == 128, "a round descriptor is one 128-byte line");
 
@@ -167,9 +171,10 @@ template <int NV> __device__ __forceinline__ void block_sums(const double (&acc)
 
 // ---- FIRST / TRIAL -------------------------------------------------------------------------------------------------------------
 // MODE 0: FIRST (evaluate at x, write g and d = -g) ; MODE 1: TRIAL (evaluate at x = xp + step*d, store nothing: the point is
-// rebuilt by the pass that needs it) ; MODE 2: MATERIALIZE (x = xp + step*d, write x and g; no sums).  Operands stream through
-// registers with 128-bit loads/stores (a shared-memory staged variant measured slower for this 1:1 read/write pass).  Objectives
-// without neighbour coupling only: the coupled ones take p_trial_halo.
+// rebuilt by the pass that needs it) ; MODE 2: MATERIALIZE of a ray point (x = xp + step*d, write x and g; no sums) ; MODE 3:
+// MATERIALIZE of a stored point (evaluate at xp, write g, and x when given: the start point xp -> x, or the point in x itself with
+// xp = x, x = nullptr; no sums).  Operands stream through registers with 128-bit loads/stores (a shared-memory staged variant
+// measured slower for this 1:1 read/write pass).  Objectives without neighbour coupling only: the coupled ones take p_trial_halo.
 template <class T, class OBJ, int MODE>
 __device__ __forceinline__ void p_trial(const OBJ& obj, const Own& own, const T* __restrict__ xp, const T* __restrict__ d, T step,
                                         T* __restrict__ x, T* __restrict__ g, T* __restrict__ dout, PShared& sh, double* dst, int G, bool evict_first)
@@ -182,7 +187,7 @@ __device__ __forceinline__ void p_trial(const OBJ& obj, const Own& own, const T*
         const int64_t i0 = q << 2;
         const int cnt = (n - i0 >= 4) ? 4 : int(n - i0);
         T xv[4], dv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
-        if (MODE != 0)
+        if (MODE == 1 || MODE == 2)
         {
             const Pack<T> px = load4<T, Hint::Stream, true>(xp, i0, cnt), pd = load4<T, Hint::Stream, true>(d, i0, cnt);
 #pragma unroll
@@ -190,7 +195,7 @@ __device__ __forceinline__ void p_trial(const OBJ& obj, const Own& own, const T*
         }
         else
         {
-            const Pack<T> px = load4<T, Hint::Stream, true>(x, i0, cnt);
+            const Pack<T> px = load4<T, Hint::Stream, true>(MODE == 3 ? xp : x, i0, cnt);
 #pragma unroll
             for (int k = 0; k < 4; k++) xv[k] = px.v[k];
         }
@@ -199,15 +204,23 @@ __device__ __forceinline__ void p_trial(const OBJ& obj, const Own& own, const T*
         {
             Pack<T> pg, po;
 #pragma unroll
-            for (int k = 0; k < 4; k++) { pg.v[k] = gv[k]; po.v[k] = (MODE == 2) ? xv[k] : T(-1) * gv[k]; }
-            T* const out0 = (MODE == 2) ? x : dout;
-            if (evict_first) { store4<T, Hint::Stream, true>(out0, i0, cnt, po); store4<T, Hint::Stream, true>(g, i0, cnt, pg); }
-            else { store4<T, Hint::Plain, true>(out0, i0, cnt, po); store4<T, Hint::Plain, true>(g, i0, cnt, pg); }
+            for (int k = 0; k < 4; k++) { pg.v[k] = gv[k]; po.v[k] = (MODE >= 2) ? xv[k] : T(-1) * gv[k]; }
+            T* const out0 = (MODE >= 2) ? x : dout;
+            if (evict_first)
+            {
+                if (MODE != 3 || out0) store4<T, Hint::Stream, true>(out0, i0, cnt, po);
+                store4<T, Hint::Stream, true>(g, i0, cnt, pg);
+            }
+            else
+            {
+                if (MODE != 3 || out0) store4<T, Hint::Plain, true>(out0, i0, cnt, po);
+                store4<T, Hint::Plain, true>(g, i0, cnt, pg);
+            }
         }
     };
 #pragma unroll 2
     for (int64_t q = (own.c0 >> 2) + threadIdx.x; q < p1; q += kPThreads) body(q);
-    if constexpr (MODE != 2)
+    if constexpr (MODE < 2)
     {
         const double dacc[4] = {(double)acc[0], (double)acc[1], (double)acc[2], (double)acc[3]};
         block_sums<4>(dacc, sh, dst, G);
@@ -311,7 +324,7 @@ __device__ __forceinline__ void p_trial_halo(const OBJ& obj, const Own& own, con
     block_sums<4>(dacc, sh, dst, G);
 }
 
-// ---- RESTORE (and MATERIALIZE of a search's start point) ----------------------------------------------------------------------
+// ---- RESTORE (neighbour-coupled objectives) -----------------------------------------------------------------------------------
 template <class T>
 __device__ __forceinline__ void p_restore(const Own& own, const T* __restrict__ xp, const T* __restrict__ gp, T* __restrict__ x, T* __restrict__ g)
 {
@@ -360,11 +373,12 @@ template <class T> __device__ __forceinline__ void mask_unit(Unit<T>& u, int cnt
     for (int k = 0; k < 16 / (int)sizeof(T); k++) u.v[k] = (k < cnt) ? u.v[k] : T(0);
 }
 
-// copies of one tile: `nrhs` right-hand vectors (sh.vecs[0..nrhs), round_up(len, 32) elements each) + the history runs of block
-// `blk`; one lane per copy.  Returns nothing; the stage's barrier has been told the byte count.
+// copies of one tile: `nrhs` right-hand rows, of which the first `nload` are loaded (sh.vecs[0..nload), round_up(len, 32) elements
+// each) and the others are left for the pass to fill, + the history runs of block `blk`; one lane per copy.  Returns nothing; the
+// stage's barrier has been told the byte count.
 template <class T>
-__device__ __forceinline__ void stage_tiled(T* dstt, int TE, int nrhs, int64_t e0, int len, const PHist<T>& h, const SlotRuns& runs, PShared& sh,
-                                            uint64_t* bar)
+__device__ __forceinline__ void stage_tiled(T* dstt, int TE, int nrhs, int nload, int64_t e0, int len, const PHist<T>& h, const SlotRuns& runs,
+                                            PShared& sh, uint64_t* bar)
 {
     const int tid = threadIdx.x;
     if (tid >= 32) return;
@@ -374,11 +388,11 @@ __device__ __forceinline__ void stage_tiled(T* dstt, int TE, int nrhs, int64_t e
     if (tid == 0)
     {
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy accesses of this stage before the copies that overwrite it
-        mbar_expect_tx(bar, rbytes * (unsigned)nrhs + abytes + bbytes);
+        mbar_expect_tx(bar, rbytes * (unsigned)nload + abytes + bbytes);
     }
     __syncwarp();
     const T* blk = h.H + (e0 >> h.bt_log) * h.bstride;
-    if (tid < nrhs) tma_load_1d(dstt + (size_t)tid * TE, static_cast<const T*>(sh.vecs[tid]) + e0, rbytes, bar);
+    if (tid < nload) tma_load_1d(dstt + (size_t)tid * TE, static_cast<const T*>(sh.vecs[tid]) + e0, rbytes, bar);
     else if (tid == nrhs && abytes) tma_load_1d(dstt + (size_t)nrhs * TE, blk + (size_t)runs.a0 * 2 * TE, abytes, bar);
     else if (tid == nrhs + 1 && bbytes) tma_load_1d(dstt + (size_t)(nrhs + 2 * (runs.a1 - runs.a0)) * TE, blk + (size_t)runs.b0 * 2 * TE, bbytes, bar);
 }
@@ -388,7 +402,8 @@ __device__ __forceinline__ void stage_tiled(T* dstt, int TE, int nrhs, int64_t e
 // point, neighbour-coupled objectives): the newest pair s = x - xp, y = g - gp is formed on the fly from the staged rows {g, x, gp, xp},
 // identically in every warp that needs it, takes part as column 0 and is written to ring slot `new_slot` by the warps that own
 // column 0.  An implied point (p_dots_implied) is formed once per element instead, see there.
-// Column j (by age) belongs to warp group j, whose `split` warps share the tile's units.  PLAIN: s.v and y.v over the old history only.
+// Column j (by age) belongs to warp group j, whose `split` warps share the tile's units.  PLAIN: s.g and y.g over the old history only;
+// for an objective without neighbour coupling g is not stored: x is staged and every column warp evaluates g = grad f(x) of its units.
 template <class T> struct PDots
 {
     int64_t n;
@@ -396,16 +411,19 @@ template <class T> struct PDots
     int c;               // columns taking part (FORM: including the new pair)
     int end, cnt_old;    // the old columns: the cnt_old slots below `end`
     int new_slot, split, cols_per_round;
-    T step;              // FORM of an implied point: its step, or (at_start) the start point
+    T step;              // FORM of an implied point: its step (PT_RAY), or the start point (PT_START)
     int at_start;
-    T *x, *g;            // FORM of an implied point: where it is written
+    T* x;                // FORM of an implied point: where it is written
 };
 
-template <class T, int ROUNDS, bool FORM>
-__device__ __forceinline__ void p_dots(const PDots<T>& a, const Own& own, T* tiles, PShared& sh, unsigned& phase_bits, double* dst, int G)
+template <class T, class OBJ, int ROUNDS, bool FORM>
+__device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const Own& own, T* tiles, PShared& sh, unsigned& phase_bits, double* dst,
+                                       int G)
 {
     constexpr int EPT = 16 / (int)sizeof(T);
-    constexpr int NRHS = FORM ? 4 : 1;                           // staged right-hand vectors: g, x, gp, xp / g
+    constexpr bool G_IMPLIED = !OBJ::kHalo;
+    static_assert(!(FORM && G_IMPLIED), "an implied point is formed by p_dots_implied");
+    constexpr int NRHS = FORM ? 4 : 1;                           // staged right-hand vectors: g, x, gp, xp / g (G_IMPLIED: x)
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int TE = a.h.BT();
     const int my_col = warp / a.split, my_part = warp % a.split;
@@ -426,7 +444,7 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const Own& own, T* til
     __syncthreads();   // sh.vecs / sh.slots are in place and the staging ring is free
     int64_t next_tile = 0;
     for (int s = 0; s < stages; s++, next_tile++)
-        if (next_tile < ntl) stage_tiled<T>(tiles + (size_t)s * nrows * TE, TE, NRHS, own.start(next_tile, TE), own.len(next_tile, TE), a.h, runs, sh, &full_bar[s]);
+        if (next_tile < ntl) stage_tiled<T>(tiles + (size_t)s * nrows * TE, TE, NRHS, NRHS, own.start(next_tile, TE), own.len(next_tile, TE), a.h, runs, sh, &full_bar[s]);
     int stage = 0;
     for (int64_t t = 0; t < ntl; t++)
     {
@@ -462,6 +480,18 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const Own& own, T* til
 #pragma unroll
                         for (int k = 0; k < EPT; k++) { usn.v[k] = ux.v[k] - uxp.v[k]; uyn.v[k] = ug.v[k] - ugp.v[k]; }
                         if (cnt < EPT) { mask_unit(usn, cnt); mask_unit(uyn, cnt); }
+                    }
+                    else if constexpr (G_IMPLIED)
+                    {
+                        // the arithmetic of every pass that evaluates the objective: bit for bit the g a stored point would have
+                        const Unit<T> uxs = lds_unit<T>(base + off);
+                        const int c4 = cnt < EPT ? cnt : EPT;
+                        T xv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
+#pragma unroll
+                        for (int k = 0; k < EPT; k++) xv[k] = (k < c4) ? uxs.v[k] : T(0);
+                        obj.eval(e0 + off, c4, xv, T(0), T(0), gv);
+#pragma unroll
+                        for (int k = 0; k < EPT; k++) ug.v[k] = gv[k];
                     }
                     else ug = lds_unit<T>(base + off);
                     bool loaded = false;
@@ -499,7 +529,7 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const Own& own, T* til
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncthreads();
-        if (next_tile < ntl) stage_tiled<T>(tiles + (size_t)stage * nrows * TE, TE, NRHS, own.start(next_tile, TE), own.len(next_tile, TE), a.h, runs, sh, &full_bar[stage]);
+        if (next_tile < ntl) stage_tiled<T>(tiles + (size_t)stage * nrows * TE, TE, NRHS, NRHS, own.start(next_tile, TE), own.len(next_tile, TE), a.h, runs, sh, &full_bar[stage]);
         next_tile++;
         stage = (stage + 1 == stages) ? 0 : stage + 1;
     }
@@ -526,9 +556,11 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const Own& own, T* til
 }
 
 // DOTS_FORM of an implied point (objectives without neighbour coupling): the sums of p_dots<FORM>, with the point rebuilt from the
-// staged rows {d, xp, gp} ONCE per element.  The forming warps take every unit of a staged tile: x = xp + step*d, g = grad f(x) with
-// the trial's own arithmetic (or x = xp, g = gp when the search ended on its start point), s = x - xp, y = g - gp; they write x, g and
-// the pair to HBM and g, s, y over d, xp, gp in the stage.  The column groups then read those rows.  The forming warps are the ones
+// staged rows {d, xp} ONCE per element.  Neither gradient is read: both are element-wise functions of a point the pass has, and the
+// objective's arithmetic gives them bit for bit as stored.  The forming warps take every unit of a staged tile: gp = grad f(xp),
+// x = xp + step*d, g = grad f(x) with the trial's own arithmetic (or x = xp, g = gp when the search ended on its start point),
+// s = x - xp, y = g - gp; they write x and the pair to HBM (g is not stored: the next pass evaluates it from x) and g, s, y into the
+// stage's three right-hand rows (d, xp and one row no copy fills).  The column groups then read those rows.  The forming warps are the ones
 // dots_geometry leaves without a column (c = 10: 4 of 24) or, when every warp has a column (c = 3, 6, 12, ...), the warps of
 // column 0, which form a tile before taking their own dots of it.  Split, columns and the unit-to-lane mapping are p_dots', and so is
 // every accumulator: the sums are bit-identical to forming the point in every column group.
@@ -541,7 +573,7 @@ __device__ __forceinline__ void p_dots_implied(const PDots<T>& a, const OBJ& obj
 {
     static_assert(!OBJ::kHalo, "neighbour-coupled objectives store their trial points: p_dots<FORM>");
     constexpr int EPT = 16 / (int)sizeof(T);
-    constexpr int NRHS = 3;                                      // staged right-hand vectors: d, xp, gp, formed into g, s_new, y_new
+    constexpr int NRHS = 3, NLOAD = 2;                           // right-hand rows: d, xp staged, formed into g, s_new, y_new
     __shared__ uint64_t formed_bar[kPMaxStages], empty_bar[kPMaxStages];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int TE = a.h.BT();
@@ -571,7 +603,7 @@ __device__ __forceinline__ void p_dots_implied(const PDots<T>& a, const OBJ& obj
     __syncthreads();   // sh.vecs / sh.slots and the barriers are in place, the staging ring is free
     int64_t next_tile = 0;
     for (int s = 0; s < stages; s++, next_tile++)
-        if (next_tile < ntl) stage_tiled<T>(tiles + (size_t)s * nrows * TE, TE, NRHS, own.start(next_tile, TE), own.len(next_tile, TE), a.h, runs, sh, &full_bar[s]);
+        if (next_tile < ntl) stage_tiled<T>(tiles + (size_t)s * nrows * TE, TE, NRHS, NLOAD, own.start(next_tile, TE), own.len(next_tile, TE), a.h, runs, sh, &full_bar[s]);
     const unsigned full_phase = phase_bits;
     int stage = 0;
     unsigned lap = 0;                                            // parity of the current use of `stage` in this pass
@@ -592,13 +624,20 @@ __device__ __forceinline__ void p_dots_implied(const PDots<T>& a, const OBJ& obj
                 if (cnt <= 0) break;
                 const Unit<T> ud = lds_unit<T>(base + off);
                 const Unit<T> uxp = lds_unit<T>(base + TE + off);
-                const Unit<T> ugp = lds_unit<T>(base + 2 * TE + off);
-                Unit<T> ux, ug, usn, uyn;
+                const int c4 = cnt < EPT ? cnt : EPT;
+                Unit<T> ux, ug, ugp, usn, uyn;
+                {
+                    T xv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
+#pragma unroll
+                    for (int k = 0; k < EPT; k++) xv[k] = (k < c4) ? uxp.v[k] : T(0);
+                    obj.eval(e0 + off, c4, xv, T(0), T(0), gv);
+#pragma unroll
+                    for (int k = 0; k < EPT; k++) ugp.v[k] = gv[k];
+                }
                 if (a.at_start) { ux = uxp; ug = ugp; }
                 else
                 {
                     // the trial's arithmetic (p_trial, and p_combine's first trial with step 1 on the stored d)
-                    const int c4 = cnt < EPT ? cnt : EPT;
                     T xv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
 #pragma unroll
                     for (int k = 0; k < EPT; k++) xv[k] = (k < c4) ? uxp.v[k] + a.step * ud.v[k] : T(0);
@@ -612,7 +651,6 @@ __device__ __forceinline__ void p_dots_implied(const PDots<T>& a, const OBJ& obj
                 st_unit<T>(s_new, off, cnt, usn);
                 st_unit<T>(s_new + TE, off, cnt, uyn);
                 st_unit<T>(a.x, e0 + off, cnt, ux);
-                st_unit<T>(a.g, e0 + off, cnt, ug);
                 *reinterpret_cast<float4*>(base + off) = *reinterpret_cast<const float4*>(ug.v);
                 *reinterpret_cast<float4*>(base + TE + off) = *reinterpret_cast<const float4*>(usn.v);
                 *reinterpret_cast<float4*>(base + 2 * TE + off) = *reinterpret_cast<const float4*>(uyn.v);
@@ -666,7 +704,7 @@ __device__ __forceinline__ void p_dots_implied(const PDots<T>& a, const OBJ& obj
         if (warp == 0 && next_tile < ntl)
         {
             mbar_wait(&empty_bar[stage], lap);
-            stage_tiled<T>(base, TE, NRHS, own.start(next_tile, TE), own.len(next_tile, TE), a.h, runs, sh, &full_bar[stage]);
+            stage_tiled<T>(base, TE, NRHS, NLOAD, own.start(next_tile, TE), own.len(next_tile, TE), a.h, runs, sh, &full_bar[stage]);
         }
         next_tile++;
         if (++stage == stages) { stage = 0; lap ^= 1u; }
@@ -709,7 +747,9 @@ __device__ __forceinline__ void dots_geometry(int c, int units, int& split, int&
 // ---- COMBINE (+ first trial) ---------------------------------------------------------------------------------------------------
 // d = cv*v + sum_j cy_j*y_j + cs_j*s_j ; FUSE: x1 = xc + d, g1 = grad f(x1) and the four trial sums (neighbour-coupled objectives:
 // x1, g1 written to (x1_out, g1_out)).
-// Staged rows of a tile: v, (xc,) then the history block's live slots; sh.slots[j] = packed row of the pair of age j.  A thread owns
+// Staged rows of a tile: v, (xc,) then the history block's live slots; sh.slots[j] = packed row of the pair of age j.  Objectives
+// without neighbour coupling (G_IMPLIED): v = grad f(xc) is not stored; xc is staged alone and each thread evaluates v of its unit
+// with the objective's arithmetic, bit for bit the stored gradient.  A thread owns
 // one 16-byte unit of the tile and adds the terms in the order the recursion would (y newest -> oldest, then s oldest -> newest), with
 // the operand loads of 8 columns in flight before their multiply-adds retire (the pass is bound by shared-memory latency otherwise).
 // HALO (neighbour-coupled objectives, one GPU): x1 goes back into the staged x row, two spare warps form d and x1 of the element on
@@ -723,8 +763,9 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
                                           Between between)
 {
     constexpr int EPT = 16 / (int)sizeof(T);
+    constexpr bool G_IMPLIED = !OBJ::kHalo;
     constexpr int DV = HALO ? OBJ::kDataVectors : 0;              // HALO: the objective's data vectors ride in the stage as well
-    constexpr int NRHS = (FUSE ? 2 : 1) + DV;                     // v (, xc) (, data0, data1)
+    constexpr int NRHS = G_IMPLIED ? 1 : (FUSE ? 2 : 1) + DV;     // v (, xc) (, data0, data1) / xc
     constexpr int PAD = EPT;                                      // HALO: room for x1 of the neighbouring element on either side of the x row
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int TE = h.BT();
@@ -740,7 +781,7 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
     // HALO: the x row is staged one granule into the stage (row 1 starts at TE + PAD), everything after it shifts by 2*PAD
     auto stage_one = [&](int64_t t, int s) {
         T* dstt = tiles + (size_t)s * stage_elems;
-        if (!HALO) { stage_tiled<T>(dstt, TE, NRHS, own.start(t, TE), own.len(t, TE), h, runs, sh, &full_bar[s]); return; }
+        if (!HALO) { stage_tiled<T>(dstt, TE, NRHS, NRHS, own.start(t, TE), own.len(t, TE), h, runs, sh, &full_bar[s]); return; }
         if (tid >= 32) return;
         const int64_t e0 = own.start(t, TE);
         const int len = own.len(t, TE);
@@ -791,14 +832,14 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
     {
         mbar_wait(&full_bar[stage], (phase_bits >> stage) & 1u);
         phase_bits ^= (1u << stage);
-        T* base = tiles + (size_t)stage * stage_elems;                          // row 0: v
-        T* xrow = base + TE + (HALO ? PAD : 0);                                   // row 1: xc (FUSE)
+        T* base = tiles + (size_t)stage * stage_elems;                          // row 0: v (G_IMPLIED: xc)
+        T* xrow = base + (G_IMPLIED ? 0 : TE) + (HALO ? PAD : 0);               // row 1: xc (FUSE)
         const T* hist = base + (size_t)NRHS * TE + (HALO ? 2 * PAD : 0);
         const int len = own.len(t, TE);
         const int64_t e0 = own.start(t, TE);
-        // d of one unit: the arithmetic every owner of an element uses
+        // d of one unit: the arithmetic every owner of an element uses (G_IMPLIED: uv comes in evaluated)
         auto direction = [&](int off, T (&r)[EPT], Unit<T>& uv) {
-            uv = lds_unit<T>(base + off);
+            if constexpr (!G_IMPLIED) uv = lds_unit<T>(base + off);
 #pragma unroll
             for (int k = 0; k < EPT; k++) r[k] = cv * uv.v[k];
 #pragma unroll 8
@@ -825,6 +866,16 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
                 const int cnt = (len - off >= EPT) ? EPT : (len - off);
                 T r[EPT];
                 Unit<T> uv;
+                if constexpr (G_IMPLIED)
+                {
+                    const Unit<T> ux = lds_unit<T>(xrow + off);
+                    T xv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
+#pragma unroll
+                    for (int k = 0; k < EPT; k++) xv[k] = (k < cnt) ? ux.v[k] : T(0);
+                    obj.eval(e0 + off, cnt, xv, T(0), T(0), gv);
+#pragma unroll
+                    for (int k = 0; k < EPT; k++) uv.v[k] = gv[k];
+                }
                 direction(off, r, uv);
                 Unit<T> out;
 #pragma unroll
@@ -969,19 +1020,20 @@ __device__ __forceinline__ void st_release_gpu_u32(unsigned* p, unsigned v)
 }
 
 // n-words a pass has to move (reads + writes of whole vectors): the roofline numerator of the persistent kernel.  stored: the
-// trials store their points (neighbour-coupled objectives)
-__device__ __forceinline__ double words_of(int op, int c, int data_vectors, bool stored)
+// trials store their points and every pass reads the stored g (neighbour-coupled objectives); otherwise g is evaluated from x
+// wherever it is needed, and only FIRST and MATERIALIZE write it.  pt: the point a MATERIALIZE writes (PT_*)
+__device__ __forceinline__ double words_of(int op, int c, int data_vectors, bool stored, int pt)
 {
     switch (op)
     {
     case POP_FIRST: return 3.0 + data_vectors;              // R x ; W g, d
     case POP_TRIAL: return (stored ? 4.0 : 2.0) + data_vectors;   // R xp, d (; W x, g)
     case POP_RESTORE: return 4.0;                           // R xp, gp ; W x, g
-    case POP_MATERIALIZE: return 4.0;                       // R xp, d (or gp) ; W x, g
-    case POP_DOTS_FORM: return 2.0 * c + (stored ? 4.0 : 5.0);   // R x, xp, g, gp / xp, d, gp, 2(c-1) columns ; (W x, g,) W s, y
-    case POP_DOTS_PLAIN: return 2.0 * c + 1.0;              // R g, 2c columns
-    case POP_COMBINE: return 2.0 * c + 2.0;                 // R g, 2c columns ; W d
-    case POP_COMBINE_TRIAL: return 2.0 * c + (stored ? 5.0 : 3.0) + data_vectors;   // R g, x, 2c columns ; W d (, x1, g1)
+    case POP_MATERIALIZE: return stored || pt == PT_RAY ? 4.0 : (pt == PT_START ? 3.0 : 2.0);   // R xp, d / xp / x ; W x, g / x, g / g
+    case POP_DOTS_FORM: return 2.0 * c + (stored ? 4.0 : 3.0);   // R x, xp, g, gp / xp, d, 2(c-1) columns ; (W x, g / W x,) W s, y
+    case POP_DOTS_PLAIN: return 2.0 * c + 1.0;              // R g (or x), 2c columns
+    case POP_COMBINE: return 2.0 * c + 2.0;                 // R g (or x), 2c columns ; W d
+    case POP_COMBINE_TRIAL: return 2.0 * c + (stored ? 5.0 : 2.0) + data_vectors;   // R g, x (or x), 2c columns ; W d (, x1, g1)
     default: return 0.0;
     }
 }
@@ -1100,7 +1152,7 @@ __device__ int leader_round(const PArgs<T>& a, int G, PShared& sh, PState<T>* ca
         if (b < a.B && state_of(b)->op != POP_IDLE)
         {
             PState<T>* st = state_of(b);
-            advance_problem<T, HALO>(st, st->raw);
+            advance_problem<T, HALO, !HALO>(st, st->raw);
             PRound<T>* rd = a.rounds + b;
             rd->x = st->x; rd->xp = st->xp; rd->g = st->g; rd->gp = st->gp; rd->drt = st->drt;
             rd->step = st->step; rd->at_start = st->at_start;
@@ -1261,7 +1313,7 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
             const int at_start = ldv(&rd->at_start);
             if (op == POP_IDLE) continue;
             acct_bucket = (acct_bucket == -1 || acct_bucket == op) ? op : 0;
-            acct_words += words_of(op, c_round, kDataVectors, HALO);
+            acct_words += words_of(op, c_round, kDataVectors, HALO, at_start);
             double* dst = a.partials + (size_t)b * a.pstride * G + cta;
             const OBJ obj{ObjGeom<T>{a.n, a.index_offset, a.n_global, (HALO && a.xc != nullptr) ? st->halo : nullptr, st->data0, st->data1}};
             switch (op)
@@ -1280,8 +1332,12 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
             case POP_MATERIALIZE:
                 if constexpr (!HALO)
                 {
-                    if (at_start) p_restore<T>(own, vxp, vgp, vx, vg);
-                    else p_trial<T, OBJ, 2>(obj, own, vxp, vd, step, vx, vg, nullptr, sh, dst, G, a.evict_first_stores);
+                    if (at_start == PT_RAY) p_trial<T, OBJ, 2>(obj, own, vxp, vd, step, vx, vg, nullptr, sh, dst, G, a.evict_first_stores);
+                    else   // PT_START: x = xp, g = grad f(xp) ; PT_X: g = grad f(x)
+                    {
+                        const bool start = at_start == PT_START;
+                        p_trial<T, OBJ, 3>(obj, own, start ? vxp : vx, nullptr, T(0), start ? vx : nullptr, vg, nullptr, sh, dst, G, a.evict_first_stores);
+                    }
                 }
                 break;
             case POP_DOTS_FORM:
@@ -1293,7 +1349,7 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
                 d.end = head;                                   // the old columns: the slots below the free slot `head`
                 d.cnt_old = form ? c_round - 1 : c_round;
                 d.new_slot = form ? head : -1;
-                d.step = step; d.at_start = at_start; d.x = vx; d.g = vg;
+                d.step = step; d.at_start = at_start; d.x = vx;
                 dots_geometry(d.c, d.h.BT() / (16 / (int)sizeof(T)), d.split, d.cols_per_round);
                 __syncthreads();   // sh.slots / sh.vecs may still be read by the previous problem's pass
                 {
@@ -1303,16 +1359,16 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
                         sh.slots[tid] = (unsigned char)runs.row_of(slot_by_age(head, d.h.M, form ? tid - 1 : tid));
                     if (tid == 0)
                     {
-                        if (form && !HALO) { sh.vecs[0] = vd; sh.vecs[1] = vxp; sh.vecs[2] = vgp; }   // the point is rebuilt from them
+                        if (!HALO) { sh.vecs[0] = form ? vd : vx; sh.vecs[1] = vxp; }   // the point is rebuilt from d, xp / g from x
                         else { sh.vecs[0] = vg; sh.vecs[1] = vx; sh.vecs[2] = vgp; sh.vecs[3] = vxp; }
                     }
                 }
                 if (form)
                 {
-                    if constexpr (HALO) p_dots<T, ROUNDS, true>(d, own, tiles, sh, phase_bits, dst, G);
+                    if constexpr (HALO) p_dots<T, OBJ, ROUNDS, true>(d, obj, own, tiles, sh, phase_bits, dst, G);
                     else p_dots_implied<T, OBJ, ROUNDS>(d, obj, own, tiles, sh, phase_bits, dst, G);
                 }
-                else p_dots<T, ROUNDS, false>(d, own, tiles, sh, phase_bits, dst, G);
+                else p_dots<T, OBJ, ROUNDS, false>(d, obj, own, tiles, sh, phase_bits, dst, G);
                 break;
             }
             case POP_COMBINE:
@@ -1337,7 +1393,7 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
                         sh.slots[j] = (unsigned char)runs.row_of(g.slots[j]);
                         sh.slotid[j] = g.slots[j];
                     }
-                    if (tid == 0) { sh.vecs[0] = vg; sh.vecs[1] = vx; sh.vecs[2] = st->data0; sh.vecs[3] = st->data1; }
+                    if (tid == 0) { sh.vecs[0] = HALO ? vg : vx; sh.vecs[1] = vx; sh.vecs[2] = st->data0; sh.vecs[3] = st->data1; }   // (!HALO: g is evaluated from x)
                 }
                 // the coefficient recursion (every CTA; CTA 0 also writes the folded Gram matrices back) and its 2c+1 results into sh.coef
                 const bool own_scratch = gram_solve_smem_elems(g.c) * sizeof(T) <= sizeof(s_gram);

@@ -17,6 +17,10 @@ constexpr int kMaxPast = 64;
 enum { POP_IDLE = 0, POP_FIRST = 1, POP_TRIAL = 2, POP_DOTS_FORM = 3, POP_DOTS_PLAIN = 4, POP_COMBINE = 5, POP_COMBINE_TRIAL = 6, POP_RESTORE = 7,
        POP_MATERIALIZE = 8 };
 
+// which point an implied (x, g) stands for (PState::at_start): the ray point xp + step*d, the search's start point, or (only when
+// the gradient itself is implied, G_IMPLIED below) the point already in x, whose g is grad f(x) but not stored
+enum { PT_RAY = 0, PT_START = 1, PT_X = 2 };
+
 // ---- the S/Y history of the solve: tiled layout ---------------------------------------------------------------------------------
 // H[block][slot][S|Y][BT]: all ring slots of one block of BT coordinates lie next to each other (BT = the largest power of two for
 // which two stages of 2m+4 rows fit the kernel's shared memory: 512 for fp64 m = 10).  A pass over a tile then needs the right-hand
@@ -57,7 +61,7 @@ template <class T> struct PState
     LBFGSpp::RunTimeCore<T> ls;
     LBFGSpp::SearchRecord<T> rec;   // fx, dg, gg, xx of the current point
     // iteration scalars.  step: the trial to evaluate, or (objectives without neighbour coupling) the step of the point (x, g)
-    // stand for while they are implied; step_kept: the step of the search's kept trial; at_start: the point is the search's start
+    // stand for while they are implied; step_kept: the step of the search's kept trial; at_start: which point they stand for (PT_*)
     T gnorm, step, step_kept;
     int at_start;
     int k;
@@ -129,19 +133,25 @@ template <class T, bool STORED> __device__ __forceinline__ void digest_trial(PSt
         break;
     case LBFGSpp::SEARCH_TAKE_START:
         if (STORED) { st->op = POP_RESTORE; return; }   // copy xp/gp back, then carry on
-        st->at_start = 1;
+        st->at_start = PT_START;
         break;
     }
     after_search<T, STORED>(st);
 }
 
-// top of an iteration (LBFGS.h:121-127): the search is armed, the current point becomes the previous one
-template <class T> __device__ __forceinline__ bool begin_search(PState<T>* st, T step)
+// top of an iteration (LBFGS.h:121-127): the search is armed, the current point becomes the previous one.  G_IMPLIED: only x of
+// the current point is stored (the pair-forming pass of an objective without neighbour coupling does not write g)
+template <class T, bool G_IMPLIED = false> __device__ __forceinline__ bool begin_search(PState<T>* st, T step)
 {
     // the search validates its inputs before anything moves (the reference throws before touching x): on failure x stays the
-    // current point (it is in (x, g): FIRST or the pair-forming pass wrote it)
+    // current point (FIRST or the pair-forming pass wrote it; G_IMPLIED: one MATERIALIZE round writes its g)
     const int rc = st->ls.init(st->ls_opt, st->rec.fx, st->rec.dg, step, st->max_step);
-    if (rc != 0) { finish(st, st->k, rc); return false; }
+    if (rc != 0)
+    {
+        if (G_IMPLIED) st->at_start = PT_X;
+        finish(st, st->k, rc, G_IMPLIED);
+        return false;
+    }
     dswap(st->xp, st->x);
     dswap(st->gp, st->g);
     st->rec.begin();
@@ -151,7 +161,9 @@ template <class T> __device__ __forceinline__ bool begin_search(PState<T>* st, T
     return true;
 }
 
-template <class T, bool STORED> __device__ void advance_problem(PState<T>* st, const double* vals)
+// G_IMPLIED (the resident solve, objectives without neighbour coupling): g is stored by FIRST and MATERIALIZE only; every other pass
+// that needs grad f of a stored point evaluates it from x, bit for bit the g that would have been stored
+template <class T, bool STORED, bool G_IMPLIED = false> __device__ void advance_problem(PState<T>* st, const double* vals)
 {
     st->rounds++;
     switch (st->op)
@@ -206,7 +218,7 @@ template <class T, bool STORED> __device__ void advance_problem(PState<T>* st, c
         if (st->pending >= 0) { st->gram_cur = 1 - st->gram_cur; st->pending = -1; }
         st->rec.dg = (T)vals[0];            // LBFGS.h:123 for the next pass
         st->k += 1;
-        if (!begin_search(st, T(1))) return;   // LBFGS.h:168
+        if (!begin_search<T, G_IMPLIED>(st, T(1))) return;   // LBFGS.h:168
         // the pass already evaluated xp + 1*d (STORED: into the buffers that the rotation just made (x, g))
         if (fused && st->ls.step() == T(1)) digest_trial<T, STORED>(st, (T)vals[1], (T)vals[2], (T)vals[3], (T)vals[4]);
         return;
