@@ -306,7 +306,11 @@ const void* lbfgs_b200_solver_final_grad(const lbfgs_b200_solver* s);   /* devic
 const void* lbfgs_b200_solver_final_grad_of(const lbfgs_b200_solver* s, int problem);
 lbfgs_b200_hist* lbfgs_b200_solver_history(lbfgs_b200_solver* s);       /* the S/Y ring of problem 0 as left by the last solve   */
 lbfgs_b200_hist* lbfgs_b200_solver_history_of(lbfgs_b200_solver* s, int problem);
-/* x_inout: device vector (start point in, solution out).  trace_host (optional): f of every evaluation. */
+/* x_inout: device vector (start point in, solution out).  trace_host (optional): f of every evaluation.
+ * data0/data1 (as the objective needs, here and in the batch entry points below): device vectors that start on a 16-byte boundary.
+ * The solve reads each problem's data with bulk copies of whole 32-element groups, up to round_up(n, 32) elements from its start
+ * (the values past n are not used); a vector of n elements from lbfgs_b200_malloc has that room.  LBFGS_B200_ERR_INVALID, before
+ * anything is launched, for a misaligned data vector. */
 lbfgs_b200_status lbfgs_b200_solver_minimize_f64(lbfgs_b200_solver* s, int objective, const double* data0, const double* data1,
                                                  const lbfgs_b200_param* prm, int line_search, double* x_inout,
                                                  double* trace_host, long long trace_cap, lbfgs_b200_outcome* out);
@@ -314,7 +318,9 @@ lbfgs_b200_status lbfgs_b200_solver_minimize_f32(lbfgs_b200_solver* s, int objec
                                                  const lbfgs_b200_param* prm, int line_search, float* x_inout,
                                                  double* trace_host, long long trace_cap, lbfgs_b200_outcome* out);
 /* Batch: problem b starts from x_inout + b*ldx (device) and leaves its solution there; data0/data1 (optional) per problem at
- * data + b*ldd (ldd = 0: shared by all problems); outs[batch]. */
+ * data + b*ldd (ldd = 0: shared by all problems); outs[batch].  ldd must be 0 or at least n, and ldd*elem_bytes a multiple of 16, so
+ * that every problem's data starts on a 16-byte boundary; the buffers must hold (batch-1)*ldd + round_up(n, 32) elements.
+ * LBFGS_B200_ERR_INVALID, before anything is launched, otherwise. */
 lbfgs_b200_status lbfgs_b200_solver_minimize_batch_f64(lbfgs_b200_solver* s, int objective, const double* data0, const double* data1,
                                                        int64_t ldd, const lbfgs_b200_param* prm, int line_search, double* x_inout,
                                                        int64_t ldx, lbfgs_b200_outcome* outs);

@@ -58,6 +58,12 @@ static lbfgs_b200_status solver_minimize(lbfgs_b200_solver* s, int objective, co
     REQUIRE(ctx, prm->past <= kMaxPast, "past > %d is not supported by the device-resident solve", kMaxPast);
     REQUIRE(ctx, ctx->nranks == 1 || ctx->x_active, "the device-resident solve needs the in-kernel exchange (comm_p2p) when sharded");
     REQUIRE(ctx, B == 1 || ldx >= s->n, "solver_minimize: the batch stride of x is shorter than n");
+    // the passes read a problem's data with bulk copies that start on 16-byte boundaries of data + b*ldd
+    REQUIRE(ctx, ldd == 0 || ldd >= s->n, "solver_minimize: the batch stride of the data (%lld) must be 0 (shared) or at least n (%lld)",
+            (long long)ldd, (long long)s->n);
+    REQUIRE(ctx, ldd * (int64_t)sizeof(T) % 16 == 0, "solver_minimize: the batch stride of the data (%lld elements) must be a multiple of 16 bytes",
+            (long long)ldd);
+    REQUIRE(ctx, (uintptr_t)data0 % 16 == 0 && (uintptr_t)data1 % 16 == 0, "solver_minimize: the data vectors must start on a 16-byte boundary");
     REQUIRE(ctx, trace_host == nullptr || B == 1, "solver_minimize: traces are recorded for single problems only");
     if (ctx->x_active) REQUIRE(ctx, (size_t)B * (s->pstride + 4) <= (size_t)kXMaxVals, "batch of %d problems with m = %d exceeds the exchange buffer", B, s->m);
     const int rounds = (s->m + kGramMaxWarps - 1) / kGramMaxWarps;   // column pairs per round of the dots pass: at most one per warp

@@ -1,5 +1,5 @@
 """Small whole solves for tests/gpu_sanitize.sh (compute-sanitizer target; not collected by pytest): both solver loops, all four line
-searches, the neighbour-coupled objectives (staged tiles with margins), fp32, a batch, the literal two-loop recursion, L-BFGS-B."""
+searches, the neighbour-coupled objectives (staged tiles with margins, fp32 at odd n, a batch with per-problem data), fp32, a batch, the literal two-loop recursion, L-BFGS-B."""
 import os
 import sys
 
@@ -23,6 +23,18 @@ for resident in (False, True):
     print("chained", "resident" if resident else "host", g["status"], g["niter"], g["nfev"], g["fx"])
 g = lb.LBFGSSolver(lb.LBFGSParam(), "MoreThuente", dtype=np.float32, resident=True).minimize(lb.OBJ_ROSENBROCK_PAIRED, np.zeros(4096))
 print("lbfgs f32 resident", g["status"], g["niter"], g["fx"])
+g = lb.LBFGSSolver(lb.LBFGSParam(m=3, max_iterations=30), "MoreThuente", dtype=np.float32, resident=True).minimize(lb.OBJ_ROSENBROCK_CHAINED, np.full(6007, 1.3))
+print("chained f32 resident odd n", g["status"], g["niter"], g["fx"])
+# per-problem data through the C ABI: problem k's d and b at offset k*ldd, ldd > n (the bulk copies read up to round_up(n, 32))
+from test_gpu_resident_implied_grad import resident  # noqa: E402
+nb, ldd = 5003, 5004
+D, R = np.zeros(2 * ldd + 5024), np.zeros(2 * ldd + 5024)
+for k in range(3):
+    D[k * ldd:k * ldd + nb], R[k * ldd:k * ldd + nb] = po.quad_tridiag_data(nb, seed=3 + k)[:2]
+ctx = lb.Context(0)
+outs, _, _, _ = resident(ctx, lb.OBJ_QUAD_TRIDIAG, np.zeros((3, nb)), lb.LBFGSParam(m=6, max_iterations=25), "MoreThuente", data0=D, data1=R, ldd=ldd)
+print("tridiag batch per-problem data", [(o.status, o.niter) for o in outs])
+ctx.close()
 bs = lb.BatchSession(lb.OBJ_ROSENBROCK_PAIRED, np.stack([np.zeros(3000), np.full(3000, 0.5), np.ones(3000)]), lb.LBFGSParam(m=6), "MoreThuente")
 res, _, _ = bs.solve()
 bs.close()

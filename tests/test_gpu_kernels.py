@@ -54,35 +54,60 @@ def objective_inputs(kind, n, rng):
     return x, None, None
 
 
-@pytest.mark.parametrize("kind", [lb.OBJ_ROSENBROCK_PAIRED, lb.OBJ_QUAD_SHIFT, lb.OBJ_ROSENBROCK_CHAINED, lb.OBJ_QUAD_TRIDIAG])
-@pytest.mark.parametrize("n", [2, 4, 6, 10, 34, 1000, 4098, (1 << 18) + 2])
-def test_objective_and_fused_trial(gpu_ctx, orc, kind, n):
+def grad_expression(kind, x, d0, d1):
+    """grad f of a built-in objective, expression by expression as the kernels evaluate it (in x's dtype)."""
+    from test_gpu_resident_coupled import chained_grad, tridiag_grad
+    from test_gpu_resident_exit_points import rosenbrock_grad
+    from test_gpu_resident_implied_grad import quad_shift_grad
+    return {lb.OBJ_ROSENBROCK_PAIRED: lambda: rosenbrock_grad(x), lb.OBJ_QUAD_SHIFT: lambda: quad_shift_grad(x),
+            lb.OBJ_ROSENBROCK_CHAINED: lambda: chained_grad(x), lb.OBJ_QUAD_TRIDIAG: lambda: tridiag_grad(x, d0, d1)}[kind]()
+
+
+# (objective, n): odd n for the objectives that allow it (the paired Rosenbrock function needs an even n)
+OBJECTIVE_SIZES = [(kind, n) for n in (2, 3, 4, 5, 6, 10, 34, 1000, 1001, 4098, (1 << 18) + 2, (1 << 18) + 3)
+                   for kind in (lb.OBJ_ROSENBROCK_PAIRED, lb.OBJ_QUAD_SHIFT, lb.OBJ_ROSENBROCK_CHAINED, lb.OBJ_QUAD_TRIDIAG)
+                   if not (kind == lb.OBJ_ROSENBROCK_PAIRED and n % 2)]
+
+
+@pytest.mark.parametrize("dtype", [np.float64, np.float32])
+@pytest.mark.parametrize("kind,n", OBJECTIVE_SIZES)
+def test_objective_and_fused_trial(gpu_ctx, orc, kind, n, dtype):
     rng = np.random.default_rng(100 * kind + n)
     xp, d0, d1 = objective_inputs(kind, n, rng)
     drt = rng.standard_normal(n)
     step = 0.173
+    if dtype == np.float32:
+        xp, drt = xp.astype(dtype), drt.astype(dtype)
+        d0, d1 = (None if v is None else v.astype(dtype) for v in (d0, d1))
+        step = dtype(step)
     x_ref = xp + step * drt
-    f_ref, g_ref = orc.objective(kind, x_ref, d0, d1)
+    eps = np.finfo(dtype).eps
     D0 = lb.DeviceArray(gpu_ctx, d0) if d0 is not None else None
     D1 = lb.DeviceArray(gpu_ctx, d1) if d1 is not None else None
     dxp, dd = lb.DeviceArray(gpu_ctx, xp), lb.DeviceArray(gpu_ctx, drt)
-    dx, dg = gpu_ctx.empty(n), gpu_ctx.empty(n)
+    dx, dg = gpu_ctx.empty(n, dtype), gpu_ctx.empty(n, dtype)
     f, gd, gg, xx = gpu_ctx.trial(kind, dxp, dd, step, dx, dg, D0, D1)
     x_gpu, g_gpu = dx.get(), dg.get()
-    assert np.max(np.abs(x_gpu - x_ref)) <= 2 * np.finfo(np.float64).eps * np.max(np.abs(xp) + np.abs(step * drt))
+    assert np.max(np.abs(x_gpu - x_ref)) <= 2 * eps * np.max(np.abs(xp) + np.abs(step * drt))
     # gradient at the GPU's own x (separates objective arithmetic from the axpy rounding)
     f_at, g_at = orc.objective(kind, x_gpu, d0, d1)
-    scale = np.max(np.abs(g_at)) + 1.0
-    assert np.max(np.abs(g_gpu - g_at)) <= 1e-13 * scale * 10
-    assert abs(f - f_at) <= 1e-12 * max(1.0, abs(f_at))
-    assert abs(gd - np.dot(g_at, drt)) <= red_tol(g_at * drt, np.float64) * 4
-    assert abs(gg - np.dot(g_at, g_at)) <= red_tol(g_at * g_at, np.float64) * 4
-    assert abs(xx - np.dot(x_gpu, x_gpu)) <= red_tol(x_gpu * x_gpu, np.float64) * 4
+    if dtype == np.float64:
+        scale = np.max(np.abs(g_at)) + 1.0
+        assert np.max(np.abs(g_gpu - g_at)) <= 1e-13 * scale * 10
+        assert abs(f - f_at) <= 1e-12 * max(1.0, abs(f_at))
+        f_ref, _ = orc.objective(kind, x_ref, d0, d1)
+        assert abs(f_ref - f) <= 1e-9 * max(1.0, abs(f_ref))
+    else:   # fp32: the expression in fp32, bit for bit (no FMA contraction); f summed in fp32
+        assert np.array_equal(g_gpu, grad_expression(kind, x_gpu, d0, d1))
+        assert abs(f - f_at) <= 1e-4 * max(1.0, abs(f_at))
+    g64 = g_at if dtype == np.float64 else g_gpu.astype(np.float64)
+    assert abs(gd - np.dot(g64, drt)) <= red_tol(g64 * drt, dtype) * 4
+    assert abs(gg - np.dot(g64, g64)) <= red_tol(g64 * g64, dtype) * 4
+    assert abs(xx - np.dot(x_gpu.astype(np.float64), x_gpu)) <= red_tol(x_gpu.astype(np.float64) * x_gpu, dtype) * 4
     # plain evaluation entry point
-    dg2 = gpu_ctx.empty(n)
+    dg2 = gpu_ctx.empty(n, dtype)
     f2, _, gg2, xx2 = gpu_ctx.objective(kind, dx, dg2, D0, D1)
     assert np.array_equal(dg2.get(), g_gpu) and f2 == f and gg2 == gg and xx2 == xx
-    assert abs(f_ref - f) <= 1e-9 * max(1.0, abs(f_ref))
 
 
 def test_paired_rosenbrock_rejects_odd_n(gpu_ctx):

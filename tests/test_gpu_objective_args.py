@@ -44,3 +44,31 @@ def test_resident_solve_rejects_before_launch(kind, n, msg, dtype):
     assert dctx.launches() == before
     with pytest.raises(ValueError, match=msg):
         lb.LBFGSSolver(lb.LBFGSParam(), "MoreThuente", dtype=dtype, resident=True).minimize(kind, np.zeros(n, dtype), raise_errors=True)
+
+
+def _tridiag_batch(ctx, dtype, B, n, ldd, offset_elems=0):
+    from test_gpu_resident_implied_grad import resident
+    size = max(ldd, n) * B + 64
+    d = lb.DeviceArray(ctx, np.ones(size, dtype), offset_elems=offset_elems)
+    b = lb.DeviceArray(ctx, np.zeros(size, dtype))
+    return resident(ctx, lb.OBJ_QUAD_TRIDIAG, np.zeros((B, n), dtype), lb.LBFGSParam(), "MoreThuente", data0=d, data1=b, ldd=ldd)
+
+
+# (batch, n, ldd, data0 offset in elements, part of the message): the resident solve reads each problem's data with bulk copies
+# that start on 16-byte boundaries of data + b*ldd
+DATA_CASES = [
+    pytest.param(2, 100, 50, 0, "at least n", id="ldd_below_n"),
+    pytest.param(2, 100, -100, 0, "at least n", id="ldd_negative"),
+    pytest.param(2, 100, 101, 0, "multiple of 16 bytes", id="ldd_misaligned"),
+    pytest.param(1, 100, 0, 1, "16-byte boundary", id="data0_misaligned"),
+]
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+@pytest.mark.parametrize("B,n,ldd,offset,msg", DATA_CASES)
+def test_resident_solve_rejects_bad_data_layout_before_launch(gpu_ctx, B, n, ldd, offset, msg, dtype):
+    before = gpu_ctx.launches()
+    with pytest.raises(lb.LbfgsB200Error, match=msg) as e:
+        _tridiag_batch(gpu_ctx, dtype, B, n, ldd, offset)
+    assert e.value.status == 1
+    assert gpu_ctx.launches() == before

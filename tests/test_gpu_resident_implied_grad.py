@@ -32,15 +32,18 @@ class _Outcome(C.Structure):    # lbfgs_b200_outcome
                 ("rounds", C.c_longlong)]
 
 
-def resident(ctx, objective, X0, prm, ls):
+def resident(ctx, objective, X0, prm, ls, data0=None, data1=None, ldd=0, on_solver=None):
     """The rows of X0 solved by one launch of the device-resident solve through the C ABI (a single problem through
     lbfgs_b200_solver_minimize, several through the batch entry point): (outcomes, X, G, rounds by pass) with G the final gradients
-    read through lbfgs_b200_solver_final_grad_of."""
+    read through lbfgs_b200_solver_final_grad_of.  data0/data1: None, a host array (uploaded in X0's dtype) or a lb.DeviceArray
+    (passed as it is), problem b's data at offset b*ldd (ldd = 0: shared).  on_solver(s): called with the solver after the solve."""
     X0 = np.atleast_2d(X0)
     dt = X0.dtype
     suf = "f64" if dt == np.float64 else "f32"
     B, n = X0.shape
     lib = ctx.lib
+    data = [v if v is None or isinstance(v, lb.DeviceArray) else ctx.array(np.asarray(v, dtype=dt)) for v in (data0, data1)]
+    d0, d1 = (None if v is None else v.ptr for v in data)
     s = C.c_void_p()
     if B == 1:
         ctx.check(lib.lbfgs_b200_solver_create(ctx.h, n, prm.m, dt.itemsize, C.byref(s)))
@@ -52,9 +55,11 @@ def resident(ctx, objective, X0, prm, ls):
         xd = ctx.array(X0.reshape(-1))
         outs = (_Outcome * B)()
         if B == 1:
-            ctx.check(getattr(lib, "lbfgs_b200_solver_minimize_" + suf)(s, objective, None, None, C.byref(p), LS[ls], xd.ptr, None, 0, outs))
+            ctx.check(getattr(lib, "lbfgs_b200_solver_minimize_" + suf)(s, objective, d0, d1, C.byref(p), LS[ls], xd.ptr, None, 0, outs))
         else:
-            ctx.check(getattr(lib, "lbfgs_b200_solver_minimize_batch_" + suf)(s, objective, None, None, 0, C.byref(p), LS[ls], xd.ptr, n, outs))
+            ctx.check(getattr(lib, "lbfgs_b200_solver_minimize_batch_" + suf)(s, objective, d0, d1, ldd, C.byref(p), LS[ls], xd.ptr, n, outs))
+        if on_solver is not None:
+            on_solver(s)
         X = xd.get().reshape(B, n)
         G = np.empty((B, n), dtype=dt)
         for b in range(B):

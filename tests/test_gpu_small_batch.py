@@ -109,26 +109,32 @@ def test_rosenbrock_from_zero_matches_checker(orc, ls, n):
 
 
 def test_other_objectives(orc):
-    # chained Rosenbrock: stored trials (x_lo / g_lo, RESTORE)
+    from test_gpu_resident_coupled import chained_grad, tridiag_grad
+    # chained Rosenbrock: stored trials (x_lo / g_lo, RESTORE); odd n leaves a ragged last pack.  The gradient a problem returns is
+    # the gradient expression at its x, bit for bit (no FMA contraction)
     prm = lb.LBFGSParam(max_iterations=MAXIT)
-    res, X, _ = small(np.full((2, 300), 1.3), prm, "NocedalWright", lb.OBJ_ROSENBROCK_CHAINED)
-    c = orc.lbfgs(po.OBJ_ROSENBROCK_CHAINED, np.full(300, 1.3), LS["NocedalWright"], cpu_param(orc, prm))
-    for b in range(2):
-        assert res[b]["status"] == c["status"] == "ok"
-        near(res[b], X[b], c, 1e-6)
-    # tridiagonal quadratic with per-problem data (ldd = n): every problem against the checker on its own d and b
-    n, B = 200, 3
-    data = [po.quad_tridiag_data(n, kappa=1e2, seed=10 + b) for b in range(B)]
-    D = np.concatenate([d for d, _, _ in data])
-    R = np.concatenate([r for _, r, _ in data])
-    prm = lb.LBFGSParam(max_iterations=MAXIT)
-    for ls in ("Bracketing", "MoreThuente"):
-        res, X, _ = small(np.zeros((B, n)), prm, ls, lb.OBJ_QUAD_TRIDIAG, data0=D, data1=R, ldd=n)
-        for b, (d, r, xs) in enumerate(data):
-            c = orc.lbfgs(po.OBJ_QUAD_TRIDIAG, np.zeros(n), LS[ls], cpu_param(orc, prm), data0=d, data1=r)
+    for n in (300, 301):
+        res, X, G = small(np.full((2, n), 1.3), prm, "NocedalWright", lb.OBJ_ROSENBROCK_CHAINED, want_grad=True)
+        c = orc.lbfgs(po.OBJ_ROSENBROCK_CHAINED, np.full(n, 1.3), LS["NocedalWright"], cpu_param(orc, prm))
+        for b in range(2):
             assert res[b]["status"] == c["status"] == "ok"
             near(res[b], X[b], c, 1e-6)
-            assert np.max(np.abs(X[b] - xs)) <= 1e-3
+            assert np.array_equal(G[b], chained_grad(X[b]))
+    # tridiagonal quadratic with per-problem data (ldd = n): every problem against the checker on its own d and b
+    B = 3
+    prm = lb.LBFGSParam(max_iterations=MAXIT)
+    for n in (200, 201):
+        data = [po.quad_tridiag_data(n, kappa=1e2, seed=10 + b) for b in range(B)]
+        D = np.concatenate([d for d, _, _ in data])
+        R = np.concatenate([r for _, r, _ in data])
+        for ls in ("Bracketing", "MoreThuente"):
+            res, X, G = small(np.zeros((B, n)), prm, ls, lb.OBJ_QUAD_TRIDIAG, data0=D, data1=R, ldd=n, want_grad=True)
+            for b, (d, r, xs) in enumerate(data):
+                c = orc.lbfgs(po.OBJ_QUAD_TRIDIAG, np.zeros(n), LS[ls], cpu_param(orc, prm), data0=d, data1=r)
+                assert res[b]["status"] == c["status"] == "ok"
+                near(res[b], X[b], c, 1e-6)
+                assert np.max(np.abs(X[b] - xs)) <= 1e-3
+                assert np.array_equal(G[b], tridiag_grad(X[b], d, r))
     # quadratic shift: 2 iterations, x = 0..9
     res, X, _ = small(np.zeros((2, 10)), lb.LBFGSParam(max_iterations=MAXIT), "NocedalWright", lb.OBJ_QUAD_SHIFT)
     assert all(r["niter"] == 2 for r in res) and np.allclose(X, np.arange(10.0), atol=1e-12)
