@@ -9,6 +9,7 @@
 //     TRIAL          x = xp + step*d, g = grad f(x)              ; {f, g.d, g.g, x.x}                       LineSearch*.h trial, LBFGS.h:130,137
 //     DOTS_FORM      s = x - xp, y = g - gp -> free ring slot    ; [S Y]'[g s y] (6 dots per column pair)   LBFGS.h:159-162, BFGSMat.h:85-92 + apply_Hv pass 1
 //     DOTS_PLAIN     (pair rejected by the curvature gate)       ; [S Y]'g over the old history
+//                    (both in p_dots: forming warps prepare each staged element once -- g, and the new pair -- the column warps read it)
 //     COMBINE        coefficient recursion (every CTA, shared memory) ; d = cv*g + sum cy_j y_j + cs_j s_j ; {g.d}   BFGSMat.h:283-301 in Gram form
 //     COMBINE_TRIAL  COMBINE + the first trial of the next line search in the same pass: the reference restarts every search
 //                    at step = 1 (LBFGS.h:168), so x1 = x + d, g1 = grad f(x1) ; {g.d, f1, g1.d, g1.g1, x1.x1}
@@ -372,6 +373,21 @@ template <class T> __device__ __forceinline__ void mask_unit(Unit<T>& u, int cnt
 #pragma unroll
     for (int k = 0; k < 16 / (int)sizeof(T); k++) u.v[k] = (k < cnt) ? u.v[k] : T(0);
 }
+// g = grad f(x) of the unit at elements i0.. of an objective without neighbour coupling (lanes past cnt: x = 0): the arithmetic of
+// every pass that evaluates the objective, so bit for bit the g a pass would have stored for that point
+template <class T, class OBJ> __device__ __forceinline__ Unit<T> grad_unit(const OBJ& obj, int64_t i0, int cnt, const Unit<T>& ux)
+{
+    constexpr int EPT = 16 / (int)sizeof(T);
+    const int c4 = cnt < EPT ? cnt : EPT;
+    T xv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
+#pragma unroll
+    for (int k = 0; k < EPT; k++) xv[k] = (k < c4) ? ux.v[k] : T(0);
+    obj.eval(i0, c4, xv, T(0), T(0), gv);
+    Unit<T> ug;
+#pragma unroll
+    for (int k = 0; k < EPT; k++) ug.v[k] = gv[k];
+    return ug;
+}
 
 // copies of one tile: `nrhs` right-hand rows, of which the first `nload` are loaded (sh.vecs[0..nload), round_up(len, 32) elements
 // each) and the others are left for the pass to fill, + the history runs of block `blk`; one lane per copy.  Returns nothing; the
@@ -398,12 +414,26 @@ __device__ __forceinline__ void stage_tiled(T* dstt, int TE, int nrhs, int nload
 }
 
 // ---- DOTS -----------------------------------------------------------------------------------------------------------------------
-// [S Y]'[v s_new y_new] over this CTA's chunk, one block (tile) at a time, everything staged by bulk copies.  FORM (p_dots: a stored
-// point, neighbour-coupled objectives): the newest pair s = x - xp, y = g - gp is formed on the fly from the staged rows {g, x, gp, xp},
-// identically in every warp that needs it, takes part as column 0 and is written to ring slot `new_slot` by the warps that own
-// column 0.  An implied point (p_dots_implied) is formed once per element instead, see there.
-// Column j (by age) belongs to warp group j, whose `split` warps share the tile's units.  PLAIN: s.g and y.g over the old history only;
-// for an objective without neighbour coupling g is not stored: x is staged and every column warp evaluates g = grad f(x) of its units.
+// [S Y]'[g s_new y_new] (FORM) or [S Y]'g over the old history (PLAIN), over this CTA's chunk, one block (tile) at a time, everything
+// staged by bulk copies.  Column j (by age) belongs to warp group j, whose `split` warps share the tile's units.  Before the column
+// groups read a staged tile, forming warps take each of its units once and leave what the columns read in its first right-hand rows:
+// g in row 0 and, in FORM, the new pair s, y in rows 1 and 2, which they also write to ring slot `new_slot`:
+//     FORM,  implied point (no neighbour coupling)   staged d, xp (+ a row no copy fills): gp = grad f(xp), x = xp + step*d and
+//                                                    g = grad f(x) with the trial's own arithmetic (or x = xp, g = gp when the search
+//                                                    ended on its start point), s = x - xp, y = g - gp; x is written as well (g is not
+//                                                    stored: the next pass evaluates it from x)
+//     FORM,  stored point (neighbour-coupled)        staged g, x, gp, xp: s = x - xp, y = g - gp (row 0 stays g)
+//     PLAIN, no neighbour coupling                   staged x: g = grad f(x)
+//     PLAIN, neighbour-coupled                       staged g: nothing to form
+// In FORM the new pair is column 0; in PLAIN every column, age 0 included, is read through sh.slots.  The forming warps are the ones
+// dots_geometry leaves without a column (c = 10: 4 of 24) or, when every warp has a column (c = 3, 6, 12, ...), the warps of column 0,
+// which form a tile before taking their own dots of it.  Neither the unit-to-lane mapping of the columns nor any accumulator depends on
+// who forms, so the sums are bit-identical to forming the pair in every column warp.
+// No CTA-wide barrier per tile (a per-tile __syncthreads() left the column warps idle ~30 % of a tile at c = 10, DESIGN.md section 3):
+// every stage has three mbarriers -- full (the bulk copies; parity in phase_bits), formed (arrivals of the forming warps, which arrive
+// also when they have nothing to form) and empty (arrivals of the column warps), the latter two initialised by the pass -- and warp 0,
+// after its own dots of a tile, waits for the stage's empty barrier and re-arms it.  So a column group starts a tile as soon as it is
+// formed.
 template <class T> struct PDots
 {
     int64_t n;
@@ -421,159 +451,9 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const 
                                        int G)
 {
     constexpr int EPT = 16 / (int)sizeof(T);
-    constexpr bool G_IMPLIED = !OBJ::kHalo;
-    static_assert(!(FORM && G_IMPLIED), "an implied point is formed by p_dots_implied");
-    constexpr int NRHS = FORM ? 4 : 1;                           // staged right-hand vectors: g, x, gp, xp / g (G_IMPLIED: x)
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int TE = a.h.BT();
-    const int my_col = warp / a.split, my_part = warp % a.split;
-    const int upp = (TE / EPT) / a.split;                        // units of a tile per warp of a column group
-    const SlotRuns runs(a.end, a.cnt_old, a.h.M);
-    const int nrows = NRHS + 2 * a.cnt_old;
-    int stages = (int)((size_t)kPStageBytes / ((size_t)nrows * TE * sizeof(T)));
-    stages = stages > kPMaxStages ? kPMaxStages : stages;
-    const int64_t ntl = own.ntiles(TE);
-    uint64_t* full_bar = sh.full_bar;
-
-    T acc[ROUNDS][kGramVals];
-#pragma unroll
-    for (int r = 0; r < ROUNDS; r++)
-#pragma unroll
-        for (int k = 0; k < kGramVals; k++) acc[r][k] = T(0);
-
-    __syncthreads();   // sh.vecs / sh.slots are in place and the staging ring is free
-    int64_t next_tile = 0;
-    for (int s = 0; s < stages; s++, next_tile++)
-        if (next_tile < ntl) stage_tiled<T>(tiles + (size_t)s * nrows * TE, TE, NRHS, NRHS, own.start(next_tile, TE), own.len(next_tile, TE), a.h, runs, sh, &full_bar[s]);
-    int stage = 0;
-    for (int64_t t = 0; t < ntl; t++)
-    {
-        mbar_wait(&full_bar[stage], (phase_bits >> stage) & 1u);
-        phase_bits ^= (1u << stage);
-        const T* base = tiles + (size_t)stage * nrows * TE;
-        const T* hist = base + (size_t)NRHS * TE;
-        const int64_t e0 = own.start(t, TE);
-        const int len = own.len(t, TE);
-#pragma unroll
-        for (int r = 0; r < ROUNDS; r++)
-        {
-            const int j = r * a.cols_per_round + my_col;
-            if (my_col < a.cols_per_round && j < a.c)
-            {
-                const bool is_new = FORM && j == 0;
-                const T* srow = hist + (size_t)2 * (is_new ? 0 : sh.slots[j]) * TE;     // sh.slots[j]: packed row of the column of age j
-                const T* yrow = srow + TE;
-                T* s_new = a.h.s_at(a.new_slot < 0 ? 0 : a.new_slot, e0);
-                for (int u = my_part * upp + lane; u < (my_part + 1) * upp; u += 32)
-                {
-                    const int off = u * EPT;
-                    const int cnt = len - off;
-                    if (cnt <= 0) break;
-                    Unit<T> ug, us, uy, usn, uyn, ux;
-                    if constexpr (FORM)
-                    {
-                        Unit<T> ugp, uxp;
-                        ug = lds_unit<T>(base + off);
-                        ux = lds_unit<T>(base + TE + off);
-                        ugp = lds_unit<T>(base + 2 * TE + off);
-                        uxp = lds_unit<T>(base + 3 * TE + off);
-#pragma unroll
-                        for (int k = 0; k < EPT; k++) { usn.v[k] = ux.v[k] - uxp.v[k]; uyn.v[k] = ug.v[k] - ugp.v[k]; }
-                        if (cnt < EPT) { mask_unit(usn, cnt); mask_unit(uyn, cnt); }
-                    }
-                    else if constexpr (G_IMPLIED)
-                    {
-                        // the arithmetic of every pass that evaluates the objective: bit for bit the g a stored point would have
-                        const Unit<T> uxs = lds_unit<T>(base + off);
-                        const int c4 = cnt < EPT ? cnt : EPT;
-                        T xv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
-#pragma unroll
-                        for (int k = 0; k < EPT; k++) xv[k] = (k < c4) ? uxs.v[k] : T(0);
-                        obj.eval(e0 + off, c4, xv, T(0), T(0), gv);
-#pragma unroll
-                        for (int k = 0; k < EPT; k++) ug.v[k] = gv[k];
-                    }
-                    else ug = lds_unit<T>(base + off);
-                    bool loaded = false;
-                    if constexpr (FORM)
-                    {
-                        if (is_new)
-                        {
-                            us = usn; uy = uyn;
-                            st_unit<T>(s_new, off, cnt, usn);
-                            st_unit<T>(s_new + TE, off, cnt, uyn);
-                            loaded = true;
-                        }
-                    }
-                    if (!loaded) { us = lds_unit<T>(srow + off); uy = lds_unit<T>(yrow + off); }
-                    if (cnt < EPT) { mask_unit(ug, cnt); mask_unit(us, cnt); mask_unit(uy, cnt); }
-#pragma unroll
-                    for (int k = 0; k < EPT; k++)
-                    {
-                        acc[r][0] += us.v[k] * ug.v[k];
-                        acc[r][1] += uy.v[k] * ug.v[k];
-                    }
-                    if constexpr (FORM)
-                    {
-#pragma unroll
-                        for (int k = 0; k < EPT; k++)
-                        {
-                            acc[r][2] += us.v[k] * uyn.v[k];
-                            acc[r][3] += uy.v[k] * uyn.v[k];
-                            acc[r][4] += uy.v[k] * usn.v[k];
-                            acc[r][5] += us.v[k] * usn.v[k];
-                        }
-                    }
-                }
-            }
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncthreads();
-        if (next_tile < ntl) stage_tiled<T>(tiles + (size_t)stage * nrows * TE, TE, NRHS, NRHS, own.start(next_tile, TE), own.len(next_tile, TE), a.h, runs, sh, &full_bar[stage]);
-        next_tile++;
-        stage = (stage + 1 == stages) ? 0 : stage + 1;
-    }
-
-    // block reduction: lanes -> warp, then the `split` warps of a column; value (j, k) -> dst[(j*6 + k) * G]
-#pragma unroll
-    for (int r = 0; r < ROUNDS; r++)
-#pragma unroll
-        for (int k = 0; k < kGramVals; k++)
-        {
-            const double w = warp_sum((double)acc[r][k]);
-            if (lane == 0) sh.red[warp][r * kGramVals + k] = w;
-        }
-    __syncthreads();
-    const int nvals = a.c * kGramVals;
-    for (int idx = tid; idx < nvals; idx += kPThreads)
-    {
-        const int j = idx / kGramVals, k = idx % kGramVals;
-        const int r = j / a.cols_per_round, col = j % a.cols_per_round;
-        double t = 0.0;
-        for (int p = 0; p < a.split; p++) t += sh.red[col * a.split + p][r * kGramVals + k];
-        dst[(size_t)idx * G] = t;
-    }
-}
-
-// DOTS_FORM of an implied point (objectives without neighbour coupling): the sums of p_dots<FORM>, with the point rebuilt from the
-// staged rows {d, xp} ONCE per element.  Neither gradient is read: both are element-wise functions of a point the pass has, and the
-// objective's arithmetic gives them bit for bit as stored.  The forming warps take every unit of a staged tile: gp = grad f(xp),
-// x = xp + step*d, g = grad f(x) with the trial's own arithmetic (or x = xp, g = gp when the search ended on its start point),
-// s = x - xp, y = g - gp; they write x and the pair to HBM (g is not stored: the next pass evaluates it from x) and g, s, y into the
-// stage's three right-hand rows (d, xp and one row no copy fills).  The column groups then read those rows.  The forming warps are the ones
-// dots_geometry leaves without a column (c = 10: 4 of 24) or, when every warp has a column (c = 3, 6, 12, ...), the warps of
-// column 0, which form a tile before taking their own dots of it.  Split, columns and the unit-to-lane mapping are p_dots', and so is
-// every accumulator: the sums are bit-identical to forming the point in every column group.
-// No CTA-wide barrier per tile: every stage has three mbarriers -- full (the bulk copies; parity in phase_bits), formed (arrivals of
-// the forming warps) and empty (arrivals of the column warps), the latter two initialised by the pass -- and warp 0, after its own
-// dots of a tile, waits for the stage's empty barrier and re-arms it.  So a column group starts a tile as soon as it is formed.
-template <class T, class OBJ, int ROUNDS>
-__device__ __forceinline__ void p_dots_implied(const PDots<T>& a, const OBJ& obj, const Own& own, T* tiles, PShared& sh, unsigned& phase_bits,
-                                               double* dst, int G)
-{
-    static_assert(!OBJ::kHalo, "neighbour-coupled objectives store their trial points: p_dots<FORM>");
-    constexpr int EPT = 16 / (int)sizeof(T);
-    constexpr int NRHS = 3, NLOAD = 2;                           // right-hand rows: d, xp staged, formed into g, s_new, y_new
+    constexpr bool HALO = OBJ::kHalo;
+    constexpr int NRHS = !FORM ? 1 : (HALO ? 4 : 3);             // right-hand rows: g / x ; FORM: g, x, gp, xp / d, xp, (formed)
+    constexpr int NLOAD = (FORM && !HALO) ? 2 : NRHS;            // ... of which the bulk copies fill the first NLOAD
     __shared__ uint64_t formed_bar[kPMaxStages], empty_bar[kPMaxStages];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int TE = a.h.BT();
@@ -616,46 +496,59 @@ __device__ __forceinline__ void p_dots_implied(const PDots<T>& a, const OBJ& obj
         if (former)
         {
             mbar_wait(&full_bar[stage], ((full_phase >> stage) & 1u) ^ lap);
-            T* s_new = a.h.s_at(a.new_slot, e0);
-            for (int u = fw * 32 + lane; u < units; u += nform * 32)
+            if constexpr (FORM || !HALO)
             {
-                const int off = u * EPT;
-                const int cnt = len - off;
-                if (cnt <= 0) break;
-                const Unit<T> ud = lds_unit<T>(base + off);
-                const Unit<T> uxp = lds_unit<T>(base + TE + off);
-                const int c4 = cnt < EPT ? cnt : EPT;
-                Unit<T> ux, ug, ugp, usn, uyn;
+                for (int u = fw * 32 + lane; u < units; u += nform * 32)
                 {
-                    T xv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
+                    const int off = u * EPT;
+                    const int cnt = len - off;
+                    if (cnt <= 0) break;
+                    if constexpr (!FORM)
+                    {
+                        const Unit<T> ug = grad_unit(obj, e0 + off, cnt, lds_unit<T>(base + off));
+                        *reinterpret_cast<float4*>(base + off) = *reinterpret_cast<const float4*>(ug.v);
+                    }
+                    else
+                    {
+                        Unit<T> ux, ug, uxp, ugp, usn, uyn;
+                        if constexpr (HALO)
+                        {
+                            ug = lds_unit<T>(base + off);
+                            ux = lds_unit<T>(base + TE + off);
+                            ugp = lds_unit<T>(base + 2 * TE + off);
+                            uxp = lds_unit<T>(base + 3 * TE + off);
+                        }
+                        else
+                        {
+                            const Unit<T> ud = lds_unit<T>(base + off);
+                            uxp = lds_unit<T>(base + TE + off);
+                            ugp = grad_unit(obj, e0 + off, cnt, uxp);
+                            if (a.at_start) { ux = uxp; ug = ugp; }
+                            else
+                            {
+                                // the trial's arithmetic (p_trial, and p_combine's first trial with step 1 on the stored d)
 #pragma unroll
-                    for (int k = 0; k < EPT; k++) xv[k] = (k < c4) ? uxp.v[k] : T(0);
-                    obj.eval(e0 + off, c4, xv, T(0), T(0), gv);
+                                for (int k = 0; k < EPT; k++) ux.v[k] = (k < cnt) ? uxp.v[k] + a.step * ud.v[k] : T(0);
+                                ug = grad_unit(obj, e0 + off, cnt, ux);
+                            }
+                        }
 #pragma unroll
-                    for (int k = 0; k < EPT; k++) ugp.v[k] = gv[k];
+                        for (int k = 0; k < EPT; k++) { usn.v[k] = ux.v[k] - uxp.v[k]; uyn.v[k] = ug.v[k] - ugp.v[k]; }
+                        if (cnt < EPT) { mask_unit(usn, cnt); mask_unit(uyn, cnt); }
+                        T* s_new = a.h.s_at(a.new_slot, e0);
+                        st_unit<T>(s_new, off, cnt, usn);
+                        st_unit<T>(s_new + TE, off, cnt, uyn);
+                        if constexpr (!HALO)
+                        {
+                            st_unit<T>(a.x, e0 + off, cnt, ux);
+                            *reinterpret_cast<float4*>(base + off) = *reinterpret_cast<const float4*>(ug.v);
+                        }
+                        *reinterpret_cast<float4*>(base + TE + off) = *reinterpret_cast<const float4*>(usn.v);
+                        *reinterpret_cast<float4*>(base + 2 * TE + off) = *reinterpret_cast<const float4*>(uyn.v);
+                    }
                 }
-                if (a.at_start) { ux = uxp; ug = ugp; }
-                else
-                {
-                    // the trial's arithmetic (p_trial, and p_combine's first trial with step 1 on the stored d)
-                    T xv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
-#pragma unroll
-                    for (int k = 0; k < EPT; k++) xv[k] = (k < c4) ? uxp.v[k] + a.step * ud.v[k] : T(0);
-                    obj.eval(e0 + off, c4, xv, T(0), T(0), gv);
-#pragma unroll
-                    for (int k = 0; k < EPT; k++) { ux.v[k] = xv[k]; ug.v[k] = gv[k]; }
-                }
-#pragma unroll
-                for (int k = 0; k < EPT; k++) { usn.v[k] = ux.v[k] - uxp.v[k]; uyn.v[k] = ug.v[k] - ugp.v[k]; }
-                if (cnt < EPT) { mask_unit(usn, cnt); mask_unit(uyn, cnt); }
-                st_unit<T>(s_new, off, cnt, usn);
-                st_unit<T>(s_new + TE, off, cnt, uyn);
-                st_unit<T>(a.x, e0 + off, cnt, ux);
-                *reinterpret_cast<float4*>(base + off) = *reinterpret_cast<const float4*>(ug.v);
-                *reinterpret_cast<float4*>(base + TE + off) = *reinterpret_cast<const float4*>(usn.v);
-                *reinterpret_cast<float4*>(base + 2 * TE + off) = *reinterpret_cast<const float4*>(uyn.v);
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // these writes before the bulk copies that re-arm the stage
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // these writes before the bulk copies that re-arm the stage
             __syncwarp();
             if (lane == 0) mbar_arrive(&formed_bar[stage]);
         }
@@ -668,16 +561,17 @@ __device__ __forceinline__ void p_dots_implied(const PDots<T>& a, const OBJ& obj
                 const int j = r * a.cols_per_round + my_col;
                 if (my_col < a.cols_per_round && j < a.c)
                 {
-                    const T* srow = hist + (size_t)2 * (j == 0 ? 0 : sh.slots[j]) * TE;     // sh.slots[j]: packed row of the column of age j
+                    const bool is_new = FORM && j == 0;
+                    const T* srow = hist + (size_t)2 * (is_new ? 0 : sh.slots[j]) * TE;     // sh.slots[j]: packed row of the column of age j
                     const T* yrow = srow + TE;
                     for (int u = my_part * upp + lane; u < (my_part + 1) * upp; u += 32)
                     {
                         const int off = u * EPT;
                         const int cnt = len - off;
                         if (cnt <= 0) break;
-                        Unit<T> ug = lds_unit<T>(base + off), us, uy;
-                        const Unit<T> usn = lds_unit<T>(base + TE + off), uyn = lds_unit<T>(base + 2 * TE + off);
-                        if (j == 0) { us = usn; uy = uyn; }
+                        Unit<T> ug = lds_unit<T>(base + off), us, uy, usn{}, uyn{};
+                        if constexpr (FORM) { usn = lds_unit<T>(base + TE + off); uyn = lds_unit<T>(base + 2 * TE + off); }
+                        if (is_new) { us = usn; uy = uyn; }
                         else { us = lds_unit<T>(srow + off); uy = lds_unit<T>(yrow + off); }
                         if (cnt < EPT) { mask_unit(ug, cnt); mask_unit(us, cnt); mask_unit(uy, cnt); }
 #pragma unroll
@@ -686,13 +580,16 @@ __device__ __forceinline__ void p_dots_implied(const PDots<T>& a, const OBJ& obj
                             acc[r][0] += us.v[k] * ug.v[k];
                             acc[r][1] += uy.v[k] * ug.v[k];
                         }
-#pragma unroll
-                        for (int k = 0; k < EPT; k++)
+                        if constexpr (FORM)
                         {
-                            acc[r][2] += us.v[k] * uyn.v[k];
-                            acc[r][3] += uy.v[k] * uyn.v[k];
-                            acc[r][4] += uy.v[k] * usn.v[k];
-                            acc[r][5] += us.v[k] * usn.v[k];
+#pragma unroll
+                            for (int k = 0; k < EPT; k++)
+                            {
+                                acc[r][2] += us.v[k] * uyn.v[k];
+                                acc[r][3] += uy.v[k] * uyn.v[k];
+                                acc[r][4] += uy.v[k] * usn.v[k];
+                                acc[r][5] += us.v[k] * usn.v[k];
+                            }
                         }
                     }
                 }
@@ -713,7 +610,8 @@ __device__ __forceinline__ void p_dots_implied(const PDots<T>& a, const OBJ& obj
     for (int s = 0; s < stages; s++)
         if (s < ntl) phase_bits ^= (unsigned)(((ntl - 1 - s) / stages + 1) & 1) << s;
 
-    // block reduction: as p_dots (the forming warps without a column contribute zeros that nobody reads)
+    // block reduction: lanes -> warp, then the `split` warps of a column; value (j, k) -> dst[(j*6 + k) * G] (the forming warps
+    // without a column contribute zeros that nobody reads)
 #pragma unroll
     for (int r = 0; r < ROUNDS; r++)
 #pragma unroll
@@ -866,16 +764,7 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
                 const int cnt = (len - off >= EPT) ? EPT : (len - off);
                 T r[EPT];
                 Unit<T> uv;
-                if constexpr (G_IMPLIED)
-                {
-                    const Unit<T> ux = lds_unit<T>(xrow + off);
-                    T xv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
-#pragma unroll
-                    for (int k = 0; k < EPT; k++) xv[k] = (k < cnt) ? ux.v[k] : T(0);
-                    obj.eval(e0 + off, cnt, xv, T(0), T(0), gv);
-#pragma unroll
-                    for (int k = 0; k < EPT; k++) uv.v[k] = gv[k];
-                }
+                if constexpr (G_IMPLIED) uv = grad_unit(obj, e0 + off, cnt, lds_unit<T>(xrow + off));
                 direction(off, r, uv);
                 Unit<T> out;
 #pragma unroll
@@ -1363,11 +1252,7 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
                         else { sh.vecs[0] = vg; sh.vecs[1] = vx; sh.vecs[2] = vgp; sh.vecs[3] = vxp; }
                     }
                 }
-                if (form)
-                {
-                    if constexpr (HALO) p_dots<T, OBJ, ROUNDS, true>(d, obj, own, tiles, sh, phase_bits, dst, G);
-                    else p_dots_implied<T, OBJ, ROUNDS>(d, obj, own, tiles, sh, phase_bits, dst, G);
-                }
+                if (form) p_dots<T, OBJ, ROUNDS, true>(d, obj, own, tiles, sh, phase_bits, dst, G);
                 else p_dots<T, OBJ, ROUNDS, false>(d, obj, own, tiles, sh, phase_bits, dst, G);
                 break;
             }

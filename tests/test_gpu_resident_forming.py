@@ -1,6 +1,7 @@
-"""The pair-forming dots pass of the device-resident solve for objectives without neighbour coupling forms the accepted point once
-per element, in the warps the dots geometry leaves without a column or, when every warp has a column (c = 3, 6, 12, and every
-c > 24), in the warps of column 0.  These runs reach the geometries an m = 10 solve does not: c = 12 with two warps per column,
+"""The pair-forming dots pass of the device-resident solve forms each element once -- for objectives without neighbour coupling the
+accepted point, its gradient and the new pair -- in the warps the dots geometry leaves without a column or, when every warp has a
+column (c = 3, 6, 12, and every c > 24), in the warps of column 0.  These runs reach the geometries an m = 10 solve does not: c = 12
+with two warps per column,
 and c > 24 where one warp forms every tile and the columns take two rounds, on a vector whose last CTA holds a ragged tile of
 fewer than 512 coordinates."""
 import numpy as np
