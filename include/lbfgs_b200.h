@@ -294,10 +294,11 @@ int lbfgs_b200_solver_batch(const lbfgs_b200_solver* s);
  * indexed by the pass a round ran: 0 = rounds in which the problems of a batch ran different passes, 1 FIRST, 2 TRIAL, 3 DOTS_FORM,
  * 4 DOTS_PLAIN, 5 COMBINE, 6 COMBINE_TRIAL, 7 RESTORE, 8 MATERIALIZE (9 unused).  ms_by_op10: the kernel's time split by round (CTA 0's cycle counter scaled
  * to kernel_ms; includes each round's synchronisation); alg_bytes_by_op10: algorithmic bytes of those passes (whole vectors read and
- * written: FIRST 3n, TRIAL 2n, DOTS_FORM (2c+3)n, DOTS_PLAIN (2c+1)n, COMBINE (2c+2)n, COMBINE_TRIAL (2c+2)n, MATERIALIZE 4n, 3n or 2n
- * words (the point on the ray, the search's start point, the point already in x: the gradient is evaluated from x, not stored, between
- * FIRST and MATERIALIZE); for the neighbour-coupled objectives, whose trials store their points and whose passes read the stored gradient:
- * TRIAL 4n, DOTS_FORM (2c+4)n, COMBINE_TRIAL (2c+5)n, RESTORE 4n; + the objective's
+ * written: FIRST 4n, TRIAL 2n, DOTS_FORM (c+2)n, DOTS_PLAIN (c+2)n, COMBINE (c+2)n, COMBINE_TRIAL (c+2)n, MATERIALIZE 4n or 3n
+ * words (the point on the ray; the search's start point or the point already in x: the gradient is evaluated from x, not stored, between
+ * FIRST and MATERIALIZE, and the history ring holds the c+1 iterates of c chained pairs, not the pairs); for the neighbour-coupled
+ * objectives, whose trials store their points, whose passes read the stored gradient and whose ring holds S|Y: FIRST 3n, TRIAL 4n,
+ * DOTS_FORM (2c+4)n, DOTS_PLAIN (2c+1)n, COMBINE (2c+2)n, COMBINE_TRIAL (2c+5)n, MATERIALIZE 4n, RESTORE 4n; + the objective's
  * data vectors per evaluation); sync_ms[3]: { the part of kernel_ms between CTA 0's arrival at a grid barrier and its release, the part of that spent waiting for
  * the last CTA to arrive, the part spent in the cross-rank exchange }. */
 lbfgs_b200_status lbfgs_b200_solver_profile(const lbfgs_b200_solver* s, double* kernel_ms, double* ms_by_op10, unsigned long long* rounds_by_op10,

@@ -24,8 +24,12 @@
 // COMBINE the read of g.  Only FIRST and MATERIALIZE write g: a problem that stops anywhere but at FIRST takes one MATERIALIZE round
 // for the point it stopped at -- on the ray, its search's start point, or the point in x (arming the next search failed).  The kept
 // best trial of a search is its step, so there is no x_lo/g_lo and no RESTORE pass.
+// History of iterates.  For the same objectives a pair is a function of its two endpoints (s = x - xp, y = grad f(x) - grad f(xp)),
+// and consecutive accepted pairs share one: the ring holds iterates (PState::pts), x and xp are rows of it, and the dots and
+// combination passes stage the c + 1 endpoints of c chained pairs instead of 2c columns and rebuild each pair where they read it,
+// with the arithmetic that formed it (point_plan).  The flat x, g hold only the caller's start point and the result.
 // Neighbour-coupled objectives (kHalo) store every trial's x, g and keep the best one by pointer swap with x_lo/g_lo, as the
-// reference's search does (LineSearchMoreThuente.h:534,553), and restore the start point with RESTORE.
+// reference's search does (LineSearchMoreThuente.h:534,553), restore the start point with RESTORE, and keep an S|Y ring.
 // Every CTA owns the same contiguous chunk (granularity: the block length of the tiled history) of EVERY vector in EVERY pass, so a CTA only ever reads vector
 // elements it wrote itself (halo coordinates excepted, those are read through L2) and streams long contiguous runs.  Between rounds there is one
 // grid-wide synchronisation: CTAs deposit their partial sums in fixed slots, CTA 0 adds them in a fixed order (deterministic: no
@@ -36,8 +40,8 @@
 // ring bookkeeping (BFGSMat.h:81-97) and the buffer rotation (pointer swaps) -- and publishes one 128-byte descriptor per problem that tells every CTA what the next round does.  The host is
 // not involved between launch and completion: 1 launch per minimize(), 2 + (T - 1) rounds per iteration with T line-search trials.
 //
-// Data movement: ALL operands of the dots and combination passes -- the right-hand vectors and the 2c history columns, which live in
-// a tiled layout (PHist) so that the columns of a tile are one or two contiguous runs -- are staged into shared memory by TMA bulk
+// Data movement: ALL operands of the dots and combination passes -- the right-hand vectors and the history rows, which live in
+// a tiled layout (PHist) so that the rows of a tile are one or two contiguous runs -- are staged into shared memory by TMA bulk
 // copies (cp.async.bulk + mbarrier) in a two-stage ring of ~90 KB stages: the bytes in flight per SM are set by the ring, not by
 // registers.  The trial pass streams through registers (128-bit loads / stores).  Vectors owned by the solver are padded to whole
 // 256-byte lines, so every tile -- the ragged end of a vector included -- is a legal bulk copy; lanes past n are masked in the
@@ -65,6 +69,7 @@ template <class T> struct alignas(128) PRound
     T step;                     // TRIAL: the trial's step; DOTS_FORM / MATERIALIZE of an implied point: the step of that point
     int op, c_round, head, pending, gram_cur;
     int at_start;               // DOTS_FORM / MATERIALIZE of an implied point: which point (PT_RAY, PT_START, PT_X)
+    int px, pxp;                // objectives without neighbour coupling: the point rows of x and xp in the ring
 };
 static_assert(sizeof(PRound<double>) == 128 && sizeof(PRound<float>) == 128, "a round descriptor is one 128-byte line");
 
@@ -120,6 +125,11 @@ struct PShared
     double margin[2][2 * kMaxM + 2];        // neighbour-coupled combination pass: products of the element on either side of a tile
     double carry[2];                        // ... and x1 of the last element of the previous tile (two slots, alternating)
     unsigned char ops[4096];                // this round's op of every problem
+    // objectives without neighbour coupling: the point rows a dots / combination pass stages (point_plan)
+    unsigned char prow[2 * kMaxM + 2];      // by point row of the ring: its row among the staged points
+    unsigned char pstart[kMaxM], pend[kMaxM];   // by column: staged row of the start / end point of its pair
+    unsigned char run_at[2 * kMaxM + 2], run_len[2 * kMaxM + 2], run_row[2 * kMaxM + 2];   // one bulk copy per run of ring rows
+    int nruns, npts, xrow;                  // copies, staged point rows, staged row of the pass's own point (x, or xp in DOTS_FORM)
 };
 
 // Ownership.  CTA i owns the contiguous chunk [c0, c1) of every vector (boundaries on multiples of the history's block length, the
@@ -171,14 +181,16 @@ template <int NV> __device__ __forceinline__ void block_sums(const double (&acc)
 }
 
 // ---- FIRST / TRIAL -------------------------------------------------------------------------------------------------------------
-// MODE 0: FIRST (evaluate at x, write g and d = -g) ; MODE 1: TRIAL (evaluate at x = xp + step*d, store nothing: the point is
-// rebuilt by the pass that needs it) ; MODE 2: MATERIALIZE of a ray point (x = xp + step*d, write x and g; no sums) ; MODE 3:
-// MATERIALIZE of a stored point (evaluate at xp, write g, and x when given: the start point xp -> x, or the point in x itself with
-// xp = x, x = nullptr; no sums).  Operands stream through registers with 128-bit loads/stores (a shared-memory staged variant
-// measured slower for this 1:1 read/write pass).  Objectives without neighbour coupling only: the coupled ones take p_trial_halo.
+// MODE 0: FIRST (evaluate at the flat x, write g, d = -g and x into point row `pout` of the ring) ; MODE 1: TRIAL (evaluate at
+// x = xp + step*d, xp = point row `pin`, store nothing: the point is rebuilt by the pass that needs it) ; MODE 2: MATERIALIZE of a ray
+// point (x = xp + step*d, write the flat x and g; no sums) ; MODE 3: MATERIALIZE of a stored point (evaluate at point row `pin`,
+// write the flat x and g; no sums).  Operands stream through registers with 128-bit loads/stores (a shared-memory staged variant
+// measured slower for this 1:1 read/write pass); a pack never crosses a block of the ring (BT >= 32).  Objectives without neighbour
+// coupling only: the coupled ones take p_trial_halo.
 template <class T, class OBJ, int MODE>
-__device__ __forceinline__ void p_trial(const OBJ& obj, const Own& own, const T* __restrict__ xp, const T* __restrict__ d, T step,
-                                        T* __restrict__ x, T* __restrict__ g, T* __restrict__ dout, PShared& sh, double* dst, int G, bool evict_first)
+__device__ __forceinline__ void p_trial(const OBJ& obj, const Own& own, const PHist<T>& h, int pin, const T* __restrict__ d, T step,
+                                        T* __restrict__ x, T* __restrict__ g, T* __restrict__ dout, int pout, PShared& sh, double* dst, int G,
+                                        bool evict_first)
 {
     static_assert(!OBJ::kHalo, "neighbour-coupled objectives take p_trial_halo");
     T acc[4] = {T(0), T(0), T(0), T(0)};
@@ -188,15 +200,16 @@ __device__ __forceinline__ void p_trial(const OBJ& obj, const Own& own, const T*
         const int64_t i0 = q << 2;
         const int cnt = (n - i0 >= 4) ? 4 : int(n - i0);
         T xv[4], dv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
+        const T* xin = (MODE == 0) ? x + i0 : h.pt_at(pin, i0);
         if (MODE == 1 || MODE == 2)
         {
-            const Pack<T> px = load4<T, Hint::Stream, true>(xp, i0, cnt), pd = load4<T, Hint::Stream, true>(d, i0, cnt);
+            const Pack<T> px = load4<T, Hint::Stream, true>(xin, 0, cnt), pd = load4<T, Hint::Stream, true>(d, i0, cnt);
 #pragma unroll
             for (int k = 0; k < 4; k++) { dv[k] = pd.v[k]; xv[k] = px.v[k] + step * pd.v[k]; }
         }
         else
         {
-            const Pack<T> px = load4<T, Hint::Stream, true>(MODE == 3 ? xp : x, i0, cnt);
+            const Pack<T> px = load4<T, Hint::Stream, true>(xin, 0, cnt);
 #pragma unroll
             for (int k = 0; k < 4; k++) xv[k] = px.v[k];
         }
@@ -207,15 +220,20 @@ __device__ __forceinline__ void p_trial(const OBJ& obj, const Own& own, const T*
 #pragma unroll
             for (int k = 0; k < 4; k++) { pg.v[k] = gv[k]; po.v[k] = (MODE >= 2) ? xv[k] : T(-1) * gv[k]; }
             T* const out0 = (MODE >= 2) ? x : dout;
+            Pack<T> pxo;
+#pragma unroll
+            for (int k = 0; k < 4; k++) pxo.v[k] = xv[k];
             if (evict_first)
             {
-                if (MODE != 3 || out0) store4<T, Hint::Stream, true>(out0, i0, cnt, po);
+                store4<T, Hint::Stream, true>(out0, i0, cnt, po);
                 store4<T, Hint::Stream, true>(g, i0, cnt, pg);
+                if (MODE == 0) store4<T, Hint::Stream, true>(h.pt_at(pout, i0), 0, cnt, pxo);
             }
             else
             {
-                if (MODE != 3 || out0) store4<T, Hint::Plain, true>(out0, i0, cnt, po);
+                store4<T, Hint::Plain, true>(out0, i0, cnt, po);
                 store4<T, Hint::Plain, true>(g, i0, cnt, pg);
+                if (MODE == 0) store4<T, Hint::Plain, true>(h.pt_at(pout, i0), 0, cnt, pxo);
             }
         }
     };
@@ -413,19 +431,96 @@ __device__ __forceinline__ void stage_tiled(T* dstt, int TE, int nrhs, int nload
     else if (tid == nrhs + 1 && bbytes) tma_load_1d(dstt + (size_t)(nrhs + 2 * (runs.a1 - runs.a0)) * TE, blk + (size_t)runs.b0 * 2 * TE, bbytes, bar);
 }
 
+// Objectives without neighbour coupling: the point rows a pass stages -- the start and end points of the pairs of ages
+// 0 .. ncols-1 (columns col0 .. col0+ncols-1) and the pass's own point `own_pt` -- in ring order, one bulk copy per run of consecutive
+// rows: a chained history (every pair starting where the older one ends) is one run, or two where it wraps.  A pair rejected by the
+// curvature gate breaks the chain and leaves more, shorter runs.  All threads call; the previous pass no longer reads sh.
+template <class T>
+__device__ void point_plan(const PState<T>* st, int head, int ncols, int col0, int own_pt, PShared& sh)
+{
+    const int tid = threadIdx.x;
+    const int M = st->hist.M, P = 2 * M;
+    for (int p = tid; p < P; p += kPThreads) sh.prow[p] = 0;
+    __syncthreads();
+    if (tid < ncols)
+    {
+        const int slot = slot_by_age(head, M, tid);
+        const unsigned char a = __ldcg(st->pts + 2 * slot), b = __ldcg(st->pts + 2 * slot + 1);
+        sh.pstart[col0 + tid] = a;
+        sh.pend[col0 + tid] = b;
+        sh.prow[a] = 1;
+        sh.prow[b] = 1;
+    }
+    if (tid == 0) sh.prow[own_pt] = 1;
+    __syncthreads();
+    if (tid == 0)
+    {
+        int rows = 0, runs = 0;
+        bool prev = false;
+        for (int p = 0; p < P; p++)
+        {
+            const bool used = sh.prow[p] != 0;
+            if (used)
+            {
+                if (!prev) { sh.run_at[runs] = (unsigned char)p; sh.run_len[runs] = 0; sh.run_row[runs] = (unsigned char)rows; runs++; }
+                sh.run_len[runs - 1]++;
+                sh.prow[p] = (unsigned char)rows++;
+            }
+            prev = used;
+        }
+        sh.nruns = runs;
+        sh.npts = rows;
+        sh.xrow = sh.prow[own_pt];
+    }
+    __syncthreads();
+    if (tid < ncols)
+    {
+        sh.pstart[col0 + tid] = sh.prow[sh.pstart[col0 + tid]];
+        sh.pend[col0 + tid] = sh.prow[sh.pend[col0 + tid]];
+    }
+    __syncthreads();
+}
+
+// copies of one tile, objectives without neighbour coupling: `nload` right-hand rows (sh.vecs), room for nrhs - nload rows the pass
+// fills, then the sh.npts point rows of point_plan; lanes of warp 0.  The stage's barrier has been told the byte count.
+template <class T>
+__device__ __forceinline__ void stage_points(T* dstt, int TE, int nrhs, int nload, int64_t e0, int len, const PHist<T>& h, const PShared& sh,
+                                             uint64_t* bar)
+{
+    const int tid = threadIdx.x;
+    if (tid >= 32) return;
+    const unsigned rbytes = (unsigned)((len + 31) & ~31) * (unsigned)sizeof(T);
+    if (tid == 0)
+    {
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy accesses of this stage before the copies that overwrite it
+        mbar_expect_tx(bar, rbytes * (unsigned)nload + (unsigned)sh.npts * (unsigned)TE * (unsigned)sizeof(T));
+    }
+    __syncwarp();
+    const T* blk = h.H + (e0 >> h.bt_log) * h.bstride;
+    T* prows = dstt + (size_t)nrhs * TE;
+    if (tid < nload) tma_load_1d(dstt + (size_t)tid * TE, static_cast<const T*>(sh.vecs[tid]) + e0, rbytes, bar);
+    for (int r = tid; r < sh.nruns; r += 32)
+        tma_load_1d(prows + (size_t)sh.run_row[r] * TE, blk + ((size_t)sh.run_at[r] << h.bt_log), (unsigned)sh.run_len[r] * (unsigned)TE * (unsigned)sizeof(T), bar);
+}
+
 // ---- DOTS -----------------------------------------------------------------------------------------------------------------------
 // [S Y]'[g s_new y_new] (FORM) or [S Y]'g over the old history (PLAIN), over this CTA's chunk, one block (tile) at a time, everything
 // staged by bulk copies.  Column j (by age) belongs to warp group j, whose `split` warps share the tile's units.  Before the column
 // groups read a staged tile, forming warps take each of its units once and leave what the columns read in its first right-hand rows:
-// g in row 0 and, in FORM, the new pair s, y in rows 1 and 2, which they also write to ring slot `new_slot`:
-//     FORM,  implied point (no neighbour coupling)   staged d, xp (+ a row no copy fills): gp = grad f(xp), x = xp + step*d and
-//                                                    g = grad f(x) with the trial's own arithmetic (or x = xp, g = gp when the search
-//                                                    ended on its start point), s = x - xp, y = g - gp; x is written as well (g is not
-//                                                    stored: the next pass evaluates it from x)
-//     FORM,  stored point (neighbour-coupled)        staged g, x, gp, xp: s = x - xp, y = g - gp (row 0 stays g)
-//     PLAIN, no neighbour coupling                   staged x: g = grad f(x)
+// g in row 0 and, in FORM, the new pair s, y in rows 1 and 2:
+//     FORM,  implied point (no neighbour coupling)   staged d (+ two rows no copy fills) and the points: gp = grad f(xp), x = xp +
+//                                                    step*d and g = grad f(x) with the trial's own arithmetic (or x = xp, g = gp when
+//                                                    the search ended on its start point), s = x - xp, y = g - gp; x is written to its
+//                                                    point row (g is not stored: the next pass evaluates it from x; nor is the pair:
+//                                                    its readers rebuild it from its endpoints)
+//     FORM,  stored point (neighbour-coupled)        staged g, x, gp, xp: s = x - xp, y = g - gp, written to ring slot `new_slot`
+//                                                    (row 0 stays g)
+//     PLAIN, no neighbour coupling                   the points: g = grad f(x)
 //     PLAIN, neighbour-coupled                       staged g: nothing to form
-// In FORM the new pair is column 0; in PLAIN every column, age 0 included, is read through sh.slots.  The forming warps are the ones
+// In FORM the new pair is column 0; in PLAIN every column, age 0 included, is an old pair.  Objectives without neighbour coupling
+// stage the pairs' endpoints (point_plan) and a column warp rebuilds s = x_end - x_start, y = grad f(x_end) - grad f(x_start) of
+// each unit with the arithmetic that formed it, bit for bit the pair the forming pass had; neighbour-coupled objectives stage the
+// ring's S|Y slots (the column of age j: sh.slots[j]).  The forming warps are the ones
 // dots_geometry leaves without a column (c = 10: 4 of 24) or, when every warp has a column (c = 3, 6, 12, ...), the warps of column 0,
 // which form a tile before taking their own dots of it.  Neither the unit-to-lane mapping of the columns nor any accumulator depends on
 // who forms, so the sums are bit-identical to forming the pair in every column warp.
@@ -443,7 +538,7 @@ template <class T> struct PDots
     int new_slot, split, cols_per_round;
     T step;              // FORM of an implied point: its step (PT_RAY), or the start point (PT_START)
     int at_start;
-    T* x;                // FORM of an implied point: where it is written
+    int px;              // FORM of an implied point: the point row it is written to
 };
 
 template <class T, class OBJ, int ROUNDS, bool FORM>
@@ -452,8 +547,8 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const 
 {
     constexpr int EPT = 16 / (int)sizeof(T);
     constexpr bool HALO = OBJ::kHalo;
-    constexpr int NRHS = !FORM ? 1 : (HALO ? 4 : 3);             // right-hand rows: g / x ; FORM: g, x, gp, xp / d, xp, (formed)
-    constexpr int NLOAD = (FORM && !HALO) ? 2 : NRHS;            // ... of which the bulk copies fill the first NLOAD
+    constexpr int NRHS = !FORM ? 1 : (HALO ? 4 : 3);             // right-hand rows: g / (formed) ; FORM: g, x, gp, xp / d, (formed) x 2
+    constexpr int NLOAD = HALO ? NRHS : (FORM ? 1 : 0);          // ... of which the bulk copies fill the first NLOAD
     __shared__ uint64_t formed_bar[kPMaxStages], empty_bar[kPMaxStages];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int TE = a.h.BT();
@@ -461,7 +556,7 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const 
     const int my_col = warp / a.split, my_part = warp % a.split;
     const int upp = units / a.split;                             // units of a tile per warp of a column group
     const SlotRuns runs(a.end, a.cnt_old, a.h.M);
-    const int nrows = NRHS + 2 * a.cnt_old;
+    const int nrows = NRHS + (HALO ? 2 * a.cnt_old : sh.npts);
     int stages = (int)((size_t)kPStageBytes / ((size_t)nrows * TE * sizeof(T)));
     stages = stages > kPMaxStages ? kPMaxStages : stages;
     const int64_t ntl = own.ntiles(TE);
@@ -482,8 +577,12 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const 
         for (int s = 0; s < stages; s++) { mbar_init(&formed_bar[s], nform); mbar_init(&empty_bar[s], col_warps); }
     __syncthreads();   // sh.vecs / sh.slots and the barriers are in place, the staging ring is free
     int64_t next_tile = 0;
+    auto stage_one = [&](T* dstt, int64_t t, uint64_t* bar) {
+        if constexpr (HALO) stage_tiled<T>(dstt, TE, NRHS, NLOAD, own.start(t, TE), own.len(t, TE), a.h, runs, sh, bar);
+        else stage_points<T>(dstt, TE, NRHS, NLOAD, own.start(t, TE), own.len(t, TE), a.h, sh, bar);
+    };
     for (int s = 0; s < stages; s++, next_tile++)
-        if (next_tile < ntl) stage_tiled<T>(tiles + (size_t)s * nrows * TE, TE, NRHS, NLOAD, own.start(next_tile, TE), own.len(next_tile, TE), a.h, runs, sh, &full_bar[s]);
+        if (next_tile < ntl) stage_one(tiles + (size_t)s * nrows * TE, next_tile, &full_bar[s]);
     const unsigned full_phase = phase_bits;
     int stage = 0;
     unsigned lap = 0;                                            // parity of the current use of `stage` in this pass
@@ -505,7 +604,7 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const 
                     if (cnt <= 0) break;
                     if constexpr (!FORM)
                     {
-                        const Unit<T> ug = grad_unit(obj, e0 + off, cnt, lds_unit<T>(base + off));
+                        const Unit<T> ug = grad_unit(obj, e0 + off, cnt, lds_unit<T>(hist + (size_t)sh.xrow * TE + off));
                         *reinterpret_cast<float4*>(base + off) = *reinterpret_cast<const float4*>(ug.v);
                     }
                     else
@@ -521,7 +620,7 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const 
                         else
                         {
                             const Unit<T> ud = lds_unit<T>(base + off);
-                            uxp = lds_unit<T>(base + TE + off);
+                            uxp = lds_unit<T>(hist + (size_t)sh.xrow * TE + off);
                             ugp = grad_unit(obj, e0 + off, cnt, uxp);
                             if (a.at_start) { ux = uxp; ug = ugp; }
                             else
@@ -535,12 +634,15 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const 
 #pragma unroll
                         for (int k = 0; k < EPT; k++) { usn.v[k] = ux.v[k] - uxp.v[k]; uyn.v[k] = ug.v[k] - ugp.v[k]; }
                         if (cnt < EPT) { mask_unit(usn, cnt); mask_unit(uyn, cnt); }
-                        T* s_new = a.h.s_at(a.new_slot, e0);
-                        st_unit<T>(s_new, off, cnt, usn);
-                        st_unit<T>(s_new + TE, off, cnt, uyn);
-                        if constexpr (!HALO)
+                        if constexpr (HALO)
                         {
-                            st_unit<T>(a.x, e0 + off, cnt, ux);
+                            T* s_new = a.h.s_at(a.new_slot, e0);
+                            st_unit<T>(s_new, off, cnt, usn);
+                            st_unit<T>(s_new + TE, off, cnt, uyn);
+                        }
+                        else
+                        {
+                            st_unit<T>(a.h.pt_at(a.px, e0), off, cnt, ux);
                             *reinterpret_cast<float4*>(base + off) = *reinterpret_cast<const float4*>(ug.v);
                         }
                         *reinterpret_cast<float4*>(base + TE + off) = *reinterpret_cast<const float4*>(usn.v);
@@ -562,8 +664,9 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const 
                 if (my_col < a.cols_per_round && j < a.c)
                 {
                     const bool is_new = FORM && j == 0;
-                    const T* srow = hist + (size_t)2 * (is_new ? 0 : sh.slots[j]) * TE;     // sh.slots[j]: packed row of the column of age j
-                    const T* yrow = srow + TE;
+                    // HALO: sh.slots[j] = packed row of the column of age j ; otherwise the staged rows of its pair's endpoints
+                    const T* srow = HALO ? hist + (size_t)2 * (is_new ? 0 : sh.slots[j]) * TE : hist + (size_t)(is_new ? 0 : sh.pstart[j]) * TE;
+                    const T* yrow = HALO ? srow + TE : hist + (size_t)(is_new ? 0 : sh.pend[j]) * TE;
                     for (int u = my_part * upp + lane; u < (my_part + 1) * upp; u += 32)
                     {
                         const int off = u * EPT;
@@ -572,7 +675,14 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const 
                         Unit<T> ug = lds_unit<T>(base + off), us, uy, usn{}, uyn{};
                         if constexpr (FORM) { usn = lds_unit<T>(base + TE + off); uyn = lds_unit<T>(base + 2 * TE + off); }
                         if (is_new) { us = usn; uy = uyn; }
-                        else { us = lds_unit<T>(srow + off); uy = lds_unit<T>(yrow + off); }
+                        else if constexpr (HALO) { us = lds_unit<T>(srow + off); uy = lds_unit<T>(yrow + off); }
+                        else
+                        {
+                            const Unit<T> ua = lds_unit<T>(srow + off), ub = lds_unit<T>(yrow + off);   // x_start, x_end
+                            const Unit<T> ga = grad_unit(obj, e0 + off, cnt, ua), gb = grad_unit(obj, e0 + off, cnt, ub);
+#pragma unroll
+                            for (int k = 0; k < EPT; k++) { us.v[k] = ub.v[k] - ua.v[k]; uy.v[k] = gb.v[k] - ga.v[k]; }
+                        }
                         if (cnt < EPT) { mask_unit(ug, cnt); mask_unit(us, cnt); mask_unit(uy, cnt); }
 #pragma unroll
                         for (int k = 0; k < EPT; k++)
@@ -601,7 +711,7 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const 
         if (warp == 0 && next_tile < ntl)
         {
             mbar_wait(&empty_bar[stage], lap);
-            stage_tiled<T>(base, TE, NRHS, NLOAD, own.start(next_tile, TE), own.len(next_tile, TE), a.h, runs, sh, &full_bar[stage]);
+            stage_one(base, next_tile, &full_bar[stage]);
         }
         next_tile++;
         if (++stage == stages) { stage = 0; lap ^= 1u; }
@@ -646,8 +756,11 @@ __device__ __forceinline__ void dots_geometry(int c, int units, int& split, int&
 // d = cv*v + sum_j cy_j*y_j + cs_j*s_j ; FUSE: x1 = xc + d, g1 = grad f(x1) and the four trial sums (neighbour-coupled objectives:
 // x1, g1 written to (x1_out, g1_out)).
 // Staged rows of a tile: v, (xc,) then the history block's live slots; sh.slots[j] = packed row of the pair of age j.  Objectives
-// without neighbour coupling (G_IMPLIED): v = grad f(xc) is not stored; xc is staged alone and each thread evaluates v of its unit
-// with the objective's arithmetic, bit for bit the stored gradient.  A thread owns
+// without neighbour coupling (G_IMPLIED): the ring holds points, and a tile stages only the point rows of point_plan -- xc and the
+// endpoints of the c pairs (c + 1 rows for a chained history, xc being the newest end).  v = grad f(xc) and the pairs are not
+// stored: each thread evaluates v of its unit and rebuilds y_j = grad f(x_end) - grad f(x_start), s_j = x_end - x_start with the
+// arithmetic that formed them, bit for bit the stored vectors; walking the y terms newest -> oldest it keeps the gradient of a pair's
+// start, which is the next pair's end in a chained history.  A thread owns
 // one 16-byte unit of the tile and adds the terms in the order the recursion would (y newest -> oldest, then s oldest -> newest), with
 // the operand loads of 8 columns in flight before their multiply-adds retire (the pass is bound by shared-memory latency otherwise).
 // HALO (neighbour-coupled objectives, one GPU): x1 goes back into the staged x row, two spare warps form d and x1 of the element on
@@ -663,12 +776,12 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
     constexpr int EPT = 16 / (int)sizeof(T);
     constexpr bool G_IMPLIED = !OBJ::kHalo;
     constexpr int DV = HALO ? OBJ::kDataVectors : 0;              // HALO: the objective's data vectors ride in the stage as well
-    constexpr int NRHS = G_IMPLIED ? 1 : (FUSE ? 2 : 1) + DV;     // v (, xc) (, data0, data1) / xc
+    constexpr int NRHS = G_IMPLIED ? 0 : (FUSE ? 2 : 1) + DV;     // v (, xc) (, data0, data1) / (xc is a point row)
     constexpr int PAD = EPT;                                      // HALO: room for x1 of the neighbouring element on either side of the x row
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int TE = h.BT();
     const SlotRuns runs(end, c, h.M);
-    const int nrows = NRHS + 2 * c;
+    const int nrows = NRHS + (G_IMPLIED ? sh.npts : 2 * c);
     const size_t stage_elems = (size_t)nrows * TE + (HALO ? 2 * PAD : 0);
     int stages = (int)((size_t)kPStageBytes / (stage_elems * sizeof(T)));
     stages = stages > kPMaxStages ? kPMaxStages : stages;
@@ -679,6 +792,7 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
     // HALO: the x row is staged one granule into the stage (row 1 starts at TE + PAD), everything after it shifts by 2*PAD
     auto stage_one = [&](int64_t t, int s) {
         T* dstt = tiles + (size_t)s * stage_elems;
+        if constexpr (G_IMPLIED) { stage_points<T>(dstt, TE, 0, 0, own.start(t, TE), own.len(t, TE), h, sh, &full_bar[s]); return; }
         if (!HALO) { stage_tiled<T>(dstt, TE, NRHS, NRHS, own.start(t, TE), own.len(t, TE), h, runs, sh, &full_bar[s]); return; }
         if (tid >= 32) return;
         const int64_t e0 = own.start(t, TE);
@@ -730,31 +844,62 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
     {
         mbar_wait(&full_bar[stage], (phase_bits >> stage) & 1u);
         phase_bits ^= (1u << stage);
-        T* base = tiles + (size_t)stage * stage_elems;                          // row 0: v (G_IMPLIED: xc)
-        T* xrow = base + (G_IMPLIED ? 0 : TE) + (HALO ? PAD : 0);               // row 1: xc (FUSE)
+        T* base = tiles + (size_t)stage * stage_elems;                          // row 0: v (G_IMPLIED: the point rows)
+        T* xrow = G_IMPLIED ? base + (size_t)sh.xrow * TE : base + TE + (HALO ? PAD : 0);   // row 1: xc (FUSE)
         const T* hist = base + (size_t)NRHS * TE + (HALO ? 2 * PAD : 0);
         const int len = own.len(t, TE);
         const int64_t e0 = own.start(t, TE);
-        // d of one unit: the arithmetic every owner of an element uses (G_IMPLIED: uv comes in evaluated)
+        // d of one unit: the arithmetic every owner of an element uses
         auto direction = [&](int off, T (&r)[EPT], Unit<T>& uv) {
-            if constexpr (!G_IMPLIED) uv = lds_unit<T>(base + off);
-#pragma unroll
-            for (int k = 0; k < EPT; k++) r[k] = cv * uv.v[k];
-#pragma unroll 8
-            for (int j = 0; j < c; j++)                        // y terms newest -> oldest
+            if constexpr (G_IMPLIED)
             {
-                const Unit<T> uy = lds_unit<T>(hist + ((size_t)2 * sh.slots[j] + 1) * TE + off);
-                const T cy = s_coef[1 + j];
+                const int64_t i0 = e0 + off;
+                const int cnt = len - off;
+                uv = grad_unit(obj, i0, cnt, lds_unit<T>(xrow + off));
 #pragma unroll
-                for (int k = 0; k < EPT; k++) r[k] += cy * uy.v[k];
+                for (int k = 0; k < EPT; k++) r[k] = cv * uv.v[k];
+                Unit<T> gk = uv;                               // grad f of staged point row `kept`
+                int kept = sh.xrow;
+                for (int j = 0; j < c; j++)                    // y terms newest -> oldest
+                {
+                    const int re = sh.pend[j], rs = sh.pstart[j];
+                    const Unit<T> ge = (re == kept) ? gk : grad_unit(obj, i0, cnt, lds_unit<T>(base + (size_t)re * TE + off));
+                    gk = grad_unit(obj, i0, cnt, lds_unit<T>(base + (size_t)rs * TE + off));
+                    kept = rs;
+                    const T cy = s_coef[1 + j];
+#pragma unroll
+                    for (int k = 0; k < EPT; k++) r[k] += cy * (ge.v[k] - gk.v[k]);
+                }
+#pragma unroll 4
+                for (int j = c - 1; j >= 0; j--)               // s terms oldest -> newest
+                {
+                    const Unit<T> ue = lds_unit<T>(base + (size_t)sh.pend[j] * TE + off), us = lds_unit<T>(base + (size_t)sh.pstart[j] * TE + off);
+                    const T cs = s_coef[1 + c + j];
+#pragma unroll
+                    for (int k = 0; k < EPT; k++) r[k] += cs * (ue.v[k] - us.v[k]);
+                }
             }
-#pragma unroll 8
-            for (int j = c - 1; j >= 0; j--)                   // s terms oldest -> newest
+            else
             {
-                const Unit<T> us = lds_unit<T>(hist + (size_t)2 * sh.slots[j] * TE + off);
-                const T cs = s_coef[1 + c + j];
+                uv = lds_unit<T>(base + off);
 #pragma unroll
-                for (int k = 0; k < EPT; k++) r[k] += cs * us.v[k];
+                for (int k = 0; k < EPT; k++) r[k] = cv * uv.v[k];
+#pragma unroll 8
+                for (int j = 0; j < c; j++)                    // y terms newest -> oldest
+                {
+                    const Unit<T> uy = lds_unit<T>(hist + ((size_t)2 * sh.slots[j] + 1) * TE + off);
+                    const T cy = s_coef[1 + j];
+#pragma unroll
+                    for (int k = 0; k < EPT; k++) r[k] += cy * uy.v[k];
+                }
+#pragma unroll 8
+                for (int j = c - 1; j >= 0; j--)               // s terms oldest -> newest
+                {
+                    const Unit<T> us = lds_unit<T>(hist + (size_t)2 * sh.slots[j] * TE + off);
+                    const T cs = s_coef[1 + c + j];
+#pragma unroll
+                    for (int k = 0; k < EPT; k++) r[k] += cs * us.v[k];
+                }
             }
         };
         if constexpr (!HALO)
@@ -764,7 +909,6 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
                 const int cnt = (len - off >= EPT) ? EPT : (len - off);
                 T r[EPT];
                 Unit<T> uv;
-                if constexpr (G_IMPLIED) uv = grad_unit(obj, e0 + off, cnt, lds_unit<T>(xrow + off));
                 direction(off, r, uv);
                 Unit<T> out;
 #pragma unroll
@@ -909,20 +1053,22 @@ __device__ __forceinline__ void st_release_gpu_u32(unsigned* p, unsigned v)
 }
 
 // n-words a pass has to move (reads + writes of whole vectors): the roofline numerator of the persistent kernel.  stored: the
-// trials store their points and every pass reads the stored g (neighbour-coupled objectives); otherwise g is evaluated from x
-// wherever it is needed, and only FIRST and MATERIALIZE write it.  pt: the point a MATERIALIZE writes (PT_*)
+// trials store their points, every pass reads the stored g and the ring holds the c pairs as 2c columns (neighbour-coupled
+// objectives).  Otherwise g is evaluated from x wherever it is needed, only FIRST and MATERIALIZE write it, and the ring holds
+// points: c chained pairs are c + 1 of them (a chain broken by the curvature gate stages up to c more, not counted here).  pt: the
+// point a MATERIALIZE writes (PT_*)
 __device__ __forceinline__ double words_of(int op, int c, int data_vectors, bool stored, int pt)
 {
     switch (op)
     {
-    case POP_FIRST: return 3.0 + data_vectors;              // R x ; W g, d
+    case POP_FIRST: return (stored ? 3.0 : 4.0) + data_vectors;   // R x ; W g, d (, x to its point row)
     case POP_TRIAL: return (stored ? 4.0 : 2.0) + data_vectors;   // R xp, d (; W x, g)
     case POP_RESTORE: return 4.0;                           // R xp, gp ; W x, g
-    case POP_MATERIALIZE: return stored || pt == PT_RAY ? 4.0 : (pt == PT_START ? 3.0 : 2.0);   // R xp, d / xp / x ; W x, g / x, g / g
-    case POP_DOTS_FORM: return 2.0 * c + (stored ? 4.0 : 3.0);   // R x, xp, g, gp / xp, d, 2(c-1) columns ; (W x, g / W x,) W s, y
-    case POP_DOTS_PLAIN: return 2.0 * c + 1.0;              // R g (or x), 2c columns
-    case POP_COMBINE: return 2.0 * c + 2.0;                 // R g (or x), 2c columns ; W d
-    case POP_COMBINE_TRIAL: return 2.0 * c + (stored ? 5.0 : 2.0) + data_vectors;   // R g, x (or x), 2c columns ; W d (, x1, g1)
+    case POP_MATERIALIZE: return stored || pt == PT_RAY ? 4.0 : 3.0;   // R xp, d / xp / x ; W x, g
+    case POP_DOTS_FORM: return stored ? 2.0 * c + 4.0 : c + 2.0;   // R x, xp, g, gp, 2(c-1) columns ; W s, y  /  R d, c points ; W x
+    case POP_DOTS_PLAIN: return stored ? 2.0 * c + 1.0 : c + 2.0;  // R g, 2c columns  /  R x, c + 1 points
+    case POP_COMBINE: return stored ? 2.0 * c + 2.0 : c + 2.0;     // R g, 2c columns / c + 1 points ; W d
+    case POP_COMBINE_TRIAL: return (stored ? 2.0 * c + 5.0 : c + 2.0) + data_vectors;   // R g, x, 2c columns / c + 1 points ; W d (, x1, g1)
     default: return 0.0;
     }
 }
@@ -1041,10 +1187,11 @@ __device__ int leader_round(const PArgs<T>& a, int G, PShared& sh, PState<T>* ca
         if (b < a.B && state_of(b)->op != POP_IDLE)
         {
             PState<T>* st = state_of(b);
-            advance_problem<T, HALO, !HALO>(st, st->raw);
+            advance_problem<T, HALO, !HALO, !HALO>(st, st->raw);
             PRound<T>* rd = a.rounds + b;
             rd->x = st->x; rd->xp = st->xp; rd->g = st->g; rd->gp = st->gp; rd->drt = st->drt;
             rd->step = st->step; rd->at_start = st->at_start;
+            if (!HALO) { rd->px = st->px; rd->pxp = st->pxp; }
             rd->c_round = st->c_round; rd->head = st->head; rd->pending = st->pending; rd->gram_cur = st->gram_cur;
             rd->op = st->op;
             running = st->op != POP_IDLE;
@@ -1200,6 +1347,7 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
             const T step = ldv(&rd->step);
             const int c_round = ldv(&rd->c_round), head = ldv(&rd->head), pending = ldv(&rd->pending), gram_cur = ldv(&rd->gram_cur);
             const int at_start = ldv(&rd->at_start);
+            const int px = HALO ? 0 : ldv(&rd->px), pxp = HALO ? 0 : ldv(&rd->pxp);
             if (op == POP_IDLE) continue;
             acct_bucket = (acct_bucket == -1 || acct_bucket == op) ? op : 0;
             acct_words += words_of(op, c_round, kDataVectors, HALO, at_start);
@@ -1209,11 +1357,11 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
             {
             case POP_FIRST:
                 if constexpr (HALO) p_trial_halo<T, OBJ, 0>(obj, own, nullptr, nullptr, T(0), vx, vg, vd, tiles, sh, phase_bits, dst, G);
-                else p_trial<T, OBJ, 0>(obj, own, nullptr, nullptr, T(0), vx, vg, vd, sh, dst, G, a.evict_first_stores);
+                else p_trial<T, OBJ, 0>(obj, own, st->hist, 0, nullptr, T(0), vx, vg, vd, px, sh, dst, G, a.evict_first_stores);
                 break;
             case POP_TRIAL:
                 if constexpr (HALO) p_trial_halo<T, OBJ, 1>(obj, own, vxp, vd, step, vx, vg, nullptr, tiles, sh, phase_bits, dst, G);
-                else p_trial<T, OBJ, 1>(obj, own, vxp, vd, step, nullptr, nullptr, nullptr, sh, dst, G, a.evict_first_stores);
+                else p_trial<T, OBJ, 1>(obj, own, st->hist, pxp, vd, step, nullptr, nullptr, nullptr, 0, sh, dst, G, a.evict_first_stores);
                 break;
             case POP_RESTORE:
                 p_restore<T>(own, vxp, vgp, vx, vg);
@@ -1221,12 +1369,9 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
             case POP_MATERIALIZE:
                 if constexpr (!HALO)
                 {
-                    if (at_start == PT_RAY) p_trial<T, OBJ, 2>(obj, own, vxp, vd, step, vx, vg, nullptr, sh, dst, G, a.evict_first_stores);
-                    else   // PT_START: x = xp, g = grad f(xp) ; PT_X: g = grad f(x)
-                    {
-                        const bool start = at_start == PT_START;
-                        p_trial<T, OBJ, 3>(obj, own, start ? vxp : vx, nullptr, T(0), start ? vx : nullptr, vg, nullptr, sh, dst, G, a.evict_first_stores);
-                    }
+                    if (at_start == PT_RAY) p_trial<T, OBJ, 2>(obj, own, st->hist, pxp, vd, step, vx, vg, nullptr, 0, sh, dst, G, a.evict_first_stores);
+                    else   // PT_START: x = xp ; PT_X: x = x (its point row) ; g = grad f(x)
+                        p_trial<T, OBJ, 3>(obj, own, st->hist, at_start == PT_START ? pxp : px, nullptr, T(0), vx, vg, nullptr, 0, sh, dst, G, a.evict_first_stores);
                 }
                 break;
             case POP_DOTS_FORM:
@@ -1238,19 +1383,22 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
                 d.end = head;                                   // the old columns: the slots below the free slot `head`
                 d.cnt_old = form ? c_round - 1 : c_round;
                 d.new_slot = form ? head : -1;
-                d.step = step; d.at_start = at_start; d.x = vx;
+                d.step = step; d.at_start = at_start; d.px = px;
                 dots_geometry(d.c, d.h.BT() / (16 / (int)sizeof(T)), d.split, d.cols_per_round);
                 __syncthreads();   // sh.slots / sh.vecs may still be read by the previous problem's pass
+                if constexpr (!HALO)
+                {
+                    // the point is rebuilt from d and xp / g from x; the old pairs (FORM: columns 1..) from their endpoints
+                    if (tid == 0) sh.vecs[0] = vd;
+                    point_plan<T>(st, head, d.cnt_old, form ? 1 : 0, form ? pxp : px, sh);
+                }
+                else
                 {
                     const SlotRuns runs(d.end, d.cnt_old, d.h.M);
                     // age j (FORM: j >= 1) -> packed row of its slot in the staged block
                     if (tid < d.c && !(form && tid == 0))
                         sh.slots[tid] = (unsigned char)runs.row_of(slot_by_age(head, d.h.M, form ? tid - 1 : tid));
-                    if (tid == 0)
-                    {
-                        if (!HALO) { sh.vecs[0] = form ? vd : vx; sh.vecs[1] = vxp; }   // the point is rebuilt from d, xp / g from x
-                        else { sh.vecs[0] = vg; sh.vecs[1] = vx; sh.vecs[2] = vgp; sh.vecs[3] = vxp; }
-                    }
+                    if (tid == 0) { sh.vecs[0] = vg; sh.vecs[1] = vx; sh.vecs[2] = vgp; sh.vecs[3] = vxp; }
                 }
                 if (form) p_dots<T, OBJ, ROUNDS, true>(d, obj, own, tiles, sh, phase_bits, dst, G);
                 else p_dots<T, OBJ, ROUNDS, false>(d, obj, own, tiles, sh, phase_bits, dst, G);
@@ -1271,6 +1419,8 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
                 __syncthreads();   // the tile area / tables may still be in use by the previous problem's pass
                 // per age: packed row of the column in a staged block, and its ring slot
                 const bool fuse = op == POP_COMBINE_TRIAL;
+                if constexpr (!HALO) point_plan<T>(st, head, g.c, 0, px, sh);   // g is evaluated from x, the pairs from their endpoints
+                else
                 {
                     const SlotRuns runs(head, g.c, g.M);
                     for (int j = tid; j < g.c; j += kPThreads)
@@ -1278,7 +1428,7 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
                         sh.slots[j] = (unsigned char)runs.row_of(g.slots[j]);
                         sh.slotid[j] = g.slots[j];
                     }
-                    if (tid == 0) { sh.vecs[0] = HALO ? vg : vx; sh.vecs[1] = vx; sh.vecs[2] = st->data0; sh.vecs[3] = st->data1; }   // (!HALO: g is evaluated from x)
+                    if (tid == 0) { sh.vecs[0] = vg; sh.vecs[1] = vx; sh.vecs[2] = st->data0; sh.vecs[3] = st->data1; }
                 }
                 // the coefficient recursion (every CTA; CTA 0 also writes the folded Gram matrices back) and its 2c+1 results into sh.coef
                 const bool own_scratch = gram_solve_smem_elems(g.c) * sizeof(T) <= sizeof(s_gram);

@@ -7,13 +7,20 @@ struct lbfgs_b200_solver
     lbfgs_b200_ctx* ctx = nullptr;
     int64_t n = 0;
     int m = 0, elem = 8, B = 1;
-    // the S/Y rings, tiled: H[problem][block][slot][S|Y][BT] (lb::PHist); small per-problem arrays in one slab each
+    // the rings, tiled: H[problem][block][slot][S|Y][BT] (lb::PHist) -- or, for objectives without neighbour coupling,
+    // H[problem][block][point][BT] with 2M points; small per-problem arrays in one slab each
     void* d_hist = nullptr;
     int bt_log = 9, M = 0;
     size_t hist_elems = 0;                // elements of one problem's tiled ring
     void* d_small = nullptr;              // [B][ ys M | alpha M | theta 1 (padded to 4) | SY,YY,SS x2: 6 M^2 ]
     size_t small_elems = 0;
+    unsigned char* d_pts = nullptr;       // [B][2M]: start and end point of the pair in each slot (lb::PState::pts)
     std::vector<int> ring_head, ring_ncorr, ring_gram_cur;   // ring state after the last solve (for the export below)
+    // how the last solve's rings hold their pairs: as points (then the export rebuilds S, Y with the objective's gradient) or as S|Y
+    bool ring_points = false;
+    int ring_objective = -1;
+    int64_t ring_gofs = 0, ring_nglob = 0;
+    std::vector<unsigned char> ring_pts;  // host copy of d_pts after the last solve
     std::vector<lbfgs_b200_hist*> exported;                   // column-major copies made on request (lbfgs_b200_solver_history_of)
     std::vector<char> export_fresh;
     void* vec_slab = nullptr;             // [B][5][vec_elems] : x, xp, g, gp, drt
@@ -112,6 +119,7 @@ static lbfgs_b200_status solver_minimize(lbfgs_b200_solver* s, int objective, co
         p.data0 = data0 ? data0 + (size_t)b * ldd : nullptr;
         p.data1 = data1 ? data1 + (size_t)b * ldd : nullptr;
         p.raw = s->d_raw + (size_t)b * s->pstride;
+        p.pts = s->d_pts + (size_t)b * 2 * s->M;
         p.halo = s->d_halo + (size_t)b * kHaloDoubles;
         init_problem_state<T>(p, *prm, ls_kind, fuse_first_trial);   // (prm->m == s->m: p.M == s->M)
         p.trace = trace_host ? s->d_trace : nullptr;
@@ -125,6 +133,7 @@ static lbfgs_b200_status solver_minimize(lbfgs_b200_solver* s, int objective, co
         const PState<T>& p = hs[b];
         hr[b].x = p.x; hr[b].xp = p.xp; hr[b].g = p.g; hr[b].gp = p.gp; hr[b].drt = p.drt;
         hr[b].step = T(0); hr[b].op = p.op; hr[b].c_round = 0; hr[b].head = 0; hr[b].pending = -1; hr[b].gram_cur = p.gram_cur;
+        hr[b].px = p.px; hr[b].pxp = p.pxp;
     }
     // BFGSMat::reset (BFGSMat.h:61-78): no pairs, theta = 1, Gram matrices cleared
     CU(ctx, cudaMemsetAsync(s->d_small, 0, sizeof(T) * s->small_elems * (size_t)B, ctx->stream));
@@ -184,6 +193,10 @@ static lbfgs_b200_status solver_minimize(lbfgs_b200_solver* s, int objective, co
         outs[b].gnorm = (double)p.gnorm;
         outs[b].rounds = p.rounds;
     }
+    s->ring_points = !stored_trials;
+    s->ring_objective = objective;
+    s->ring_gofs = geo.gofs; s->ring_nglob = geo.n_glob;
+    if (s->ring_points) CU(ctx, cudaMemcpyAsync(s->ring_pts.data(), s->d_pts, s->ring_pts.size(), cudaMemcpyDeviceToHost, ctx->stream));
     if (trace_host)
     {
         const long long cnt = hs[0].nfev < trace_cap ? hs[0].nfev : trace_cap;
@@ -204,6 +217,34 @@ template <class T> __global__ void k_untile_history(lb::PHist<T> h, int64_t n, i
         Y[(int64_t)slot * ld + i] = *h.y_at(slot, i);
     }
 }
+// ... of a ring of points: pair slot `slot` from its endpoints (ends[2 slot], ends[2 slot + 1]; -1: no live pair, zeros), with the
+// arithmetic of the passes that read it, 16-byte unit by 16-byte unit: bit for bit the s and y the solve used
+struct PairEnds { short v[2 * (lb::kMaxM + 1)]; };
+template <class T, class OBJ> __global__ void k_untile_points(lb::PHist<T> h, OBJ obj, PairEnds ends, int64_t n, int64_t ld, T* __restrict__ S, T* __restrict__ Y)
+{
+    constexpr int EPT = 16 / (int)sizeof(T);
+    const int slot = blockIdx.y;
+    const int ps = ends.v[2 * slot], pe = ends.v[2 * slot + 1];
+    for (int64_t i0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * EPT; i0 < n; i0 += (int64_t)gridDim.x * blockDim.x * EPT)
+    {
+        const int cnt = n - i0 >= EPT ? EPT : (int)(n - i0);
+        lb::Unit<T> us, uy;
+        if (ps >= 0)
+        {
+            const lb::Unit<T> ua = lb::lds_unit<T>(h.pt_at(ps, i0)), ub = lb::lds_unit<T>(h.pt_at(pe, i0));
+            const lb::Unit<T> ga = lb::grad_unit(obj, i0, cnt, ua), gb = lb::grad_unit(obj, i0, cnt, ub);
+#pragma unroll
+            for (int k = 0; k < EPT; k++) { us.v[k] = ub.v[k] - ua.v[k]; uy.v[k] = gb.v[k] - ga.v[k]; }
+        }
+        else
+            for (int k = 0; k < EPT; k++) us.v[k] = uy.v[k] = T(0);
+        for (int k = 0; k < cnt; k++)
+        {
+            S[(int64_t)slot * ld + i0 + k] = us.v[k];
+            Y[(int64_t)slot * ld + i0 + k] = uy.v[k];
+        }
+    }
+}
 #if defined(LBFGS_B200_PERSIST_F64)
 template <class T> static lbfgs_b200_hist* export_history(lbfgs_b200_solver* s, int b)
 {
@@ -215,7 +256,28 @@ template <class T> static lbfgs_b200_hist* export_history(lbfgs_b200_solver* s, 
     ph.H = static_cast<T*>(s->d_hist) + (size_t)b * s->hist_elems;
     ph.bt_log = s->bt_log; ph.M = s->M; ph.bstride = (int64_t)s->M * 2 * ((int64_t)1 << s->bt_log);
     const dim3 grid((unsigned)std::min<int64_t>((s->n + 255) / 256, 4 * ctx->sm_count), (unsigned)s->M);
-    k_untile_history<T><<<grid, 256, 0, ctx->stream>>>(ph, s->n, h->ld, static_cast<T*>(h->S), static_cast<T*>(h->Y));
+    if (s->ring_points)
+    {
+        // the live pairs: ages 0 .. ncorr-1 below head
+        PairEnds ends;
+        for (int k = 0; k < 2 * s->M; k++) ends.v[k] = -1;
+        const unsigned char* pts = s->ring_pts.data() + (size_t)b * 2 * s->M;
+        for (int age = 0; age < s->ring_ncorr[(size_t)b]; age++)
+        {
+            const int slot = lb::slot_by_age(s->ring_head[(size_t)b], s->M, age);
+            ends.v[2 * slot] = pts[2 * slot];
+            ends.v[2 * slot + 1] = pts[2 * slot + 1];
+        }
+        const lb::ObjGeom<T> geo{s->n, s->ring_gofs, s->ring_nglob, nullptr, nullptr, nullptr};
+        if (with_objective<T>(ctx, s->ring_objective, [&](auto tag) {
+                using OBJ = decltype(tag);
+                if constexpr (!OBJ::kHalo)
+                    k_untile_points<T, OBJ><<<grid, 256, 0, ctx->stream>>>(ph, OBJ{geo}, ends, s->n, h->ld, static_cast<T*>(h->S), static_cast<T*>(h->Y));
+                return LBFGS_B200_OK;
+            }) != LBFGS_B200_OK)
+            return nullptr;
+    }
+    else k_untile_history<T><<<grid, 256, 0, ctx->stream>>>(ph, s->n, h->ld, static_cast<T*>(h->S), static_cast<T*>(h->Y));
     const T* small = static_cast<const T*>(s->d_small) + (size_t)b * s->small_elems;
     const size_t mm = (size_t)s->M * s->M;
     cudaMemcpyAsync(h->ys, small, sizeof(T) * s->M, cudaMemcpyDeviceToDevice, ctx->stream);
@@ -261,6 +323,7 @@ lbfgs_b200_status lbfgs_b200_solver_create_batch(lbfgs_b200_ctx* ctx, int64_t n,
     s->hist_elems = (size_t)nblocks * s->M * 2 * ((size_t)1 << s->bt_log);
     s->small_elems = (size_t)2 * s->M + 4 + 6 * (size_t)s->M * s->M;
     s->ring_head.assign((size_t)batch, 0); s->ring_ncorr.assign((size_t)batch, 0); s->ring_gram_cur.assign((size_t)batch, 0);
+    s->ring_pts.assign((size_t)batch * 2 * s->M, 0);
     s->exported.assign((size_t)batch, nullptr); s->export_fresh.assign((size_t)batch, 0);
     cudaError_t e = cudaSuccess;
     s->vec_elems = (((size_t)n * elem_bytes + 255) & ~size_t(255)) / elem_bytes;
@@ -269,6 +332,7 @@ lbfgs_b200_status lbfgs_b200_solver_create_batch(lbfgs_b200_ctx* ctx, int64_t n,
     if (e == cudaSuccess) e = pool_alloc(ctx, (void**)&s->vec_slab, (size_t)batch * 5 * s->vec_elems * elem_bytes);
     if (e == cudaSuccess) e = pool_alloc(ctx, (void**)&s->d_hist, (size_t)batch * s->hist_elems * elem_bytes);
     if (e == cudaSuccess) e = pool_alloc(ctx, (void**)&s->d_small, (size_t)batch * s->small_elems * elem_bytes);
+    if (e == cudaSuccess) e = pool_alloc(ctx, (void**)&s->d_pts, (size_t)batch * 2 * s->M);
     if (e == cudaSuccess) e = pool_alloc(ctx, (void**)&s->d_state, state_bytes);
     if (e == cudaSuccess) e = pool_alloc(ctx, (void**)&s->d_rounds, (elem_bytes == 8 ? sizeof(lb::PRound<double>) : sizeof(lb::PRound<float>)) * (size_t)batch);
     if (e == cudaSuccess) e = pool_alloc(ctx, (void**)&s->d_ctl, sizeof(lb::PCtl));
@@ -296,7 +360,7 @@ void lbfgs_b200_solver_destroy(lbfgs_b200_solver* s)
     if (!s) return;
     if (s->ctx && s->ctx->stream) cudaStreamSynchronize(s->ctx->stream);   // the events below must not be in use
     for (void* p : {(void*)s->vec_slab, (void*)s->lo_slab, (void*)s->d_state, (void*)s->d_rounds, (void*)s->d_ctl, (void*)s->d_partials, (void*)s->d_raw, (void*)s->d_halo,
-                    (void*)s->d_trace, (void*)s->d_hist, (void*)s->d_small})
+                    (void*)s->d_trace, (void*)s->d_hist, (void*)s->d_small, (void*)s->d_pts})
         pool_free(s->ctx, p);
     if (s->ev0) cudaEventDestroy(s->ev0);
     if (s->ev1) cudaEventDestroy(s->ev1);

@@ -35,6 +35,8 @@ template <class T> struct PHist
     __device__ __forceinline__ int BT() const { return 1 << bt_log; }
     __device__ __forceinline__ T* s_at(int slot, int64_t i) const { return H + (i >> bt_log) * bstride + ((int64_t)slot << (bt_log + 1)) + (i & (BT() - 1)); }
     __device__ __forceinline__ T* y_at(int slot, int64_t i) const { return s_at(slot, i) + BT(); }
+    // the ring as 2M point rows (objectives without neighbour coupling, see PState::pts): row `p` of element i
+    __device__ __forceinline__ T* pt_at(int p, int64_t i) const { return H + (i >> bt_log) * bstride + ((int64_t)p << bt_log) + (i & (BT() - 1)); }
 };
 
 // ---- per-problem state (device memory; the leader CTA's working copy) ----------------------------------------------------------
@@ -70,13 +72,18 @@ template <class T> struct PState
     int finished;
     int niter;      // return value of minimize()
     T fx_hist[kMaxPast];
+    // POINTS (the resident solve, objectives without neighbour coupling): the ring's 2M rows per block hold iterates instead of M
+    // pairs S|Y.  x and xp are rows of it (the flat x, g stay the caller's start point and result); a pair is rebuilt from its two
+    // endpoints wherever it is read: s = x_end - x_start, y = grad f(x_end) - grad f(x_start).
+    int px, pxp;                // point rows of x and xp
+    unsigned char* pts;         // [2M] device memory: start and end point row of the pair in each pair slot (read by every CTA)
     double* trace;              // optional: f of every evaluation
     long long trace_cap;
     long long rounds;           // rounds this problem took part in
 };
 
 template <class P> __device__ __forceinline__ void dswap(P& a, P& b) { P t = a; a = b; b = t; }
-__device__ __forceinline__ int slot_by_age(int head, int M, int age) { return ((head - 1 - age) % M + M) % M; }
+__host__ __device__ __forceinline__ int slot_by_age(int head, int M, int age) { return ((head - 1 - age) % M + M) % M; }
 
 // ---- the leader's work between two rounds ------------------------------------------------------------------------------------
 template <class T> __device__ __forceinline__ void record_eval(PState<T>* st, T fx)
@@ -93,9 +100,32 @@ template <class T> __device__ __forceinline__ void finish(PState<T>* st, int nit
     st->op = implied ? POP_MATERIALIZE : POP_IDLE;
 }
 
+// POINTS: the point row the pair-forming pass writes x to -- the first row after xp's, cyclically, that neither xp nor an endpoint
+// of a live pair holds.  A chained history then stays one cyclic run of rows.  2M rows always leave one free: m live pairs have at
+// most 2m endpoints.
+template <class T> __device__ int free_point(const PState<T>* st)
+{
+    const int P = 2 * st->M;
+    unsigned long long used[3] = {0ull, 0ull, 0ull};   // 2M <= 2 (kMaxM + 1) rows
+    auto mark = [&](int p) { used[p >> 6] |= 1ull << (p & 63); };
+    mark(st->pxp);
+    for (int age = 0; age < st->ncorr; age++)
+    {
+        const int s = slot_by_age(st->head, st->M, age);
+        mark(ldv(st->pts + 2 * s));
+        mark(ldv(st->pts + 2 * s + 1));
+    }
+    for (int k = 1; k < P; k++)
+    {
+        const int p = (st->pxp + k) % P;
+        if (!((used[p >> 6] >> (p & 63)) & 1ull)) return p;
+    }
+    return st->pxp;   // (not reached)
+}
+
 // after a search has produced its point -- in (x, g) when STORED, else implied by (step, at_start): the stopping rules
 // (LBFGS.h:137-154), then on to the pair-forming dots
-template <class T, bool STORED> __device__ __forceinline__ void after_search(PState<T>* st)
+template <class T, bool STORED, bool POINTS = false> __device__ __forceinline__ void after_search(PState<T>* st)
 {
     using namespace LBFGSpp;
     const int k = st->k;
@@ -108,11 +138,12 @@ template <class T, bool STORED> __device__ __forceinline__ void after_search(PSt
     }
     st->op = POP_DOTS_FORM;
     st->c_round = st->ncorr < st->m ? st->ncorr + 1 : st->m;
+    if (POINTS) st->px = free_point(st);
 }
 
 // the trial at st->step has been evaluated: {fx, dg, gg, xx}.  Sets the next op.  STORED: the trial is in (x, g), a kept trial
 // moves to (x_lo, g_lo) by pointer swap; otherwise a trial is its step, and the kept one is st->step_kept.
-template <class T, bool STORED> __device__ __forceinline__ void digest_trial(PState<T>* st, T fx, T dg, T gg, T xx)
+template <class T, bool STORED, bool POINTS = false> __device__ __forceinline__ void digest_trial(PState<T>* st, T fx, T dg, T gg, T xx)
 {
     record_eval(st, fx);
     bool keep = false;
@@ -136,12 +167,13 @@ template <class T, bool STORED> __device__ __forceinline__ void digest_trial(PSt
         st->at_start = PT_START;
         break;
     }
-    after_search<T, STORED>(st);
+    after_search<T, STORED, POINTS>(st);
 }
 
 // top of an iteration (LBFGS.h:121-127): the search is armed, the current point becomes the previous one.  G_IMPLIED: only x of
 // the current point is stored (the pair-forming pass of an objective without neighbour coupling does not write g)
-template <class T, bool G_IMPLIED = false> __device__ __forceinline__ bool begin_search(PState<T>* st, T step)
+// POINTS: x and xp are point rows; the flat x, g are left alone (they only ever hold the start point and the result)
+template <class T, bool G_IMPLIED = false, bool POINTS = false> __device__ __forceinline__ bool begin_search(PState<T>* st, T step)
 {
     // the search validates its inputs before anything moves (the reference throws before touching x): on failure x stays the
     // current point (FIRST or the pair-forming pass wrote it; G_IMPLIED: one MATERIALIZE round writes its g)
@@ -152,8 +184,12 @@ template <class T, bool G_IMPLIED = false> __device__ __forceinline__ bool begin
         finish(st, st->k, rc, G_IMPLIED);
         return false;
     }
-    dswap(st->xp, st->x);
-    dswap(st->gp, st->g);
+    if (POINTS) dswap(st->pxp, st->px);
+    else
+    {
+        dswap(st->xp, st->x);
+        dswap(st->gp, st->g);
+    }
     st->rec.begin();
     st->at_start = 0;
     st->op = POP_TRIAL;
@@ -162,8 +198,9 @@ template <class T, bool G_IMPLIED = false> __device__ __forceinline__ bool begin
 }
 
 // G_IMPLIED (the resident solve, objectives without neighbour coupling): g is stored by FIRST and MATERIALIZE only; every other pass
-// that needs grad f of a stored point evaluates it from x, bit for bit the g that would have been stored
-template <class T, bool STORED, bool G_IMPLIED = false> __device__ void advance_problem(PState<T>* st, const double* vals)
+// that needs grad f of a stored point evaluates it from x, bit for bit the g that would have been stored.  POINTS (the same solve):
+// the ring holds iterates (see PState::pts)
+template <class T, bool STORED, bool G_IMPLIED = false, bool POINTS = false> __device__ void advance_problem(PState<T>* st, const double* vals)
 {
     st->rounds++;
     switch (st->op)
@@ -179,14 +216,14 @@ template <class T, bool STORED, bool G_IMPLIED = false> __device__ void advance_
         st->gnorm = std::sqrt(gg);
         if (LBFGSpp::gradient_converged(st->gnorm, xx, st->epsilon, st->epsilon_rel)) { finish(st, 1); return; }
         st->rec.dg = -gg;                   // grad . (-grad)
-        begin_search(st, T(1) / st->gnorm); // LBFGS.h:108
+        begin_search<T, false, POINTS>(st, T(1) / st->gnorm); // LBFGS.h:108
         return;
     }
     case POP_TRIAL:
-        digest_trial<T, STORED>(st, (T)vals[0], (T)vals[1], (T)vals[2], (T)vals[3]);
+        digest_trial<T, STORED, POINTS>(st, (T)vals[0], (T)vals[1], (T)vals[2], (T)vals[3]);
         return;
     case POP_RESTORE:           // (x, g) now hold the search's start point; its sums were restored before
-        after_search<T, STORED>(st);
+        after_search<T, STORED, POINTS>(st);
         return;
     case POP_MATERIALIZE:       // (x, g) now hold the point the problem stopped at
         st->op = POP_IDLE;
@@ -198,6 +235,7 @@ template <class T, bool STORED, bool G_IMPLIED = false> __device__ void advance_
         if (LBFGSpp::curvature_ok(sy, yy, LBFGSpp::lsdetail::eps_of<T>()))
         {
             st->ys[st->head] = sy;
+            if (POINTS) { st->pts[2 * st->head] = (unsigned char)st->pxp; st->pts[2 * st->head + 1] = (unsigned char)st->px; }
             *st->theta = yy / sy;
             st->pending = st->head;
             st->head = (st->head + 1) % st->M;
@@ -218,9 +256,9 @@ template <class T, bool STORED, bool G_IMPLIED = false> __device__ void advance_
         if (st->pending >= 0) { st->gram_cur = 1 - st->gram_cur; st->pending = -1; }
         st->rec.dg = (T)vals[0];            // LBFGS.h:123 for the next pass
         st->k += 1;
-        if (!begin_search<T, G_IMPLIED>(st, T(1))) return;   // LBFGS.h:168
+        if (!begin_search<T, G_IMPLIED, POINTS>(st, T(1))) return;   // LBFGS.h:168
         // the pass already evaluated xp + 1*d (STORED: into the buffers that the rotation just made (x, g))
-        if (fused && st->ls.step() == T(1)) digest_trial<T, STORED>(st, (T)vals[1], (T)vals[2], (T)vals[3], (T)vals[4]);
+        if (fused && st->ls.step() == T(1)) digest_trial<T, STORED, POINTS>(st, (T)vals[1], (T)vals[2], (T)vals[3], (T)vals[4]);
         return;
     }
     default: return;
@@ -245,6 +283,7 @@ template <class T> inline void init_problem_state(PState<T>& p, const lbfgs_b200
 {
     p.head = 0; p.ncorr = 0; p.M = prm.m + 1; p.m = prm.m; p.gram_cur = 0; p.pending = -1;
     p.op = POP_FIRST; p.c_round = 0;
+    p.px = 0; p.pxp = 0;
     p.epsilon = (T)prm.epsilon; p.epsilon_rel = (T)prm.epsilon_rel; p.delta = (T)prm.delta; p.max_step = (T)prm.max_step;
     p.past = prm.past; p.max_iterations = prm.max_iterations;
     p.fuse_first_trial = fuse_first_trial;
