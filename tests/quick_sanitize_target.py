@@ -1,5 +1,5 @@
 """Small whole solves for tests/gpu_sanitize.sh (compute-sanitizer target; not collected by pytest): both solver loops, all four line
-searches, the neighbour-coupled objectives (staged tiles with margins, fp32 at odd n, a batch with per-problem data, plain dots rounds), fp32, a batch, the literal two-loop recursion, L-BFGS-B."""
+searches, the neighbour-coupled objectives (staged tiles with margins, fp32 at odd n, a batch with per-problem data, plain dots rounds), fp32, a batch, the literal two-loop recursion, histories of 64 pairs, L-BFGS-B."""
 import os
 import sys
 
@@ -47,5 +47,20 @@ bs.close()
 print("batch", [(r["status"], r["niter"]) for r in res])
 g = lb.LBFGSSolver(lb.LBFGSParam(m=5), "NocedalWright", hv_algo=lb.HV_TWO_LOOP).minimize(lb.OBJ_ROSENBROCK_CHAINED, np.full(3000, 1.3))
 print("lbfgs two-loop chained", g["status"], g["niter"], g["fx"])
+# long histories: a resident solve past c = 48 (the third round of columns, 64-element history blocks) and an m = 64 Gram apply_Hv
+d, b, _ = po.quad_tridiag_data(6003, seed=1)
+g = lb.LBFGSSolver(lb.LBFGSParam(m=64, max_iterations=52), "MoreThuente", resident=True).minimize(lb.OBJ_QUAD_TRIDIAG, np.zeros(6003), data0=d, data1=b)
+print("tridiag resident m=64", g["status"], g["niter"], g["nfev"], g["fx"])
+ctx = lb.Context(0)
+rng = np.random.default_rng(64)
+h = lb.History(ctx, 6003, 64)
+for _ in range(70):
+    s = rng.standard_normal(6003)
+    h.add(ctx.array(s), ctx.array(s + 0.1 * rng.standard_normal(6003)))
+res = ctx.empty(6003)
+h.apply_Hv(ctx.array(rng.standard_normal(6003)), -1.0, res, lb.HV_GRAM)
+print("apply_Hv gram m=64 c=%d" % h.ncorr, float(np.abs(res.get()).max()))
+del h, res
+ctx.close()
 g = lb.LBFGSBSolver(lb.LBFGSBParam()).minimize(lb.OBJ_ROSENBROCK_CHAINED, np.full(5000, 3.0), 2.0, 4.0)
 print("lbfgsb", g["status"], g["niter"], g["nfev"], g["fx"])
