@@ -755,12 +755,8 @@ __device__ __forceinline__ void dots_geometry(int c, int units, int& split, int&
 // ---- COMBINE (+ first trial) ---------------------------------------------------------------------------------------------------
 // d = cv*v + sum_j cy_j*y_j + cs_j*s_j ; FUSE: x1 = xc + d, g1 = grad f(x1) and the four trial sums (neighbour-coupled objectives:
 // x1, g1 written to (x1_out, g1_out)).
-// Staged rows of a tile: v, (xc,) then the history block's live slots; sh.slots[j] = packed row of the pair of age j.  Objectives
-// without neighbour coupling (G_IMPLIED): the ring holds points, and a tile stages only the point rows of point_plan -- xc and the
-// endpoints of the c pairs (c + 1 rows for a chained history, xc being the newest end).  v = grad f(xc) and the pairs are not
-// stored: each thread evaluates v of its unit and rebuilds y_j = grad f(x_end) - grad f(x_start), s_j = x_end - x_start with the
-// arithmetic that formed them, bit for bit the stored vectors; walking the y terms newest -> oldest it keeps the gradient of a pair's
-// start, which is the next pair's end in a chained history.  A thread owns
+// Staged rows of a tile: v, (xc,) then the history block's live slots; sh.slots[j] = packed row of the pair of age j (objectives
+// without neighbour coupling stage points instead and take p_combine_points).  A thread owns
 // one 16-byte unit of the tile and adds the terms in the order the recursion would (y newest -> oldest, then s oldest -> newest), with
 // the operand loads of 8 columns in flight before their multiply-adds retire (the pass is bound by shared-memory latency otherwise).
 // HALO (neighbour-coupled objectives, one GPU): x1 goes back into the staged x row, two spare warps form d and x1 of the element on
@@ -774,14 +770,14 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
                                           Between between)
 {
     constexpr int EPT = 16 / (int)sizeof(T);
-    constexpr bool G_IMPLIED = !OBJ::kHalo;
+    static_assert(OBJ::kHalo, "objectives without neighbour coupling take p_combine_points");
     constexpr int DV = HALO ? OBJ::kDataVectors : 0;              // HALO: the objective's data vectors ride in the stage as well
-    constexpr int NRHS = G_IMPLIED ? 0 : (FUSE ? 2 : 1) + DV;     // v (, xc) (, data0, data1) / (xc is a point row)
+    constexpr int NRHS = (FUSE ? 2 : 1) + DV;                     // v (, xc) (, data0, data1)
     constexpr int PAD = EPT;                                      // HALO: room for x1 of the neighbouring element on either side of the x row
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int TE = h.BT();
     const SlotRuns runs(end, c, h.M);
-    const int nrows = NRHS + (G_IMPLIED ? sh.npts : 2 * c);
+    const int nrows = NRHS + 2 * c;
     const size_t stage_elems = (size_t)nrows * TE + (HALO ? 2 * PAD : 0);
     int stages = (int)((size_t)kPStageBytes / (stage_elems * sizeof(T)));
     stages = stages > kPMaxStages ? kPMaxStages : stages;
@@ -792,7 +788,6 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
     // HALO: the x row is staged one granule into the stage (row 1 starts at TE + PAD), everything after it shifts by 2*PAD
     auto stage_one = [&](int64_t t, int s) {
         T* dstt = tiles + (size_t)s * stage_elems;
-        if constexpr (G_IMPLIED) { stage_points<T>(dstt, TE, 0, 0, own.start(t, TE), own.len(t, TE), h, sh, &full_bar[s]); return; }
         if (!HALO) { stage_tiled<T>(dstt, TE, NRHS, NRHS, own.start(t, TE), own.len(t, TE), h, runs, sh, &full_bar[s]); return; }
         if (tid >= 32) return;
         const int64_t e0 = own.start(t, TE);
@@ -817,21 +812,17 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
 
     T acc[5] = {T(0), T(0), T(0), T(0), T(0)};
     T pre[5] = {T(0), T(0), T(0), T(0), T(0)};   // HALO, right-margin warp: operands of the element after the current tile
-    // FUSE: the trial of one unit at x1 = xv (lanes past EPT: 0, or x1 of the right neighbour) -> acc[1..4]; x1 and g1 stored for a
-    // neighbour-coupled objective only (otherwise the pair-forming pass rebuilds the point if the search accepts it)
+    // FUSE: the trial of one unit at x1 = xv (lanes past EPT: 0, or x1 of the right neighbour) -> acc[1..4]; x1 and g1 stored
     auto first_trial = [&](const OBJ& o, int64_t i0, int cnt, const T (&xv)[4], T xl, T xr, const T (&r)[EPT]) {
         T dv[EPT], gv[4];
 #pragma unroll
         for (int k = 0; k < EPT; k++) dv[k] = (k < cnt) ? r[k] : T(0);   // (past cnt, d comes from whatever the vectors' padding holds)
         eval_pack(o, i0, cnt, xv, xl, xr, dv, gv, acc + 1);
-        if constexpr (OBJ::kHalo)
-        {
-            Unit<T> ug, uo;
+        Unit<T> ug, uo;
 #pragma unroll
-            for (int k = 0; k < EPT; k++) { ug.v[k] = gv[k]; uo.v[k] = xv[k]; }
-            st_unit<T>(x1_out, i0, cnt, uo);
-            st_unit<T>(g1_out, i0, cnt, ug);
-        }
+        for (int k = 0; k < EPT; k++) { ug.v[k] = gv[k]; uo.v[k] = xv[k]; }
+        st_unit<T>(x1_out, i0, cnt, uo);
+        st_unit<T>(g1_out, i0, cnt, ug);
     };
     __syncthreads();   // sh.vecs / sh.slots are in place and the staging ring is free
     int64_t next_tile = 0;
@@ -844,62 +835,31 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
     {
         mbar_wait(&full_bar[stage], (phase_bits >> stage) & 1u);
         phase_bits ^= (1u << stage);
-        T* base = tiles + (size_t)stage * stage_elems;                          // row 0: v (G_IMPLIED: the point rows)
-        T* xrow = G_IMPLIED ? base + (size_t)sh.xrow * TE : base + TE + (HALO ? PAD : 0);   // row 1: xc (FUSE)
+        T* base = tiles + (size_t)stage * stage_elems;                          // row 0: v
+        T* xrow = base + TE + (HALO ? PAD : 0);                                  // row 1: xc (FUSE)
         const T* hist = base + (size_t)NRHS * TE + (HALO ? 2 * PAD : 0);
         const int len = own.len(t, TE);
         const int64_t e0 = own.start(t, TE);
         // d of one unit: the arithmetic every owner of an element uses
         auto direction = [&](int off, T (&r)[EPT], Unit<T>& uv) {
-            if constexpr (G_IMPLIED)
+            uv = lds_unit<T>(base + off);
+#pragma unroll
+            for (int k = 0; k < EPT; k++) r[k] = cv * uv.v[k];
+#pragma unroll 8
+            for (int j = 0; j < c; j++)                    // y terms newest -> oldest
             {
-                const int64_t i0 = e0 + off;
-                const int cnt = len - off;
-                uv = grad_unit(obj, i0, cnt, lds_unit<T>(xrow + off));
+                const Unit<T> uy = lds_unit<T>(hist + ((size_t)2 * sh.slots[j] + 1) * TE + off);
+                const T cy = s_coef[1 + j];
 #pragma unroll
-                for (int k = 0; k < EPT; k++) r[k] = cv * uv.v[k];
-                Unit<T> gk = uv;                               // grad f of staged point row `kept`
-                int kept = sh.xrow;
-                for (int j = 0; j < c; j++)                    // y terms newest -> oldest
-                {
-                    const int re = sh.pend[j], rs = sh.pstart[j];
-                    const Unit<T> ge = (re == kept) ? gk : grad_unit(obj, i0, cnt, lds_unit<T>(base + (size_t)re * TE + off));
-                    gk = grad_unit(obj, i0, cnt, lds_unit<T>(base + (size_t)rs * TE + off));
-                    kept = rs;
-                    const T cy = s_coef[1 + j];
-#pragma unroll
-                    for (int k = 0; k < EPT; k++) r[k] += cy * (ge.v[k] - gk.v[k]);
-                }
-#pragma unroll 4
-                for (int j = c - 1; j >= 0; j--)               // s terms oldest -> newest
-                {
-                    const Unit<T> ue = lds_unit<T>(base + (size_t)sh.pend[j] * TE + off), us = lds_unit<T>(base + (size_t)sh.pstart[j] * TE + off);
-                    const T cs = s_coef[1 + c + j];
-#pragma unroll
-                    for (int k = 0; k < EPT; k++) r[k] += cs * (ue.v[k] - us.v[k]);
-                }
+                for (int k = 0; k < EPT; k++) r[k] += cy * uy.v[k];
             }
-            else
+#pragma unroll 8
+            for (int j = c - 1; j >= 0; j--)               // s terms oldest -> newest
             {
-                uv = lds_unit<T>(base + off);
+                const Unit<T> us = lds_unit<T>(hist + (size_t)2 * sh.slots[j] * TE + off);
+                const T cs = s_coef[1 + c + j];
 #pragma unroll
-                for (int k = 0; k < EPT; k++) r[k] = cv * uv.v[k];
-#pragma unroll 8
-                for (int j = 0; j < c; j++)                    // y terms newest -> oldest
-                {
-                    const Unit<T> uy = lds_unit<T>(hist + ((size_t)2 * sh.slots[j] + 1) * TE + off);
-                    const T cy = s_coef[1 + j];
-#pragma unroll
-                    for (int k = 0; k < EPT; k++) r[k] += cy * uy.v[k];
-                }
-#pragma unroll 8
-                for (int j = c - 1; j >= 0; j--)               // s terms oldest -> newest
-                {
-                    const Unit<T> us = lds_unit<T>(hist + (size_t)2 * sh.slots[j] * TE + off);
-                    const T cs = s_coef[1 + c + j];
-#pragma unroll
-                    for (int k = 0; k < EPT; k++) r[k] += cs * us.v[k];
-                }
+                for (int k = 0; k < EPT; k++) r[k] += cs * us.v[k];
             }
         };
         if constexpr (!HALO)
@@ -1035,6 +995,185 @@ __device__ __forceinline__ void p_combine(const OBJ& obj, const Own& own, const 
     {
         const double dacc[1] = {(double)acc[0]};
         block_sums<1>(dacc, sh, dst, G);
+    }
+}
+
+// ---- COMBINE (+ first trial), objectives without neighbour coupling --------------------------------------------------------------
+// The same d and trial sums as p_combine.  The ring holds points, and a tile stages only the point rows of point_plan -- xc and the
+// endpoints of the c pairs (c + 1 rows for a chained history, xc being the newest end).  v = grad f(xc) and the pairs are not stored:
+// they are rebuilt with the arithmetic that formed them, y_j = grad f(x_end) - grad f(x_start), s_j = x_end - x_start, bit for bit the
+// stored vectors.  The c + 1 gradient evaluations per unit are most of the pass's arithmetic, so the CTA's warps take a tile in two roles:
+//     gradient warps   v = grad f(xc) and d = cv*v + sum_j cy_j*y_j (newest -> oldest, keeping the gradient of a pair's start, which
+//                      is the next pair's end in a chained history) + sum_j cs_j*s_j (oldest -> newest), into a hand-off slot after
+//                      the staging ring.  They work in `ng` groups, group k taking tiles k, k + ng, ... with a slot of its own.
+//                      With 512 units per tile (fp64, m <= 4) the 8 spare warps are too few: ng = 0, and the owners form their units
+//     owner warps      thread u owns unit u of every tile -- the thread that owned it when one thread did a unit's whole arithmetic,
+//                      so each per-thread sum adds the same terms in the same order: stores d, adds v.d and, FUSE, the first trial
+//                      at x1 = xc + 1*d
+// (Also handing the s terms to the owners measured slower: 0.328 against 0.320 ms per round on config 2, DESIGN.md section 10.)
+// Which thread computes a value does not change its bits, so d and the sums are those of one thread doing a unit's whole arithmetic.
+// No CTA-wide barrier per tile: a stage has a full barrier (the bulk copies; parity in phase_bits) and an empty one (the owner warps,
+// which read a tile after its gradient warps); a hand-off slot has a formed barrier (its gradient warps) and a free one (the owner
+// warps).  Warp 0 re-arms a stage once its empty barrier completes.
+template <class T, class OBJ, bool FUSE, class Between>
+__device__ __forceinline__ void p_combine_points(const OBJ& obj, const Own& own, const PHist<T>& h, int c, T* tiles, T* __restrict__ res,
+                                                 PShared& sh, unsigned& phase_bits, double* dst, int G, Between between)
+{
+    static_assert(!OBJ::kHalo, "neighbour-coupled objectives take p_combine");
+    constexpr int EPT = 16 / (int)sizeof(T);
+    constexpr int kMaxGroups = kPMaxStages - 1;                  // a group works ahead of the owners on a loaded stage: at most stages - 1 tiles
+    __shared__ uint64_t empty_bar[kPMaxStages], formed_bar[kMaxGroups], free_bar[kMaxGroups];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int TE = h.BT();
+    const int units = TE / EPT;                                  // 32 .. 512
+    const int ow = (units + 31) / 32;                            // owner warps: 0 .. ow-1, one unit per thread
+    const int spare = kPWarps - ow;
+    const int gs = ow < spare ? ow : spare;                      // warps per gradient group
+    int ng = spare < ow ? 0 : spare / gs;                        // 0: the owners form their own units (512 units: 8 spare warps are too few)
+    ng = ng > kMaxGroups ? kMaxGroups : ng;
+    const size_t stage_elems = (size_t)sh.npts * TE;
+    int stages = (int)(((size_t)kPStageBytes / sizeof(T) - (size_t)ng * 2 * TE) / stage_elems);   // (>= 2: see bt_log in persist_host.cuh)
+    stages = stages > kPMaxStages ? kPMaxStages : stages;
+    ng = ng > stages - 1 ? stages - 1 : ng;
+    T* const hand = tiles + (size_t)stages * stage_elems;       // slot k: v, d (TE elements each)
+    const int64_t ntl = own.ntiles(TE);
+    const T* s_coef = reinterpret_cast<const T*>(sh.coef);
+    uint64_t* full_bar = sh.full_bar;
+    const bool owner = warp < ow;
+    const int grp = owner ? -1 : (warp - ow) / gs, gw = owner ? 0 : (warp - ow) % gs;
+
+    T acc[5] = {T(0), T(0), T(0), T(0), T(0)};
+    if (tid == 0)
+    {
+        for (int s = 0; s < stages; s++) mbar_init(&empty_bar[s], ow);
+        for (int k = 0; k < ng; k++) { mbar_init(&formed_bar[k], gs); mbar_init(&free_bar[k], ow); }
+    }
+    __syncthreads();   // sh.vecs / point_plan are in place, the barriers initialised and the staging ring is free
+    for (int s = 0; s < stages; s++)
+        if (s < ntl) stage_points<T>(tiles + (size_t)s * stage_elems, TE, 0, 0, own.start(s, TE), own.len(s, TE), h, sh, &full_bar[s]);
+    between();         // (ends with a barrier when it runs the recursion: sh.coef is in place)
+    const unsigned full_phase = phase_bits;
+    // v = grad f(xc) and d of one unit (lanes past cnt: x = 0), in the order of the recursion
+    auto form = [&](const T* base, int64_t i0, int off, int cnt, Unit<T>& uv, Unit<T>& ud) {
+        const T cv = s_coef[0];
+        uv = grad_unit(obj, i0, cnt, lds_unit<T>(base + (size_t)sh.xrow * TE + off));
+#pragma unroll
+        for (int k = 0; k < EPT; k++) ud.v[k] = cv * uv.v[k];
+        Unit<T> gk = uv;                                       // grad f of staged point row `kept`
+        int kept = sh.xrow;
+        for (int j = 0; j < c; j++)                            // y terms newest -> oldest
+        {
+            const int re = sh.pend[j], rs = sh.pstart[j];
+            const Unit<T> ge = (re == kept) ? gk : grad_unit(obj, i0, cnt, lds_unit<T>(base + (size_t)re * TE + off));
+            gk = grad_unit(obj, i0, cnt, lds_unit<T>(base + (size_t)rs * TE + off));
+            kept = rs;
+            const T cy = s_coef[1 + j];
+#pragma unroll
+            for (int k = 0; k < EPT; k++) ud.v[k] += cy * (ge.v[k] - gk.v[k]);
+        }
+#pragma unroll 4
+        for (int j = c - 1; j >= 0; j--)                       // s terms oldest -> newest
+        {
+            const Unit<T> ue = lds_unit<T>(base + (size_t)sh.pend[j] * TE + off), us = lds_unit<T>(base + (size_t)sh.pstart[j] * TE + off);
+            const T cs = s_coef[1 + c + j];
+#pragma unroll
+            for (int k = 0; k < EPT; k++) ud.v[k] += cs * (ue.v[k] - us.v[k]);
+        }
+    };
+    if (owner)
+    {
+        for (int64_t t = 0; t < ntl; t++)
+        {
+            const int stage = (int)(t % stages), slot = ng ? (int)(t % ng) : 0;
+            const unsigned lap = (unsigned)(t / stages) & 1u;
+            const T* base = tiles + (size_t)stage * stage_elems;
+            const T* xrow = base + (size_t)sh.xrow * TE;
+            const T* hv = hand + (size_t)slot * 2 * TE;
+            const int len = own.len(t, TE);
+            const int64_t e0 = own.start(t, TE);
+            mbar_wait(&full_bar[stage], ((full_phase >> stage) & 1u) ^ lap);
+            if (ng) mbar_wait(&formed_bar[slot], (unsigned)(t / ng) & 1u);
+            for (int off = tid * EPT; off < len; off += ow * 32 * EPT)
+            {
+                const int cnt = (len - off >= EPT) ? EPT : (len - off);
+                Unit<T> uv, ud;
+                if (ng) { uv = lds_unit<T>(hv + off); ud = lds_unit<T>(hv + TE + off); }
+                else form(base, e0 + off, off, len - off, uv, ud);
+#pragma unroll
+                for (int k = 0; k < EPT; k++) acc[0] += (k < cnt) ? uv.v[k] * ud.v[k] : T(0);
+                const int64_t i0 = e0 + off;
+                st_unit<T>(res, i0, cnt, ud);
+                if constexpr (FUSE)
+                {
+                    // the trial at x1 = xc + 1*d -> acc[1..4] (nothing stored: the pair-forming pass rebuilds the point if the search
+                    // accepts it)
+                    const Unit<T> ux = lds_unit<T>(xrow + off);
+                    T xv[4] = {T(0), T(0), T(0), T(0)}, dv[EPT], gv[4];
+#pragma unroll
+                    for (int k = 0; k < EPT; k++)
+                    {
+                        xv[k] = (k < cnt) ? ux.v[k] + T(1) * ud.v[k] : T(0);
+                        dv[k] = (k < cnt) ? ud.v[k] : T(0);
+                    }
+                    eval_pack(obj, i0, cnt, xv, T(0), T(0), dv, gv, acc + 1);
+                }
+            }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // these reads before the bulk copies that re-arm the stage
+            __syncwarp();
+            if (lane == 0) { if (ng) mbar_arrive(&free_bar[slot]); mbar_arrive(&empty_bar[stage]); }
+            if (warp == 0 && t + stages < ntl)
+            {
+                mbar_wait(&empty_bar[stage], lap);
+                stage_points<T>(tiles + (size_t)stage * stage_elems, TE, 0, 0, own.start(t + stages, TE), own.len(t + stages, TE), h, sh,
+                                &full_bar[stage]);
+            }
+        }
+    }
+    else if (grp < ng)
+    {
+        T* const hv = hand + (size_t)grp * 2 * TE;
+        for (int64_t t = grp; t < ntl; t += ng)
+        {
+            const int stage = (int)(t % stages);
+            const T* base = tiles + (size_t)stage * stage_elems;
+            const int len = own.len(t, TE);
+            const int64_t e0 = own.start(t, TE);
+            // A parity wait is only right when the barrier's previous phase has completed.  The stage's previous occupant in this pass is
+            // tile t - stages, which another group may have formed, so first wait until the owners are done with this slot's previous
+            // tile t - ng: they have then waited on the full barrier of every tile up to t - ng >= t - stages + 1 (ng < stages).  For
+            // t < ng this is the stage's first tile of the pass, and every earlier phase completed in an earlier pass.
+            if (t >= ng) mbar_wait(&free_bar[grp], (unsigned)(t / ng - 1) & 1u);
+            mbar_wait(&full_bar[stage], ((full_phase >> stage) & 1u) ^ ((unsigned)(t / stages) & 1u));
+            for (int off = (gw * 32 + lane) * EPT; off < len; off += gs * 32 * EPT)
+            {
+                Unit<T> uv, ud;
+                form(base, e0 + off, off, len - off, uv, ud);
+                *reinterpret_cast<float4*>(hv + off) = *reinterpret_cast<const float4*>(uv.v);
+                *reinterpret_cast<float4*>(hv + TE + off) = *reinterpret_cast<const float4*>(ud.v);
+            }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // these accesses before later bulk copies into this memory
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&formed_bar[grp]);
+        }
+    }
+    // the full barriers: one completed phase per tile a stage carried (every thread keeps the same parities, waiting or not)
+    for (int s = 0; s < stages; s++)
+        if (s < ntl) phase_bits ^= (unsigned)(((ntl - 1 - s) / stages + 1) & 1) << s;
+    if (FUSE)
+    {
+        const double dacc[5] = {(double)acc[0], (double)acc[1], (double)acc[2], (double)acc[3], (double)acc[4]};
+        block_sums<5>(dacc, sh, dst, G);
+    }
+    else
+    {
+        const double dacc[1] = {(double)acc[0]};
+        block_sums<1>(dacc, sh, dst, G);
+    }
+    // (block_sums began with a barrier: every arrival on and wait for the pass's barriers is done)
+    if (tid == 0)
+    {
+        for (int s = 0; s < stages; s++) mbar_inval(&empty_bar[s]);
+        for (int k = 0; k < ng; k++) { mbar_inval(&formed_bar[k]); mbar_inval(&free_bar[k]); }
     }
 }
 
@@ -1441,7 +1580,12 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
                 };
                 if (!own_scratch) solve_into(tiles);   // a long history: the staging ring is the scratch, the copies start afterwards
                 auto between = [&]() { if (own_scratch) solve_into(reinterpret_cast<T*>(s_gram)); };
-                if (fuse) p_combine<T, OBJ, true, OBJ::kHalo>(obj, own, st->hist, g.c, head, tiles, vd, vxp, vgp, sh, phase_bits, dst, G, between);
+                if constexpr (!HALO)
+                {
+                    if (fuse) p_combine_points<T, OBJ, true>(obj, own, st->hist, g.c, tiles, vd, sh, phase_bits, dst, G, between);
+                    else p_combine_points<T, OBJ, false>(obj, own, st->hist, g.c, tiles, vd, sh, phase_bits, dst, G, between);
+                }
+                else if (fuse) p_combine<T, OBJ, true, true>(obj, own, st->hist, g.c, head, tiles, vd, vxp, vgp, sh, phase_bits, dst, G, between);
                 else p_combine<T, OBJ, false, false>(obj, own, st->hist, g.c, head, tiles, vd, nullptr, nullptr, sh, phase_bits, dst, G, between);
                 break;
             }
