@@ -9,6 +9,8 @@
 #ifndef LBFGSPP_B200_LBFGS_SMALL_BATCH_H
 #define LBFGSPP_B200_LBFGS_SMALL_BATCH_H
 
+#include <limits>
+#include <stdexcept>
 #include <vector>
 
 #include "LBFGSBatch.h"
@@ -22,12 +24,26 @@ template <> struct small_batch_abi<double>
     static lbfgs_b200_status minimize(lbfgs_b200_ctx* c, int obj, const double* d0, const double* d1, int64_t ldd, int64_t n, int64_t B,
                                       const lbfgs_b200_param* p, int ls, double* X, int64_t ldx, double* G, lbfgs_b200_outcome* o)
     { return lbfgs_b200_small_minimize_f64(c, obj, d0, d1, ldd, n, B, p, ls, X, ldx, G, o); }
+    static lbfgs_b200_status minimize_keep(lbfgs_b200_ctx* c, int obj, const double* d0, const double* d1, int64_t ldd, int64_t n, int64_t B,
+                                           const lbfgs_b200_param* p, int ls, double* X, int64_t ldx, double* G, lbfgs_b200_outcome* o,
+                                           lbfgs_b200_small_hist* h)
+    { return lbfgs_b200_small_minimize_keep_f64(c, obj, d0, d1, ldd, n, B, p, ls, X, ldx, G, o, h); }
+    static lbfgs_b200_status times(lbfgs_b200_small_hist* h, int inv, int64_t b0, int64_t count, int k, const double* V, int64_t ldv,
+                                   int64_t ldvp, double* OUT, int64_t ldo, int64_t ldop)
+    { return lbfgs_b200_small_hist_times_f64(h, inv, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop); }
 };
 template <> struct small_batch_abi<float>
 {
     static lbfgs_b200_status minimize(lbfgs_b200_ctx* c, int obj, const float* d0, const float* d1, int64_t ldd, int64_t n, int64_t B,
                                       const lbfgs_b200_param* p, int ls, float* X, int64_t ldx, float* G, lbfgs_b200_outcome* o)
     { return lbfgs_b200_small_minimize_f32(c, obj, d0, d1, ldd, n, B, p, ls, X, ldx, G, o); }
+    static lbfgs_b200_status minimize_keep(lbfgs_b200_ctx* c, int obj, const float* d0, const float* d1, int64_t ldd, int64_t n, int64_t B,
+                                           const lbfgs_b200_param* p, int ls, float* X, int64_t ldx, float* G, lbfgs_b200_outcome* o,
+                                           lbfgs_b200_small_hist* h)
+    { return lbfgs_b200_small_minimize_keep_f32(c, obj, d0, d1, ldd, n, B, p, ls, X, ldx, G, o, h); }
+    static lbfgs_b200_status times(lbfgs_b200_small_hist* h, int inv, int64_t b0, int64_t count, int k, const float* V, int64_t ldv,
+                                   int64_t ldvp, float* OUT, int64_t ldo, int64_t ldop)
+    { return lbfgs_b200_small_hist_times_f32(h, inv, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop); }
 };
 }  // namespace detail
 
@@ -41,12 +57,29 @@ private:
     const LBFGSParam<Scalar>& m_param;
     Vector m_grad;          // B*n final gradients
     std::ptrdiff_t m_n;
+    long m_B;
+    bool m_keep;                    // keep_final_approx()
+    lbfgs_b200_small_hist* m_hist;  // the final approximations of the last minimize(), when it kept them
+    Device* m_dev;
+    bool m_kept;                    // the last minimize() filled m_hist
 
     LBFGSSmallBatchSolver(const LBFGSSmallBatchSolver&);
     LBFGSSmallBatchSolver& operator=(const LBFGSSmallBatchSolver&);
 
 public:
-    LBFGSSmallBatchSolver(const LBFGSParam<Scalar>& param) : m_param(param), m_n(0) { m_param.check_param(); }
+    LBFGSSmallBatchSolver(const LBFGSParam<Scalar>& param)
+        : m_param(param), m_n(0), m_B(0), m_keep(false), m_hist(nullptr), m_dev(nullptr), m_kept(false)
+    {
+        m_param.check_param();
+    }
+    ~LBFGSSmallBatchSolver()
+    {
+        if (m_hist) lbfgs_b200_small_hist_destroy(m_hist);
+    }
+
+    // Keep every problem's final L-BFGS approximation on the device in the next minimize() calls (off by default): B*(2m*n + m + 3m^2
+    // + 2) elements of device memory, see lbfgs_b200_small_hist_create.  Off, minimize() allocates nothing for it.
+    void keep_final_approx(bool on) { m_keep = on; }
 
     // largest n a problem may have for history size m and built-in objective `objective` (LBFGS_B200_OBJ_*); 0 if none
     static std::ptrdiff_t max_n(int m, int objective) { return std::ptrdiff_t(lbfgs_b200_small_max_n(m, int(sizeof(Scalar)), objective)); }
@@ -61,11 +94,29 @@ public:
         const std::ptrdiff_t n = X.size() / B;
         m_grad = Vector(dev, X.size());
         m_n = n;
+        m_B = B;
+        m_kept = false;
         const lbfgs_b200_param p = detail::abi_param(m_param);
         std::vector<lbfgs_b200_outcome> raw((size_t)B);
-        dev.check(detail::small_batch_abi<Scalar>::minimize(dev.ctx(), f.builtin_kind(), f.builtin_data0(), f.builtin_data1(), int64_t(ldd), int64_t(n),
-                                                            int64_t(B), &p, detail::line_search_id<LineSearch>::value, X.data(), int64_t(n),
-                                                            m_grad.data(), raw.data()));
+        if (m_keep)
+        {
+            if (m_hist && (m_dev != &dev || !same_shape(n, B)))
+            {
+                lbfgs_b200_small_hist_destroy(m_hist);
+                m_hist = nullptr;
+            }
+            if (!m_hist) dev.check(lbfgs_b200_small_hist_create(dev.ctx(), int64_t(n), m_param.m, int(sizeof(Scalar)), int64_t(B), &m_hist));
+            m_dev = &dev;
+            m_hist_n = n; m_hist_B = B; m_hist_m = m_param.m;
+            dev.check(detail::small_batch_abi<Scalar>::minimize_keep(dev.ctx(), f.builtin_kind(), f.builtin_data0(), f.builtin_data1(), int64_t(ldd),
+                                                                     int64_t(n), int64_t(B), &p, detail::line_search_id<LineSearch>::value, X.data(),
+                                                                     int64_t(n), m_grad.data(), raw.data(), m_hist));
+            m_kept = true;
+        }
+        else
+            dev.check(detail::small_batch_abi<Scalar>::minimize(dev.ctx(), f.builtin_kind(), f.builtin_data0(), f.builtin_data1(), int64_t(ldd), int64_t(n),
+                                                                int64_t(B), &p, detail::line_search_id<LineSearch>::value, X.data(), int64_t(n),
+                                                                m_grad.data(), raw.data()));
         std::vector<BatchOutcome<Scalar> > out((size_t)B);
         for (size_t b = 0; b < size_t(B); b++)
         {
@@ -77,6 +128,65 @@ public:
     }
     // gradient of problem b at its solution (device pointer into the solver's own B*n buffer, valid until the next minimize())
     const Scalar* final_grad(long b) const { return m_grad.data() + std::ptrdiff_t(b) * m_n; }
+
+    // The final approximations of the last minimize() (keep_final_approx(true)) as operators, every problem in one launch: V holds
+    // B*k vectors back to back, problem b's vector j at [(b*k + j)*n, ...); OUT (resized to match) receives B_b or H_b times each.
+    void final_approx_hessian_times(const Vector& V, Vector& OUT) { all_times(V, OUT, false); }
+    void final_approx_inverse_hessian_times(const Vector& V, Vector& OUT) { all_times(V, OUT, true); }
+    // One problem b: OUT = B_b V or H_b V, V holding k = V.size()/n vectors back to back (the signatures of LBFGSBatchSolver).
+    void final_approx_hessian_times(long b, const Vector& V, Vector& OUT) { one_times(b, V, OUT, false); }
+    void final_approx_inverse_hessian_times(long b, const Vector& V, Vector& OUT) { one_times(b, V, OUT, true); }
+    // The dense n x n matrices of problem b (LBFGSSolver::final_approx_hessian / final_approx_inverse_hessian), formed on the device
+    // as the products with the columns of I.
+    SmallMatrix<Scalar> final_approx_hessian(long b) { return dense(b, false); }
+    SmallMatrix<Scalar> final_approx_inverse_hessian(long b) { return dense(b, true); }
+
+private:
+    std::ptrdiff_t m_hist_n = 0;
+    long m_hist_B = 0;
+    int m_hist_m = 0;
+    bool same_shape(std::ptrdiff_t n, long B) const { return m_hist_n == n && m_hist_B == B && m_hist_m == m_param.m; }
+
+    void require_kept() const
+    {
+        if (!m_kept) throw std::logic_error("LBFGSSmallBatchSolver: no final approximation kept (call keep_final_approx(true) before minimize())");
+    }
+    void all_times(const Vector& V, Vector& OUT, bool inverse)
+    {
+        require_kept();
+        const std::ptrdiff_t per = m_n * std::ptrdiff_t(m_B);
+        if (V.size() < 1 || V.size() % per != 0 || V.size() / per > std::numeric_limits<int>::max())
+            throw std::invalid_argument("V.size() must be a positive multiple of B * n");
+        const int k = int(V.size() / per);
+        OUT.resize(V.size());
+        m_dev->check(detail::small_batch_abi<Scalar>::times(m_hist, inverse, 0, int64_t(m_B), k, V.data(), int64_t(m_n), int64_t(k) * m_n,
+                                                            OUT.data(), int64_t(m_n), int64_t(k) * m_n));
+    }
+    void one_times(long b, const Vector& V, Vector& OUT, bool inverse)
+    {
+        require_kept();
+        if (b < 0 || b >= m_B) throw std::invalid_argument("LBFGSSmallBatchSolver: problem index out of range");
+        const int k = BFGSMat<Scalar>::block_count(V.size(), m_n);
+        OUT.resize(V.size());
+        m_dev->check(detail::small_batch_abi<Scalar>::times(m_hist, inverse, int64_t(b), 1, k, V.data(), int64_t(m_n), 0, OUT.data(),
+                                                            int64_t(m_n), 0));
+    }
+    SmallMatrix<Scalar> dense(long b, bool inverse)
+    {
+        require_kept();
+        if (b < 0 || b >= m_B) throw std::invalid_argument("LBFGSSmallBatchSolver: problem index out of range");
+        const int n = int(m_n);
+        std::vector<Scalar> eye(size_t(n) * size_t(n), Scalar(0));
+        for (int i = 0; i < n; i++) eye[size_t(i) * size_t(n) + size_t(i)] = Scalar(1);
+        Vector I(*m_dev), OUT(*m_dev);
+        I.copy_from_host(eye.data(), std::ptrdiff_t(n) * n);
+        one_times(b, I, OUT, inverse);
+        OUT.copy_to_host(eye.data());
+        SmallMatrix<Scalar> A(n, n);
+        for (int j = 0; j < n; j++)   // column j of A is the product with e_j
+            for (int i = 0; i < n; i++) A(i, j) = eye[size_t(j) * size_t(n) + size_t(i)];
+        return A;
+    }
 };
 
 }  // namespace LBFGSpp

@@ -16,6 +16,7 @@
 
 #include "DeviceVector.h"
 #include "BKLDLT.h"
+#include "CompactForm.h"
 #include "SmallDense.h"
 
 namespace LBFGSpp {
@@ -174,19 +175,7 @@ public:
         m_SS = SmallMatrix<Scalar>(c, c);
         m_dev->check(detail::BoxAbi<Scalar>::hist_gram(m_hist, m_SY.data(), m_SS.data(), nullptr, nullptr, &m_theta_host));
         m_Minv = SmallMatrix<Scalar>(2 * c, 2 * c);
-        for (int a = 0; a < c; a++)
-        {
-            m_Minv(a, a) = -m_SY(a, a);
-            for (int b = 0; b < c; b++)
-            {
-                if (a < b)  // age a < age b: pair a is the newer one
-                {
-                    m_Minv(c + a, b) = m_SY(a, b);
-                    m_Minv(b, c + a) = m_SY(a, b);
-                }
-                m_Minv(c + a, c + b) = m_theta_host * m_SS(a, b);
-            }
-        }
+        compact_minv(c, m_SY.data(), m_SS.data(), c, m_theta_host, m_Minv.data());
         m_Msolver.compute(m_Minv);
         m_M = SmallMatrix<Scalar>(2 * c, 2 * c);
         std::vector<Scalar> e(size_t(2 * c));
@@ -332,7 +321,7 @@ public:
 
     // The operator form of the same two matrices, at any n: OUT = B V or H V for k vectors stored back to back in V (OUT is resized
     // to match), in groups of 16 vectors.  Per group one pass over the history for W'V (lbfgs_b200_hist_wt_dot_multi), the 2c x 2c
-    // algebra on the host, and one pass for the combination (lbfgs_b200_hist_lincomb_multi):
+    // algebra of CompactForm.h on the host, and one pass for the combination (lbfgs_b200_hist_lincomb_multi):
     //   B v = theta v - W M W'v                  C = -M W'v in W's [Y ; theta S] convention, a0 = theta
     //   H v = v/theta + S u_s + Y u_y/theta      u_y = -R^-1 S'v,  u_s = R^-T ((D + Y'Y/theta) R^-1 S'v - Y'v/theta),  a0 = 1/theta
     // (the compact form of H above, with triangular solves per vector; B is never inverted).  With c = 0: B = theta I, H = I/theta.
@@ -356,23 +345,18 @@ private:
         refresh_middle();
         const int c = m_c_host;
         const Scalar theta = m_theta_host;
-        // H: R(t, u) = s_t'y_u (t <= u) and Y'Y in chronological order t = c - 1 - age
+        // H: R and Y'Y in chronological order (compact_h_setup)
         SmallMatrix<Scalar> R(c, c), YY(c, c);
         if (inverse && c > 0)
         {
             SmallMatrix<Scalar> YYage(c, c);
             m_dev->check(detail::BoxAbi<Scalar>::hist_gram(m_hist, nullptr, nullptr, YYage.data(), nullptr, nullptr));
-            for (int t = 0; t < c; t++)
-                for (int u = 0; u < c; u++)
-                {
-                    R(t, u) = t <= u ? m_SY(c - 1 - t, c - 1 - u) : Scalar(0);
-                    YY(t, u) = YYage(c - 1 - t, c - 1 - u);
-                }
+            compact_h_setup(c, m_SY.data(), YYage.data(), c, R.data(), YY.data());
         }
         OUT.resize(V.size());
         const int kGroup = 16;
         const size_t cs = static_cast<size_t>(c);
-        std::vector<Scalar> Wv, C, p(cs), q(cs), w(cs), us(cs), u(2 * cs);
+        std::vector<Scalar> Wv, C, w(cs), us(cs);
         for (int j0 = 0; j0 < k; j0 += kGroup)
         {
             const int kk = std::min(kGroup, k - j0);
@@ -385,48 +369,8 @@ private:
             }
             for (int j = 0; j < kk && c > 0; j++)
             {
-                auto Cy = [&](int age) -> Scalar& { return C[size_t(age * kk + j)]; };
-                auto Cs = [&](int age) -> Scalar& { return C[size_t((c + age) * kk + j)]; };
-                if (!inverse)
-                {
-                    for (int a = 0; a < c; a++)
-                    {
-                        u[size_t(a)] = Wv[size_t(a * kk + j)];
-                        u[size_t(c + a)] = theta * Wv[size_t((c + a) * kk + j)];
-                    }
-                    const std::vector<Scalar> Mu = m_M.times(u);
-                    for (int a = 0; a < c; a++)
-                    {
-                        Cy(a) = -Mu[size_t(a)];
-                        Cs(a) = -theta * Mu[size_t(c + a)];
-                    }
-                    continue;
-                }
-                for (int t = 0; t < c; t++)
-                {
-                    p[size_t(t)] = Wv[size_t((c + c - 1 - t) * kk + j)];   // s_t'v
-                    q[size_t(t)] = Wv[size_t((c - 1 - t) * kk + j)];       // y_t'v
-                }
-                for (int t = c - 1; t >= 0; t--)   // w = R^-1 S'v
-                {
-                    Scalar acc = p[size_t(t)];
-                    for (int s = t + 1; s < c; s++) acc -= R(t, s) * w[size_t(s)];
-                    w[size_t(t)] = acc / R(t, t);
-                }
-                for (int t = 0; t < c; t++)        // u_s = R^-T ((D + Y'Y/theta) w - Y'v/theta)
-                {
-                    Scalar z = R(t, t) * w[size_t(t)];
-                    Scalar yyw = Scalar(0);
-                    for (int s = 0; s < c; s++) yyw += YY(t, s) * w[size_t(s)];
-                    z += (yyw - q[size_t(t)]) / theta;
-                    for (int s = 0; s < t; s++) z -= R(s, t) * us[size_t(s)];
-                    us[size_t(t)] = z / R(t, t);
-                }
-                for (int t = 0; t < c; t++)
-                {
-                    Cy(c - 1 - t) = -w[size_t(t)] / theta;
-                    Cs(c - 1 - t) = us[size_t(t)];
-                }
+                if (inverse) compact_h_coef(c, R.data(), YY.data(), theta, Wv.data() + j, kk, w.data(), us.data(), 1, C.data() + j, kk);
+                else compact_b_coef(c, m_M.data(), theta, Wv.data() + j, kk, C.data() + j, kk);
             }
             m_dev->check(detail::BoxAbi<Scalar>::hist_lincomb_multi(m_hist, inverse ? Scalar(1) / theta : theta, kk, v, m_n,
                                                                     c > 0 ? C.data() : nullptr, OUT.data() + std::ptrdiff_t(j0) * m_n, m_n));

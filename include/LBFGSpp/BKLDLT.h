@@ -14,11 +14,10 @@
 #ifndef LBFGSPP_B200_BKLDLT_H
 #define LBFGSPP_B200_BKLDLT_H
 
-#include <cmath>
 #include <stdexcept>
-#include <utility>
 #include <vector>
 
+#include "CompactForm.h"
 #include "SmallDense.h"
 
 namespace LBFGSpp {
@@ -28,131 +27,34 @@ enum BKLDLT_UPLO { Lower = 0, Upper = 1 };
 template <typename Scalar>
 class BKLDLT
 {
-    enum BlockTag : unsigned char { SINGLE = 0, PAIR_HEAD = 1, PAIR_TAIL = 2 };
-
     int m_n;
-    SmallMatrix<Scalar> m_w;       // strictly lower part: L;  diagonal (and sub-diagonal inside a pair): D
-    std::vector<int> m_order;      // m_order[i] = original index now at position i
-    std::vector<BlockTag> m_tag;
+    SmallMatrix<Scalar> m_w;              // strictly lower part: L;  diagonal (and sub-diagonal inside a pair): D
+    std::vector<int> m_order;             // m_order[i] = original index now at position i
+    std::vector<unsigned char> m_tag;     // BK_SINGLE / BK_PAIR_HEAD / BK_PAIR_TAIL
     int m_info;
-
-    // symmetric interchange of positions p < q: whole rows (carries the finished columns of L along) and, in the
-    // not-yet-eliminated block starting at `from`, the columns
-    void interchange(int p, int q, int from)
-    {
-        if (p == q) return;
-        for (int j = 0; j < m_n; j++) std::swap(m_w(p, j), m_w(q, j));
-        for (int i = from; i < m_n; i++) std::swap(m_w(i, p), m_w(i, q));
-        std::swap(m_order[size_t(p)], m_order[size_t(q)]);
-    }
 
 public:
     BKLDLT() : m_n(0), m_info(NOT_COMPUTED) {}
     explicit BKLDLT(const SmallMatrix<Scalar>& mat, int uplo = Lower) : m_n(0), m_info(NOT_COMPUTED) { compute(mat, uplo); }
 
-    // Only the `uplo` triangle of `mat` is read.
+    // Only the `uplo` triangle of `mat` is read.  The factorisation itself is bk_factor (CompactForm.h).
     void compute(const SmallMatrix<Scalar>& mat, int uplo = Lower)
     {
-        using std::abs;
         if (mat.rows() != mat.cols()) throw std::invalid_argument("BKLDLT: matrix must be square");
         const int n = m_n = mat.rows();
         m_w = SmallMatrix<Scalar>(n, n);
         for (int i = 0; i < n; i++)
             for (int j = 0; j <= i; j++) m_w(i, j) = m_w(j, i) = (uplo == Lower) ? mat(i, j) : mat(j, i);
         m_order.resize(size_t(n));
-        for (int i = 0; i < n; i++) m_order[size_t(i)] = i;
-        m_tag.assign(size_t(n), SINGLE);
-        m_info = SUCCESSFUL;
-        const Scalar alpha = Scalar((1.0 + std::sqrt(17.0)) / 8.0);
-
-        int k = 0;
-        while (k < n)
-        {
-            // largest off-diagonal magnitude of column k in the active block
-            int r = k;
-            Scalar colmax = Scalar(0);
-            for (int i = k + 1; i < n; i++)
-                if (abs(m_w(i, k)) > colmax) { colmax = abs(m_w(i, k)); r = i; }
-            const Scalar akk = abs(m_w(k, k));
-            bool pair = false;
-            if (colmax > Scalar(0) && akk < alpha * colmax)
-            {
-                Scalar rowmax = Scalar(0);  // largest off-diagonal magnitude of row/column r in the active block
-                for (int j = k; j < n; j++)
-                    if (j != r && abs(m_w(r, j)) > rowmax) rowmax = abs(m_w(r, j));
-                if (akk * rowmax >= alpha * colmax * colmax) { /* a(k,k) is acceptable after all */ }
-                else if (abs(m_w(r, r)) >= alpha * rowmax) interchange(k, r, k);
-                else { interchange(k + 1, r, k); pair = true; }
-            }
-            if (!pair)
-            {
-                const Scalar d = m_w(k, k);
-                if (d == Scalar(0)) { m_info = NUMERICAL_ISSUE; return; }
-                for (int i = k + 1; i < n; i++)
-                {
-                    const Scalar li = m_w(i, k) / d;
-                    for (int j = k + 1; j <= i; j++) m_w(i, j) -= li * m_w(k, j);  // row k still holds column k unscaled
-                    m_w(i, k) = li;
-                }
-                for (int i = k + 1; i < n; i++)
-                    for (int j = i + 1; j < n; j++) m_w(i, j) = m_w(j, i);
-                k += 1;
-            }
-            else
-            {
-                const Scalar a = m_w(k, k), b = m_w(k + 1, k), c = m_w(k + 1, k + 1);
-                const Scalar det = a * c - b * b;
-                if (det == Scalar(0)) { m_info = NUMERICAL_ISSUE; return; }
-                m_tag[size_t(k)] = PAIR_HEAD;
-                m_tag[size_t(k + 1)] = PAIR_TAIL;
-                for (int i = k + 2; i < n; i++)
-                {
-                    const Scalar u = m_w(i, k), v = m_w(i, k + 1);
-                    const Scalar l1 = (u * c - v * b) / det, l2 = (v * a - u * b) / det;
-                    for (int j = k + 2; j <= i; j++) m_w(i, j) -= l1 * m_w(k, j) + l2 * m_w(k + 1, j);
-                    m_w(i, k) = l1;
-                    m_w(i, k + 1) = l2;
-                }
-                // mirror the updated block: the pivot search and the next elimination read rows as well as columns
-                for (int i = k + 2; i < n; i++)
-                    for (int j = i + 1; j < n; j++) m_w(i, j) = m_w(j, i);
-                k += 2;
-            }
-        }
+        m_tag.assign(size_t(n), (unsigned char)BK_SINGLE);
+        m_info = bk_factor(m_w.data(), n, m_order.data(), m_tag.data()) == 0 ? SUCCESSFUL : NUMERICAL_ISSUE;
     }
 
     void solve_inplace(std::vector<Scalar>& b) const
     {
         if (m_info == NOT_COMPUTED) throw std::logic_error("BKLDLT: need to call compute() first");
-        const int n = m_n;
-        std::vector<Scalar> z(static_cast<size_t>(n));
-        for (int i = 0; i < n; i++) z[size_t(i)] = b[size_t(m_order[size_t(i)])];
-        // L z' = z : columns of a pair carry no entry on the pair's own rows
-        for (int k = 0; k < n; k++)
-        {
-            const int first = (m_tag[size_t(k)] == PAIR_HEAD) ? k + 2 : k + 1;
-            for (int i = first; i < n; i++) z[size_t(i)] -= m_w(i, k) * z[size_t(k)];
-        }
-        for (int k = 0; k < n; k++)
-        {
-            if (m_tag[size_t(k)] == SINGLE)
-                z[size_t(k)] /= m_w(k, k);
-            else if (m_tag[size_t(k)] == PAIR_HEAD)
-            {
-                const Scalar a = m_w(k, k), bb = m_w(k + 1, k), c = m_w(k + 1, k + 1), det = a * c - bb * bb;
-                const Scalar u = z[size_t(k)], v = z[size_t(k + 1)];
-                z[size_t(k)] = (u * c - v * bb) / det;
-                z[size_t(k + 1)] = (v * a - u * bb) / det;
-            }
-        }
-        for (int k = n - 1; k >= 0; k--)
-        {
-            const int first = (m_tag[size_t(k)] == PAIR_HEAD) ? k + 2 : k + 1;
-            Scalar acc = Scalar(0);
-            for (int i = first; i < n; i++) acc += m_w(i, k) * z[size_t(i)];
-            z[size_t(k)] -= acc;
-        }
-        for (int i = 0; i < n; i++) b[size_t(m_order[size_t(i)])] = z[size_t(i)];
+        std::vector<Scalar> z(static_cast<size_t>(m_n));
+        bk_solve(m_w.data(), m_n, m_order.data(), m_tag.data(), b.data(), 1, z.data());
     }
     std::vector<Scalar> solve(std::vector<Scalar> b) const
     {

@@ -1,0 +1,209 @@
+// LBFGSpp/CompactForm.h -- the 2c x 2c algebra of the compact L-BFGS representation over raw arrays, written once for the host
+// (BFGSMat.h, BKLDLT.h) and the device (the small-batch products of csrc/small_batch.cuh).  Compiled by g++ and nvcc alike; with
+// -ffp-contract=off / -fmad=false both compute the same bits from the same inputs.
+//
+// Conventions: history columns by AGE (0 = newest pair); the c x c Gram blocks by age, row-major with leading dimension ldg:
+// SY(a, b) = s_a'y_b, SS(a, b) = s_a's_b, YY(a, b) = y_a'y_b.  Per vector, wv[r * ldw] holds the dots [Y S]'v (rows y by age, then
+// s by age) and the coefficients are written to C[r * ldc] in the same row order.
+//   B v = theta v - W M W'v,  W = [Y, theta S],  M = Minv^-1,  Minv = [ -D   L' ; L   theta S'S ]
+//       (D = diag(s_a'y_a), L(a, b) = s_a'y_b when pair a is newer than pair b)          C = -M W'v in W's convention, a0 = theta
+//   H v = v/theta + S u_s + Y u_y/theta,  R = triu(S'Y) in chronological order t = c - 1 - age:
+//       u_y = -R^-1 S'v,  u_s = R^-T ((D + Y'Y/theta) R^-1 S'v - Y'v/theta)                                    a0 = 1/theta
+// With c = 0: B = theta I, H = I / theta.
+#ifndef LBFGSPP_B200_COMPACT_FORM_H
+#define LBFGSPP_B200_COMPACT_FORM_H
+
+#include <cmath>
+
+#include "LineSearchCore.h"
+
+namespace LBFGSpp {
+
+// ---- Bunch-Kaufman LDL' of a symmetric indefinite n x n matrix (the pivot rule is documented in BKLDLT.h) ----------------------
+enum { BK_SINGLE = 0, BK_PAIR_HEAD = 1, BK_PAIR_TAIL = 2 };
+
+// w: the full symmetric matrix, row-major, factorised in place (strictly lower part: L; diagonal and the sub-diagonal inside a
+// pair: D).  order[i]: original index now at position i; tag[i]: BK_*.  Returns 0 (SUCCESSFUL) or 2 (NUMERICAL_ISSUE).
+template <typename T>
+LBFGS_HD inline int bk_factor(T* w, int n, int* order, unsigned char* tag)
+{
+    using std::abs;
+    auto W = [&](int i, int j) -> T& { return w[i * n + j]; };
+    // symmetric interchange of positions p < q: whole rows, and the columns of the not-yet-eliminated block starting at `from`
+    auto interchange = [&](int p, int q, int from) {
+        if (p == q) return;
+        for (int j = 0; j < n; j++) { const T t = W(p, j); W(p, j) = W(q, j); W(q, j) = t; }
+        for (int i = from; i < n; i++) { const T t = W(i, p); W(i, p) = W(i, q); W(i, q) = t; }
+        const int t = order[p]; order[p] = order[q]; order[q] = t;
+    };
+    for (int i = 0; i < n; i++) { order[i] = i; tag[i] = BK_SINGLE; }
+    const T alpha = T((1.0 + std::sqrt(17.0)) / 8.0);
+    int k = 0;
+    while (k < n)
+    {
+        // largest off-diagonal magnitude of column k in the active block
+        int r = k;
+        T colmax = T(0);
+        for (int i = k + 1; i < n; i++)
+            if (abs(W(i, k)) > colmax) { colmax = abs(W(i, k)); r = i; }
+        const T akk = abs(W(k, k));
+        bool pair = false;
+        if (colmax > T(0) && akk < alpha * colmax)
+        {
+            T rowmax = T(0);  // largest off-diagonal magnitude of row/column r in the active block
+            for (int j = k; j < n; j++)
+                if (j != r && abs(W(r, j)) > rowmax) rowmax = abs(W(r, j));
+            if (akk * rowmax >= alpha * colmax * colmax) { /* a(k,k) is acceptable after all */ }
+            else if (abs(W(r, r)) >= alpha * rowmax) interchange(k, r, k);
+            else { interchange(k + 1, r, k); pair = true; }
+        }
+        if (!pair)
+        {
+            const T d = W(k, k);
+            if (d == T(0)) return 2;
+            for (int i = k + 1; i < n; i++)
+            {
+                const T li = W(i, k) / d;
+                for (int j = k + 1; j <= i; j++) W(i, j) -= li * W(k, j);  // row k still holds column k unscaled
+                W(i, k) = li;
+            }
+            for (int i = k + 1; i < n; i++)
+                for (int j = i + 1; j < n; j++) W(i, j) = W(j, i);
+            k += 1;
+        }
+        else
+        {
+            const T a = W(k, k), b = W(k + 1, k), c = W(k + 1, k + 1);
+            const T det = a * c - b * b;
+            if (det == T(0)) return 2;
+            tag[k] = BK_PAIR_HEAD;
+            tag[k + 1] = BK_PAIR_TAIL;
+            for (int i = k + 2; i < n; i++)
+            {
+                const T u = W(i, k), v = W(i, k + 1);
+                const T l1 = (u * c - v * b) / det, l2 = (v * a - u * b) / det;
+                for (int j = k + 2; j <= i; j++) W(i, j) -= l1 * W(k, j) + l2 * W(k + 1, j);
+                W(i, k) = l1;
+                W(i, k + 1) = l2;
+            }
+            // mirror the updated block: the pivot search and the next elimination read rows as well as columns
+            for (int i = k + 2; i < n; i++)
+                for (int j = i + 1; j < n; j++) W(i, j) = W(j, i);
+            k += 2;
+        }
+    }
+    return 0;
+}
+
+// b <- A^-1 b for the factorisation above; b[i * bstride], z: n elements of scratch
+template <typename T>
+LBFGS_HD inline void bk_solve(const T* w, int n, const int* order, const unsigned char* tag, T* b, int bstride, T* z)
+{
+    auto W = [&](int i, int j) { return w[i * n + j]; };
+    for (int i = 0; i < n; i++) z[i] = b[order[i] * bstride];
+    // L z' = z : columns of a pair carry no entry on the pair's own rows
+    for (int k = 0; k < n; k++)
+    {
+        const int first = (tag[k] == BK_PAIR_HEAD) ? k + 2 : k + 1;
+        for (int i = first; i < n; i++) z[i] -= W(i, k) * z[k];
+    }
+    for (int k = 0; k < n; k++)
+    {
+        if (tag[k] == BK_SINGLE)
+            z[k] /= W(k, k);
+        else if (tag[k] == BK_PAIR_HEAD)
+        {
+            const T a = W(k, k), bb = W(k + 1, k), c = W(k + 1, k + 1), det = a * c - bb * bb;
+            const T u = z[k], v = z[k + 1];
+            z[k] = (u * c - v * bb) / det;
+            z[k + 1] = (v * a - u * bb) / det;
+        }
+    }
+    for (int k = n - 1; k >= 0; k--)
+    {
+        const int first = (tag[k] == BK_PAIR_HEAD) ? k + 2 : k + 1;
+        T acc = T(0);
+        for (int i = first; i < n; i++) acc += W(i, k) * z[i];
+        z[k] -= acc;
+    }
+    for (int i = 0; i < n; i++) b[order[i] * bstride] = z[i];
+}
+
+// ---- the compact form ---------------------------------------------------------------------------------------------------------
+// Minv [2c x 2c], row-major (every entry written)
+template <typename T>
+LBFGS_HD inline void compact_minv(int c, const T* SY, const T* SS, int ldg, T theta, T* Minv)
+{
+    const int w = 2 * c;
+    for (int i = 0; i < w * w; i++) Minv[i] = T(0);
+    for (int a = 0; a < c; a++)
+    {
+        Minv[a * w + a] = -SY[a * ldg + a];
+        for (int b = 0; b < c; b++)
+        {
+            if (a < b)  // age a < age b: pair a is the newer one
+            {
+                Minv[(c + a) * w + b] = SY[a * ldg + b];
+                Minv[b * w + c + a] = SY[a * ldg + b];
+            }
+            Minv[(c + a) * w + c + b] = theta * SS[a * ldg + b];
+        }
+    }
+}
+
+// B: C = -M u with u = [Y'v ; theta S'v] (M: the 2c x 2c inverse of Minv, row-major)
+template <typename T>
+LBFGS_HD inline void compact_b_coef(int c, const T* M, T theta, const T* wv, int ldw, T* C, int ldc)
+{
+    const int w = 2 * c;
+    for (int i = 0; i < w; i++)
+    {
+        T acc = T(0);
+        for (int j = 0; j < w; j++) acc += M[i * w + j] * (j < c ? wv[j * ldw] : theta * wv[j * ldw]);
+        C[i * ldc] = i < c ? -acc : -theta * acc;
+    }
+}
+
+// H: R(t, u) = s_t'y_u (t <= u, else 0) and Y'Y, both c x c in chronological order t = c - 1 - age
+template <typename T>
+LBFGS_HD inline void compact_h_setup(int c, const T* SY, const T* YY, int ldg, T* R, T* YYc)
+{
+    for (int t = 0; t < c; t++)
+        for (int u = 0; u < c; u++)
+        {
+            R[t * c + u] = t <= u ? SY[(c - 1 - t) * ldg + (c - 1 - u)] : T(0);
+            YYc[t * c + u] = YY[(c - 1 - t) * ldg + (c - 1 - u)];
+        }
+}
+
+// H: the coefficients of one vector.  w, us: c elements of scratch each (stride ldt)
+template <typename T>
+LBFGS_HD inline void compact_h_coef(int c, const T* R, const T* YYc, T theta, const T* wv, int ldw, T* w, T* us, int ldt, T* C, int ldc)
+{
+    auto p = [&](int t) { return wv[(c + c - 1 - t) * ldw]; };   // s_t'v
+    auto q = [&](int t) { return wv[(c - 1 - t) * ldw]; };       // y_t'v
+    for (int t = c - 1; t >= 0; t--)   // w = R^-1 S'v
+    {
+        T acc = p(t);
+        for (int s = t + 1; s < c; s++) acc -= R[t * c + s] * w[s * ldt];
+        w[t * ldt] = acc / R[t * c + t];
+    }
+    for (int t = 0; t < c; t++)        // u_s = R^-T ((D + Y'Y/theta) w - Y'v/theta)
+    {
+        T z = R[t * c + t] * w[t * ldt];
+        T yyw = T(0);
+        for (int s = 0; s < c; s++) yyw += YYc[t * c + s] * w[s * ldt];
+        z += (yyw - q(t)) / theta;
+        for (int s = 0; s < t; s++) z -= R[s * c + t] * us[s * ldt];
+        us[t * ldt] = z / R[t * c + t];
+    }
+    for (int t = 0; t < c; t++)
+    {
+        C[(c - 1 - t) * ldc] = -w[t * ldt] / theta;
+        C[(c + c - 1 - t) * ldc] = us[t * ldt];
+    }
+}
+
+}  // namespace LBFGSpp
+
+#endif  // LBFGSPP_B200_COMPACT_FORM_H

@@ -356,6 +356,40 @@ lbfgs_b200_status lbfgs_b200_small_minimize_f32(lbfgs_b200_ctx* ctx, int objecti
                                                 int64_t n, int64_t B, const lbfgs_b200_param* prm, int line_search,
                                                 float* X, int64_t ldx, float* G, lbfgs_b200_outcome* outs_host);
 
+/* The final quasi-Newton approximations of a small-batch solve, kept on the device (the small-batch counterpart of
+ * final_approx_hessian() / final_approx_inverse_hessian(), reference LBFGS.h:192-197, BFGSMat.h:150-271).  A history made for
+ * (n, m, precision, B) receives, from lbfgs_b200_small_minimize_keep_*, every problem's pairs, ys, theta and Gram blocks as BFGSMat
+ * holds them when minimize() returns (the last step's pair is not among them).  Device memory: B*(2m*n + m + 3m^2 + 2) elements
+ * plus B ints; fp64, B = 65536, n = 256, m = 10: about 2.8 GB.  LBFGS_B200_ERR_ALLOC when that cannot be had. */
+typedef struct lbfgs_b200_small_hist lbfgs_b200_small_hist;
+lbfgs_b200_status lbfgs_b200_small_hist_create(lbfgs_b200_ctx* ctx, int64_t n, int m, int elem_bytes, int64_t B, lbfgs_b200_small_hist** out);
+void lbfgs_b200_small_hist_destroy(lbfgs_b200_small_hist* h);
+/* device pointers to s / y of problem b at `age` (0 = newest; meaningful for age < its pair count), for tests; NULL out of range */
+const void* lbfgs_b200_small_hist_s_col(const lbfgs_b200_small_hist* h, int64_t b, int age);
+const void* lbfgs_b200_small_hist_y_col(const lbfgs_b200_small_hist* h, int64_t b, int age);
+
+#define LBFGS_B200_DECLARE_SMALL_HIST(T, SUF)                                                                                     \
+    /* lbfgs_b200_small_minimize_* that also fills `hist`, whose n, m, precision and B must match the solve's             \
+     * (LBFGS_B200_ERR_INVALID before anything is launched otherwise).  Everything else is the same launch.            */ \
+    lbfgs_b200_status lbfgs_b200_small_minimize_keep_##SUF(lbfgs_b200_ctx* ctx, int objective, const T* data0, const T* data1,   \
+                                                           int64_t ldd, int64_t n, int64_t B, const lbfgs_b200_param* prm,        \
+                                                           int line_search, T* X, int64_t ldx, T* G, lbfgs_b200_outcome* outs_host, \
+                                                           lbfgs_b200_small_hist* hist);                                        \
+    /* per problem: its pair count c (c_host[B]) and theta (theta_host[B]); either may be NULL.  Synchronises.            */ \
+    lbfgs_b200_status lbfgs_b200_small_hist_info_##SUF(lbfgs_b200_small_hist* h, int* c_host, T* theta_host);                    \
+    /* OUT_p = B_b V_p (inverse = 0) or H_b V_p (inverse != 0) for the problems b = b0 + p, p < count, in one launch: k >= 1   \
+     * vectors each, vector j of problem p at V + p*ldvp + j*ldv (ldvp = 0: one V for every problem), its product at          \
+     * OUT + p*ldop + j*ldo; ldv, ldo >= n.  The arithmetic of LBFGSSolver::final_approx_*_times: [Y S]'V summed in fp64, the   \
+     * coefficients of the compact form (include/LBFGSpp/CompactForm.h), OUT = a0 V + sum cy_a y_a + sum cs_a s_a in that order. \
+     * A problem's products depend on n only, not on b0, count or k.  OUT may be V only with the same layout (ldo == ldv,       \
+     * ldop == ldvp) and, for count > 1, vectors of its own per problem.  LBFGS_B200_ERR_INVALID for k < 1, ldv or ldo < n, a     \
+     * problem range outside [0, B), NULL pointers or a history no solve has filled.  Asynchronous.                          */ \
+    lbfgs_b200_status lbfgs_b200_small_hist_times_##SUF(lbfgs_b200_small_hist* h, int inverse, int64_t b0, int64_t count, int k, \
+                                                        const T* V, int64_t ldv, int64_t ldvp, T* OUT, int64_t ldo, int64_t ldop);
+
+LBFGS_B200_DECLARE_SMALL_HIST(double, f64)
+LBFGS_B200_DECLARE_SMALL_HIST(float, f32)
+
 #ifdef __cplusplus
 }
 #endif

@@ -159,6 +159,17 @@ def _declare(lib):
         lib.lbfgs_b200_small_max_n.argtypes = [ci, ci, ci]
         for suf in ("f64", "f32"):
             getattr(lib, "lbfgs_b200_small_minimize_" + suf).argtypes = [vp, ci, vp, vp, i64, i64, i64, vp, ci, vp, i64, vp, vp]
+    if hasattr(lib, "lbfgs_b200_small_hist_create"):
+        lib.lbfgs_b200_small_hist_create.argtypes = [vp, i64, ci, ci, i64, C.POINTER(vp)]
+        lib.lbfgs_b200_small_hist_destroy.argtypes = [vp]
+        lib.lbfgs_b200_small_hist_destroy.restype = None
+        for name in ("lbfgs_b200_small_hist_s_col", "lbfgs_b200_small_hist_y_col"):
+            getattr(lib, name).restype = vp
+            getattr(lib, name).argtypes = [vp, i64, ci]
+        for suf in ("f64", "f32"):
+            getattr(lib, "lbfgs_b200_small_minimize_keep_" + suf).argtypes = [vp, ci, vp, vp, i64, i64, i64, vp, ci, vp, i64, vp, vp, vp]
+            getattr(lib, "lbfgs_b200_small_hist_info_" + suf).argtypes = [vp, vp, vp]
+            getattr(lib, "lbfgs_b200_small_hist_times_" + suf).argtypes = [vp, ci, i64, i64, ci, vp, i64, i64, vp, i64, i64]
     lib._typed = True
     return lib
 
@@ -172,6 +183,19 @@ class _DrvParam(C.Structure):
 
 class _BatchItem(C.Structure):
     _fields_ = [("status", C.c_int), ("niter", C.c_int), ("nfev", C.c_long), ("fx", C.c_double), ("gnorm", C.c_double)]
+
+
+class _AbiParam(C.Structure):
+    """lbfgs_b200_param"""
+    _fields_ = [("m", C.c_int), ("epsilon", C.c_double), ("epsilon_rel", C.c_double), ("past", C.c_int), ("delta", C.c_double),
+                ("max_iterations", C.c_int), ("linesearch", C.c_int), ("max_linesearch", C.c_int), ("min_step", C.c_double),
+                ("max_step", C.c_double), ("ftol", C.c_double), ("wolfe", C.c_double)]
+
+
+class _Outcome(C.Structure):
+    """lbfgs_b200_outcome"""
+    _fields_ = [("status", C.c_int), ("niter", C.c_int), ("nfev", C.c_longlong), ("fx", C.c_double), ("gnorm", C.c_double),
+                ("rounds", C.c_longlong)]
 
 
 class _SmallItem(C.Structure):
@@ -243,6 +267,10 @@ def _declare_driver(lib):
         for suf, pt in (("f64", dp), ("f32", fp)):
             getattr(lib, "lbfgsb200_drv_small_batch_" + suf).argtypes = [ci, ci, cl, cl, pt, pt, pt, cl, ci, prm, pt, pt,
                                                                          C.POINTER(_SmallItem), err, errlen]
+    if hasattr(lib, "lbfgsb200_drv_small_batch_hessian_times_f64"):
+        for suf, pt in (("f64", dp), ("f32", fp)):
+            getattr(lib, "lbfgsb200_drv_small_batch_hessian_times_" + suf).argtypes = [ci, ci, cl, cl, pt, pt, pt, cl, ci, prm, pt, cl, ci, pt,
+                                                                                      pt, pt, pt, C.POINTER(_SmallItem), err, errlen]
     lib._drv_typed = True
     return lib
 
@@ -841,6 +869,92 @@ def solve_small_batch(objective, X0, param=None, linesearch="MoreThuente", dtype
     res = [dict(status=STATUS_NAMES[it.kind], code=it.code, niter=it.niter, nfev=it.nfev, fx=it.fx, gnorm=it.gnorm, rounds=it.rounds)
            for it in items]
     return res, X, G
+
+
+def small_batch_hessian_times(objective, X0, V, param=None, linesearch="MoreThuente", dtype=np.float64, data0=None, data1=None, ldd=0,
+                              device=0, lib=None):
+    """solve_small_batch with every problem's final approximation kept (LBFGSSmallBatchSolver::keep_final_approx), then its products
+    with the vectors V: shape (k, n), shared by all problems, or (B, k, n).  Returns (outcomes, X, B V, H V, H (B V)), the products
+    of shape (B, k, n)."""
+    drv = driver(lib)
+    X0 = np.ascontiguousarray(X0, dtype=dtype)
+    B, n = X0.shape
+    V = np.ascontiguousarray(V, dtype=dtype)
+    shared = V.ndim == 2
+    k = V.shape[-2]
+    if V.shape[-1] != n or (not shared and (V.ndim != 3 or V.shape[0] != B)):
+        raise ValueError("V must have shape (k, n) or (B, k, n)")
+    p = (param if param is not None else LBFGSParam())._c()
+    d0 = None if data0 is None else np.ascontiguousarray(data0, dtype=dtype).reshape(-1)
+    d1 = None if data1 is None else np.ascontiguousarray(data1, dtype=dtype).reshape(-1)
+    X = np.empty_like(X0)
+    BV, HV, HBV = (np.empty((B, k, n), dtype=dtype) for _ in range(3))
+    items = (_SmallItem * B)()
+    suf = "f32" if np.dtype(dtype) == np.float32 else "f64"
+    fn = getattr(drv, "lbfgsb200_drv_small_batch_hessian_times_" + suf)
+    err = C.create_string_buffer(256)
+    r = fn(device, objective, n, B, _ptr(X0), _ptr(d0), _ptr(d1), int(ldd), _ls_id(linesearch), C.byref(p), _ptr(V), k, int(shared), _ptr(X),
+           _ptr(BV), _ptr(HV), _ptr(HBV), items, err, len(err))
+    if r < 0:
+        raise (ValueError if r == -1 else RuntimeError)("small_batch_hessian_times failed: %s" % err.value.decode())
+    res = [dict(status=STATUS_NAMES[it.kind], code=it.code, niter=it.niter, nfev=it.nfev, fx=it.fx, gnorm=it.gnorm, rounds=it.rounds)
+           for it in items]
+    return res, X, BV, HV, HBV
+
+
+class SmallHistory:
+    """The kept final approximations of a small-batch solve (lbfgs_b200_small_hist) through the C ABI: create, minimize-keep, info,
+    columns and products."""
+
+    def __init__(self, ctx, n, m, B, dtype=np.float64):
+        self.ctx, self.n, self.m, self.B, self.dtype = ctx, n, m, B, np.dtype(dtype)
+        self.suf = "f64" if self.dtype == np.float64 else "f32"
+        self.ct = C.c_double if self.dtype == np.float64 else C.c_float
+        self.h = C.c_void_p()
+        ctx.check(ctx.lib.lbfgs_b200_small_hist_create(ctx.h, n, m, self.dtype.itemsize, B, C.byref(self.h)))
+
+    def __del__(self):
+        try:
+            if self.h and self.ctx.h:
+                self.ctx.lib.lbfgs_b200_small_hist_destroy(self.h)
+            self.h = None
+        except Exception:
+            pass
+
+    def minimize(self, objective, X, param, linesearch="MoreThuente", data0=None, data1=None, ldd=0, ldx=None, G=None, keep=True):
+        """lbfgs_b200_small_minimize_keep_* (keep=False: the plain lbfgs_b200_small_minimize_*) on DeviceArrays; returns the raw
+        outcomes (a ctypes array of lbfgs_b200_outcome)."""
+        outs = (_Outcome * self.B)()
+        p = _AbiParam(*(getattr(param, f) for f, _ in _AbiParam._fields_))
+        args = [self.ctx.h, objective, data0.ptr if data0 is not None else None, data1.ptr if data1 is not None else None, ldd, self.n, self.B,
+                C.byref(p), _ls_id(linesearch), X.ptr, self.n if ldx is None else ldx, G.ptr if G is not None else None, outs]
+        if keep:
+            self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_small_minimize_keep_" + self.suf)(*args, self.h))
+        else:
+            self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_small_minimize_" + self.suf)(*args))
+        return outs
+
+    def info(self):
+        """(c, theta): per-problem pair counts and theta, arrays of B."""
+        c = np.zeros(self.B, dtype=np.int32)
+        th = np.zeros(self.B, dtype=self.dtype)
+        self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_small_hist_info_" + self.suf)(self.h, c.ctypes.data_as(C.c_void_p),
+                                                                                        th.ctypes.data_as(C.c_void_p)))
+        return c, th
+
+    def column(self, which, b, age):
+        fn = self.ctx.lib.lbfgs_b200_small_hist_s_col if which == "s" else self.ctx.lib.lbfgs_b200_small_hist_y_col
+        p = fn(self.h, b, age)
+        if not p:
+            raise IndexError("no such column")
+        out = np.empty(self.n, dtype=self.dtype)
+        self.ctx.check(self.ctx.lib.lbfgs_b200_memcpy_d2h(self.ctx.h, out.ctypes.data_as(C.c_void_p), p, out.nbytes))
+        return out
+
+    def times(self, inverse, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop):
+        """lbfgs_b200_small_hist_times_* on DeviceArrays (asynchronous)."""
+        self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_small_hist_times_" + self.suf)(self.h, int(inverse), b0, count, k, V.ptr, ldv, ldvp,
+                                                                                         OUT.ptr, ldo, ldop))
 
 
 def phase_clock(on=True):

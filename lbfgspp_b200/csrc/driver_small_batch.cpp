@@ -5,8 +5,18 @@
 #include "../../include/LBFGSpp/DeviceObjectives.h"
 #include "driver_common.h"
 
+#include <algorithm>
+#include <cstdio>
+#include <type_traits>
+
 #pragma weak lbfgs_b200_small_minimize_f64
 #pragma weak lbfgs_b200_small_minimize_f32
+#pragma weak lbfgs_b200_small_minimize_keep_f64
+#pragma weak lbfgs_b200_small_minimize_keep_f32
+#pragma weak lbfgs_b200_small_hist_create
+#pragma weak lbfgs_b200_small_hist_destroy
+#pragma weak lbfgs_b200_small_hist_times_f64
+#pragma weak lbfgs_b200_small_hist_times_f32
 
 using namespace LBFGSpp;
 using namespace lbfgsb200_drv;
@@ -32,9 +42,11 @@ namespace {
 // B problems (rows of x0s_host, n each) minimised by LBFGSSmallBatchSolver; data0/data1 (optional, host) per problem at data + b*ldd
 // (ldd = 0: shared).  xs_out / gs_out (optional): solutions and final gradients.  Returns the number of problems that did not end
 // cleanly, -1 (err holds the message) when the call was refused as an invalid argument, -2 on any other failure.
-template <class Scalar>
+// `after(solver, dev)` (optional) runs on the solver once minimize() has returned; `keep`: minimize() keeps the final approximations
+template <class Scalar, class After = std::nullptr_t>
 int small_batch(int device_ordinal, int objective, long n, long B, const Scalar* x0s_host, const Scalar* data0_host, const Scalar* data1_host,
-                long ldd, int ls, const drv_param* q, Scalar* xs_out, Scalar* gs_out, drv_small_item* items, char* err, int errlen)
+                long ldd, int ls, const drv_param* q, Scalar* xs_out, Scalar* gs_out, drv_small_item* items, char* err, int errlen,
+                bool keep = false, After after = nullptr)
 {
     int invalid = 0;
     const int r = reported(err, errlen, -2, [&]() {
@@ -53,6 +65,7 @@ int small_batch(int device_ordinal, int objective, long n, long B, const Scalar*
             int bad = 0;
             with_line_search(ls, [&](auto tag) {
                 typename decltype(tag)::template SmallBatchSolver<Scalar> solver(prm);
+                solver.keep_final_approx(keep);
                 const std::vector<BatchOutcome<Scalar> > out = solver.minimize(obj, X, B, ldd);
                 for (long b = 0; b < B; b++)
                 {
@@ -65,6 +78,7 @@ int small_batch(int device_ordinal, int objective, long n, long B, const Scalar*
                 }
                 if (gs_out)
                     dev.check(lbfgs_b200_memcpy_d2h(dev.ctx(), gs_out, solver.final_grad(0), sizeof(Scalar) * size_t(n) * size_t(B)));
+                if constexpr (!std::is_same_v<After, std::nullptr_t>) after(solver, dev);
             });
             if (xs_out) X.copy_to_host(xs_out);
             return bad;
@@ -78,7 +92,58 @@ int small_batch(int device_ordinal, int objective, long n, long B, const Scalar*
     return (r == -2 && invalid) ? -1 : r;
 }
 
+// small_batch with the final approximations kept, then B_b V_b, H_b V_b and H_b (B_b V_b) for every problem b.  V_host: k vectors
+// of n shared by all problems (shared != 0) or B*k of them, problem b's at [(b*k + j)*n, ...); BV/HV/HBV: B*k*n each.
+template <class Scalar>
+int small_batch_hessian_times(int device_ordinal, int objective, long n, long B, const Scalar* x0s_host, const Scalar* data0_host,
+                              const Scalar* data1_host, long ldd, int ls, const drv_param* q, const Scalar* V_host, long k, int shared,
+                              Scalar* xs_out, Scalar* BV, Scalar* HV, Scalar* HBV, drv_small_item* items, char* err, int errlen)
+{
+    if (!lbfgs_b200_small_hist_create || !lbfgs_b200_small_hist_destroy ||
+        (sizeof(Scalar) == 8 ? !lbfgs_b200_small_minimize_keep_f64 || !lbfgs_b200_small_hist_times_f64
+                             : !lbfgs_b200_small_minimize_keep_f32 || !lbfgs_b200_small_hist_times_f32))
+    {
+        std::snprintf(err, size_t(errlen), "the C ABI library in use has no kept small-batch approximations (lbfgs_b200_small_minimize_keep_*, "
+                                           "lbfgs_b200_small_hist_*)");
+        return -2;
+    }
+    return small_batch<Scalar>(device_ordinal, objective, n, B, x0s_host, data0_host, data1_host, ldd, ls, q, xs_out, nullptr, items, err, errlen,
+                               true, [&](auto& solver, Device& dev) {
+        const size_t total = size_t(B) * size_t(k) * size_t(n);
+        std::vector<Scalar> v(total);
+        for (long b = 0; b < B; b++)
+            std::copy(V_host + (shared ? 0 : size_t(b) * size_t(k) * size_t(n)), V_host + (shared ? 0 : size_t(b) * size_t(k) * size_t(n)) + size_t(k) * size_t(n),
+                      v.begin() + std::ptrdiff_t(size_t(b) * size_t(k) * size_t(n)));
+        DeviceVector<Scalar> Vd(dev), Bd(dev), Hd(dev), HBd(dev);
+        Vd.copy_from_host(v.data(), std::ptrdiff_t(total));
+        solver.final_approx_hessian_times(Vd, Bd);
+        solver.final_approx_inverse_hessian_times(Vd, Hd);
+        solver.final_approx_inverse_hessian_times(Bd, HBd);
+        Bd.copy_to_host(BV);
+        Hd.copy_to_host(HV);
+        HBd.copy_to_host(HBV);
+    });
+}
+
 }  // namespace
+
+extern "C" int lbfgsb200_drv_small_batch_hessian_times_f64(int device_ordinal, int objective, long n, long B, const double* x0s_host,
+                                                           const double* data0_host, const double* data1_host, long ldd, int ls, const drv_param* q,
+                                                           const double* V_host, long k, int shared, double* xs_out, double* BV, double* HV,
+                                                           double* HBV, drv_small_item* items, char* err, int errlen)
+{
+    return small_batch_hessian_times<double>(device_ordinal, objective, n, B, x0s_host, data0_host, data1_host, ldd, ls, q, V_host, k, shared, xs_out,
+                                             BV, HV, HBV, items, err, errlen);
+}
+
+extern "C" int lbfgsb200_drv_small_batch_hessian_times_f32(int device_ordinal, int objective, long n, long B, const float* x0s_host,
+                                                           const float* data0_host, const float* data1_host, long ldd, int ls, const drv_param* q,
+                                                           const float* V_host, long k, int shared, float* xs_out, float* BV, float* HV,
+                                                           float* HBV, drv_small_item* items, char* err, int errlen)
+{
+    return small_batch_hessian_times<float>(device_ordinal, objective, n, B, x0s_host, data0_host, data1_host, ldd, ls, q, V_host, k, shared, xs_out,
+                                            BV, HV, HBV, items, err, errlen);
+}
 
 extern "C" int lbfgsb200_drv_small_batch_f64(int device_ordinal, int objective, long n, long B, const double* x0s_host, const double* data0_host,
                                              const double* data1_host, long ldd, int ls, const drv_param* q, double* xs_out, double* gs_out,

@@ -3,6 +3,17 @@
 #include "two_loop_gram.cuh"
 #include "small_batch.cuh"
 
+// the kept final histories of a small-batch solve (SmallHistLayout per problem) and their pair counts
+struct lbfgs_b200_small_hist
+{
+    lbfgs_b200_ctx* ctx = nullptr;
+    int64_t n = 0, B = 0;
+    int m = 0, elem = 8;
+    void* data = nullptr;
+    int* counts = nullptr;
+    bool filled = false;   // a solve has written every problem's record
+};
+
 namespace {
 
 // what a built-in objective adds to the vectors of a problem: x_lo/g_lo when its trials are stored, and its data vectors
@@ -20,7 +31,8 @@ bool small_objective_shape(int objective, bool& stored, int& data_vectors)
 
 template <class T>
 lbfgs_b200_status small_minimize(lbfgs_b200_ctx* ctx, int objective, const T* data0, const T* data1, int64_t ldd, int64_t n, int64_t B,
-                                 const lbfgs_b200_param* prm, int ls_kind, T* X, int64_t ldx, T* G, lbfgs_b200_outcome* outs_host)
+                                 const lbfgs_b200_param* prm, int ls_kind, T* X, int64_t ldx, T* G, lbfgs_b200_outcome* outs_host,
+                                 lbfgs_b200_small_hist* keep = nullptr)
 {
     using namespace lb;
     if (!ctx) return LBFGS_B200_ERR_INVALID;
@@ -46,6 +58,11 @@ lbfgs_b200_status small_minimize(lbfgs_b200_ctx* ctx, int objective, const T* da
             return objective_geometry<OBJ>(ctx, n, data0, data1, geo);
         }))
         return st;
+    if (keep)
+        REQUIRE(ctx, keep->ctx == ctx && keep->n == n && keep->m == prm->m && keep->elem == (int)sizeof(T) && keep->B == B,
+                "small_minimize_keep: the history was made (on this context?) for n = %lld, m = %d, %s, B = %lld; the solve has n = %lld, m = %d, %s, B = %lld",
+                (long long)keep->n, keep->m, keep->elem == 8 ? "fp64" : "fp32", (long long)keep->B, (long long)n, prm->m,
+                sizeof(T) == 8 ? "fp64" : "fp32", (long long)B);
     const int64_t max_n = lbfgs_b200_small_max_n(prm->m, (int)sizeof(T), objective);
     REQUIRE(ctx, n <= max_n, "small_minimize: n = %lld exceeds %lld, the largest n whose solve fits one CTA's shared memory for m = %d and this "
             "objective in %s; solve larger problems with LBFGSBatchSolver", (long long)n, (long long)max_n, prm->m, sizeof(T) == 8 ? "fp64" : "fp32");
@@ -66,6 +83,12 @@ lbfgs_b200_status small_minimize(lbfgs_b200_ctx* ctx, int objective, const T* da
     a.data0 = data0; a.data1 = data1; a.ldd = ldd;
     a.X = X; a.ldx = ldx; a.G = G;
     a.outs = static_cast<lbfgs_b200_outcome*>(buf);
+    if (keep)
+    {
+        keep->filled = false;
+        a.hist = static_cast<T*>(keep->data);
+        a.hist_c = keep->counts;
+    }
     auto run = [&]() -> cudaError_t {
         cudaError_t e = cudaMemcpyAsync((void*)a.proto, &proto, sizeof(PState<T>), cudaMemcpyHostToDevice, ctx->stream);
         if (e == cudaSuccess) e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)a.L.total);
@@ -79,6 +102,57 @@ lbfgs_b200_status small_minimize(lbfgs_b200_ctx* ctx, int objective, const T* da
     const cudaError_t e = run();
     pool_free(ctx, buf);
     CU(ctx, e);
+    if (keep) keep->filled = true;
+    return LBFGS_B200_OK;
+}
+
+template <class T> lbfgs_b200_status small_hist_check(lbfgs_b200_small_hist* h, const char* what)
+{
+    if (!h) return LBFGS_B200_ERR_INVALID;
+    REQUIRE(h->ctx, h->elem == (int)sizeof(T), "%s: the history holds %s values", what, h->elem == 8 ? "fp64" : "fp32");
+    REQUIRE(h->ctx, h->filled, "%s: no solve has filled the history", what);
+    return LBFGS_B200_OK;
+}
+
+template <class T> lbfgs_b200_status small_hist_info(lbfgs_b200_small_hist* h, int* c_host, T* theta_host)
+{
+    if (auto st = small_hist_check<T>(h, "small_hist_info")) return st;
+    lbfgs_b200_ctx* ctx = h->ctx;
+    const lb::SmallHistLayout HL{h->n, h->m};
+    if (c_host) CU(ctx, cudaMemcpyAsync(c_host, h->counts, sizeof(int) * (size_t)h->B, cudaMemcpyDeviceToHost, ctx->stream));
+    if (theta_host)
+        CU(ctx, cudaMemcpy2DAsync(theta_host, sizeof(T), static_cast<const T*>(h->data) + HL.theta(), sizeof(T) * (size_t)HL.rec(), sizeof(T),
+                                  (size_t)h->B, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(ctx, cudaStreamSynchronize(ctx->stream));
+    return LBFGS_B200_OK;
+}
+
+template <class T>
+lbfgs_b200_status small_hist_times(lbfgs_b200_small_hist* h, int inverse, int64_t b0, int64_t count, int k, const T* V, int64_t ldv, int64_t ldvp,
+                                   T* OUT, int64_t ldo, int64_t ldop)
+{
+    using namespace lb;
+    if (auto st = small_hist_check<T>(h, "small_hist_times")) return st;
+    lbfgs_b200_ctx* ctx = h->ctx;
+    const int64_t n = h->n;
+    REQUIRE(ctx, V && OUT, "small_hist_times: NULL argument");
+    REQUIRE(ctx, k >= 1 && (k + kSGroup - 1) / kSGroup <= 65535, "small_hist_times: k must be in 1..%d (got %d)", 65535 * kSGroup, k);
+    REQUIRE(ctx, b0 >= 0 && count >= 1 && count <= h->B - b0, "small_hist_times: problems [%lld, %lld) are not within the %lld of the history",
+            (long long)b0, (long long)(b0 + count), (long long)h->B);
+    REQUIRE(ctx, ldv >= n && ldo >= n, "small_hist_times: leading dimensions ldv = %lld, ldo = %lld must be at least n = %lld", (long long)ldv,
+            (long long)ldo, (long long)n);
+    REQUIRE(ctx, ldvp >= 0 && ldop >= 0, "small_hist_times: negative problem stride");
+    REQUIRE(ctx, (const void*)V != (const void*)OUT || (ldo == ldv && ldop == ldvp && (ldvp > 0 || count == 1)),
+            "small_hist_times: OUT may be V only with the same layout (ldo == ldv, ldop == ldvp) and vectors of its own per problem");
+    SmallTimesArgs<T> a{};
+    a.hist = static_cast<const T*>(h->data); a.hist_c = h->counts; a.HL = SmallHistLayout{n, h->m};
+    a.b0 = b0; a.k = k; a.inverse = inverse ? 1 : 0;
+    a.V = V; a.ldv = ldv; a.ldvp = ldvp; a.OUT = OUT; a.ldo = ldo; a.ldop = ldop;
+    const size_t smem = small_times_smem(h->m, (int)sizeof(T));
+    CU(ctx, cudaFuncSetAttribute(k_small_hist_times<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_small_hist_times<T><<<dim3((unsigned)count, (unsigned)((k + kSGroup - 1) / kSGroup)), small_threads(n), smem, ctx->stream>>>(a);
+    CU(ctx, cudaGetLastError());
+    ctx->launches++;
     return LBFGS_B200_OK;
 }
 
@@ -96,6 +170,64 @@ int64_t lbfgs_b200_small_max_n(int m, int elem_bytes, int objective)
     const int64_t per_coord = (int64_t)elem_bytes * L.nvec;               // every vector holds round_up(n, 4) elements
     return (((int64_t)(lb::kSSmemLimit - L.vecs) / per_coord) / 4) * 4;
 }
+
+lbfgs_b200_status lbfgs_b200_small_hist_create(lbfgs_b200_ctx* ctx, int64_t n, int m, int elem_bytes, int64_t B, lbfgs_b200_small_hist** out)
+{
+    if (!ctx) return LBFGS_B200_ERR_INVALID;
+    REQUIRE(ctx, out, "small_hist_create: NULL argument");
+    *out = nullptr;
+    REQUIRE(ctx, n >= 1 && m >= 1 && m <= lb::kMaxM && (elem_bytes == 8 || elem_bytes == 4) && B >= 1 && B <= 0x7fffffff,
+            "small_hist_create: need n >= 1, 1 <= m <= %d, elem_bytes 8 or 4 and 1 <= B <= 2^31 - 1", lb::kMaxM);
+    REQUIRE(ctx, lb::small_times_smem(m, elem_bytes) <= lb::kSSmemLimit, "small_hist_create: m = %d is too large for the products", m);
+    auto* h = new lbfgs_b200_small_hist();
+    h->ctx = ctx; h->n = n; h->m = m; h->elem = elem_bytes; h->B = B;
+    const lb::SmallHistLayout HL{n, m};
+    cudaError_t e = pool_alloc(ctx, &h->data, (size_t)elem_bytes * (size_t)HL.rec() * (size_t)B);
+    if (e == cudaSuccess) e = pool_alloc(ctx, reinterpret_cast<void**>(&h->counts), sizeof(int) * (size_t)B);
+    if (e != cudaSuccess)
+    {
+        lbfgs_b200_small_hist_destroy(h);
+        cudaGetLastError();
+        return fail(ctx, e == cudaErrorMemoryAllocation ? LBFGS_B200_ERR_ALLOC : LBFGS_B200_ERR_CUDA, "small_hist_create: %s", cudaGetErrorString(e));
+    }
+    *out = h;
+    return LBFGS_B200_OK;
+}
+
+void lbfgs_b200_small_hist_destroy(lbfgs_b200_small_hist* h)
+{
+    if (!h) return;
+    pool_free(h->ctx, h->data);
+    pool_free(h->ctx, h->counts);
+    delete h;
+}
+
+static const void* small_hist_col(const lbfgs_b200_small_hist* h, int64_t b, int age, bool y)
+{
+    if (!h || b < 0 || b >= h->B || age < 0 || age >= h->m) return nullptr;
+    const lb::SmallHistLayout HL{h->n, h->m};
+    return static_cast<const char*>(h->data) + (size_t)h->elem * (size_t)(b * HL.rec() + (y ? HL.y(age) : HL.s(age)));
+}
+const void* lbfgs_b200_small_hist_s_col(const lbfgs_b200_small_hist* h, int64_t b, int age) { return small_hist_col(h, b, age, false); }
+const void* lbfgs_b200_small_hist_y_col(const lbfgs_b200_small_hist* h, int64_t b, int age) { return small_hist_col(h, b, age, true); }
+
+#define LBFGS_B200_SMALL_KEEP(T, SUF)                                                                                              \
+    lbfgs_b200_status lbfgs_b200_small_minimize_keep_##SUF(lbfgs_b200_ctx* ctx, int objective, const T* data0, const T* data1,     \
+                                                           int64_t ldd, int64_t n, int64_t B, const lbfgs_b200_param* prm,          \
+                                                           int line_search, T* X, int64_t ldx, T* G, lbfgs_b200_outcome* outs_host, \
+                                                           lbfgs_b200_small_hist* hist)                                           \
+    {                                                                                                                              \
+        if (ctx) REQUIRE(ctx, hist, "small_minimize_keep: NULL history");                                                           \
+        return small_minimize<T>(ctx, objective, data0, data1, ldd, n, B, prm, line_search, X, ldx, G, outs_host, hist);          \
+    }                                                                                                                              \
+    lbfgs_b200_status lbfgs_b200_small_hist_info_##SUF(lbfgs_b200_small_hist* h, int* c_host, T* theta_host)                       \
+    { return small_hist_info<T>(h, c_host, theta_host); }                                                                         \
+    lbfgs_b200_status lbfgs_b200_small_hist_times_##SUF(lbfgs_b200_small_hist* h, int inverse, int64_t b0, int64_t count, int k,   \
+                                                        const T* V, int64_t ldv, int64_t ldvp, T* OUT, int64_t ldo, int64_t ldop)  \
+    { return small_hist_times<T>(h, inverse, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop); }
+
+LBFGS_B200_SMALL_KEEP(double, f64)
+LBFGS_B200_SMALL_KEEP(float, f32)
 
 lbfgs_b200_status lbfgs_b200_small_minimize_f64(lbfgs_b200_ctx* ctx, int objective, const double* data0, const double* data1, int64_t ldd,
                                                 int64_t n, int64_t B, const lbfgs_b200_param* prm, int line_search, double* X, int64_t ldx,

@@ -29,6 +29,7 @@
 //     (x_lo g_lo), (data0 data1) ]          with M = m + 1 ring slots and p = round_up(max(6m, 8), 8)
 #pragma once
 
+#include "../../include/LBFGSpp/CompactForm.h"
 #include "problem_machine.cuh"
 
 namespace lb {
@@ -65,6 +66,23 @@ inline SmallLayout small_layout(int64_t n, int m, int elem, bool stored, int dat
     return L;
 }
 
+// The final history of one problem as kept for the products (lbfgs_b200_small_hist): c = its pair count <= m, every block by age
+// (0 = newest pair), T elements from the problem's record start: s_a at a*n, y_a at (m + a)*n, ys_a, the c x c Gram blocks S'Y, Y'Y,
+// S'S (row-major, leading dimension c), theta.  rec = 2m*n + m + 3m^2 + 2 elements per problem.
+struct SmallHistLayout
+{
+    int64_t n;
+    int m;
+    __host__ __device__ int64_t s(int age) const { return age * n; }
+    __host__ __device__ int64_t y(int age) const { return (m + age) * n; }
+    __host__ __device__ int64_t ys() const { return 2 * m * n; }
+    __host__ __device__ int64_t SY() const { return ys() + m; }
+    __host__ __device__ int64_t YY() const { return SY() + (int64_t)m * m; }
+    __host__ __device__ int64_t SS() const { return YY() + (int64_t)m * m; }
+    __host__ __device__ int64_t theta() const { return SS() + (int64_t)m * m; }
+    __host__ __device__ int64_t rec() const { return theta() + 2; }
+};
+
 template <class T> struct SmallArgs
 {
     const PState<T>* proto;     // options and initial ring / op (init_problem_state), the same for every problem (device memory)
@@ -77,6 +95,8 @@ template <class T> struct SmallArgs
     int64_t ldx;
     T* G;                       // optional: final gradients, same layout as X
     lbfgs_b200_outcome* outs;   // [B]
+    T* hist;                    // optional: the final history of problem b at hist + b*SmallHistLayout::rec (see there)
+    int* hist_c;                // [B] with hist: its pair count
 };
 
 // block sums of NV per-thread values -> raw[0..NV): a fixed shuffle tree per warp, warp totals in warp order.  All threads call.
@@ -95,6 +115,34 @@ template <int NV> __device__ __forceinline__ void small_sums(const double (&v)[N
         double t = 0.0;
         for (int w = 0; w < nw; w++) t += red[w * ps + threadIdx.x];
         raw[threadIdx.x] = t;
+    }
+}
+
+// the export after the solve, out of line so that it leaves the solve loop's register allocation alone
+template <class T>
+__device__ __noinline__ void small_export_history(const PState<T>* st, const T* ring, int64_t ld, T* rec, int* c_out, int64_t n)
+{
+    const int tid = threadIdx.x, nt = blockDim.x, M = st->M;
+    const SmallHistLayout HL{n, M - 1};
+    const int c = st->ncorr, head = st->head, cur = st->gram_cur;
+    for (int age = 0; age < c; age++)
+    {
+        const T* sj = ring + 2 * (int64_t)slot_by_age(head, M, age) * ld;
+        const T* yj = sj + ld;
+        for (int64_t i = tid; i < n; i += nt) { rec[HL.s(age) + i] = sj[i]; rec[HL.y(age) + i] = yj[i]; }
+    }
+    for (int idx = tid; idx < c * c; idx += nt)
+    {
+        const int pi = slot_by_age(head, M, idx / c), pj = slot_by_age(head, M, idx % c);
+        rec[HL.SY() + idx] = st->SY[cur][pi * M + pj];
+        rec[HL.YY() + idx] = st->YY[cur][pi * M + pj];
+        rec[HL.SS() + idx] = st->SS[cur][pi * M + pj];
+    }
+    for (int age = tid; age < c; age += nt) rec[HL.ys() + age] = st->ys[slot_by_age(head, M, age)];
+    if (tid == 0)
+    {
+        rec[HL.theta()] = *st->theta;
+        *c_out = c;
     }
 }
 
@@ -395,6 +443,15 @@ __global__ void __launch_bounds__(kSMaxThreads) k_small_batch(const SmallArgs<T>
         if (tid == 0) advance_problem<T, STORED>(st, raw);
     }
 
+    // ---- the final history (optional): what BFGSMat holds when minimize() returns.  A solve stops only in after_search (before the
+    // pair-forming dots of that iteration, so the last step's pair never enters: reference LBFGS.h:137-162), in digest_trial (a
+    // line-search error) or in begin_search (a search that refuses to start); all three run when no pair is pending.  The
+    // combination pass of the iteration that accepted the newest pair folded its Gram rows and columns into SY/YY/SS[1 - gram_cur]
+    // and advance_problem flipped gram_cur and cleared `pending` in the same step, and a rejected pair (DOTS_PLAIN) touches neither
+    // the ring nor the Gram blocks.  So at every exit -- max_iterations, past/delta, a line-search error, convergence at x0 with
+    // ncorr = 0 -- SY/YY/SS[gram_cur] hold exactly the dots of the ncorr pairs that head, ys and theta describe.
+    if (a.hist) small_export_history(st, s_col(0), ld, a.hist + b * SmallHistLayout{n, M - 1}.rec(), a.hist_c + b, n);
+
     // ---- results: the point (and gradient) the problem stopped at, and its outcome ----
     {
         T* const xo = a.X + b * a.ldx;
@@ -413,6 +470,138 @@ __global__ void __launch_bounds__(kSMaxThreads) k_small_batch(const SmallArgs<T>
             o.fx = (double)st->rec.fx; o.gnorm = (double)st->gnorm; o.rounds = st->rounds;
             a.outs[b] = o;
         }
+    }
+}
+
+
+// ---- products with the kept approximations: OUT_p = B_b V_p or H_b V_p for problems b = b0 + p --------------------------------
+// One CTA per (problem, group of up to kSGroup vectors), small_threads(n) threads: the dots [Y S]'V (per thread in fp64 over the
+// coordinates i = tid, tid + nt, ..., then small_sums), the coefficients of CompactForm.h (B: Minv factorised by thread 0, the 2c
+// columns of M = Minv^-1 solved by 2c threads; H: R and Y'Y set up once; one thread per vector for its coefficients), and
+// OUT = a0 V + sum_a cy_a y_a + sum_a cs_a s_a (terms in that order).  Every sum's order depends on n only, so a problem's products
+// do not depend on b0, count or its position, and column j of a call equals a one-vector call on that column.
+constexpr int kSGroup = 16;
+
+template <class T> struct SmallTimesArgs
+{
+    const T* hist;              // records of SmallHistLayout
+    const int* hist_c;
+    SmallHistLayout HL;
+    int64_t b0;
+    int k, inverse;
+    const T* V;                 // problem p's vector j at V + p*ldvp + j*ldv
+    int64_t ldv, ldvp;
+    T* OUT;                     // at OUT + p*ldop + j*ldo
+    int64_t ldo, ldop;
+};
+
+// dynamic shared memory of k_small_hist_times (bytes): block sums, [Y S]'V and the coefficients (2m x kSGroup each), and the
+// algebra: B needs Minv's factor and M (2m x 2m each), H needs R, Y'Y (m x m each) and two scratch rows per vector
+inline size_t small_times_smem(int m, int elem)
+{
+    const size_t w = 2 * (size_t)m;
+    const size_t alg_b = 2 * w * w, alg_h = 2 * (size_t)m * m + 2 * (size_t)m * kSGroup;
+    return sizeof(double) * (size_t)kSMaxWarps * kSGroup + (size_t)elem * (2 * w * kSGroup + (alg_b > alg_h ? alg_b : alg_h));
+}
+
+template <class T>
+__global__ void __launch_bounds__(kSMaxThreads) k_small_hist_times(const SmallTimesArgs<T> a)
+{
+    extern __shared__ __align__(16) unsigned char s_smem[];
+    __shared__ int s_order[2 * kMaxM];
+    __shared__ unsigned char s_tag[2 * kMaxM];
+    const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5;
+    const int64_t p = blockIdx.x, b = a.b0 + p, n = a.HL.n;
+    const int m = a.HL.m, j0 = blockIdx.y * kSGroup, kk = min(kSGroup, a.k - j0);
+    const T* rec = a.hist + b * a.HL.rec();
+    const T* V = a.V + p * a.ldvp + j0 * a.ldv;
+    T* OUT = a.OUT + p * a.ldop + j0 * a.ldo;
+    const int c = a.hist_c[b];
+    const T theta = rec[a.HL.theta()];
+    const T a0 = a.inverse ? T(1) / theta : theta;
+    double* red = reinterpret_cast<double*>(s_smem);
+    T* wv = reinterpret_cast<T*>(red + kSMaxWarps * kSGroup);        // [2c][kSGroup]
+    T* C = wv + 2 * m * kSGroup;                                     // [2c][kSGroup]
+    T* alg = C + 2 * m * kSGroup;
+    if (c > 0)
+    {
+        // [Y S]'V, one history row at a time
+        for (int r = 0; r < 2 * c; r++)
+        {
+            const T* h = rec + (r < c ? a.HL.y(r) : a.HL.s(r - c));
+            double acc[kSGroup];
+#pragma unroll
+            for (int j = 0; j < kSGroup; j++) acc[j] = 0.0;
+            for (int64_t i = tid; i < n; i += nt)
+            {
+                const double hv = (double)h[i];
+#pragma unroll
+                for (int j = 0; j < kSGroup; j++)
+                    if (j < kk) acc[j] += hv * (double)V[j * a.ldv + i];
+            }
+            // block sums as small_sums takes them: a fixed shuffle tree per warp, warp totals in warp order
+#pragma unroll
+            for (int j = 0; j < kSGroup; j++)
+            {
+                const double w = warp_sum(acc[j]);
+                if (lane == 0) red[warp * kSGroup + j] = w;
+            }
+            __syncthreads();
+            if (tid < kk)
+            {
+                double t = 0.0;
+                for (int w = 0; w < (nt >> 5); w++) t += red[w * kSGroup + tid];
+                wv[r * kSGroup + tid] = (T)t;
+            }
+            __syncthreads();
+        }
+        const T* SY = rec + a.HL.SY();
+        if (!a.inverse)
+        {
+            const int w = 2 * c;
+            T* F = alg;            // Minv, factorised in place
+            T* Mm = alg + w * w;   // M = Minv^-1
+            if (tid == 0)
+            {
+                LBFGSpp::compact_minv(c, SY, rec + a.HL.SS(), c, theta, F);
+                LBFGSpp::bk_factor(F, w, s_order, s_tag);
+            }
+            __syncthreads();
+            for (int j = tid; j < w; j += nt)   // column j of M: Minv^-1 e_j
+            {
+                T z[2 * kMaxM];
+                for (int i = 0; i < w; i++) Mm[i * w + j] = i == j ? T(1) : T(0);
+                LBFGSpp::bk_solve(F, w, s_order, s_tag, Mm + j, w, z);
+            }
+            __syncthreads();
+            if (tid < kk) LBFGSpp::compact_b_coef(c, Mm, theta, wv + tid, kSGroup, C + tid, kSGroup);
+        }
+        else
+        {
+            T* R = alg;
+            T* YYc = R + c * c;
+            T* scr = YYc + c * c;   // per vector: w, us (c each), column tid
+            if (tid == 0) LBFGSpp::compact_h_setup(c, SY, rec + a.HL.YY(), c, R, YYc);
+            __syncthreads();
+            if (tid < kk) LBFGSpp::compact_h_coef(c, R, YYc, theta, wv + tid, kSGroup, scr + tid, scr + c * kSGroup + tid, kSGroup, C + tid, kSGroup);
+        }
+        __syncthreads();
+    }
+    // OUT = a0 V + sum_a cy_a y_a + sum_a cs_a s_a
+    for (int64_t i = tid; i < n; i += nt)
+    {
+        T r[kSGroup];
+#pragma unroll
+        for (int j = 0; j < kSGroup; j++) r[j] = j < kk ? a0 * V[j * a.ldv + i] : T(0);
+        for (int row = 0; row < 2 * c; row++)
+        {
+            const T hv = rec[(row < c ? a.HL.y(row) : a.HL.s(row - c)) + i];
+#pragma unroll
+            for (int j = 0; j < kSGroup; j++) r[j] += C[row * kSGroup + j] * hv;
+        }
+#pragma unroll
+        for (int j = 0; j < kSGroup; j++)
+            if (j < kk) OUT[j * a.ldo + i] = r[j];
     }
 }
 
