@@ -303,8 +303,20 @@ public:
     // before the first one, std::invalid_argument when V.size() is not a positive multiple of n.
     void final_approx_hessian_times(const Vector& V, Vector& OUT) { approx_times(V, OUT, false); }
     void final_approx_inverse_hessian_times(const Vector& V, Vector& OUT) { approx_times(V, OUT, true); }
+    // Their diagonals at any n (standard errors sqrt(diag H), a Jacobi preconditioner diag B): out (resized to n) from one pass over
+    // the history, no products (BFGSMat::hessian_diagonal).  Valid after minimize() in either loop; std::logic_error before the first.
+    void final_approx_hessian_diagonal(Vector& out) { approx_diagonal(out, false); }
+    void final_approx_inverse_hessian_diagonal(Vector& out) { approx_diagonal(out, true); }
 
 private:
+    void approx_diagonal(Vector& out, bool inverse)
+    {
+        sync_history();
+        m_bfgs.require_history();
+        if (inverse) m_bfgs.inverse_hessian_diagonal(out);
+        else m_bfgs.hessian_diagonal(out);
+    }
+
     void approx_times(const Vector& V, Vector& OUT, bool inverse)
     {
         sync_history();

@@ -105,8 +105,24 @@ public:
     // or H_b V, V holding k = V.size()/n vectors back to back.  The products are those of the same problem solved alone.
     void final_approx_hessian_times(int b, const Vector& V, Vector& OUT) { approx_times(b, V, OUT, false); }
     void final_approx_inverse_hessian_times(int b, const Vector& V, Vector& OUT) { approx_times(b, V, OUT, true); }
+    // LBFGSSolver::final_approx_hessian_diagonal / final_approx_inverse_hessian_diagonal for problem b: bit-identical to the same
+    // problem's diagonal solved alone.
+    void final_approx_hessian_diagonal(int b, Vector& out) { approx_diagonal(b, out, false); }
+    void final_approx_inverse_hessian_diagonal(int b, Vector& out) { approx_diagonal(b, out, true); }
 
 private:
+    void approx_diagonal(int b, Vector& out, bool inverse)
+    {
+        if (!m_solver) throw std::logic_error("LBFGSBatchSolver: no history yet (minimize() has not run)");
+        if (b < 0 || b >= m_B) throw std::invalid_argument("LBFGSBatchSolver: problem index out of range");
+        lbfgs_b200_hist* h = lbfgs_b200_solver_history_of(m_solver, b);   // column-major copy of problem b's ring
+        if (!h) m_dev->check(LBFGS_B200_ERR_CUDA);
+        BFGSMat<Scalar> mat;
+        mat.borrow(*m_dev, h, m_n, m_m);
+        if (inverse) mat.inverse_hessian_diagonal(out);
+        else mat.hessian_diagonal(out);
+    }
+
     void approx_times(int b, const Vector& V, Vector& OUT, bool inverse)
     {
         if (!m_solver) throw std::logic_error("LBFGSBatchSolver: no history yet (minimize() has not run)");

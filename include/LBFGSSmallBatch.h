@@ -31,6 +31,8 @@ template <> struct small_batch_abi<double>
     static lbfgs_b200_status times(lbfgs_b200_small_hist* h, int inv, int64_t b0, int64_t count, int k, const double* V, int64_t ldv,
                                    int64_t ldvp, double* OUT, int64_t ldo, int64_t ldop)
     { return lbfgs_b200_small_hist_times_f64(h, inv, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop); }
+    static lbfgs_b200_status diag(lbfgs_b200_small_hist* h, int inv, int64_t b0, int64_t count, double* OUT, int64_t ldo)
+    { return lbfgs_b200_small_hist_diag_f64(h, inv, b0, count, OUT, ldo); }
 };
 template <> struct small_batch_abi<float>
 {
@@ -44,6 +46,8 @@ template <> struct small_batch_abi<float>
     static lbfgs_b200_status times(lbfgs_b200_small_hist* h, int inv, int64_t b0, int64_t count, int k, const float* V, int64_t ldv,
                                    int64_t ldvp, float* OUT, int64_t ldo, int64_t ldop)
     { return lbfgs_b200_small_hist_times_f32(h, inv, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop); }
+    static lbfgs_b200_status diag(lbfgs_b200_small_hist* h, int inv, int64_t b0, int64_t count, float* OUT, int64_t ldo)
+    { return lbfgs_b200_small_hist_diag_f32(h, inv, b0, count, OUT, ldo); }
 };
 }  // namespace detail
 
@@ -140,6 +144,12 @@ public:
     // as the products with the columns of I.
     SmallMatrix<Scalar> final_approx_hessian(long b) { return dense(b, false); }
     SmallMatrix<Scalar> final_approx_inverse_hessian(long b) { return dense(b, true); }
+    // Their diagonals, formed on the device with no products (lbfgs_b200_small_hist_diag): every problem in one launch, OUT resized
+    // to B*n with problem b's at [b*n, (b + 1)*n), or problem b alone, OUT resized to n.  A problem's diagonal is the same either way.
+    void final_approx_hessian_diagonal(Vector& OUT) { diagonal(0, m_B, OUT, false); }
+    void final_approx_inverse_hessian_diagonal(Vector& OUT) { diagonal(0, m_B, OUT, true); }
+    void final_approx_hessian_diagonal(long b, Vector& OUT) { one_diagonal(b, OUT, false); }
+    void final_approx_inverse_hessian_diagonal(long b, Vector& OUT) { one_diagonal(b, OUT, true); }
 
 private:
     std::ptrdiff_t m_hist_n = 0;
@@ -170,6 +180,18 @@ private:
         OUT.resize(V.size());
         m_dev->check(detail::small_batch_abi<Scalar>::times(m_hist, inverse, int64_t(b), 1, k, V.data(), int64_t(m_n), 0, OUT.data(),
                                                             int64_t(m_n), 0));
+    }
+    void diagonal(long b0, long count, Vector& OUT, bool inverse)
+    {
+        require_kept();
+        OUT.resize(m_n * std::ptrdiff_t(count));
+        m_dev->check(detail::small_batch_abi<Scalar>::diag(m_hist, inverse, int64_t(b0), int64_t(count), OUT.data(), int64_t(m_n)));
+    }
+    void one_diagonal(long b, Vector& OUT, bool inverse)
+    {
+        require_kept();
+        if (b < 0 || b >= m_B) throw std::invalid_argument("LBFGSSmallBatchSolver: problem index out of range");
+        diagonal(b, 1, OUT, inverse);
     }
     SmallMatrix<Scalar> dense(long b, bool inverse)
     {

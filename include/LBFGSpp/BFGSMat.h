@@ -337,7 +337,41 @@ public:
     }
     std::ptrdiff_t dim() const { return m_n; }
 
+    // The diagonals of the same two matrices at any n, with no products: written over the raw columns W = [Y S] as
+    // B = theta I + W K_B W' and H = I/theta + W K_H W' (CompactForm.h, compact_kb / compact_kh, K formed here on the host), entry i is
+    // a0 + r_i' K r_i with r_i row i of W: one pass over the history (lbfgs_b200_hist_quad_diag).  out is resized to n.  With c = 0:
+    // theta and 1/theta.
+    void hessian_diagonal(Vector& out) { diagonal(out, false); }
+    void inverse_hessian_diagonal(Vector& out) { diagonal(out, true); }
+
 private:
+    void diagonal(Vector& out, bool inverse)
+    {
+        require_history();
+        refresh_middle();
+        const int c = m_c_host, w = 2 * c;
+        const Scalar theta = m_theta_host;
+        std::vector<Scalar> K(size_t(w) * size_t(w));
+        if (c > 0)
+        {
+            std::vector<Scalar> unit(size_t(2 * w - 1), Scalar(0));
+            unit[size_t(w - 1)] = Scalar(1);
+            if (inverse)
+            {
+                SmallMatrix<Scalar> YYage(c, c), R(c, c), YY(c, c);
+                m_dev->check(detail::BoxAbi<Scalar>::hist_gram(m_hist, nullptr, nullptr, YYage.data(), nullptr, nullptr));
+                compact_h_setup(c, m_SY.data(), YYage.data(), c, R.data(), YY.data());
+                std::vector<Scalar> scr(static_cast<size_t>(w));
+                compact_kh(c, R.data(), YY.data(), theta, unit.data(), 0, 1, scr.data(), 1, K.data());
+            }
+            else
+                compact_kb(c, m_M.data(), theta, unit.data(), 0, 1, K.data());
+            compact_k_symmetrise(w, K.data(), 0, 1);
+        }
+        out.resize(m_n);
+        m_dev->check(detail::BoxAbi<Scalar>::hist_quad_diag(m_hist, inverse ? Scalar(1) / theta : theta, c > 0 ? K.data() : nullptr, out.data()));
+    }
+
     void times(const Vector& V, int k, Vector& OUT, bool inverse)
     {
         require_history();

@@ -10,6 +10,8 @@
 //   H v = v/theta + S u_s + Y u_y/theta,  R = triu(S'Y) in chronological order t = c - 1 - age:
 //       u_y = -R^-1 S'v,  u_s = R^-T ((D + Y'Y/theta) R^-1 S'v - Y'v/theta)                                    a0 = 1/theta
 // With c = 0: B = theta I, H = I / theta.
+// The same two matrices as B = theta I + W K_B W' and H = I/theta + W K_H W' over the raw W = [Y S]: compact_kb / compact_kh, whose
+// diagonals a0 + r_i' K r_i (r_i: row i of W) need no products.
 #ifndef LBFGSPP_B200_COMPACT_FORM_H
 #define LBFGSPP_B200_COMPACT_FORM_H
 
@@ -202,6 +204,40 @@ LBFGS_HD inline void compact_h_coef(int c, const T* R, const T* YYc, T theta, co
         C[(c - 1 - t) * ldc] = -w[t * ldt] / theta;
         C[(c + c - 1 - t) * ldc] = us[t * ldt];
     }
+}
+
+// ---- the middle matrices over the raw columns: B = theta I + W K_B W',  H = I/theta + W K_H W',  W = [Y S] by age ----------------
+// K_B = -diag(I, theta I) M diag(I, theta I); K_H = [ 0  -R^-1/theta ; -R^-T/theta  R^-T (D + Y'Y/theta) R^-1 ] (the blocks in
+// chronological order).  Column r of K is the coefficient vector compact_b_coef / compact_h_coef make for e_r, so the two functions
+// below write columns r0, r0 + dr, ... of K [2c x 2c] (row-major, rows y by age then s by age) and several threads can share a K;
+// compact_k_symmetrise then makes it exactly symmetric.  unit: 4c - 1 elements, zero but unit[2c - 1] = 1, so that unit + 2c - 1 - r
+// is e_r with stride 1.
+template <typename T>
+LBFGS_HD inline void compact_kb(int c, const T* M, T theta, const T* unit, int r0, int dr, T* K)
+{
+    const int w = 2 * c;
+    for (int r = r0; r < w; r += dr) compact_b_coef(c, M, theta, unit + (w - 1 - r), 1, K + r, w);
+}
+
+// scr: compact_h_coef's w and us for one column, 2c elements at stride ldt
+template <typename T>
+LBFGS_HD inline void compact_kh(int c, const T* R, const T* YYc, T theta, const T* unit, int r0, int dr, T* scr, int ldt, T* K)
+{
+    const int w = 2 * c;
+    for (int r = r0; r < w; r += dr) compact_h_coef(c, R, YYc, theta, unit + (w - 1 - r), 1, scr, scr + c * ldt, ldt, K + r, w);
+}
+
+// K = (K + K')/2 on rows i0, i0 + di, ...: row i owns the pairs (i, j > i), so rows may be done by different threads at once
+template <typename T>
+LBFGS_HD inline void compact_k_symmetrise(int w, T* K, int i0, int di)
+{
+    for (int i = i0; i < w; i += di)
+        for (int j = i + 1; j < w; j++)
+        {
+            const T v = (K[i * w + j] + K[j * w + i]) * T(0.5);
+            K[i * w + j] = v;
+            K[j * w + i] = v;
+        }
 }
 
 }  // namespace LBFGSpp

@@ -231,6 +231,13 @@ void* lbfgs_b200_box_vector(lbfgs_b200_box* b, int which);               /* LBFG
      * element the terms are added in that order (with k = 1 the arithmetic of hist_lincomb).  OUT may be V when ldo == ldv. */ \
     lbfgs_b200_status lbfgs_b200_hist_lincomb_multi_##SUF(lbfgs_b200_hist* h, T a0, int k, const T* V,         \
                                                           int64_t ldv, const T* C_host, T* OUT, int64_t ldo);  \
+    /* The diagonal of the final approximation (LBFGSSolver::final_approx_hessian_diagonal / _inverse_hessian_diagonal): with  \
+     * B or H = a0 I + W K W', W = [Y S] (include/LBFGSpp/CompactForm.h, compact_kb / compact_kh), out_i = a0 + r_i' K r_i for   \
+     * i < n, r_i = (y_0[i] .. y_{c-1}[i], s_0[i] .. s_{c-1}[i]).  K_host [2c][2c] row-major, symmetric: only its upper triangle \
+     * is read (NULL allowed when c = 0).  One pass over the 2c history columns, no reductions; per element the sum is taken   \
+     * in fp64 in a fixed order (lbfgsb_kernels.cuh, k_hist_quad_diag), so out_i depends on row i and K only.  Any m; replicas \
+     * only (a context with more than one rank is refused).  Entries of out past n are not written.                          */ \
+    lbfgs_b200_status lbfgs_b200_hist_quad_diag_##SUF(lbfgs_b200_hist* h, T a0, const T* K_host, T* out);      \
     /* Cauchy.h:111-129: breakpoints, d = -g on movable coordinates, class bytes.                                      \
      * out5 = { #fixed, #never-bounded, #with a finite breakpoint, d.d, smallest breakpoint } */                       \
     lbfgs_b200_status lbfgs_b200_box_cauchy_breaks_##SUF(lbfgs_b200_box*, const T* x, const T* g, const T* lb, \
@@ -385,7 +392,15 @@ const void* lbfgs_b200_small_hist_y_col(const lbfgs_b200_small_hist* h, int64_t 
      * ldop == ldvp) and, for count > 1, vectors of its own per problem.  LBFGS_B200_ERR_INVALID for k < 1, ldv or ldo < n, a     \
      * problem range outside [0, B), NULL pointers or a history no solve has filled.  Asynchronous.                          */ \
     lbfgs_b200_status lbfgs_b200_small_hist_times_##SUF(lbfgs_b200_small_hist* h, int inverse, int64_t b0, int64_t count, int k, \
-                                                        const T* V, int64_t ldv, int64_t ldvp, T* OUT, int64_t ldo, int64_t ldop);
+                                                        const T* V, int64_t ldv, int64_t ldvp, T* OUT, int64_t ldo, int64_t ldop);   \
+    /* OUT + p*ldo = diag(B_b) (inverse = 0) or diag(H_b) (inverse != 0) for the problems b = b0 + p, p < count, in one launch  \
+     * (one block per problem): the block forms its problem's K of CompactForm.h on the chip and makes one pass over its 2c    \
+     * history columns, out_i = a0 + r_i' K r_i in the order of lbfgs_b200_hist_quad_diag.  A problem's diagonal depends on its   \
+     * history only, not on b0, count or its position; with c = 0 it is theta (B) or 1/theta (H).  LBFGS_B200_ERR_INVALID for  \
+     * ldo < n, a problem range outside [0, B), a NULL OUT, a history no solve has filled or a context with more than one      \
+     * rank.  Asynchronous.                                                                                                   */ \
+    lbfgs_b200_status lbfgs_b200_small_hist_diag_##SUF(lbfgs_b200_small_hist* h, int inverse, int64_t b0, int64_t count, T* OUT,   \
+                                                       int64_t ldo);
 
 LBFGS_B200_DECLARE_SMALL_HIST(double, f64)
 LBFGS_B200_DECLARE_SMALL_HIST(float, f32)

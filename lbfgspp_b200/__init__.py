@@ -133,6 +133,8 @@ def _declare(lib):
         if hasattr(lib, "lbfgs_b200_hist_wt_dot_multi_" + suf):   # the k-vector passes (a test double of the ABI may lack them)
             getattr(lib, "lbfgs_b200_hist_wt_dot_multi_" + suf).argtypes = [vp, ci, vp, i64, pt]
             getattr(lib, "lbfgs_b200_hist_lincomb_multi_" + suf).argtypes = [vp, ct, ci, vp, i64, pt, vp, i64]
+        if hasattr(lib, "lbfgs_b200_hist_quad_diag_" + suf):      # the diagonal pass (a test double of the ABI may lack it)
+            getattr(lib, "lbfgs_b200_hist_quad_diag_" + suf).argtypes = [vp, ct, pt, vp]
         getattr(lib, "lbfgs_b200_box_cauchy_breaks_" + suf).argtypes = [vp, vp, vp, vp, vp, pt]
         getattr(lib, "lbfgs_b200_box_cauchy_sweep_" + suf).argtypes = [vp, vp, pt, pt, ct, ct, i64, i64, pt]
         getattr(lib, "lbfgs_b200_box_cauchy_build_" + suf).argtypes = [vp, vp, vp, vp, ct, ct, pt]
@@ -170,6 +172,7 @@ def _declare(lib):
             getattr(lib, "lbfgs_b200_small_minimize_keep_" + suf).argtypes = [vp, ci, vp, vp, i64, i64, i64, vp, ci, vp, i64, vp, vp, vp]
             getattr(lib, "lbfgs_b200_small_hist_info_" + suf).argtypes = [vp, vp, vp]
             getattr(lib, "lbfgs_b200_small_hist_times_" + suf).argtypes = [vp, ci, i64, i64, ci, vp, i64, i64, vp, i64, i64]
+            getattr(lib, "lbfgs_b200_small_hist_diag_" + suf).argtypes = [vp, ci, i64, i64, vp, i64]
     lib._typed = True
     return lib
 
@@ -271,6 +274,14 @@ def _declare_driver(lib):
         for suf, pt in (("f64", dp), ("f32", fp)):
             getattr(lib, "lbfgsb200_drv_small_batch_hessian_times_" + suf).argtypes = [ci, ci, cl, cl, pt, pt, pt, cl, ci, prm, pt, cl, ci, pt,
                                                                                       pt, pt, pt, C.POINTER(_SmallItem), err, errlen]
+    # the diagonals of the final approximation (csrc/driver_hessian_diag.cpp)
+    if hasattr(lib, "lbfgsb200_drv_solve_hessian_diag_f64"):
+        lib.lbfgsb200_drv_solve_hessian_diag_f64.argtypes = [ci, ci, cl, ci, prm, ci, dp, dp, dp, C.POINTER(ci), err, errlen]
+        lib.lbfgsb200_drv_batch_hessian_diag_f64.argtypes = [ci, ci, cl, ci, dp, ci, prm, ci, dp, dp, err, errlen]
+        lib.lbfgsb200_drv_hist_diag_f64.argtypes = [ci, cl, ci, ci, dp, dp, dp, dp, err, errlen]
+        for suf, pt in (("f64", dp), ("f32", fp)):
+            getattr(lib, "lbfgsb200_drv_small_batch_hessian_diag_" + suf).argtypes = [ci, ci, cl, cl, pt, pt, pt, cl, ci, prm, pt, pt, pt,
+                                                                                     C.POINTER(_SmallItem), err, errlen]
     lib._drv_typed = True
     return lib
 
@@ -620,6 +631,13 @@ class History:
         self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_hist_lincomb_multi_" + self.suf)(
             self.h, a0, k, V.ptr, ldv, coef.ctypes.data_as(C.POINTER(self.ct)) if coef.size else None, OUT.ptr, ldo))
 
+    def quad_diag(self, a0, K, out):
+        """out_i = a0 + r_i' K r_i into the DeviceArray out (lbfgs_b200_hist_quad_diag): K (2c, 2c), symmetric, rows y by age then s by
+        age; only its upper triangle is read."""
+        Kc = np.ascontiguousarray(K, dtype=self.dtype).reshape(-1)
+        self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_hist_quad_diag_" + self.suf)(
+            self.h, a0, Kc.ctypes.data_as(C.POINTER(self.ct)) if Kc.size else None, out.ptr))
+
     def column(self, which, age):
         fn = self.ctx.lib.lbfgs_b200_hist_s_col if which == "s" else self.ctx.lib.lbfgs_b200_hist_y_col
         p = fn(self.h, age)
@@ -841,6 +859,45 @@ def batch_hessian_times(objective, X0, b, V, param=None, linesearch="MoreThuente
         device, objective, n, B, _ptr(X0), _ls_id(linesearch), C.byref(p), b, _ptr(v), vlen, _ptr(bv), _ptr(hv), _ptr(hbv), *err)), V, n)
 
 
+def solve_hessian_diagonal(objective, x0, param=None, linesearch="NocedalWright", resident=True, device=0, lib=None):
+    """minimize(), then the diagonals of the final approximation (LBFGSSolver::final_approx_hessian_diagonal /
+    final_approx_inverse_hessian_diagonal).  Returns (niter, x, diag B, diag H)."""
+    drv = driver(lib)
+    x = np.array(x0, dtype=np.float64, order="C").copy()
+    n = x.size
+    p = (param if param is not None else LBFGSParam())._c()
+    niter = C.c_int(0)
+    dB, dH = np.zeros(n), np.zeros(n)
+    _checked("solve_hessian_diagonal", lambda *err: drv.lbfgsb200_drv_solve_hessian_diag_f64(
+        device, objective, n, _ls_id(linesearch), C.byref(p), int(resident), _ptr(x), _ptr(dB), _ptr(dH), C.byref(niter), *err))
+    return niter.value, x, dB, dH
+
+
+def batch_hessian_diagonal(objective, X0, b, param=None, linesearch="MoreThuente", device=0, lib=None):
+    """A batch (rows of X0) minimised by LBFGSBatchSolver, then the diagonals of problem b's final approximation.
+    Returns (diag B, diag H)."""
+    drv = driver(lib)
+    X0 = np.ascontiguousarray(X0, dtype=np.float64)
+    B, n = X0.shape
+    p = (param if param is not None else LBFGSParam())._c()
+    dB, dH = np.zeros(n), np.zeros(n)
+    _checked("batch_hessian_diagonal", lambda *err: drv.lbfgsb200_drv_batch_hessian_diag_f64(
+        device, objective, n, B, _ptr(X0), _ls_id(linesearch), C.byref(p), b, _ptr(dB), _ptr(dH), *err))
+    return dB, dH
+
+
+def hist_diagonal(S, Y, m=None, device=0, lib=None):
+    """diag B and diag H of the history built by adding the pairs (S[k], Y[k]) in order to a ring of size m (default: all of them)."""
+    drv = driver(lib)
+    S = np.ascontiguousarray(S, dtype=np.float64)
+    Y = np.ascontiguousarray(Y, dtype=np.float64)
+    npairs, n = S.shape
+    dB, dH = np.zeros(n), np.zeros(n)
+    _checked("hist_diagonal", lambda *err: drv.lbfgsb200_drv_hist_diag_f64(device, n, npairs if m is None else m, npairs, _ptr(S), _ptr(Y),
+                                                                          _ptr(dB), _ptr(dH), *err))
+    return dB, dH
+
+
 def small_max_n(m, objective, dtype=np.float64):
     """Largest n of a problem the small-batch solve takes for history size m and built-in objective `objective` (0 if none)."""
     return int(abi().lbfgs_b200_small_max_n(int(m), np.dtype(dtype).itemsize, int(objective)))
@@ -902,6 +959,32 @@ def small_batch_hessian_times(objective, X0, V, param=None, linesearch="MoreThue
     return res, X, BV, HV, HBV
 
 
+def small_batch_hessian_diagonal(objective, X0, param=None, linesearch="MoreThuente", dtype=np.float64, data0=None, data1=None, ldd=0,
+                                 device=0, lib=None):
+    """solve_small_batch with every problem's final approximation kept (LBFGSSmallBatchSolver::keep_final_approx), then the diagonals
+    of all of them, one launch each (final_approx_hessian_diagonal / final_approx_inverse_hessian_diagonal).  Returns (outcomes, X,
+    diag B, diag H), the diagonals of shape (B, n)."""
+    drv = driver(lib)
+    X0 = np.ascontiguousarray(X0, dtype=dtype)
+    B, n = X0.shape
+    p = (param if param is not None else LBFGSParam())._c()
+    d0 = None if data0 is None else np.ascontiguousarray(data0, dtype=dtype).reshape(-1)
+    d1 = None if data1 is None else np.ascontiguousarray(data1, dtype=dtype).reshape(-1)
+    X = np.empty_like(X0)
+    dB, dH = np.empty((B, n), dtype=dtype), np.empty((B, n), dtype=dtype)
+    items = (_SmallItem * B)()
+    suf = "f32" if np.dtype(dtype) == np.float32 else "f64"
+    fn = getattr(drv, "lbfgsb200_drv_small_batch_hessian_diag_" + suf)
+    err = C.create_string_buffer(256)
+    r = fn(device, objective, n, B, _ptr(X0), _ptr(d0), _ptr(d1), int(ldd), _ls_id(linesearch), C.byref(p), _ptr(X), _ptr(dB), _ptr(dH), items,
+           err, len(err))
+    if r < 0:
+        raise (ValueError if r == -1 else RuntimeError)("small_batch_hessian_diagonal failed: %s" % err.value.decode())
+    res = [dict(status=STATUS_NAMES[it.kind], code=it.code, niter=it.niter, nfev=it.nfev, fx=it.fx, gnorm=it.gnorm, rounds=it.rounds)
+           for it in items]
+    return res, X, dB, dH
+
+
 class SmallHistory:
     """The kept final approximations of a small-batch solve (lbfgs_b200_small_hist) through the C ABI: create, minimize-keep, info,
     columns and products."""
@@ -955,6 +1038,10 @@ class SmallHistory:
         """lbfgs_b200_small_hist_times_* on DeviceArrays (asynchronous)."""
         self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_small_hist_times_" + self.suf)(self.h, int(inverse), b0, count, k, V.ptr, ldv, ldvp,
                                                                                          OUT.ptr, ldo, ldop))
+
+    def diagonal(self, inverse, b0, count, OUT, ldo):
+        """lbfgs_b200_small_hist_diag_* into the DeviceArray OUT, problem b0 + p's diagonal at offset p*ldo (asynchronous)."""
+        self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_small_hist_diag_" + self.suf)(self.h, int(inverse), b0, count, OUT.ptr, ldo))
 
 
 def phase_clock(on=True):

@@ -208,6 +208,7 @@ struct lbfgs_b200_hist
     int head = 0;   // physical slot the next pair is written to
     int ncorr = 0;  // valid pairs (<= m)
     void* multi = nullptr;  // scratch of the k-vector passes (hist_wt_dot_multi / hist_lincomb_multi), made on first use
+    void* quad = nullptr;   // the packed K of hist_quad_diag (m(2m + 1) doubles), made on first use
     // physical slot of the pair with the given age (0 = newest)
     int slot(int age) const { return ((head - 1 - age) % M + M) % M; }
     template <class T> T* s_col(int phys) const { return static_cast<T*>(S) + (int64_t)phys * ld; }

@@ -1277,7 +1277,7 @@ void lbfgs_b200_hist_destroy(lbfgs_b200_hist* h)
 {
     if (!h) return;
     // (no synchronisation: the blocks go back to the context's pool and everything that used them is ordered on its stream)
-    for (void* p : {h->S, h->Y, h->ys, h->alpha, h->theta, h->SY[0], h->YY[0], h->SS[0], h->SY[1], h->YY[1], h->SS[1], h->multi}) pool_free(h->ctx, p);
+    for (void* p : {h->S, h->Y, h->ys, h->alpha, h->theta, h->SY[0], h->YY[0], h->SS[0], h->SY[1], h->YY[1], h->SS[1], h->multi, h->quad}) pool_free(h->ctx, p);
     delete h;
 }
 

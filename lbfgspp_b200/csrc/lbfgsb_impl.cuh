@@ -202,6 +202,47 @@ static lbfgs_b200_status do_hist_lincomb_multi(lbfgs_b200_hist* h, T a0, int k, 
     return launch_lincomb<T>(h, a0, k, V, ldv, static_cast<const T*>(coef), nullptr, 0, OUT, ldo);
 }
 
+// out_i = a0 + r_i' K r_i (see k_hist_quad_diag): K's upper triangle is packed, off-diagonal entries doubled, on the host (exact
+// in binary floating point), and the kernel's width is chosen from c alone, so a row's arithmetic depends on c, K and the row only
+template <class T> static lbfgs_b200_status do_hist_quad_diag(lbfgs_b200_hist* h, T a0, const T* K_host, T* out)
+{
+    if (auto st = hist_check<T>(h)) return st;
+    lbfgs_b200_ctx* ctx = h->ctx;
+    REQUIRE(ctx, ctx->nranks == 1, "hist_quad_diag: replicas only, not for a context with %d ranks", ctx->nranks);
+    const int c = h->ncorr, w = 2 * c;
+    REQUIRE(ctx, out && (c == 0 || K_host), "hist_quad_diag: NULL argument");
+    const int nk = w * (w + 1) / 2;
+    std::vector<double> kp((size_t)(nk > 0 ? nk : 1));
+    for (int p = 0, e = 0; p < w; p++)
+        for (int q = p; q < w; q++, e++) kp[(size_t)e] = (q == p ? 1.0 : 2.0) * (double)K_host[p * w + q];
+    if (!h->quad)
+    {
+        const cudaError_t e = pool_alloc(ctx, &h->quad, sizeof(double) * (size_t)h->m * (2 * h->m + 1));
+        if (e != cudaSuccess)
+            return fail(ctx, e == cudaErrorMemoryAllocation ? LBFGS_B200_ERR_ALLOC : LBFGS_B200_ERR_CUDA, "history scratch: %s", cudaGetErrorString(e));
+    }
+    if (nk > 0)
+    {
+        CU(ctx, cudaMemcpyAsync(h->quad, kp.data(), sizeof(double) * (size_t)nk, cudaMemcpyHostToDevice, ctx->stream));
+        CU(ctx, cudaStreamSynchronize(ctx->stream));   // kp is freed on return
+    }
+    QuadDiagArgs<T> a{};
+    a.n = h->n; a.ld = h->ld; a.S = static_cast<const T*>(h->S); a.Y = static_cast<const T*>(h->Y);
+    a.Kp = static_cast<const double*>(h->quad); a.a0 = (double)a0; a.out = out; a.c = c;
+    fill_slots<T>(h, a.slots);
+    const size_t smem = sizeof(double) * (size_t)nk;
+    auto launch = [&](auto kernel, int rpt) -> lbfgs_b200_status {
+        if (smem > 48 * 1024) CU(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        const int64_t span = (int64_t)kThreads * rpt, want = (h->n + span - 1) / span, cap = (int64_t)ctx->sm_count * 8;
+        kernel<<<(int)(want < 1 ? 1 : want < cap ? want : cap), kThreads, smem, ctx->stream>>>(a);
+        return post_launch(ctx, "k_hist_quad_diag");
+    };
+    if (w <= 16) return launch(k_hist_quad_diag<T, 16>, quad_diag_rpt<16>());
+    if (w <= 32) return launch(k_hist_quad_diag<T, 32>, quad_diag_rpt<32>());
+    if (w <= 64) return launch(k_hist_quad_diag<T, 64>, quad_diag_rpt<64>());
+    return launch(k_hist_quad_diag<T, kMaxW>, quad_diag_rpt<kMaxW>());
+}
+
 // G[(2c)x(2c)] over rows with (cls & mask) != 0, ordering [Y by age, S by age]   (WP'WP of BFGSMat.h:529-565)
 template <class T>
 static lbfgs_b200_status do_hist_masked_gram(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, int mask, T* G_host)
@@ -502,6 +543,8 @@ void* lbfgs_b200_box_vector(lbfgs_b200_box* b, int which)
     lbfgs_b200_status lbfgs_b200_hist_lincomb_multi_##SUF(lbfgs_b200_hist* h, T a0, int k, const T* V, int64_t ldv,         \
                                                           const T* C_host, T* OUT, int64_t ldo)                             \
     { return do_hist_lincomb_multi<T>(h, a0, k, V, ldv, C_host, OUT, ldo); }                                                \
+    lbfgs_b200_status lbfgs_b200_hist_quad_diag_##SUF(lbfgs_b200_hist* h, T a0, const T* K_host, T* out)                    \
+    { return do_hist_quad_diag<T>(h, a0, K_host, out); }                                                                    \
     lbfgs_b200_status lbfgs_b200_box_cauchy_breaks_##SUF(lbfgs_b200_box* b, const T* x, const T* g, const T* lb,            \
                                                          const T* ub, T* out5_host)                                         \
     { return do_box_cauchy_breaks<T>(b, x, g, lb, ub, out5_host); }                                                         \

@@ -6,7 +6,8 @@
 //   W'(mask o v)       -> k_gram_dots on the masked vector            (apply_WtPv, compute_FtBAb; BFGSMat.h:382-433,486-522)
 //   (W_P)'(W_P)        -> k_masked_gram                                (solve_PtBP; BFGSMat.h:529-565)
 //   W_P * coef         -> k_hist_lincomb                               (apply_PtWMv, apply_PtBQv; BFGSMat.h:435-478,570-615)
-// (k_hist_lincomb and k_hist_wt_dot_multi also serve blocks of up to 16 vectors: the operator form of the final approximation)
+// (k_hist_lincomb and k_hist_wt_dot_multi also serve blocks of up to 16 vectors: the operator form of the final approximation;
+// k_hist_quad_diag forms its diagonal)
 // The generalized Cauchy point (Cauchy.h:86-284) is sort + prefix sums: after sorting the breakpoints, the state of the
 // reference's sequential sweep just after crossing sorted position k is a function of prefix sums over positions <= k
 // (sum g^2, sum g*w, sum t*g*w with w = row of W), so all segments are examined in parallel and the first one whose
@@ -535,6 +536,86 @@ template <class T, int KMAX> __global__ void __launch_bounds__(kThreads) k_hist_
 #pragma unroll
         for (int j = 0; j < KMAX; j++)
             if (j < k) a.out[j * a.ldo + i] = r[j];
+    }
+}
+
+// The diagonal of a0 I + W K W' (W = [Y S] by age, K symmetric 2c x 2c): out_i = a0 + r_i' K r_i, r_i = row i of W.  Kp holds the
+// upper triangle packed row by row with the off-diagonal entries doubled, in double: row p is K_pp, 2K_p,p+1, ..., 2K_p,2c-1.  Per
+// element, with every operation in fp64 (fp32 storage is taken up to double) and every multiply-add a fused fma:
+//     t_p = Kp_pp r_p,  t_p = fma(Kp_pq, r_q, t_p) for q = p+1, ..., 2c-1;   acc = 0,  acc = fma(r_p, t_p, acc) for p = 0, ..., 2c-1;
+//     out_i = a0 + acc
+// so out_i depends on row i and K only (not on the grid, n or i).  2c^2 + 3c multiply-adds per element over (2c + 1) words.
+// WMAX >= 2c: the row sits in registers (loops unrolled for WMAX <= 64; at 64 part of it stays on the stack) and each K value read
+// from shared memory serves RPT rows; WMAX = kMaxW (c > 32) keeps the row in local memory.
+template <class T> struct QuadDiagArgs
+{
+    int64_t n, ld;
+    const T* S;
+    const T* Y;
+    const double* Kp;   // device, w(w+1)/2 values
+    double a0;
+    T* out;
+    int c;
+    unsigned char slots[kMaxM];
+};
+
+template <int WMAX> __host__ __device__ constexpr int quad_diag_rpt() { return WMAX <= 32 ? 64 / WMAX : 1; }
+
+template <class T, int WMAX> __global__ void __launch_bounds__(kThreads) k_hist_quad_diag(QuadDiagArgs<T> a)
+{
+    constexpr int RPT = quad_diag_rpt<WMAX>();
+    constexpr int UNROLL = WMAX <= 64 ? WMAX : 1;
+    extern __shared__ double s_kp[];
+    __shared__ const T* s_col[kMaxW];
+    const int c = a.c, w = 2 * c;
+    for (int e = threadIdx.x; e < w * (w + 1) / 2; e += kThreads) s_kp[e] = a.Kp[e];
+    for (int q = threadIdx.x; q < w; q += kThreads) s_col[q] = (q < c ? a.Y + (int64_t)a.slots[q] * a.ld : a.S + (int64_t)a.slots[q - c] * a.ld);
+    __syncthreads();
+    const int64_t span = (int64_t)kThreads * RPT;
+    for (int64_t i0 = (int64_t)blockIdx.x * span + threadIdx.x; i0 < a.n; i0 += (int64_t)gridDim.x * span)
+    {
+        double r[RPT][WMAX];
+#pragma unroll
+        for (int j = 0; j < RPT; j++)
+        {
+            const int64_t i = i0 + (int64_t)j * kThreads;
+#pragma unroll UNROLL
+            for (int q = 0; q < WMAX; q++)
+                if (q < w) r[j][q] = i < a.n ? (double)s_col[q][i] : 0.0;
+        }
+        double acc[RPT];
+#pragma unroll
+        for (int j = 0; j < RPT; j++) acc[j] = 0.0;
+        int off = 0;   // row p of the packed triangle starts at off
+#pragma unroll UNROLL
+        for (int p = 0; p < WMAX; p++)
+        {
+            if (p < w)
+            {
+                double t[RPT];
+#pragma unroll
+                for (int j = 0; j < RPT; j++) t[j] = s_kp[off] * r[j][p];
+#pragma unroll UNROLL
+                for (int q = p + 1; q < WMAX; q++)
+                {
+                    if (q < w)
+                    {
+                        const double kq = s_kp[off + q - p];
+#pragma unroll
+                        for (int j = 0; j < RPT; j++) t[j] = fma(kq, r[j][q], t[j]);
+                    }
+                }
+#pragma unroll
+                for (int j = 0; j < RPT; j++) acc[j] = fma(r[j][p], t[j], acc[j]);
+                off += w - p;
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < RPT; j++)
+        {
+            const int64_t i = i0 + (int64_t)j * kThreads;
+            if (i < a.n) a.out[i] = (T)(a.a0 + acc[j]);
+        }
     }
 }
 

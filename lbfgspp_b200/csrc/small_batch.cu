@@ -156,6 +156,29 @@ lbfgs_b200_status small_hist_times(lbfgs_b200_small_hist* h, int inverse, int64_
     return LBFGS_B200_OK;
 }
 
+template <class T>
+lbfgs_b200_status small_hist_diag(lbfgs_b200_small_hist* h, int inverse, int64_t b0, int64_t count, T* OUT, int64_t ldo)
+{
+    using namespace lb;
+    if (auto st = small_hist_check<T>(h, "small_hist_diag")) return st;
+    lbfgs_b200_ctx* ctx = h->ctx;
+    const int64_t n = h->n;
+    REQUIRE(ctx, OUT, "small_hist_diag: NULL argument");
+    REQUIRE(ctx, b0 >= 0 && count >= 1 && count <= h->B - b0, "small_hist_diag: problems [%lld, %lld) are not within the %lld of the history",
+            (long long)b0, (long long)(b0 + count), (long long)h->B);
+    REQUIRE(ctx, ldo >= n, "small_hist_diag: leading dimension ldo = %lld must be at least n = %lld", (long long)ldo, (long long)n);
+    REQUIRE(ctx, ctx->nranks == 1, "small_hist_diag: one CTA holds a whole problem, so n cannot be sharded (the context has %d ranks)", ctx->nranks);
+    SmallDiagArgs<T> a{};
+    a.hist = static_cast<const T*>(h->data); a.hist_c = h->counts; a.HL = SmallHistLayout{n, h->m};
+    a.b0 = b0; a.inverse = inverse ? 1 : 0; a.OUT = OUT; a.ldo = ldo;
+    const size_t smem = small_diag_smem(h->m, (int)sizeof(T));
+    CU(ctx, cudaFuncSetAttribute(k_small_hist_diag<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_small_hist_diag<T><<<(unsigned)count, small_threads(n), smem, ctx->stream>>>(a);
+    CU(ctx, cudaGetLastError());
+    ctx->launches++;
+    return LBFGS_B200_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -224,7 +247,10 @@ const void* lbfgs_b200_small_hist_y_col(const lbfgs_b200_small_hist* h, int64_t 
     { return small_hist_info<T>(h, c_host, theta_host); }                                                                         \
     lbfgs_b200_status lbfgs_b200_small_hist_times_##SUF(lbfgs_b200_small_hist* h, int inverse, int64_t b0, int64_t count, int k,   \
                                                         const T* V, int64_t ldv, int64_t ldvp, T* OUT, int64_t ldo, int64_t ldop)  \
-    { return small_hist_times<T>(h, inverse, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop); }
+    { return small_hist_times<T>(h, inverse, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop); }                                      \
+    lbfgs_b200_status lbfgs_b200_small_hist_diag_##SUF(lbfgs_b200_small_hist* h, int inverse, int64_t b0, int64_t count, T* OUT,    \
+                                                       int64_t ldo)                                                                \
+    { return small_hist_diag<T>(h, inverse, b0, count, OUT, ldo); }
 
 LBFGS_B200_SMALL_KEEP(double, f64)
 LBFGS_B200_SMALL_KEEP(float, f32)

@@ -504,6 +504,38 @@ inline size_t small_times_smem(int m, int elem)
     return sizeof(double) * (size_t)kSMaxWarps * kSGroup + (size_t)elem * (2 * w * kSGroup + (alg_b > alg_h ? alg_b : alg_h));
 }
 
+// The 2c x 2c algebra of a kept problem, on the chip, for the products and the diagonal.  Every thread of the CTA calls it; it ends
+// with a barrier.  B: Minv factorised in place by thread 0 in alg[0, w^2) (w = 2c), then M = Minv^-1 in alg[w^2, 2w^2), column j
+// solved by thread j.  H: R and Y'Y in chronological order in alg[0, c^2) and alg[c^2, 2c^2), set up by thread 0.
+template <class T>
+__device__ __forceinline__ void small_compact_setup(const T* rec, const SmallHistLayout& HL, int c, T theta, bool inverse, T* alg, int* order,
+                                                    unsigned char* tag)
+{
+    const int tid = threadIdx.x, nt = blockDim.x;
+    const T* SY = rec + HL.SY();
+    if (!inverse)
+    {
+        const int w = 2 * c;
+        T* F = alg;            // Minv, factorised in place
+        T* Mm = alg + w * w;   // M = Minv^-1
+        if (tid == 0)
+        {
+            LBFGSpp::compact_minv(c, SY, rec + HL.SS(), c, theta, F);
+            LBFGSpp::bk_factor(F, w, order, tag);
+        }
+        __syncthreads();
+        for (int j = tid; j < w; j += nt)   // column j of M: Minv^-1 e_j
+        {
+            T z[2 * kMaxM];
+            for (int i = 0; i < w; i++) Mm[i * w + j] = i == j ? T(1) : T(0);
+            LBFGSpp::bk_solve(F, w, order, tag, Mm + j, w, z);
+        }
+    }
+    else if (tid == 0)
+        LBFGSpp::compact_h_setup(c, SY, rec + HL.YY(), c, alg, alg + c * c);
+    __syncthreads();
+}
+
 template <class T>
 __global__ void __launch_bounds__(kSMaxThreads) k_small_hist_times(const SmallTimesArgs<T> a)
 {
@@ -555,35 +587,15 @@ __global__ void __launch_bounds__(kSMaxThreads) k_small_hist_times(const SmallTi
             }
             __syncthreads();
         }
-        const T* SY = rec + a.HL.SY();
-        if (!a.inverse)
+        small_compact_setup(rec, a.HL, c, theta, a.inverse != 0, alg, s_order, s_tag);
+        if (tid < kk)
         {
-            const int w = 2 * c;
-            T* F = alg;            // Minv, factorised in place
-            T* Mm = alg + w * w;   // M = Minv^-1
-            if (tid == 0)
+            if (!a.inverse) LBFGSpp::compact_b_coef(c, alg + 4 * c * c, theta, wv + tid, kSGroup, C + tid, kSGroup);
+            else
             {
-                LBFGSpp::compact_minv(c, SY, rec + a.HL.SS(), c, theta, F);
-                LBFGSpp::bk_factor(F, w, s_order, s_tag);
+                T* scr = alg + 2 * c * c;   // per vector: w, us (c each), column tid
+                LBFGSpp::compact_h_coef(c, alg, alg + c * c, theta, wv + tid, kSGroup, scr + tid, scr + c * kSGroup + tid, kSGroup, C + tid, kSGroup);
             }
-            __syncthreads();
-            for (int j = tid; j < w; j += nt)   // column j of M: Minv^-1 e_j
-            {
-                T z[2 * kMaxM];
-                for (int i = 0; i < w; i++) Mm[i * w + j] = i == j ? T(1) : T(0);
-                LBFGSpp::bk_solve(F, w, s_order, s_tag, Mm + j, w, z);
-            }
-            __syncthreads();
-            if (tid < kk) LBFGSpp::compact_b_coef(c, Mm, theta, wv + tid, kSGroup, C + tid, kSGroup);
-        }
-        else
-        {
-            T* R = alg;
-            T* YYc = R + c * c;
-            T* scr = YYc + c * c;   // per vector: w, us (c each), column tid
-            if (tid == 0) LBFGSpp::compact_h_setup(c, SY, rec + a.HL.YY(), c, R, YYc);
-            __syncthreads();
-            if (tid < kk) LBFGSpp::compact_h_coef(c, R, YYc, theta, wv + tid, kSGroup, scr + tid, scr + c * kSGroup + tid, kSGroup, C + tid, kSGroup);
         }
         __syncthreads();
     }
@@ -602,6 +614,76 @@ __global__ void __launch_bounds__(kSMaxThreads) k_small_hist_times(const SmallTi
 #pragma unroll
         for (int j = 0; j < kSGroup; j++)
             if (j < kk) OUT[j * a.ldo + i] = r[j];
+    }
+}
+
+
+// ---- the diagonals of the kept approximations: OUT + p*ldo = diag(B_b) or diag(H_b) for problems b = b0 + p ----------------------
+// One CTA per problem, small_threads(n) threads.  The CTA forms K of B = theta I + W K_B W' or H = I/theta + W K_H W' (W = [Y S] by
+// age; CompactForm.h: compact_kb / compact_kh column by column, then compact_k_symmetrise) after small_compact_setup, and makes one
+// pass over its rows: out_i = a0 + r_i' K r_i in the order of k_hist_quad_diag (lbfgsb_kernels.cuh), all in fp64:
+//     t_p = K_pp r_p,  t_p = fma(2 K_pq, r_q, t_p) for q = p+1, ..., 2c-1;   acc = fma(r_p, t_p, acc) for p = 0, ..., 2c-1;  a0 + acc
+// Nothing depends on b0, count or the problem's position.
+template <class T> struct SmallDiagArgs
+{
+    const T* hist;              // records of SmallHistLayout
+    const int* hist_c;
+    SmallHistLayout HL;
+    int64_t b0;
+    int inverse;
+    T* OUT;                     // problem p's diagonal at OUT + p*ldo
+    int64_t ldo;
+};
+
+// elements of the algebra region: B needs Minv's factor (K takes its place once M is formed) and M; H needs R, Y'Y, the scratch of
+// kSGroup columns and K.  With the unit vector of compact_kb / compact_kh (4m - 1) this never exceeds small_times_smem.
+__host__ __device__ inline size_t small_diag_alg(int m)
+{
+    const size_t w = 2 * (size_t)m;
+    const size_t alg_b = 2 * w * w, alg_h = 2 * (size_t)m * m + 2 * (size_t)m * kSGroup + w * w;
+    return alg_b > alg_h ? alg_b : alg_h;
+}
+inline size_t small_diag_smem(int m, int elem) { return (size_t)elem * (small_diag_alg(m) + 4 * (size_t)m); }
+
+template <class T>
+__global__ void __launch_bounds__(kSMaxThreads) k_small_hist_diag(const SmallDiagArgs<T> a)
+{
+    extern __shared__ __align__(16) unsigned char s_smem[];
+    __shared__ int s_order[2 * kMaxM];
+    __shared__ unsigned char s_tag[2 * kMaxM];
+    const int tid = threadIdx.x, nt = blockDim.x;
+    const int64_t p = blockIdx.x, b = a.b0 + p, n = a.HL.n;
+    const T* rec = a.hist + b * a.HL.rec();
+    T* out = a.OUT + p * a.ldo;
+    const int c = a.hist_c[b], w = 2 * c;
+    const T theta = rec[a.HL.theta()];
+    const double a0 = (double)(a.inverse ? T(1) / theta : theta);
+    T* alg = reinterpret_cast<T*>(s_smem);
+    T* unit = alg + small_diag_alg(a.HL.m);
+    T* K = a.inverse ? alg + 2 * c * c + 2 * c * kSGroup : alg;
+    if (c > 0)
+    {
+        for (int e = tid; e < 2 * w - 1; e += nt) unit[e] = e == w - 1 ? T(1) : T(0);
+        small_compact_setup(rec, a.HL, c, theta, a.inverse != 0, alg, s_order, s_tag);
+        if (!a.inverse) LBFGSpp::compact_kb(c, alg + w * w, theta, unit, tid, nt, K);
+        else if (tid < kSGroup) LBFGSpp::compact_kh(c, alg, alg + c * c, theta, unit, tid, kSGroup, alg + 2 * c * c + tid, kSGroup, K);
+        __syncthreads();
+        LBFGSpp::compact_k_symmetrise(w, K, tid, nt);
+        __syncthreads();
+    }
+    for (int64_t i = tid; i < n; i += nt)
+    {
+        double r[2 * kMaxM];
+        for (int q = 0; q < w; q++) r[q] = (double)rec[(q < c ? a.HL.y(q) : a.HL.s(q - c)) + i];
+        double acc = 0.0;
+        for (int pp = 0; pp < w; pp++)
+        {
+            const T* kr = K + pp * w;
+            double t = (double)kr[pp] * r[pp];
+            for (int q = pp + 1; q < w; q++) t = fma(2.0 * (double)kr[q], r[q], t);
+            acc = fma(r[pp], t, acc);
+        }
+        out[i] = (T)(a0 + acc);
     }
 }
 
