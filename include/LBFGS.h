@@ -308,6 +308,29 @@ public:
     void final_approx_hessian_diagonal(Vector& out) { approx_diagonal(out, false); }
     void final_approx_inverse_hessian_diagonal(Vector& out) { approx_diagonal(out, true); }
 
+    // N(x*, H), the Laplace approximation at the solution, without forming H (BFGSMat::inverse_hessian_factor_times / sample /
+    // inverse_hessian_logdet): OUT = L V for V holding k = V.size()/n vectors, where H = L L'; OUT = mean + L z_j for the k draws
+    // first .. first+k-1 of stream 0 (resized to k*n; a draw depends on (seed, stream, j, i) only); log det H (NaN if the kept pairs
+    // fail the positive-curvature check).  Valid after minimize() in either loop; std::logic_error before the first.
+    void final_approx_inverse_hessian_factor_times(const Vector& V, Vector& OUT)
+    {
+        sync_history();
+        m_bfgs.require_history();
+        m_bfgs.inverse_hessian_factor_times(V, BFGSMat<Scalar>::block_count(V.size(), m_bfgs.dim()), OUT);
+    }
+    void final_approx_sample(const Vector& mean, unsigned long long seed, uint32_t first, int k, Vector& OUT)
+    {
+        sync_history();
+        m_bfgs.require_history();
+        m_bfgs.sample(&mean, seed, 0u, first, k, OUT);
+    }
+    double final_approx_inverse_hessian_logdet()
+    {
+        sync_history();
+        m_bfgs.require_history();
+        return m_bfgs.inverse_hessian_logdet();
+    }
+
 private:
     void approx_diagonal(Vector& out, bool inverse)
     {

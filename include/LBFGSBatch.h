@@ -110,7 +110,37 @@ public:
     void final_approx_hessian_diagonal(int b, Vector& out) { approx_diagonal(b, out, false); }
     void final_approx_inverse_hessian_diagonal(int b, Vector& out) { approx_diagonal(b, out, true); }
 
+    // LBFGSSolver::final_approx_inverse_hessian_factor_times / final_approx_sample / final_approx_inverse_hessian_logdet for problem
+    // b, its draws from stream b: the same values as problem b solved alone with stream b.
+    void final_approx_inverse_hessian_factor_times(int b, const Vector& V, Vector& OUT)
+    {
+        BFGSMat<Scalar> mat;
+        borrow(b, mat);
+        mat.inverse_hessian_factor_times(V, BFGSMat<Scalar>::block_count(V.size(), m_n), OUT);
+    }
+    void final_approx_sample(int b, const Vector& mean, unsigned long long seed, uint32_t first, int k, Vector& OUT)
+    {
+        BFGSMat<Scalar> mat;
+        borrow(b, mat);
+        mat.sample(&mean, seed, uint32_t(b), first, k, OUT);
+    }
+    double final_approx_inverse_hessian_logdet(int b)
+    {
+        BFGSMat<Scalar> mat;
+        borrow(b, mat);
+        return mat.inverse_hessian_logdet();
+    }
+
 private:
+    void borrow(int b, BFGSMat<Scalar>& mat)
+    {
+        if (!m_solver) throw std::logic_error("LBFGSBatchSolver: no history yet (minimize() has not run)");
+        if (b < 0 || b >= m_B) throw std::invalid_argument("LBFGSBatchSolver: problem index out of range");
+        lbfgs_b200_hist* h = lbfgs_b200_solver_history_of(m_solver, b);   // column-major copy of problem b's ring
+        if (!h) m_dev->check(LBFGS_B200_ERR_CUDA);
+        mat.borrow(*m_dev, h, m_n, m_m);
+    }
+
     void approx_diagonal(int b, Vector& out, bool inverse)
     {
         if (!m_solver) throw std::logic_error("LBFGSBatchSolver: no history yet (minimize() has not run)");

@@ -33,6 +33,14 @@ template <> struct small_batch_abi<double>
     { return lbfgs_b200_small_hist_times_f64(h, inv, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop); }
     static lbfgs_b200_status diag(lbfgs_b200_small_hist* h, int inv, int64_t b0, int64_t count, double* OUT, int64_t ldo)
     { return lbfgs_b200_small_hist_diag_f64(h, inv, b0, count, OUT, ldo); }
+    static lbfgs_b200_status factor_times(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, int k, const double* V, int64_t ldv, int64_t ldvp,
+                                          double* OUT, int64_t ldo, int64_t ldop)
+    { return lbfgs_b200_small_hist_factor_times_f64(h, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop); }
+    static lbfgs_b200_status sample(lbfgs_b200_small_hist* h, uint64_t seed, uint32_t first, int64_t b0, int64_t count, int k, const double* M,
+                                    int64_t ldm, double* OUT, int64_t ldo, int64_t ldop)
+    { return lbfgs_b200_small_hist_sample_f64(h, seed, first, b0, count, k, M, ldm, OUT, ldo, ldop); }
+    static lbfgs_b200_status logdet(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, double* out)
+    { return lbfgs_b200_small_hist_logdet_f64(h, b0, count, out); }
 };
 template <> struct small_batch_abi<float>
 {
@@ -48,6 +56,14 @@ template <> struct small_batch_abi<float>
     { return lbfgs_b200_small_hist_times_f32(h, inv, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop); }
     static lbfgs_b200_status diag(lbfgs_b200_small_hist* h, int inv, int64_t b0, int64_t count, float* OUT, int64_t ldo)
     { return lbfgs_b200_small_hist_diag_f32(h, inv, b0, count, OUT, ldo); }
+    static lbfgs_b200_status factor_times(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, int k, const float* V, int64_t ldv, int64_t ldvp,
+                                          float* OUT, int64_t ldo, int64_t ldop)
+    { return lbfgs_b200_small_hist_factor_times_f32(h, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop); }
+    static lbfgs_b200_status sample(lbfgs_b200_small_hist* h, uint64_t seed, uint32_t first, int64_t b0, int64_t count, int k, const float* M,
+                                    int64_t ldm, float* OUT, int64_t ldo, int64_t ldop)
+    { return lbfgs_b200_small_hist_sample_f32(h, seed, first, b0, count, k, M, ldm, OUT, ldo, ldop); }
+    static lbfgs_b200_status logdet(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, double* out)
+    { return lbfgs_b200_small_hist_logdet_f32(h, b0, count, out); }
 };
 }  // namespace detail
 
@@ -151,6 +167,52 @@ public:
     void final_approx_hessian_diagonal(long b, Vector& OUT) { one_diagonal(b, OUT, false); }
     void final_approx_inverse_hessian_diagonal(long b, Vector& OUT) { one_diagonal(b, OUT, true); }
 
+    // N(x_b, H_b) for every kept problem without forming H_b (lbfgs_b200_small_hist_factor_times / _sample / _logdet, H_b = L_b L_b'):
+    // OUT = L_b V in the layouts of final_approx_inverse_hessian_times; OUT = X_b + L_b z_j for the k draws first .. first+k-1 of
+    // stream b (X holds the B means back to back; OUT is resized to B*k vectors, problem b's draw j at [(b*k + j)*n, ...)); log det H_b.
+    // One problem b alone: the same values.  A problem whose pairs fail the positive-curvature check gets NaN.
+    void final_approx_inverse_hessian_factor_times(const Vector& V, Vector& OUT)
+    {
+        require_kept();
+        const int k = all_count(V);
+        OUT.resize(V.size());
+        m_dev->check(detail::small_batch_abi<Scalar>::factor_times(m_hist, 0, int64_t(m_B), k, V.data(), int64_t(m_n), int64_t(k) * m_n, OUT.data(),
+                                                                   int64_t(m_n), int64_t(k) * m_n));
+    }
+    void final_approx_inverse_hessian_factor_times(long b, const Vector& V, Vector& OUT)
+    {
+        require_one(b);
+        const int k = BFGSMat<Scalar>::block_count(V.size(), m_n);
+        OUT.resize(V.size());
+        m_dev->check(detail::small_batch_abi<Scalar>::factor_times(m_hist, int64_t(b), 1, k, V.data(), int64_t(m_n), 0, OUT.data(), int64_t(m_n), 0));
+    }
+    void final_approx_sample(const Vector& X, unsigned long long seed, uint32_t first, int k, Vector& OUT)
+    {
+        require_kept();
+        if (X.size() != m_n * std::ptrdiff_t(m_B)) throw std::invalid_argument("X must hold B * n values");
+        draws(0, m_B, X.data(), seed, first, k, OUT);
+    }
+    void final_approx_sample(long b, const Vector& mean, unsigned long long seed, uint32_t first, int k, Vector& OUT)
+    {
+        require_one(b);
+        if (mean.size() != m_n) throw std::invalid_argument("mean must hold n values");
+        draws(b, 1, mean.data(), seed, first, k, OUT);
+    }
+    std::vector<double> final_approx_inverse_hessian_logdet()
+    {
+        require_kept();
+        std::vector<double> out(static_cast<size_t>(m_B));
+        m_dev->check(detail::small_batch_abi<Scalar>::logdet(m_hist, 0, int64_t(m_B), out.data()));
+        return out;
+    }
+    double final_approx_inverse_hessian_logdet(long b)
+    {
+        require_one(b);
+        double out = 0.0;
+        m_dev->check(detail::small_batch_abi<Scalar>::logdet(m_hist, int64_t(b), 1, &out));
+        return out;
+    }
+
 private:
     std::ptrdiff_t m_hist_n = 0;
     long m_hist_B = 0;
@@ -160,6 +222,25 @@ private:
     void require_kept() const
     {
         if (!m_kept) throw std::logic_error("LBFGSSmallBatchSolver: no final approximation kept (call keep_final_approx(true) before minimize())");
+    }
+    void require_one(long b) const
+    {
+        require_kept();
+        if (b < 0 || b >= m_B) throw std::invalid_argument("LBFGSSmallBatchSolver: problem index out of range");
+    }
+    int all_count(const Vector& V) const
+    {
+        const std::ptrdiff_t per = m_n * std::ptrdiff_t(m_B);
+        if (V.size() < 1 || V.size() % per != 0 || V.size() / per > std::numeric_limits<int>::max())
+            throw std::invalid_argument("V.size() must be a positive multiple of B * n");
+        return int(V.size() / per);
+    }
+    void draws(long b0, long count, const Scalar* mean, unsigned long long seed, uint32_t first, int k, Vector& OUT)
+    {
+        if (k < 1 || uint64_t(first) + uint64_t(k) > (uint64_t(1) << 32)) throw std::invalid_argument("need k >= 1 and first + k <= 2^32");
+        OUT.resize(m_n * std::ptrdiff_t(k) * std::ptrdiff_t(count));
+        m_dev->check(detail::small_batch_abi<Scalar>::sample(m_hist, seed, first, int64_t(b0), int64_t(count), k, mean, int64_t(m_n), OUT.data(),
+                                                             int64_t(m_n), int64_t(k) * m_n));
     }
     void all_times(const Vector& V, Vector& OUT, bool inverse)
     {

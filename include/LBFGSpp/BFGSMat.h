@@ -9,6 +9,8 @@
 #define LBFGSPP_B200_BFGS_MAT_H
 
 #include <algorithm>
+#include <cmath>
+#include <cstdint>
 #include <limits>
 #include <stdexcept>
 
@@ -344,7 +346,77 @@ public:
     void hessian_diagonal(Vector& out) { diagonal(out, false); }
     void inverse_hessian_diagonal(Vector& out) { diagonal(out, true); }
 
+    // A square-root factor of H and its log-determinant (CompactForm.h, compact_factor_setup / compact_factor_coef): H = L L' with
+    //   L = (I + s_{c-1} b_{c-1}') ... (I + s_0 b_0') / sqrt(theta),   log det H = -n log theta + sum_t log(rho_t s_t'B_t s_t)
+    // formed from the Gram blocks alone.  inverse_hessian_factor_times: OUT = L V for k vectors back to back, in groups of 16 through
+    // the k-vector passes (W'V, the algebra on the host, then the combination).  sample: OUT = mean + L z_j for the k draws
+    // first .. first+k-1 of stream `stream` (mean == nullptr: zero), z_j generated inside both passes and never stored
+    // (lbfgs_b200_hist_wt_dot_normal / lincomb_normal).  With c = 0: L = I/sqrt(theta).  Pairs without positive curvature
+    // (impossible after a solve, whose curvature gate refuses them): std::runtime_error, and NaN from inverse_hessian_logdet.
+    void inverse_hessian_factor_times(const Vector& V, int k, Vector& OUT) { factor(&V, nullptr, 0, 0, 0, k, OUT); }
+    void sample(const Vector* mean, unsigned long long seed, uint32_t stream, uint32_t first, int k, Vector& OUT)
+    {
+        if (mean && mean->size() != m_n) throw std::invalid_argument("mean must hold n values");
+        factor(nullptr, mean, seed, stream, first, k, OUT);
+    }
+    double inverse_hessian_logdet()
+    {
+        require_history();
+        std::vector<double> beta, Tm;
+        double ls = 0.0;
+        const Scalar theta = factor_setup(beta, Tm, ls);
+        return std::isnan(ls) ? ls : -double(m_n) * std::log(double(theta)) + ls;
+    }
+
 private:
+    // compact_factor_setup from the history's Gram blocks; ls = NaN when its check fails.  Returns theta.
+    Scalar factor_setup(std::vector<double>& beta, std::vector<double>& Tm, double& ls)
+    {
+        const int c = lbfgs_b200_hist_ncorr(m_hist);
+        const size_t cs = size_t(c > 0 ? c : 1);
+        std::vector<Scalar> SY(cs * cs), SS(cs * cs), YY(cs * cs);
+        Scalar theta = Scalar(1);
+        m_dev->check(detail::BoxAbi<Scalar>::hist_gram(m_hist, SY.data(), SS.data(), YY.data(), nullptr, &theta));
+        beta.assign(2 * cs * cs, 0.0);
+        Tm.assign(cs * cs, 0.0);
+        if (compact_factor_setup(c, SY.data(), SS.data(), YY.data(), c, theta, beta.data(), Tm.data(), &ls) != 0)
+            ls = std::numeric_limits<double>::quiet_NaN();
+        return theta;
+    }
+
+    void factor(const Vector* V, const Vector* mean, unsigned long long seed, uint32_t stream, uint32_t first, int k, Vector& OUT)
+    {
+        require_history();
+        if (V && block_count(V->size(), m_n) != k) throw std::invalid_argument("V.size() must be k * n");
+        if (!V && (k < 1 || uint64_t(first) + uint64_t(k) > (uint64_t(1) << 32))) throw std::invalid_argument("need k >= 1 and first + k <= 2^32");
+        std::vector<double> beta, Tm;
+        double ls = 0.0;
+        const Scalar theta = factor_setup(beta, Tm, ls);
+        if (std::isnan(ls)) throw std::runtime_error("BFGSMat: the kept pairs do not define a positive definite H");
+        const int c = lbfgs_b200_hist_ncorr(m_hist);
+        const double rsq = 1.0 / std::sqrt(double(theta));
+        OUT.resize(std::ptrdiff_t(k) * m_n);
+        const int kGroup = 16;
+        std::vector<Scalar> Wv, C;
+        for (int j0 = 0; j0 < k; j0 += kGroup)
+        {
+            const int kk = std::min(kGroup, k - j0);
+            const Scalar* v = V ? V->data() + std::ptrdiff_t(j0) * m_n : nullptr;
+            C.assign(size_t(2 * c * kk), Scalar(0));
+            if (c > 0)
+            {
+                Wv.assign(size_t(2 * c * kk), Scalar(0));
+                if (V) m_dev->check(detail::BoxAbi<Scalar>::hist_wt_dot_multi(m_hist, kk, v, m_n, Wv.data()));
+                else m_dev->check(detail::BoxAbi<Scalar>::hist_wt_dot_normal(m_hist, seed, stream, first + uint32_t(j0), kk, Wv.data()));
+                for (int j = 0; j < kk; j++) compact_factor_coef(c, beta.data(), Tm.data(), rsq, Wv.data() + j, kk, C.data() + j, kk);
+            }
+            Scalar* out = OUT.data() + std::ptrdiff_t(j0) * m_n;
+            if (V) m_dev->check(detail::BoxAbi<Scalar>::hist_lincomb_multi(m_hist, Scalar(rsq), kk, v, m_n, c > 0 ? C.data() : nullptr, out, m_n));
+            else m_dev->check(detail::BoxAbi<Scalar>::hist_lincomb_normal(m_hist, Scalar(rsq), seed, stream, first + uint32_t(j0), kk,
+                                                                          mean ? mean->data() : nullptr, c > 0 ? C.data() : nullptr, out, m_n));
+        }
+    }
+
     void diagonal(Vector& out, bool inverse)
     {
         require_history();

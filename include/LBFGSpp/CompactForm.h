@@ -240,6 +240,78 @@ LBFGS_HD inline void compact_k_symmetrise(int w, T* K, int i0, int di)
         }
 }
 
+// ---- a square-root factor of H: H = L L' (Brodlie-Gourlay-Greenstadt) ----------------------------------------------------------
+// Pairs in chronological order t = c - 1 - age, rho_t = 1/(y_t's_t), B_t the BFGS matrix after pairs 0..t-1 from theta I,
+// p_t = B_t s_t, sigma_t = s_t'p_t.  H_{t+1} = (I + s_t b_t') H_t (I + b_t s_t') with b_t = -rho_t y_t + sqrt(rho_t / sigma_t) p_t, so
+//     L = (I + s_{c-1} b_{c-1}') ... (I + s_0 b_0') / sqrt(theta),     log det H = -n log theta + sum_t log(rho_t sigma_t)
+// and 1 + b_t's_t = sqrt(rho_t sigma_t) > 0.  p_t lies in span(W), W = [Y S]:
+//     p_t = theta s_t + sum_{j<t} ( -p_j (p_j's_t) / sigma_j + rho_j y_j (y_j's_t) )
+// needs only Gram entries, so b_t = W beta_t with beta_t in R^2c.  L z = z/sqrt(theta) + sum_t alpha_t s_t with the unit lower
+// triangular recursion alpha_t = beta_t'(W'z)/sqrt(theta) + sum_{j<t} T(t, j) alpha_j, T(t, j) = beta_t'W's_j.
+//
+// compact_factor_setup: beta [2c][c] (row r in W's order: y by age, then s by age; column t chronological) and Tm [c][c]: T(t, j) in
+// its strictly lower part (Tm[t * c + j], j < t); its diagonal holds sigma_t and its upper part p_t's_u (u > t), the intermediates.
+// Everything is evaluated in fp64 whatever T is.  *logsum = sum_t log(rho_t sigma_t).  Returns 0, or 2 (NUMERICAL_ISSUE) when some
+// rho_t or sigma_t is not positive and finite (beta and Tm are then incomplete).  O(c^3).
+template <typename T>
+LBFGS_HD inline int compact_factor_setup(int c, const T* SY, const T* SS, const T* YY, int ldg, T theta, double* beta, double* Tm,
+                                         double* logsum)
+{
+    (void)YY;   // y'y never enters: b_t is tested against s columns only
+    const double th = double(theta), big = 1.7976931348623157e308;
+    auto sy = [&](int t, int u) { return double(SY[(c - 1 - t) * ldg + (c - 1 - u)]); };   // s_t'y_u, chronological
+    *logsum = 0.0;
+    for (int t = 0; t < c; t++)
+    {
+        // pi_t (the coefficients of p_t) in column t of beta
+        for (int r = 0; r < 2 * c; r++) beta[r * c + t] = 0.0;
+        beta[(2 * c - 1 - t) * c + t] = th;
+        for (int j = 0; j < t; j++)
+        {
+            const double f = -Tm[j * c + t] / Tm[j * c + j];
+            for (int r = 0; r < 2 * c; r++) beta[r * c + t] += f * beta[r * c + j];
+            beta[(c - 1 - j) * c + t] += sy(t, j) / sy(j, j);
+        }
+        // row t of Tm: s_u'p_t for every u
+        for (int u = 0; u < c; u++)
+        {
+            const int au = c - 1 - u;
+            double acc = 0.0;
+            for (int a = 0; a < c; a++) acc += beta[a * c + t] * double(SY[au * ldg + a]) + beta[(c + a) * c + t] * double(SS[au * ldg + a]);
+            Tm[t * c + u] = acc;
+        }
+        const double rho = 1.0 / sy(t, t), sigma = Tm[t * c + t];
+        if (!(rho > 0.0 && rho <= big && sigma > 0.0 && sigma <= big)) return 2;
+        *logsum += std::log(rho * sigma);
+    }
+    // beta_t = -rho_t e_{y_t} + kappa_t pi_t,  T(t, j) = -rho_t y_t's_j + kappa_t p_t's_j,  kappa_t = sqrt(rho_t / sigma_t)
+    for (int t = 0; t < c; t++)
+    {
+        const double rho = 1.0 / sy(t, t), kappa = std::sqrt(rho / Tm[t * c + t]);
+        for (int r = 0; r < 2 * c; r++) beta[r * c + t] *= kappa;
+        beta[(c - 1 - t) * c + t] -= rho;
+        for (int j = 0; j < t; j++) Tm[t * c + j] = kappa * Tm[t * c + j] - rho * sy(j, t);
+    }
+    return 0;
+}
+
+// L z for one vector from its dots wv[r * ldw] = (W'z)_r: C[r * ldc] in compact_b_coef's row order, the y rows zero and the s row of
+// age c - 1 - t holding alpha_t, so that L z = a0 z + sum_r C_r W_r with a0 = rsq = 1/sqrt(theta).  Sums in fp64; alpha_j is read back
+// from C (as T).
+template <typename T>
+LBFGS_HD inline void compact_factor_coef(int c, const double* beta, const double* Tm, double rsq, const T* wv, int ldw, T* C, int ldc)
+{
+    for (int a = 0; a < c; a++) C[a * ldc] = T(0);
+    for (int t = 0; t < c; t++)
+    {
+        double acc = 0.0;
+        for (int r = 0; r < 2 * c; r++) acc += beta[r * c + t] * double(wv[r * ldw]);
+        acc *= rsq;
+        for (int j = 0; j < t; j++) acc += Tm[t * c + j] * double(C[(2 * c - 1 - j) * ldc]);
+        C[(2 * c - 1 - t) * ldc] = T(acc);
+    }
+}
+
 }  // namespace LBFGSpp
 
 #endif  // LBFGSPP_B200_COMPACT_FORM_H

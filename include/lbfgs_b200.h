@@ -238,6 +238,17 @@ void* lbfgs_b200_box_vector(lbfgs_b200_box* b, int which);               /* LBFG
      * in fp64 in a fixed order (lbfgsb_kernels.cuh, k_hist_quad_diag), so out_i depends on row i and K only.  Any m; replicas \
      * only (a context with more than one rank is refused).  Entries of out past n are not written.                          */ \
     lbfgs_b200_status lbfgs_b200_hist_quad_diag_##SUF(lbfgs_b200_hist* h, T a0, const T* K_host, T* out);      \
+    /* The sampler of N(mean, H) (BFGSMat::sample): the two k-vector passes above with V = Z generated in the kernels, never   \
+     * stored, z_j = the standard normals of draw first + j of stream `stream` (Philox4x32-10, counter layout in              \
+     * csrc/philox.cuh; a draw depends on (seed, stream, j, i) only).  wt_dot_normal: R_host[2c][k] = [Y S]' Z in the order of  \
+     * hist_wt_dot_multi (column j of a call equals a k = 1 call with first + j).  lincomb_normal: OUT_j = mean + a0 z_j +      \
+     * sum_a C[c+a][j] s_a (C_host [2c][k] as hist_lincomb_multi takes it; its y rows are not read; mean may be NULL: zero).   \
+     * 1 <= k <= 16, first + k <= 2^32; replicas only.                                                                       */ \
+    lbfgs_b200_status lbfgs_b200_hist_wt_dot_normal_##SUF(lbfgs_b200_hist* h, uint64_t seed, uint32_t stream, uint32_t first, \
+                                                          int k, T* R_host);                                               \
+    lbfgs_b200_status lbfgs_b200_hist_lincomb_normal_##SUF(lbfgs_b200_hist* h, T a0, uint64_t seed, uint32_t stream,         \
+                                                           uint32_t first, int k, const T* mean, const T* C_host, T* OUT,   \
+                                                           int64_t ldo);                                                    \
     /* Cauchy.h:111-129: breakpoints, d = -g on movable coordinates, class bytes.                                      \
      * out5 = { #fixed, #never-bounded, #with a finite breakpoint, d.d, smallest breakpoint } */                       \
     lbfgs_b200_status lbfgs_b200_box_cauchy_breaks_##SUF(lbfgs_b200_box*, const T* x, const T* g, const T* lb, \
@@ -400,7 +411,19 @@ const void* lbfgs_b200_small_hist_y_col(const lbfgs_b200_small_hist* h, int64_t 
      * ldo < n, a problem range outside [0, B), a NULL OUT, a history no solve has filled or a context with more than one      \
      * rank.  Asynchronous.                                                                                                   */ \
     lbfgs_b200_status lbfgs_b200_small_hist_diag_##SUF(lbfgs_b200_small_hist* h, int inverse, int64_t b0, int64_t count, T* OUT,   \
-                                                       int64_t ldo);
+                                                       int64_t ldo);                                                              \
+    /* The square-root factor H_b = L_b L_b' of include/LBFGSpp/CompactForm.h (compact_factor_setup / compact_factor_coef), formed \
+     * on the chip per problem.  factor_times: OUT = L_b V in the layout of small_hist_times.  sample: OUT + p*ldop + j*ldo =    \
+     * MEAN + p*ldm + L_b z_j, z_j = draw first + j of stream b (the absolute problem index; philox.cuh), so a problem's draws do \
+     * not depend on b0 or count; MEAN may be NULL (zero).  The sampler uses OUT as scratch: with count > 1 it needs ldop >= k*ldo, and MEAN may not overlap OUT.  A problem whose pairs fail the check of compact_factor_setup gets NaN \
+     * outputs.  logdet: out_host[p] = log det H_b (NaN on that failure), synchronous.  Errors as small_hist_times.            */ \
+    lbfgs_b200_status lbfgs_b200_small_hist_factor_times_##SUF(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, int k,         \
+                                                               const T* V, int64_t ldv, int64_t ldvp, T* OUT, int64_t ldo,       \
+                                                               int64_t ldop);                                                    \
+    lbfgs_b200_status lbfgs_b200_small_hist_sample_##SUF(lbfgs_b200_small_hist* h, uint64_t seed, uint32_t first, int64_t b0,       \
+                                                         int64_t count, int k, const T* MEAN, int64_t ldm, T* OUT, int64_t ldo,  \
+                                                         int64_t ldop);                                                          \
+    lbfgs_b200_status lbfgs_b200_small_hist_logdet_##SUF(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, double* out_host);
 
 LBFGS_B200_DECLARE_SMALL_HIST(double, f64)
 LBFGS_B200_DECLARE_SMALL_HIST(float, f32)

@@ -135,6 +135,9 @@ def _declare(lib):
             getattr(lib, "lbfgs_b200_hist_lincomb_multi_" + suf).argtypes = [vp, ct, ci, vp, i64, pt, vp, i64]
         if hasattr(lib, "lbfgs_b200_hist_quad_diag_" + suf):      # the diagonal pass (a test double of the ABI may lack it)
             getattr(lib, "lbfgs_b200_hist_quad_diag_" + suf).argtypes = [vp, ct, pt, vp]
+        if hasattr(lib, "lbfgs_b200_hist_wt_dot_normal_" + suf):  # the sampler's passes (a test double of the ABI may lack them)
+            getattr(lib, "lbfgs_b200_hist_wt_dot_normal_" + suf).argtypes = [vp, C.c_uint64, C.c_uint32, C.c_uint32, ci, pt]
+            getattr(lib, "lbfgs_b200_hist_lincomb_normal_" + suf).argtypes = [vp, ct, C.c_uint64, C.c_uint32, C.c_uint32, ci, vp, pt, vp, i64]
         getattr(lib, "lbfgs_b200_box_cauchy_breaks_" + suf).argtypes = [vp, vp, vp, vp, vp, pt]
         getattr(lib, "lbfgs_b200_box_cauchy_sweep_" + suf).argtypes = [vp, vp, pt, pt, ct, ct, i64, i64, pt]
         getattr(lib, "lbfgs_b200_box_cauchy_build_" + suf).argtypes = [vp, vp, vp, vp, ct, ct, pt]
@@ -173,6 +176,10 @@ def _declare(lib):
             getattr(lib, "lbfgs_b200_small_hist_info_" + suf).argtypes = [vp, vp, vp]
             getattr(lib, "lbfgs_b200_small_hist_times_" + suf).argtypes = [vp, ci, i64, i64, ci, vp, i64, i64, vp, i64, i64]
             getattr(lib, "lbfgs_b200_small_hist_diag_" + suf).argtypes = [vp, ci, i64, i64, vp, i64]
+            if hasattr(lib, "lbfgs_b200_small_hist_sample_" + suf):
+                getattr(lib, "lbfgs_b200_small_hist_factor_times_" + suf).argtypes = [vp, i64, i64, ci, vp, i64, i64, vp, i64, i64]
+                getattr(lib, "lbfgs_b200_small_hist_sample_" + suf).argtypes = [vp, C.c_uint64, C.c_uint32, i64, i64, ci, vp, i64, vp, i64, i64]
+                getattr(lib, "lbfgs_b200_small_hist_logdet_" + suf).argtypes = [vp, i64, i64, C.POINTER(C.c_double)]
     lib._typed = True
     return lib
 
@@ -282,6 +289,16 @@ def _declare_driver(lib):
         for suf, pt in (("f64", dp), ("f32", fp)):
             getattr(lib, "lbfgsb200_drv_small_batch_hessian_diag_" + suf).argtypes = [ci, ci, cl, cl, pt, pt, pt, cl, ci, prm, pt, pt, pt,
                                                                                      C.POINTER(_SmallItem), err, errlen]
+    # N(x*, H) from the final approximation (csrc/driver_hessian_sample.cpp)
+    if hasattr(lib, "lbfgsb200_drv_solve_hessian_sample_f64"):
+        u64, u32 = C.c_uint64, C.c_uint32
+        lib.lbfgsb200_drv_solve_hessian_sample_f64.argtypes = [ci, ci, cl, ci, prm, ci, dp, ci, dp, dp, u64, u32, ci, dp, dp, C.POINTER(ci), err,
+                                                               errlen]
+        lib.lbfgsb200_drv_batch_hessian_sample_f64.argtypes = [ci, ci, cl, ci, dp, ci, prm, ci, ci, dp, dp, u64, u32, ci, dp, dp, dp, err, errlen]
+        lib.lbfgsb200_drv_hist_sample_f64.argtypes = [ci, cl, ci, ci, dp, dp, ci, dp, dp, dp, u64, u32, u32, ci, dp, dp, err, errlen]
+        for suf, pt in (("f64", dp), ("f32", fp)):
+            getattr(lib, "lbfgsb200_drv_small_batch_hessian_sample_" + suf).argtypes = [ci, ci, cl, cl, pt, pt, pt, cl, ci, prm, pt, ci, pt, pt, u64,
+                                                                                       u32, ci, pt, dp, C.POINTER(_SmallItem), err, errlen]
     lib._drv_typed = True
     return lib
 
@@ -638,6 +655,21 @@ class History:
         self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_hist_quad_diag_" + self.suf)(
             self.h, a0, Kc.ctypes.data_as(C.POINTER(self.ct)) if Kc.size else None, out.ptr))
 
+    def wt_dot_normal(self, seed, stream, first, k):
+        """[Y S]'Z for the draws first .. first+k-1 of stream `stream`, generated in the pass (lbfgs_b200_hist_wt_dot_normal): (2c, k)."""
+        c = self.ncorr
+        R = (self.ct * max(1, 2 * c * k))()
+        self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_hist_wt_dot_normal_" + self.suf)(self.h, seed, stream, first, k, R))
+        return np.array(R[:2 * c * k], dtype=self.dtype).reshape(2 * c, k)
+
+    def lincomb_normal(self, a0, seed, stream, first, k, mean, C_coef, OUT, ldo):
+        """OUT[:, j] = mean + a0 z_j + sum_a C[c + a, j] s_a, z_j generated in the pass (lbfgs_b200_hist_lincomb_normal); mean: a
+        DeviceArray or None."""
+        coef = np.ascontiguousarray(C_coef, dtype=self.dtype).reshape(-1)
+        self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_hist_lincomb_normal_" + self.suf)(
+            self.h, a0, seed, stream, first, k, mean.ptr if mean is not None else None,
+            coef.ctypes.data_as(C.POINTER(self.ct)) if coef.size else None, OUT.ptr, ldo))
+
     def column(self, which, age):
         fn = self.ctx.lib.lbfgs_b200_hist_s_col if which == "s" else self.ctx.lib.lbfgs_b200_hist_y_col
         p = fn(self.h, age)
@@ -898,6 +930,94 @@ def hist_diagonal(S, Y, m=None, device=0, lib=None):
     return dB, dH
 
 
+def solve_hessian_sample(objective, x0, V=None, seed=0, first=0, k=0, param=None, linesearch="NocedalWright", resident=True, device=0,
+                         lib=None):
+    """minimize(), then N(x*, H) from the final approximation (LBFGSSolver::final_approx_inverse_hessian_factor_times /
+    final_approx_sample / final_approx_inverse_hessian_logdet): L V for the rows of V (H = L L'), the k draws x* + L z_j,
+    j = first .. first+k-1 of stream 0, and log det H.  Returns (niter, x, LV, draws, logdet)."""
+    drv = driver(lib)
+    x = np.array(x0, dtype=np.float64, order="C").copy()
+    n = x.size
+    p = (param if param is not None else LBFGSParam())._c()
+    v = None if V is None else np.ascontiguousarray(V, dtype=np.float64).reshape(-1, n)
+    kv = 0 if v is None else v.shape[0]
+    LV = None if v is None else np.zeros_like(v)
+    D = np.zeros((k, n)) if k else None
+    ld, niter = C.c_double(0.0), C.c_int(0)
+    _checked("solve_hessian_sample", lambda *err: drv.lbfgsb200_drv_solve_hessian_sample_f64(
+        device, objective, n, _ls_id(linesearch), C.byref(p), int(resident), _ptr(x), kv, _ptr(v), _ptr(LV), seed, first, k, _ptr(D),
+        C.byref(ld), C.byref(niter), *err))
+    return niter.value, x, LV, D, ld.value
+
+
+def batch_hessian_sample(objective, X0, b, V=None, seed=0, first=0, k=0, param=None, linesearch="MoreThuente", device=0, lib=None):
+    """A batch (rows of X0) minimised by LBFGSBatchSolver, then problem b's L V, draws X_b + L z_j from stream b and log det H.
+    Returns (X, LV, draws, logdet)."""
+    drv = driver(lib)
+    X0 = np.ascontiguousarray(X0, dtype=np.float64)
+    B, n = X0.shape
+    p = (param if param is not None else LBFGSParam())._c()
+    v = None if V is None else np.ascontiguousarray(V, dtype=np.float64).reshape(-1, n)
+    kv = 0 if v is None else v.shape[0]
+    LV = None if v is None else np.zeros_like(v)
+    D = np.zeros((k, n)) if k else None
+    X = np.zeros_like(X0)
+    ld = C.c_double(0.0)
+    _checked("batch_hessian_sample", lambda *err: drv.lbfgsb200_drv_batch_hessian_sample_f64(
+        device, objective, n, B, _ptr(X0), _ls_id(linesearch), C.byref(p), b, kv, _ptr(v), _ptr(LV), seed, first, k, _ptr(D), C.byref(ld),
+        _ptr(X), *err))
+    return X, LV, D, ld.value
+
+
+def hist_sample(S, Y, m=None, V=None, mean=None, seed=0, stream=0, first=0, k=0, device=0, lib=None):
+    """BFGSMat's factor, sampler and log-determinant on the history built by adding the pairs (S[k], Y[k]) in order to a ring of size m
+    (default: all of them).  Returns (LV, draws, logdet)."""
+    drv = driver(lib)
+    S = np.ascontiguousarray(S, dtype=np.float64)
+    Y = np.ascontiguousarray(Y, dtype=np.float64)
+    npairs, n = S.shape
+    v = None if V is None else np.ascontiguousarray(V, dtype=np.float64).reshape(-1, n)
+    kv = 0 if v is None else v.shape[0]
+    LV = None if v is None else np.zeros_like(v)
+    mu = None if mean is None else np.ascontiguousarray(mean, dtype=np.float64)
+    D = np.zeros((k, n)) if k else None
+    ld = C.c_double(0.0)
+    _checked("hist_sample", lambda *err: drv.lbfgsb200_drv_hist_sample_f64(device, n, npairs if m is None else m, npairs, _ptr(S), _ptr(Y), kv,
+                                                                          _ptr(v), _ptr(LV), _ptr(mu), seed, stream, first, k, _ptr(D),
+                                                                          C.byref(ld), *err))
+    return LV, D, ld.value
+
+
+def small_batch_hessian_sample(objective, X0, V=None, seed=0, first=0, k=0, param=None, linesearch="MoreThuente", dtype=np.float64, data0=None,
+                               data1=None, ldd=0, device=0, lib=None):
+    """solve_small_batch with every problem's final approximation kept, then for all problems at once (LBFGSSmallBatchSolver):
+    L_b V_b (V: (B, kv, n)), the k draws X_b + L_b z_j from stream b, and log det H_b.  Returns (outcomes, X, LV, draws (B, k, n),
+    logdet (B,))."""
+    drv = driver(lib)
+    X0 = np.ascontiguousarray(X0, dtype=dtype)
+    B, n = X0.shape
+    p = (param if param is not None else LBFGSParam())._c()
+    d0 = None if data0 is None else np.ascontiguousarray(data0, dtype=dtype).reshape(-1)
+    d1 = None if data1 is None else np.ascontiguousarray(data1, dtype=dtype).reshape(-1)
+    v = None if V is None else np.ascontiguousarray(V, dtype=dtype).reshape(B, -1, n)
+    kv = 0 if v is None else v.shape[1]
+    LV = None if v is None else np.zeros_like(v)
+    D = np.zeros((B, k, n), dtype=dtype) if k else None
+    X = np.empty_like(X0)
+    ld = np.zeros(B)
+    items = (_SmallItem * B)()
+    suf = "f32" if np.dtype(dtype) == np.float32 else "f64"
+    err = C.create_string_buffer(256)
+    r = getattr(drv, "lbfgsb200_drv_small_batch_hessian_sample_" + suf)(device, objective, n, B, _ptr(X0), _ptr(d0), _ptr(d1), int(ldd),
+                                                                       _ls_id(linesearch), C.byref(p), _ptr(X), kv, _ptr(v), _ptr(LV), seed,
+                                                                       first, k, _ptr(D), _ptr(ld), items, err, len(err))
+    if r < 0:
+        raise (ValueError if r == -1 else RuntimeError)("small_batch_hessian_sample failed: %s" % err.value.decode())
+    res = [dict(status=STATUS_NAMES[it.kind], code=it.code, niter=it.niter, nfev=it.nfev, fx=it.fx, gnorm=it.gnorm, rounds=it.rounds)
+           for it in items]
+    return res, X, LV, D, ld
+
+
 def small_max_n(m, objective, dtype=np.float64):
     """Largest n of a problem the small-batch solve takes for history size m and built-in objective `objective` (0 if none)."""
     return int(abi().lbfgs_b200_small_max_n(int(m), np.dtype(dtype).itemsize, int(objective)))
@@ -1042,6 +1162,24 @@ class SmallHistory:
     def diagonal(self, inverse, b0, count, OUT, ldo):
         """lbfgs_b200_small_hist_diag_* into the DeviceArray OUT, problem b0 + p's diagonal at offset p*ldo (asynchronous)."""
         self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_small_hist_diag_" + self.suf)(self.h, int(inverse), b0, count, OUT.ptr, ldo))
+
+    def factor_times(self, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop):
+        """lbfgs_b200_small_hist_factor_times_*: OUT = L_b V with H_b = L_b L_b', on DeviceArrays (asynchronous)."""
+        self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_small_hist_factor_times_" + self.suf)(self.h, b0, count, k, V.ptr, ldv, ldvp, OUT.ptr,
+                                                                                                ldo, ldop))
+
+    def sample(self, seed, first, b0, count, k, MEAN, ldm, OUT, ldo, ldop):
+        """lbfgs_b200_small_hist_sample_*: OUT = MEAN_b + L_b z_j, z_j draw first + j of stream b; MEAN a DeviceArray or None."""
+        self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_small_hist_sample_" + self.suf)(
+            self.h, seed, first, b0, count, k, MEAN.ptr if MEAN is not None else None, ldm, OUT.ptr, ldo, ldop))
+
+    def logdet(self, b0=0, count=None):
+        """lbfgs_b200_small_hist_logdet_*: log det H_b for problems b0 .. b0+count-1 (NaN where the pairs fail the check)."""
+        count = self.B - b0 if count is None else count
+        out = np.zeros(count)
+        self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_small_hist_logdet_" + self.suf)(self.h, b0, count,
+                                                                                          out.ctypes.data_as(C.POINTER(C.c_double))))
+        return out
 
 
 def phase_clock(on=True):

@@ -63,7 +63,8 @@ def build_kernels(force=False, verbose=False):
     return LIB
 
 
-DRIVER_UNITS = ["driver.cpp", "driver_hessian_ops.cpp", "driver_small_batch.cpp", "driver_hessian_diag.cpp"]   # g++ units of the driver library
+DRIVER_UNITS = ["driver.cpp", "driver_hessian_ops.cpp", "driver_small_batch.cpp", "driver_hessian_diag.cpp",
+               "driver_hessian_sample.cpp"]   # g++ units of the driver library
 
 
 def build_driver(force=False):

@@ -37,7 +37,7 @@ namespace lbfgsb200_drv {
 // B problems (rows of x0s_host, n each) minimised by LBFGSSmallBatchSolver; data0/data1 (optional, host) per problem at data + b*ldd
 // (ldd = 0: shared).  xs_out / gs_out (optional): solutions and final gradients.  Returns the number of problems that did not end
 // cleanly, -1 (err holds the message) when the call was refused as an invalid argument, -2 on any other failure.
-// `after(solver, dev)` (optional) runs on the solver once minimize() has returned; `keep`: minimize() keeps the final approximations
+// `after(solver, dev)` or `after(solver, dev, X)` (optional, X: the solutions on the device) runs on the solver once minimize() has returned; `keep`: minimize() keeps the final approximations
 template <class Scalar, class After = std::nullptr_t>
 int small_batch(int device_ordinal, int objective, long n, long B, const Scalar* x0s_host, const Scalar* data0_host, const Scalar* data1_host,
                 long ldd, int ls, const drv_param* q, Scalar* xs_out, Scalar* gs_out, drv_small_item* items, char* err, int errlen,
@@ -73,7 +73,8 @@ int small_batch(int device_ordinal, int objective, long n, long B, const Scalar*
                 }
                 if (gs_out)
                     dev.check(lbfgs_b200_memcpy_d2h(dev.ctx(), gs_out, solver.final_grad(0), sizeof(Scalar) * size_t(n) * size_t(B)));
-                if constexpr (!std::is_same_v<After, std::nullptr_t>) after(solver, dev);
+                if constexpr (std::is_invocable_v<After&, decltype(solver)&, Device&, DeviceVector<Scalar>&>) after(solver, dev, X);
+                else if constexpr (!std::is_same_v<After, std::nullptr_t>) after(solver, dev);
             });
             if (xs_out) X.copy_to_host(xs_out);
             return bad;

@@ -202,6 +202,71 @@ static lbfgs_b200_status do_hist_lincomb_multi(lbfgs_b200_hist* h, T a0, int k, 
     return launch_lincomb<T>(h, a0, k, V, ldv, static_cast<const T*>(coef), nullptr, 0, OUT, ldo);
 }
 
+// The sampler's two passes: the k-vector passes above with the vectors generated in the kernels (philox.cuh), draws first .. first+k-1
+template <class T> static lbfgs_b200_status normal_check(lbfgs_b200_hist* h, int k, uint32_t first, const char* what)
+{
+    if (auto st = multi_check<T>(h, k, h ? h->n : 0, what)) return st;
+    REQUIRE(h->ctx, (uint64_t)first + (uint64_t)k <= 0x100000000ull, "%s: draws %u + %d run past 2^32", what, first, k);
+    return LBFGS_B200_OK;
+}
+
+template <class T>
+static lbfgs_b200_status do_hist_wt_dot_normal(lbfgs_b200_hist* h, uint64_t seed, uint32_t stream, uint32_t first, int k, T* R_host)
+{
+    if (auto st = normal_check<T>(h, k, first, "hist_wt_dot_normal")) return st;
+    lbfgs_b200_ctx* ctx = h->ctx;
+    REQUIRE(ctx, R_host, "hist_wt_dot_normal: NULL argument");
+    const int c = h->ncorr, w = 2 * c;
+    if (c == 0) return LBFGS_B200_OK;
+    double *partials, *result;
+    void* coef;
+    if (auto st = multi_scratch(h, &partials, &result, &coef)) return st;
+    WtDotNormalArgs<T> a{};
+    a.n = h->n; a.ld = h->ld; a.ldv = 0; a.S = static_cast<const T*>(h->S); a.Y = static_cast<const T*>(h->Y); a.V = nullptr;
+    a.c = c; a.k = k; a.partials = partials; a.ticket = ctx->rb.ticket; a.result = result;
+    a.src = NormalSrc{(unsigned long long)seed, stream, first};
+    fill_slots<T>(h, a.slots);
+    auto kernel = k_hist_wt_dot_multi<T, WtDotNormalArgs<T>>;
+    const size_t smem = (size_t)(w + k) * kWtPitch * sizeof(T);
+    if (smem > 48 * 1024) CU(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<wt_multi_grid(h), kThreads, smem, ctx->stream>>>(a);
+    if (auto st = post_launch(ctx, "k_hist_wt_dot_normal")) return st;
+    std::vector<double> tmp((size_t)w * k);
+    CU(ctx, cudaMemcpyAsync(tmp.data(), result, sizeof(double) * w * k, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(ctx, cudaStreamSynchronize(ctx->stream));
+    for (int e = 0; e < w * k; e++) R_host[e] = (T)tmp[(size_t)e];
+    return LBFGS_B200_OK;
+}
+
+template <class T>
+static lbfgs_b200_status do_hist_lincomb_normal(lbfgs_b200_hist* h, T a0, uint64_t seed, uint32_t stream, uint32_t first, int k, const T* mean,
+                                                const T* C_host, T* OUT, int64_t ldo)
+{
+    if (auto st = normal_check<T>(h, k, first, "hist_lincomb_normal")) return st;
+    lbfgs_b200_ctx* ctx = h->ctx;
+    REQUIRE(ctx, OUT, "hist_lincomb_normal: NULL argument");
+    REQUIRE(ctx, ldo >= h->n, "hist_lincomb_normal: leading dimension %lld is smaller than n = %lld", (long long)ldo, (long long)h->n);
+    const int c = h->ncorr;
+    double *partials, *result;
+    void* coef;
+    if (auto st = multi_scratch(h, &partials, &result, &coef)) return st;
+    if (c > 0)
+    {
+        REQUIRE(ctx, C_host != nullptr, "hist_lincomb_normal: NULL argument");
+        CU(ctx, cudaMemcpyAsync(coef, C_host, sizeof(T) * 2 * c * k, cudaMemcpyHostToDevice, ctx->stream));
+        CU(ctx, cudaStreamSynchronize(ctx->stream));   // C_host may be a stack array of the caller
+    }
+    LincombNormalArgs<T> a{};
+    a.n = h->n; a.ld = h->ld; a.ldv = 0; a.ldo = ldo; a.S = static_cast<const T*>(h->S); a.Y = static_cast<const T*>(h->Y);
+    a.V = nullptr; a.a0 = a0; a.coef = static_cast<const T*>(coef); a.cls = nullptr; a.mask = 0; a.out = OUT; a.c = c; a.k = k;
+    a.mean = mean; a.src = NormalSrc{(unsigned long long)seed, stream, first};
+    fill_slots<T>(h, a.slots);
+    const int64_t npairs = (h->n + 1) / 2;
+    if (k == 1) k_hist_lincomb<T, 1, LincombNormalArgs<T>><<<grid_for(ctx, npairs * 4, 4), kThreads, 0, ctx->stream>>>(a);
+    else k_hist_lincomb<T, kMaxK, LincombNormalArgs<T>><<<grid_for(ctx, npairs * 4, 4), kThreads, 0, ctx->stream>>>(a);
+    return post_launch(ctx, "k_hist_lincomb_normal");
+}
+
 // out_i = a0 + r_i' K r_i (see k_hist_quad_diag): K's upper triangle is packed, off-diagonal entries doubled, on the host (exact
 // in binary floating point), and the kernel's width is chosen from c alone, so a row's arithmetic depends on c, K and the row only
 template <class T> static lbfgs_b200_status do_hist_quad_diag(lbfgs_b200_hist* h, T a0, const T* K_host, T* out)
@@ -545,6 +610,13 @@ void* lbfgs_b200_box_vector(lbfgs_b200_box* b, int which)
     { return do_hist_lincomb_multi<T>(h, a0, k, V, ldv, C_host, OUT, ldo); }                                                \
     lbfgs_b200_status lbfgs_b200_hist_quad_diag_##SUF(lbfgs_b200_hist* h, T a0, const T* K_host, T* out)                    \
     { return do_hist_quad_diag<T>(h, a0, K_host, out); }                                                                    \
+    lbfgs_b200_status lbfgs_b200_hist_wt_dot_normal_##SUF(lbfgs_b200_hist* h, uint64_t seed, uint32_t stream, uint32_t first,  \
+                                                          int k, T* R_host)                                                 \
+    { return do_hist_wt_dot_normal<T>(h, seed, stream, first, k, R_host); }                                                  \
+    lbfgs_b200_status lbfgs_b200_hist_lincomb_normal_##SUF(lbfgs_b200_hist* h, T a0, uint64_t seed, uint32_t stream,          \
+                                                           uint32_t first, int k, const T* mean, const T* C_host, T* OUT,    \
+                                                           int64_t ldo)                                                      \
+    { return do_hist_lincomb_normal<T>(h, a0, seed, stream, first, k, mean, C_host, OUT, ldo); }                            \
     lbfgs_b200_status lbfgs_b200_box_cauchy_breaks_##SUF(lbfgs_b200_box* b, const T* x, const T* g, const T* lb,            \
                                                          const T* ub, T* out5_host)                                         \
     { return do_box_cauchy_breaks<T>(b, x, g, lb, ub, out5_host); }                                                         \

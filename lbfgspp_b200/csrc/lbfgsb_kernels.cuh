@@ -17,6 +17,7 @@
 
 #include "device_utils.cuh"
 #include "two_loop_gram.cuh"
+#include "philox.cuh"
 
 namespace lb {
 
@@ -498,9 +499,71 @@ template <class T> struct LincombArgs
     unsigned char slots[kMaxM];
 };
 
-// KMAX: 1 (the L-BFGS-B pass) or kMaxK; the k running sums of an element stay in registers
-template <class T, int KMAX> __global__ void __launch_bounds__(kThreads) k_hist_lincomb(LincombArgs<T> a)
+// The sampler's form (LincombNormalArgs): V is not read but generated, z_j = the normals of draw first + j (philox.cuh), and
+// OUT[:,j] = mean + a0*z_j + sum_a C[c+a][j]*s_a (mean == nullptr: no mean term; the y rows of C are not read, they are zero).  A
+// thread takes the coordinate pair (2q, 2q + 1) that one generator call serves; per element the terms are added in the order
+// mean, a0*z, s by age.
+template <class T> struct LincombNormalArgs : LincombArgs<T>
 {
+    const T* mean;
+    NormalSrc src;
+};
+
+template <class T, int KMAX> __device__ __forceinline__ void k_hist_lincomb_normal(const LincombNormalArgs<T>& a)
+{
+    __shared__ T s_coef[kMaxW * KMAX];
+    __shared__ const T* s_s[kMaxM];
+    const int k = KMAX == 1 ? 1 : a.k;
+    for (int e = threadIdx.x; e < 2 * a.c * k; e += kThreads) s_coef[e] = a.coef[e];
+    for (int j = threadIdx.x; j < a.c; j += kThreads) s_s[j] = a.S + (int64_t)a.slots[j] * a.ld;
+    __syncthreads();
+    const int64_t npairs = (a.n + 1) / 2;
+    for (int64_t q = (int64_t)blockIdx.x * kThreads + threadIdx.x; q < npairs; q += (int64_t)gridDim.x * kThreads)
+    {
+        const int64_t i0 = 2 * q;
+        const bool two = i0 + 1 < a.n;
+        const T m0 = a.mean ? a.mean[i0] : T(0), m1 = a.mean && two ? a.mean[i0 + 1] : T(0);
+        T r0[KMAX], r1[KMAX];
+#pragma unroll
+        for (int j = 0; j < KMAX; j++)
+            if (j < k)
+            {
+                double z0, z1;
+                normal_pair(a.src.seed, a.src.stream, a.src.first + (uint32_t)j, (unsigned long long)q, z0, z1);
+                r0[j] = a.mean ? m0 + a.a0 * (T)z0 : a.a0 * (T)z0;
+                r1[j] = a.mean ? m1 + a.a0 * (T)z1 : a.a0 * (T)z1;
+            }
+        for (int p = 0; p < a.c; p++)
+        {
+            const T s0 = s_s[p][i0], s1 = two ? s_s[p][i0 + 1] : T(0);
+#pragma unroll
+            for (int j = 0; j < KMAX; j++)
+                if (j < k)
+                {
+                    r0[j] += s_coef[(a.c + p) * k + j] * s0;
+                    r1[j] += s_coef[(a.c + p) * k + j] * s1;
+                }
+        }
+#pragma unroll
+        for (int j = 0; j < KMAX; j++)
+            if (j < k)
+            {
+                a.out[j * a.ldo + i0] = r0[j];
+                if (two) a.out[j * a.ldo + i0 + 1] = r1[j];
+            }
+    }
+}
+
+// KMAX: 1 (the L-BFGS-B pass) or kMaxK; the k running sums of an element stay in registers
+template <class T, int KMAX, class A = LincombArgs<T>> __global__ void __launch_bounds__(kThreads) k_hist_lincomb(A a)
+{
+    if constexpr (!std::is_same<A, LincombArgs<T>>::value)
+    {
+        k_hist_lincomb_normal<T, KMAX>(a);
+        return;
+    }
+    else
+    {
     __shared__ T s_coef[kMaxW * KMAX];
     __shared__ const T* s_y[kMaxM];
     __shared__ const T* s_s[kMaxM];
@@ -536,6 +599,7 @@ template <class T, int KMAX> __global__ void __launch_bounds__(kThreads) k_hist_
 #pragma unroll
         for (int j = 0; j < KMAX; j++)
             if (j < k) a.out[j * a.ldo + i] = r[j];
+    }
     }
 }
 
@@ -639,14 +703,23 @@ template <class T> struct WtDotMultiArgs
     unsigned char slots[kMaxM];
 };
 
-template <class T> __global__ void __launch_bounds__(kThreads) k_hist_wt_dot_multi(WtDotMultiArgs<T> a)
+// The sampler's form (WtDotNormalArgs): the k vectors are not read but generated, vector j = the normals of draw first + j
+// (philox.cuh), staged into the same strip rows as loaded vectors, so every dot keeps the order above.
+template <class T> struct WtDotNormalArgs : WtDotMultiArgs<T>
 {
+    NormalSrc src;
+};
+
+template <class T, class A = WtDotMultiArgs<T>> __global__ void __launch_bounds__(kThreads) k_hist_wt_dot_multi(A a)
+{
+    constexpr bool kGen = !std::is_same<A, WtDotMultiArgs<T>>::value;
     extern __shared__ __align__(16) unsigned char wt_smem[];
     T* rows = reinterpret_cast<T*>(wt_smem);   // [2c + k][kWtPitch]: y by age, s by age, then the k vectors
     __shared__ const T* s_col[kMaxW + kMaxK];
     __shared__ bool s_last;
     const int w = 2 * a.c, k = a.k, nrows = w + k, tid = threadIdx.x;
-    for (int q = tid; q < nrows; q += kThreads)
+    const int nload = kGen ? w : nrows;   // rows staged from memory
+    for (int q = tid; q < nload; q += kThreads)
         s_col[q] = q < a.c ? a.Y + (int64_t)a.slots[q] * a.ld : q < w ? a.S + (int64_t)a.slots[q - a.c] * a.ld : a.V + (int64_t)(q - w) * a.ldv;
     const int groups = kThreads / k, j = tid % k, g = tid / k;
     const bool active = g < groups;
@@ -659,12 +732,22 @@ template <class T> __global__ void __launch_bounds__(kThreads) k_hist_wt_dot_mul
     for (int64_t strip = blockIdx.x; strip < nstrips; strip += gridDim.x)
     {
         const int64_t r0 = strip * kWtRows;
-        for (int t = tid; t < nrows * kWtRows; t += kThreads)
+        for (int t = tid; t < nload * kWtRows; t += kThreads)
         {
             const int q = t / kWtRows, r = t % kWtRows;
             const int64_t i = r0 + r;
             rows[q * kWtPitch + r] = i < a.n ? __ldcs(s_col[q] + i) : T(0);
         }
+        if constexpr (kGen)
+            for (int t = tid; t < k * (kWtRows / 2); t += kThreads)   // one generator call per coordinate pair (r0 is even)
+            {
+                const int jv = t / (kWtRows / 2), r = 2 * (t % (kWtRows / 2));
+                const int64_t i = r0 + r;
+                double z0, z1;
+                normal_pair(a.src.seed, a.src.stream, a.src.first + (uint32_t)jv, (unsigned long long)(i / 2), z0, z1);
+                rows[(w + jv) * kWtPitch + r] = i < a.n ? (T)z0 : T(0);
+                rows[(w + jv) * kWtPitch + r + 1] = i + 1 < a.n ? (T)z1 : T(0);
+            }
         __syncthreads();
         if (active)
         {

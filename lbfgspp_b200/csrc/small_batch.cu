@@ -179,6 +179,75 @@ lbfgs_b200_status small_hist_diag(lbfgs_b200_small_hist* h, int inverse, int64_t
     return LBFGS_B200_OK;
 }
 
+template <class T>
+lbfgs_b200_status small_hist_factor(lbfgs_b200_small_hist* h, bool gen, uint64_t seed, uint32_t first, int64_t b0, int64_t count, int k,
+                                    const T* V, int64_t ldv, int64_t ldvp, T* OUT, int64_t ldo, int64_t ldop)
+{
+    using namespace lb;
+    const char* what = gen ? "small_hist_sample" : "small_hist_factor_times";
+    if (auto st = small_hist_check<T>(h, what)) return st;
+    lbfgs_b200_ctx* ctx = h->ctx;
+    const int64_t n = h->n;
+    REQUIRE(ctx, OUT && (gen || V), "%s: NULL argument", what);
+    REQUIRE(ctx, k >= 1 && (k + kSGroup - 1) / kSGroup <= 65535, "%s: k must be in 1..%d (got %d)", what, 65535 * kSGroup, k);
+    REQUIRE(ctx, !gen || (uint64_t)first + (uint64_t)k <= 0x100000000ull, "%s: draws %u + %d run past 2^32", what, first, k);
+    REQUIRE(ctx, b0 >= 0 && count >= 1 && count <= h->B - b0, "%s: problems [%lld, %lld) are not within the %lld of the history", what,
+            (long long)b0, (long long)(b0 + count), (long long)h->B);
+    REQUIRE(ctx, (gen || ldv >= n) && ldo >= n, "%s: leading dimensions ldv = %lld, ldo = %lld must be at least n = %lld", what,
+            (long long)ldv, (long long)ldo, (long long)n);
+    REQUIRE(ctx, ldvp >= 0 && ldop >= 0, "%s: negative problem stride", what);
+    REQUIRE(ctx, gen || (const void*)V != (const void*)OUT || (ldo == ldv && ldop == ldvp && (ldvp > 0 || count == 1)),
+            "%s: OUT may be V only with the same layout (ldo == ldv, ldop == ldvp) and vectors of its own per problem", what);
+    // the sampler writes its draws into OUT and reads them back: problems' output ranges must not overlap, nor may MEAN lie in OUT
+    REQUIRE(ctx, !gen || count == 1 || ldop >= (int64_t)k * ldo, "%s: problems' draws overlap (ldop = %lld < k * ldo = %lld)", what,
+            (long long)ldop, (long long)k * ldo);
+    if (gen && V)
+    {
+        const T* out_end = OUT + (count - 1) * ldop + (int64_t)(k - 1) * ldo + n;
+        const T* mean_end = V + (count - 1) * ldvp + n;
+        REQUIRE(ctx, mean_end <= OUT || out_end <= V, "%s: MEAN overlaps OUT", what);
+    }
+    REQUIRE(ctx, ctx->nranks == 1, "%s: one CTA holds a whole problem, so n cannot be sharded (the context has %d ranks)", what, ctx->nranks);
+    SmallFactorArgs<T> a{};
+    a.hist = static_cast<const T*>(h->data); a.hist_c = h->counts; a.HL = SmallHistLayout{n, h->m};
+    a.b0 = b0; a.k = k; a.V = V; a.ldv = ldv; a.ldvp = ldvp; a.OUT = OUT; a.ldo = ldo; a.ldop = ldop; a.seed = seed; a.first = first;
+    const size_t smem = small_factor_smem(h->m, (int)sizeof(T));
+    auto kernel = gen ? k_small_hist_factor<T, true> : k_small_hist_factor<T, false>;
+    CU(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<dim3((unsigned)count, (unsigned)((k + kSGroup - 1) / kSGroup)), small_threads(n), smem, ctx->stream>>>(a);
+    CU(ctx, cudaGetLastError());
+    ctx->launches++;
+    return LBFGS_B200_OK;
+}
+
+template <class T> lbfgs_b200_status small_hist_logdet(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, double* out_host)
+{
+    using namespace lb;
+    if (auto st = small_hist_check<T>(h, "small_hist_logdet")) return st;
+    lbfgs_b200_ctx* ctx = h->ctx;
+    REQUIRE(ctx, out_host, "small_hist_logdet: NULL argument");
+    REQUIRE(ctx, b0 >= 0 && count >= 1 && count <= h->B - b0, "small_hist_logdet: problems [%lld, %lld) are not within the %lld of the history",
+            (long long)b0, (long long)(b0 + count), (long long)h->B);
+    REQUIRE(ctx, ctx->nranks == 1, "small_hist_logdet: a context with %d ranks", ctx->nranks);
+    double* d = nullptr;
+    cudaError_t e = pool_alloc(ctx, reinterpret_cast<void**>(&d), sizeof(double) * (size_t)count);
+    if (e != cudaSuccess)
+        return fail(ctx, e == cudaErrorMemoryAllocation ? LBFGS_B200_ERR_ALLOC : LBFGS_B200_ERR_CUDA, "small_hist_logdet: %s", cudaGetErrorString(e));
+    const size_t smem = sizeof(double) * 3 * (size_t)h->m * h->m;
+    e = cudaFuncSetAttribute(k_small_hist_logdet<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess)
+    {
+        k_small_hist_logdet<T><<<(unsigned)count, 32, smem, ctx->stream>>>(static_cast<const T*>(h->data), h->counts, SmallHistLayout{h->n, h->m}, b0, d);
+        e = cudaGetLastError();
+        ctx->launches++;
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(out_host, d, sizeof(double) * (size_t)count, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    pool_free(ctx, d);
+    CU(ctx, e);
+    return LBFGS_B200_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -250,7 +319,17 @@ const void* lbfgs_b200_small_hist_y_col(const lbfgs_b200_small_hist* h, int64_t 
     { return small_hist_times<T>(h, inverse, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop); }                                      \
     lbfgs_b200_status lbfgs_b200_small_hist_diag_##SUF(lbfgs_b200_small_hist* h, int inverse, int64_t b0, int64_t count, T* OUT,    \
                                                        int64_t ldo)                                                                \
-    { return small_hist_diag<T>(h, inverse, b0, count, OUT, ldo); }
+    { return small_hist_diag<T>(h, inverse, b0, count, OUT, ldo); }                                                            \
+    lbfgs_b200_status lbfgs_b200_small_hist_factor_times_##SUF(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, int k,         \
+                                                               const T* V, int64_t ldv, int64_t ldvp, T* OUT, int64_t ldo,       \
+                                                               int64_t ldop)                                                     \
+    { return small_hist_factor<T>(h, false, 0, 0, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop); }                                  \
+    lbfgs_b200_status lbfgs_b200_small_hist_sample_##SUF(lbfgs_b200_small_hist* h, uint64_t seed, uint32_t first, int64_t b0,       \
+                                                         int64_t count, int k, const T* MEAN, int64_t ldm, T* OUT, int64_t ldo,  \
+                                                         int64_t ldop)                                                           \
+    { return small_hist_factor<T>(h, true, seed, first, b0, count, k, MEAN, 0, ldm, OUT, ldo, ldop); }                            \
+    lbfgs_b200_status lbfgs_b200_small_hist_logdet_##SUF(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, double* out_host)    \
+    { return small_hist_logdet<T>(h, b0, count, out_host); }
 
 LBFGS_B200_SMALL_KEEP(double, f64)
 LBFGS_B200_SMALL_KEEP(float, f32)

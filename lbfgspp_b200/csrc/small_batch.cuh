@@ -31,6 +31,7 @@
 
 #include "../../include/LBFGSpp/CompactForm.h"
 #include "problem_machine.cuh"
+#include "philox.cuh"
 
 namespace lb {
 
@@ -685,6 +686,150 @@ __global__ void __launch_bounds__(kSMaxThreads) k_small_hist_diag(const SmallDia
         }
         out[i] = (T)(a0 + acc);
     }
+}
+
+
+// ---- the square-root factor of the kept H_b: OUT = L_b V (factor_times) or MEAN + L_b Z (sample) -----------------------------------
+// One CTA per (problem, group of <= kSGroup vectors or draws), small_threads(n) threads, the shape of k_small_hist_times: [Y S]'V in
+// fp64 through the same block sums, the algebra of CompactForm.h on the chip (compact_factor_setup by thread 0, then
+// compact_factor_coef, one thread per vector) and the combination L v = v/sqrt(theta) + sum_a alpha_a s_a (terms a0 v, then s by age;
+// the sampler adds the mean first).  GEN: the vectors are draws first + j0 + j of stream b (philox.cuh), generated once into OUT
+// (one generator call per coordinate pair) and read back from there, each element by the thread that overwrites it.  Nothing depends
+// on b0, count or the problem's position.  A problem whose pairs fail compact_factor_setup's check gets NaN.
+template <class T> struct SmallFactorArgs
+{
+    const T* hist;              // records of SmallHistLayout
+    const int* hist_c;
+    SmallHistLayout HL;
+    int64_t b0;
+    int k;
+    const T* V;                 // loaded: problem p's vector j at V + p*ldvp + j*ldv;  GEN: the mean of problem p at V + p*ldvp (or NULL)
+    int64_t ldv, ldvp;
+    T* OUT;                     // at OUT + p*ldop + j*ldo
+    int64_t ldo, ldop;
+    unsigned long long seed;
+    uint32_t first;
+};
+
+// dynamic shared memory of k_small_hist_factor (bytes): block sums, [Y S]'V and the coefficients (2m x kSGroup each, as
+// small_times_smem), then beta (2m x m) and Tm (m x m) in double: never more than small_times_smem
+inline size_t small_factor_smem(int m, int elem)
+{
+    return sizeof(double) * (size_t)kSMaxWarps * kSGroup + (size_t)elem * 4 * (size_t)m * kSGroup + sizeof(double) * 3 * (size_t)m * m;
+}
+
+template <class T, bool GEN>
+__global__ void __launch_bounds__(kSMaxThreads) k_small_hist_factor(const SmallFactorArgs<T> a)
+{
+    extern __shared__ __align__(16) unsigned char s_smem[];
+    __shared__ int s_ok;
+    const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5;
+    const int64_t p = blockIdx.x, b = a.b0 + p, n = a.HL.n;
+    const int m = a.HL.m, j0 = blockIdx.y * kSGroup, kk = min(kSGroup, a.k - j0);
+    const T* rec = a.hist + b * a.HL.rec();
+    T* OUT = a.OUT + p * a.ldop + j0 * a.ldo;
+    const T* V = GEN ? OUT : a.V + p * a.ldvp + j0 * a.ldv;
+    const int64_t ldv = GEN ? a.ldo : a.ldv;
+    const T* mean = GEN && a.V ? a.V + p * a.ldvp : nullptr;
+    const int c = a.hist_c[b];
+    const T theta = rec[a.HL.theta()];
+    const double rsq = 1.0 / sqrt((double)theta);
+    const T a0 = (T)rsq;
+    double* red = reinterpret_cast<double*>(s_smem);
+    T* wv = reinterpret_cast<T*>(red + kSMaxWarps * kSGroup);        // [2c][kSGroup]
+    T* C = wv + 2 * m * kSGroup;                                     // [2c][kSGroup]
+    double* beta = reinterpret_cast<double*>(C + 2 * m * kSGroup);   // [2c][c]
+    double* Tm = beta + 2 * m * m;                                   // [c][c]
+    if (GEN)
+    {
+        for (int64_t q = tid; 2 * q < n; q += nt)
+#pragma unroll
+            for (int j = 0; j < kSGroup; j++)
+                if (j < kk)
+                {
+                    double z0, z1;
+                    normal_pair(a.seed, (uint32_t)b, a.first + (uint32_t)(j0 + j), (unsigned long long)q, z0, z1);
+                    OUT[j * a.ldo + 2 * q] = (T)z0;
+                    if (2 * q + 1 < n) OUT[j * a.ldo + 2 * q + 1] = (T)z1;
+                }
+        __syncthreads();
+    }
+    bool ok = true;
+    if (c > 0)
+    {
+        // [Y S]'V, one history row at a time (the sums of k_small_hist_times)
+        for (int r = 0; r < 2 * c; r++)
+        {
+            const T* h = rec + (r < c ? a.HL.y(r) : a.HL.s(r - c));
+            double acc[kSGroup];
+#pragma unroll
+            for (int j = 0; j < kSGroup; j++) acc[j] = 0.0;
+            for (int64_t i = tid; i < n; i += nt)
+            {
+                const double hv = (double)h[i];
+#pragma unroll
+                for (int j = 0; j < kSGroup; j++)
+                    if (j < kk) acc[j] += hv * (double)V[j * ldv + i];
+            }
+#pragma unroll
+            for (int j = 0; j < kSGroup; j++)
+            {
+                const double w = warp_sum(acc[j]);
+                if (lane == 0) red[warp * kSGroup + j] = w;
+            }
+            __syncthreads();
+            if (tid < kk)
+            {
+                double t = 0.0;
+                for (int w = 0; w < (nt >> 5); w++) t += red[w * kSGroup + tid];
+                wv[r * kSGroup + tid] = (T)t;
+            }
+            __syncthreads();
+        }
+        if (tid == 0)
+        {
+            double ls;
+            s_ok = LBFGSpp::compact_factor_setup(c, rec + a.HL.SY(), rec + a.HL.SS(), rec + a.HL.YY(), c, theta, beta, Tm, &ls) == 0;
+        }
+        __syncthreads();
+        ok = s_ok != 0;
+        if (ok && tid < kk) LBFGSpp::compact_factor_coef(c, beta, Tm, rsq, wv + tid, kSGroup, C + tid, kSGroup);
+        __syncthreads();
+    }
+    // OUT = [mean +] a0 V + sum_a cs_a s_a
+    const T nan = (T)__longlong_as_double(0x7ff8000000000000ll);
+    for (int64_t i = tid; i < n; i += nt)
+    {
+        T r[kSGroup];
+        const T mi = mean ? mean[i] : T(0);
+#pragma unroll
+        for (int j = 0; j < kSGroup; j++) r[j] = j < kk ? (mean ? mi + a0 * V[j * ldv + i] : a0 * V[j * ldv + i]) : T(0);
+        for (int q = 0; q < c; q++)
+        {
+            const T sv = rec[a.HL.s(q) + i];
+#pragma unroll
+            for (int j = 0; j < kSGroup; j++) r[j] += C[(c + q) * kSGroup + j] * sv;
+        }
+#pragma unroll
+        for (int j = 0; j < kSGroup; j++)
+            if (j < kk) OUT[j * a.ldo + i] = ok ? r[j] : nan;
+    }
+}
+
+// log det H_b = -n log theta + sum_t log(rho_t sigma_t) (compact_factor_setup) for problems b0 + p: one CTA of one warp per problem,
+// thread 0 does the O(c^3) recursion in dynamic shared memory (3c^2 doubles).  NaN when the check fails.
+template <class T> __global__ void k_small_hist_logdet(const T* hist, const int* hist_c, SmallHistLayout HL, int64_t b0, double* out)
+{
+    extern __shared__ __align__(16) unsigned char s_smem[];
+    if (threadIdx.x != 0) return;
+    const int64_t p = blockIdx.x, b = b0 + p;
+    const T* rec = hist + b * HL.rec();
+    const int c = hist_c[b];
+    const T theta = rec[HL.theta()];
+    double* beta = reinterpret_cast<double*>(s_smem);
+    double ls = 0.0;
+    const int st = LBFGSpp::compact_factor_setup(c, rec + HL.SY(), rec + HL.SS(), rec + HL.YY(), c, theta, beta, beta + 2 * c * c, &ls);
+    out[p] = st ? __longlong_as_double(0x7ff8000000000000ll) : -(double)HL.n * log((double)theta) + ls;
 }
 
 }  // namespace lb
