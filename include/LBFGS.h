@@ -331,7 +331,32 @@ public:
         return m_bfgs.inverse_hessian_logdet();
     }
 
+    // Whitening and log densities under N(x*, H) with the same factor (BFGSMat::inverse_hessian_factor_transpose_times / _solve /
+    // _transpose_solve / log_density): OUT = L' V, L^-1 V or L^-T V for V holding k = V.size()/n vectors (z = L^-1 (x - x*) whitens
+    // a point, L' maps a gradient to standard coordinates, L^-T z is a draw from N(0, B)); log N(x_j; mean, H) for the k points of X
+    // (NaN if the kept pairs fail the positive-curvature check).  Valid after minimize() in either loop; std::logic_error before
+    // the first.
+    void final_approx_inverse_hessian_factor_transpose_times(const Vector& V, Vector& OUT) { factor_op(LBFGS_B200_FACTOR_LT, V, OUT); }
+    void final_approx_inverse_hessian_factor_solve(const Vector& V, Vector& OUT) { factor_op(LBFGS_B200_FACTOR_LINV, V, OUT); }
+    void final_approx_inverse_hessian_factor_transpose_solve(const Vector& V, Vector& OUT) { factor_op(LBFGS_B200_FACTOR_LINVT, V, OUT); }
+    std::vector<double> final_approx_log_density(const Vector& mean, const Vector& X)
+    {
+        sync_history();
+        m_bfgs.require_history();
+        return m_bfgs.log_density(mean, X, BFGSMat<Scalar>::block_count(X.size(), m_bfgs.dim()));
+    }
+
 private:
+    void factor_op(int op, const Vector& V, Vector& OUT)
+    {
+        sync_history();
+        m_bfgs.require_history();
+        const int k = BFGSMat<Scalar>::block_count(V.size(), m_bfgs.dim());
+        if (op == LBFGS_B200_FACTOR_LT) m_bfgs.inverse_hessian_factor_transpose_times(V, k, OUT);
+        else if (op == LBFGS_B200_FACTOR_LINV) m_bfgs.inverse_hessian_factor_solve(V, k, OUT);
+        else m_bfgs.inverse_hessian_factor_transpose_solve(V, k, OUT);
+    }
+
     void approx_diagonal(Vector& out, bool inverse)
     {
         sync_history();

@@ -131,7 +131,29 @@ public:
         return mat.inverse_hessian_logdet();
     }
 
+    // LBFGSSolver::final_approx_inverse_hessian_factor_transpose_times / _solve / _transpose_solve / final_approx_log_density for
+    // problem b: the same values as problem b solved alone.
+    void final_approx_inverse_hessian_factor_transpose_times(int b, const Vector& V, Vector& OUT) { factor_op(b, LBFGS_B200_FACTOR_LT, V, OUT); }
+    void final_approx_inverse_hessian_factor_solve(int b, const Vector& V, Vector& OUT) { factor_op(b, LBFGS_B200_FACTOR_LINV, V, OUT); }
+    void final_approx_inverse_hessian_factor_transpose_solve(int b, const Vector& V, Vector& OUT) { factor_op(b, LBFGS_B200_FACTOR_LINVT, V, OUT); }
+    std::vector<double> final_approx_log_density(int b, const Vector& mean, const Vector& X)
+    {
+        BFGSMat<Scalar> mat;
+        borrow(b, mat);
+        return mat.log_density(mean, X, BFGSMat<Scalar>::block_count(X.size(), m_n));
+    }
+
 private:
+    void factor_op(int b, int op, const Vector& V, Vector& OUT)
+    {
+        BFGSMat<Scalar> mat;
+        borrow(b, mat);
+        const int k = BFGSMat<Scalar>::block_count(V.size(), m_n);
+        if (op == LBFGS_B200_FACTOR_LT) mat.inverse_hessian_factor_transpose_times(V, k, OUT);
+        else if (op == LBFGS_B200_FACTOR_LINV) mat.inverse_hessian_factor_solve(V, k, OUT);
+        else mat.inverse_hessian_factor_transpose_solve(V, k, OUT);
+    }
+
     void borrow(int b, BFGSMat<Scalar>& mat)
     {
         if (!m_solver) throw std::logic_error("LBFGSBatchSolver: no history yet (minimize() has not run)");

@@ -41,6 +41,12 @@ template <> struct small_batch_abi<double>
     { return lbfgs_b200_small_hist_sample_f64(h, seed, first, b0, count, k, M, ldm, OUT, ldo, ldop); }
     static lbfgs_b200_status logdet(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, double* out)
     { return lbfgs_b200_small_hist_logdet_f64(h, b0, count, out); }
+    static lbfgs_b200_status factor_apply(lbfgs_b200_small_hist* h, int op, int64_t b0, int64_t count, int k, const double* V, int64_t ldv,
+                                          int64_t ldvp, double* OUT, int64_t ldo, int64_t ldop)
+    { return lbfgs_b200_small_hist_factor_apply_f64(h, op, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop); }
+    static lbfgs_b200_status log_density(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, int k, const double* X, int64_t ldx, int64_t ldxp,
+                                         const double* M, int64_t ldm, double* out)
+    { return lbfgs_b200_small_hist_log_density_f64(h, b0, count, k, X, ldx, ldxp, M, ldm, out); }
 };
 template <> struct small_batch_abi<float>
 {
@@ -64,6 +70,12 @@ template <> struct small_batch_abi<float>
     { return lbfgs_b200_small_hist_sample_f32(h, seed, first, b0, count, k, M, ldm, OUT, ldo, ldop); }
     static lbfgs_b200_status logdet(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, double* out)
     { return lbfgs_b200_small_hist_logdet_f32(h, b0, count, out); }
+    static lbfgs_b200_status factor_apply(lbfgs_b200_small_hist* h, int op, int64_t b0, int64_t count, int k, const float* V, int64_t ldv,
+                                          int64_t ldvp, float* OUT, int64_t ldo, int64_t ldop)
+    { return lbfgs_b200_small_hist_factor_apply_f32(h, op, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop); }
+    static lbfgs_b200_status log_density(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, int k, const float* X, int64_t ldx, int64_t ldxp,
+                                         const float* M, int64_t ldm, double* out)
+    { return lbfgs_b200_small_hist_log_density_f32(h, b0, count, k, X, ldx, ldxp, M, ldm, out); }
 };
 }  // namespace detail
 
@@ -213,7 +225,53 @@ public:
         return out;
     }
 
+    // Whitening and log densities under N(x_b, H_b) for every kept problem (lbfgs_b200_small_hist_factor_apply / _log_density):
+    // OUT = L_b' V, L_b^-1 V or L_b^-T V in the layouts of final_approx_inverse_hessian_factor_times; log N(x; MEAN_b, H_b) for the k
+    // points of each problem, X holding B*k points (problem b's point j at [(b*k + j)*n, ...)) and MEANS the B means back to back,
+    // out[b*k + j].  One problem b alone: the same values.  A problem whose pairs fail the positive-curvature check gets NaN.
+    void final_approx_inverse_hessian_factor_transpose_times(const Vector& V, Vector& OUT) { all_factor(LBFGS_B200_FACTOR_LT, V, OUT); }
+    void final_approx_inverse_hessian_factor_solve(const Vector& V, Vector& OUT) { all_factor(LBFGS_B200_FACTOR_LINV, V, OUT); }
+    void final_approx_inverse_hessian_factor_transpose_solve(const Vector& V, Vector& OUT) { all_factor(LBFGS_B200_FACTOR_LINVT, V, OUT); }
+    void final_approx_inverse_hessian_factor_transpose_times(long b, const Vector& V, Vector& OUT) { one_factor(b, LBFGS_B200_FACTOR_LT, V, OUT); }
+    void final_approx_inverse_hessian_factor_solve(long b, const Vector& V, Vector& OUT) { one_factor(b, LBFGS_B200_FACTOR_LINV, V, OUT); }
+    void final_approx_inverse_hessian_factor_transpose_solve(long b, const Vector& V, Vector& OUT) { one_factor(b, LBFGS_B200_FACTOR_LINVT, V, OUT); }
+    std::vector<double> final_approx_log_density(const Vector& MEANS, const Vector& X)
+    {
+        require_kept();
+        if (MEANS.size() != m_n * std::ptrdiff_t(m_B)) throw std::invalid_argument("MEANS must hold B * n values");
+        const int k = all_count(X);
+        std::vector<double> out(static_cast<size_t>(k) * static_cast<size_t>(m_B));
+        m_dev->check(detail::small_batch_abi<Scalar>::log_density(m_hist, 0, int64_t(m_B), k, X.data(), int64_t(m_n), int64_t(k) * m_n, MEANS.data(),
+                                                                  int64_t(m_n), out.data()));
+        return out;
+    }
+    std::vector<double> final_approx_log_density(long b, const Vector& mean, const Vector& X)
+    {
+        require_one(b);
+        if (mean.size() != m_n) throw std::invalid_argument("mean must hold n values");
+        const int k = BFGSMat<Scalar>::block_count(X.size(), m_n);
+        std::vector<double> out(static_cast<size_t>(k));
+        m_dev->check(detail::small_batch_abi<Scalar>::log_density(m_hist, int64_t(b), 1, k, X.data(), int64_t(m_n), 0, mean.data(), 0, out.data()));
+        return out;
+    }
+
 private:
+    void all_factor(int op, const Vector& V, Vector& OUT)
+    {
+        require_kept();
+        const int k = all_count(V);
+        OUT.resize(V.size());
+        m_dev->check(detail::small_batch_abi<Scalar>::factor_apply(m_hist, op, 0, int64_t(m_B), k, V.data(), int64_t(m_n), int64_t(k) * m_n,
+                                                                   OUT.data(), int64_t(m_n), int64_t(k) * m_n));
+    }
+    void one_factor(long b, int op, const Vector& V, Vector& OUT)
+    {
+        require_one(b);
+        const int k = BFGSMat<Scalar>::block_count(V.size(), m_n);
+        OUT.resize(V.size());
+        m_dev->check(detail::small_batch_abi<Scalar>::factor_apply(m_hist, op, int64_t(b), 1, k, V.data(), int64_t(m_n), 0, OUT.data(), int64_t(m_n), 0));
+    }
+
     std::ptrdiff_t m_hist_n = 0;
     long m_hist_B = 0;
     int m_hist_m = 0;

@@ -353,51 +353,105 @@ public:
     // first .. first+k-1 of stream `stream` (mean == nullptr: zero), z_j generated inside both passes and never stored
     // (lbfgs_b200_hist_wt_dot_normal / lincomb_normal).  With c = 0: L = I/sqrt(theta).  Pairs without positive curvature
     // (impossible after a solve, whose curvature gate refuses them): std::runtime_error, and NaN from inverse_hessian_logdet.
-    void inverse_hessian_factor_times(const Vector& V, int k, Vector& OUT) { factor(&V, nullptr, 0, 0, 0, k, OUT); }
+    void inverse_hessian_factor_times(const Vector& V, int k, Vector& OUT) { factor<LBFGS_B200_FACTOR_L>(&V, nullptr, 0, 0, 0, k, OUT); }
     void sample(const Vector* mean, unsigned long long seed, uint32_t stream, uint32_t first, int k, Vector& OUT)
     {
         if (mean && mean->size() != m_n) throw std::invalid_argument("mean must hold n values");
-        factor(nullptr, mean, seed, stream, first, k, OUT);
+        factor<LBFGS_B200_FACTOR_L>(nullptr, mean, seed, stream, first, k, OUT);
     }
     double inverse_hessian_logdet()
     {
         require_history();
-        std::vector<double> beta, Tm;
-        double ls = 0.0;
-        const Scalar theta = factor_setup(beta, Tm, ls);
-        return std::isnan(ls) ? ls : -double(m_n) * std::log(double(theta)) + ls;
+        const FactorSetup f = factor_setup(false);
+        return f.logdet;
+    }
+
+    // Whitening and log densities under N(mean, H) with the same factor (CompactForm.h, compact_factor_t_coef / _inv_coef /
+    // _invt_coef / compact_factor_quad): OUT = L' V, L^-1 V or L^-T V for k vectors back to back, in groups of 16, each one dots
+    // pass and one combination pass (L' and L^-T read only S for their dots: lbfgs_b200_hist_s_dot_multi).  log_density: log N(x_j;
+    // mean, H) for the k points of X, from W'(x_j - mean) and |x_j - mean|^2 alone (lbfgs_b200_hist_wt_dot_diff; no combination
+    // pass).  With c = 0: L' = I/sqrt(theta), L^-1 = L^-T = sqrt(theta) I.  Pairs without positive curvature: std::runtime_error from
+    // the products, NaN from log_density.
+    void inverse_hessian_factor_transpose_times(const Vector& V, int k, Vector& OUT) { factor<LBFGS_B200_FACTOR_LT>(&V, nullptr, 0, 0, 0, k, OUT); }
+    void inverse_hessian_factor_solve(const Vector& V, int k, Vector& OUT) { factor<LBFGS_B200_FACTOR_LINV>(&V, nullptr, 0, 0, 0, k, OUT); }
+    void inverse_hessian_factor_transpose_solve(const Vector& V, int k, Vector& OUT) { factor<LBFGS_B200_FACTOR_LINVT>(&V, nullptr, 0, 0, 0, k, OUT); }
+    std::vector<double> log_density(const Vector& mean, const Vector& X, int k)
+    {
+        require_history();
+        if (mean.size() != m_n) throw std::invalid_argument("mean must hold n values");
+        if (block_count(X.size(), m_n) != k) throw std::invalid_argument("X.size() must be k * n");
+        const FactorSetup f = factor_setup(true);
+        std::vector<double> out(static_cast<size_t>(k), std::numeric_limits<double>::quiet_NaN());
+        if (std::isnan(f.logdet)) return out;
+        const int c = lbfgs_b200_hist_ncorr(m_hist), kGroup = 16;
+        std::vector<double> Wv, nrm, z(size_t(c > 0 ? c : 1));   // the dots as summed (fp64): q cancels when v lies mostly in span S
+        for (int j0 = 0; j0 < k; j0 += kGroup)
+        {
+            const int kk = std::min(kGroup, k - j0);
+            Wv.assign(size_t(std::max(1, 2 * c * kk)), 0.0);
+            nrm.assign(size_t(kk), 0.0);
+            m_dev->check(detail::BoxAbi<Scalar>::hist_wt_dot_diff(m_hist, kk, X.data() + std::ptrdiff_t(j0) * m_n, m_n, mean.data(), Wv.data(),
+                                                                  nrm.data()));
+            for (int j = 0; j < kk; j++)
+            {
+                const double q = compact_factor_quad(c, f.beta.data(), f.Tm.data(), f.SS.data(), c, f.theta, Wv.data() + j, kk, nrm[size_t(j)], z.data());
+                out[size_t(j0 + j)] = compact_log_density(q, f.logdet, double(m_n));
+            }
+        }
+        return out;
     }
 
 private:
-    // compact_factor_setup from the history's Gram blocks; ls = NaN when its check fails.  Returns theta.
-    Scalar factor_setup(std::vector<double>& beta, std::vector<double>& Tm, double& ls)
+    // compact_factor_setup from the history's Gram blocks (and compact_factor_upper when `upper`, for the inverses); logdet = log det H,
+    // NaN when the setup's check fails
+    struct FactorSetup
     {
+        std::vector<double> beta, Tm;
+        std::vector<Scalar> SY, SS;
+        Scalar theta = Scalar(1);
+        double logdet = 0.0;
+    };
+    FactorSetup factor_setup(bool upper)
+    {
+        FactorSetup f;
         const int c = lbfgs_b200_hist_ncorr(m_hist);
         const size_t cs = size_t(c > 0 ? c : 1);
-        std::vector<Scalar> SY(cs * cs), SS(cs * cs), YY(cs * cs);
-        Scalar theta = Scalar(1);
-        m_dev->check(detail::BoxAbi<Scalar>::hist_gram(m_hist, SY.data(), SS.data(), YY.data(), nullptr, &theta));
-        beta.assign(2 * cs * cs, 0.0);
-        Tm.assign(cs * cs, 0.0);
-        if (compact_factor_setup(c, SY.data(), SS.data(), YY.data(), c, theta, beta.data(), Tm.data(), &ls) != 0)
-            ls = std::numeric_limits<double>::quiet_NaN();
-        return theta;
+        std::vector<Scalar> YY(cs * cs);
+        f.SY.assign(cs * cs, Scalar(0));
+        f.SS.assign(cs * cs, Scalar(0));
+        m_dev->check(detail::BoxAbi<Scalar>::hist_gram(m_hist, f.SY.data(), f.SS.data(), YY.data(), nullptr, &f.theta));
+        f.beta.assign(2 * cs * cs, 0.0);
+        f.Tm.assign(cs * cs, 0.0);
+        double ls = 0.0;
+        if (compact_factor_setup(c, f.SY.data(), f.SS.data(), YY.data(), c, f.theta, f.beta.data(), f.Tm.data(), &ls) != 0)
+            f.logdet = std::numeric_limits<double>::quiet_NaN();
+        else
+        {
+            f.logdet = -double(m_n) * std::log(double(f.theta)) + ls;
+            if (upper) compact_factor_upper(c, f.SY.data(), c, f.Tm.data());
+        }
+        return f;
     }
 
+    // OUT = OP(L) V (V given) or the draws mean + L z_j (V == nullptr, OP L), OP one of LBFGS_B200_FACTOR_*.  A template argument, so
+    // that the factor and the sampler refer to no pass they do not use.
+    template <int OP>
     void factor(const Vector* V, const Vector* mean, unsigned long long seed, uint32_t stream, uint32_t first, int k, Vector& OUT)
     {
         require_history();
         if (V && block_count(V->size(), m_n) != k) throw std::invalid_argument("V.size() must be k * n");
         if (!V && (k < 1 || uint64_t(first) + uint64_t(k) > (uint64_t(1) << 32))) throw std::invalid_argument("need k >= 1 and first + k <= 2^32");
-        std::vector<double> beta, Tm;
-        double ls = 0.0;
-        const Scalar theta = factor_setup(beta, Tm, ls);
-        if (std::isnan(ls)) throw std::runtime_error("BFGSMat: the kept pairs do not define a positive definite H");
+        constexpr bool inv = OP == LBFGS_B200_FACTOR_LINV || OP == LBFGS_B200_FACTOR_LINVT;
+        constexpr bool sdots = OP == LBFGS_B200_FACTOR_LT || OP == LBFGS_B200_FACTOR_LINVT;   // S'V suffices
+        const FactorSetup f = factor_setup(inv);
+        if (std::isnan(f.logdet)) throw std::runtime_error("BFGSMat: the kept pairs do not define a positive definite H");
         const int c = lbfgs_b200_hist_ncorr(m_hist);
-        const double rsq = 1.0 / std::sqrt(double(theta));
+        const double rsq = 1.0 / std::sqrt(double(f.theta)), sq = std::sqrt(double(f.theta));
+        const Scalar a0 = inv ? Scalar(sq) : Scalar(rsq);
         OUT.resize(std::ptrdiff_t(k) * m_n);
         const int kGroup = 16;
         std::vector<Scalar> Wv, C;
+        std::vector<double> z(size_t(c > 0 ? c : 1));
         for (int j0 = 0; j0 < k; j0 += kGroup)
         {
             const int kk = std::min(kGroup, k - j0);
@@ -405,14 +459,23 @@ private:
             C.assign(size_t(2 * c * kk), Scalar(0));
             if (c > 0)
             {
-                Wv.assign(size_t(2 * c * kk), Scalar(0));
-                if (V) m_dev->check(detail::BoxAbi<Scalar>::hist_wt_dot_multi(m_hist, kk, v, m_n, Wv.data()));
-                else m_dev->check(detail::BoxAbi<Scalar>::hist_wt_dot_normal(m_hist, seed, stream, first + uint32_t(j0), kk, Wv.data()));
-                for (int j = 0; j < kk; j++) compact_factor_coef(c, beta.data(), Tm.data(), rsq, Wv.data() + j, kk, C.data() + j, kk);
+                Wv.assign(size_t((sdots ? 1 : 2) * c * kk), Scalar(0));
+                if (!V) m_dev->check(detail::BoxAbi<Scalar>::hist_wt_dot_normal(m_hist, seed, stream, first + uint32_t(j0), kk, Wv.data()));
+                else if constexpr (sdots) m_dev->check(detail::BoxAbi<Scalar>::hist_s_dot_multi(m_hist, kk, v, m_n, Wv.data()));
+                else m_dev->check(detail::BoxAbi<Scalar>::hist_wt_dot_multi(m_hist, kk, v, m_n, Wv.data()));
+                for (int j = 0; j < kk; j++)
+                {
+                    const double* beta = f.beta.data();
+                    const double* Tm = f.Tm.data();
+                    if constexpr (OP == LBFGS_B200_FACTOR_LT) compact_factor_t_coef(c, beta, Tm, rsq, Wv.data() + j, kk, z.data(), C.data() + j, kk);
+                    else if constexpr (OP == LBFGS_B200_FACTOR_LINV) compact_factor_inv_coef(c, beta, Tm, sq, Wv.data() + j, kk, z.data(), C.data() + j, kk);
+                    else if constexpr (OP == LBFGS_B200_FACTOR_LINVT) compact_factor_invt_coef(c, beta, Tm, sq, Wv.data() + j, kk, z.data(), C.data() + j, kk);
+                    else compact_factor_coef(c, beta, Tm, rsq, Wv.data() + j, kk, C.data() + j, kk);
+                }
             }
             Scalar* out = OUT.data() + std::ptrdiff_t(j0) * m_n;
-            if (V) m_dev->check(detail::BoxAbi<Scalar>::hist_lincomb_multi(m_hist, Scalar(rsq), kk, v, m_n, c > 0 ? C.data() : nullptr, out, m_n));
-            else m_dev->check(detail::BoxAbi<Scalar>::hist_lincomb_normal(m_hist, Scalar(rsq), seed, stream, first + uint32_t(j0), kk,
+            if (V) m_dev->check(detail::BoxAbi<Scalar>::hist_lincomb_multi(m_hist, a0, kk, v, m_n, c > 0 ? C.data() : nullptr, out, m_n));
+            else m_dev->check(detail::BoxAbi<Scalar>::hist_lincomb_normal(m_hist, a0, seed, stream, first + uint32_t(j0), kk,
                                                                           mean ? mean->data() : nullptr, c > 0 ? C.data() : nullptr, out, m_n));
         }
     }

@@ -312,6 +312,115 @@ LBFGS_HD inline void compact_factor_coef(int c, const double* beta, const double
     }
 }
 
+// ---- the transpose and the inverses of the factor, and the quadratic form of B = H^-1 ------------------------------------------
+// (I + s b')^-1 = I - s b'/(1 + b's) with 1 + b_t's_t = d_t = sqrt(rho_t sigma_t) > 0, so with U(t, j) = b_t's_j (j > t):
+//     L' v     = (v + W sum_t beta_t gamma_t) / sqrt(theta),   gamma_t = s_t'v + sum_{j>t} T(j, t) gamma_j          (t = c-1 .. 0)
+//     L^-1 v   = sqrt(theta) (v + sum_t alpha_t s_t),           alpha_t = -(beta_t'W'v + sum_{j>t} U(t, j) alpha_j) / d_t   (t = c-1 .. 0)
+//     L^-T v   = sqrt(theta) (v - W sum_t beta_t delta_t),      delta_t = (s_t'v - sum_{j<t} U(j, t) delta_j) / d_t  (t = 0 .. c-1)
+//     v'B v    = |L^-1 v|^2 = theta (v'v + 2 alpha'S'v + alpha'S'S alpha)
+// L' and L^-T need only S'v.  The coefficient functions take the dots of one vector (sv[a * ldw] = s_a'v by age; wv as above for
+// L^-1), run the recursion in fp64 in z[0, c) (scratch of the caller) and write C[r * ldc] in compact_factor_coef's row order; the
+// product is then a0 v + sum_r C_r W_r with a0 = 1/sqrt(theta) for L' and sqrt(theta) for both inverses.
+
+// compact_factor_upper: after a successful compact_factor_setup, Tm's strict upper part becomes U(t, j) (j > t) and its diagonal d_t.
+// The strict lower part (T) is left as it is.  Only the inverses call it, so the factor itself keeps its arithmetic.
+template <typename T>
+LBFGS_HD inline void compact_factor_upper(int c, const T* SY, int ldg, double* Tm)
+{
+    auto sy = [&](int t, int u) { return double(SY[(c - 1 - t) * ldg + (c - 1 - u)]); };   // s_t'y_u, chronological
+    for (int t = 0; t < c; t++)
+    {
+        const double rho = 1.0 / sy(t, t), sigma = Tm[t * c + t], kappa = std::sqrt(rho / sigma);
+        for (int j = t + 1; j < c; j++) Tm[t * c + j] = kappa * Tm[t * c + j] - rho * sy(j, t);   // b_t's_j = kappa p_t's_j - rho y_t's_j
+        Tm[t * c + t] = std::sqrt(rho * sigma);
+    }
+}
+
+// L' v: every row of C
+template <typename T>
+LBFGS_HD inline void compact_factor_t_coef(int c, const double* beta, const double* Tm, double rsq, const T* sv, int ldw, double* z, T* C, int ldc)
+{
+    for (int t = c - 1; t >= 0; t--)
+    {
+        double acc = double(sv[(c - 1 - t) * ldw]);
+        for (int j = t + 1; j < c; j++) acc += Tm[j * c + t] * z[j];
+        z[t] = acc;
+    }
+    for (int r = 0; r < 2 * c; r++)
+    {
+        double acc = 0.0;
+        for (int t = 0; t < c; t++) acc += beta[r * c + t] * z[t];
+        C[r * ldc] = T(rsq * acc);
+    }
+}
+
+// alpha of L^-1 v into z (Tm after compact_factor_upper)
+template <typename T>
+LBFGS_HD inline void compact_factor_inv_alpha(int c, const double* beta, const double* Tm, const T* wv, int ldw, double* z)
+{
+    for (int t = c - 1; t >= 0; t--)
+    {
+        double acc = 0.0;
+        for (int r = 0; r < 2 * c; r++) acc += beta[r * c + t] * double(wv[r * ldw]);
+        for (int j = t + 1; j < c; j++) acc += Tm[t * c + j] * z[j];
+        z[t] = -acc / Tm[t * c + t];
+    }
+}
+
+// L^-1 v: the y rows zero, the s row of age c - 1 - t holding sqrt(theta) alpha_t
+template <typename T>
+LBFGS_HD inline void compact_factor_inv_coef(int c, const double* beta, const double* Tm, double sq, const T* wv, int ldw, double* z, T* C, int ldc)
+{
+    compact_factor_inv_alpha(c, beta, Tm, wv, ldw, z);
+    for (int t = 0; t < c; t++)
+    {
+        C[(c - 1 - t) * ldc] = T(0);
+        C[(2 * c - 1 - t) * ldc] = T(sq * z[t]);
+    }
+}
+
+// L^-T v: every row of C
+template <typename T>
+LBFGS_HD inline void compact_factor_invt_coef(int c, const double* beta, const double* Tm, double sq, const T* sv, int ldw, double* z, T* C, int ldc)
+{
+    for (int t = 0; t < c; t++)
+    {
+        double acc = double(sv[(c - 1 - t) * ldw]);
+        for (int j = 0; j < t; j++) acc -= Tm[j * c + t] * z[j];
+        z[t] = acc / Tm[t * c + t];
+    }
+    for (int r = 0; r < 2 * c; r++)
+    {
+        double acc = 0.0;
+        for (int t = 0; t < c; t++) acc += beta[r * c + t] * z[t];
+        C[r * ldc] = T(-sq * acc);
+    }
+}
+
+// q = v'B v = |L^-1 v|^2 from the dots wv = W'v and vv = v'v alone (no pass over v); the log density of N(mu, H) at x = mu + v is
+// -q/2 - log det H / 2 - (n/2) log 2 pi.  With c = 0: theta v'v.
+template <typename T, typename TW>
+LBFGS_HD inline double compact_factor_quad(int c, const double* beta, const double* Tm, const T* SS, int ldg, T theta, const TW* wv, int ldw,
+                                           double vv, double* z)
+{
+    compact_factor_inv_alpha(c, beta, Tm, wv, ldw, z);
+    double q = vv;
+    for (int t = 0; t < c; t++)
+    {
+        const int at = c - 1 - t;
+        double acc = 2.0 * double(wv[(c + at) * ldw]);
+        for (int u = 0; u < c; u++) acc += double(SS[at * ldg + (c - 1 - u)]) * z[u];
+        q += z[t] * acc;
+    }
+    return double(theta) * q;
+}
+
+// log N(x; mu, H) from q = (x - mu)'B(x - mu) and log det H
+LBFGS_HD inline double compact_log_density(double q, double logdet, double n)
+{
+    return -0.5 * q - 0.5 * logdet - 0.5 * n * 1.8378770664093453;   // log(2 pi)
+}
+
 }  // namespace LBFGSpp
 
 #endif  // LBFGSPP_B200_COMPACT_FORM_H

@@ -130,6 +130,8 @@ template <class Scalar> struct BoxAbi;
         static lbfgs_b200_status hist_lincomb_multi(lbfgs_b200_hist* h, T a0, int k, const T* V, int64_t ldv, const T* C, T* OUT, int64_t ldo) { return lbfgs_b200_hist_lincomb_multi_##SUF(h, a0, k, V, ldv, C, OUT, ldo); } \
         static lbfgs_b200_status hist_quad_diag(lbfgs_b200_hist* h, T a0, const T* K, T* out) { return lbfgs_b200_hist_quad_diag_##SUF(h, a0, K, out); } \
         static lbfgs_b200_status hist_wt_dot_normal(lbfgs_b200_hist* h, uint64_t seed, uint32_t stream, uint32_t first, int k, T* R) { return lbfgs_b200_hist_wt_dot_normal_##SUF(h, seed, stream, first, k, R); } \
+        static lbfgs_b200_status hist_s_dot_multi(lbfgs_b200_hist* h, int k, const T* V, int64_t ldv, T* R) { return lbfgs_b200_hist_s_dot_multi_##SUF(h, k, V, ldv, R); } \
+        static lbfgs_b200_status hist_wt_dot_diff(lbfgs_b200_hist* h, int k, const T* X, int64_t ldx, const T* mean, double* R, double* nrm) { return lbfgs_b200_hist_wt_dot_diff_##SUF(h, k, X, ldx, mean, R, nrm); } \
         static lbfgs_b200_status hist_lincomb_normal(lbfgs_b200_hist* h, T a0, uint64_t seed, uint32_t stream, uint32_t first, int k, const T* mean, const T* C, T* OUT, int64_t ldo) { return lbfgs_b200_hist_lincomb_normal_##SUF(h, a0, seed, stream, first, k, mean, C, OUT, ldo); } \
         static lbfgs_b200_status cauchy_breaks(lbfgs_b200_box* b, const T* x, const T* g, const T* lb, const T* ub, T* o5) { return lbfgs_b200_box_cauchy_breaks_##SUF(b, x, g, lb, ub, o5); } \
         static lbfgs_b200_status cauchy_sweep(lbfgs_b200_box* b, const T* g, const T* M, const T* p0, T theta, T gt, int64_t nord, int64_t ninf, T* out) { return lbfgs_b200_box_cauchy_sweep_##SUF(b, g, M, p0, theta, gt, nord, ninf, out); } \

@@ -249,6 +249,16 @@ void* lbfgs_b200_box_vector(lbfgs_b200_box* b, int which);               /* LBFG
     lbfgs_b200_status lbfgs_b200_hist_lincomb_normal_##SUF(lbfgs_b200_hist* h, T a0, uint64_t seed, uint32_t stream,         \
                                                            uint32_t first, int k, const T* mean, const T* C_host, T* OUT,   \
                                                            int64_t ldo);                                                    \
+    /* Whitening and log densities under N(mean, H) (BFGSMat::inverse_hessian_factor_transpose_times / _solve /              \
+     * _transpose_solve / log_density; each replaces hist_wt_dot_multi on a full W'V).  s_dot_multi: R_host[c][k] = S'V, rows s  \
+     * by age, row a bit-identical to the s row of age a from hist_wt_dot_multi on the same V; only the c s columns are read.    \
+     * wt_dot_diff: R_host[2c][k] = [Y S]'(X - mean) and nrm_host[j] = |x_j - mean|^2, both as summed in fp64 (no rounding to T), \
+     * the differences formed in the pass as x - mean in T (R rounded to T is bit-identical to hist_wt_dot_multi on X - mean    \
+     * from lbfgs_b200_axpy_out(x, -1, mean)).                                                                                  \
+     * 1 <= k <= 16, ldv, ldx >= n, any m; replicas only.                                                                       */ \
+    lbfgs_b200_status lbfgs_b200_hist_s_dot_multi_##SUF(lbfgs_b200_hist* h, int k, const T* V, int64_t ldv, T* R_host);      \
+    lbfgs_b200_status lbfgs_b200_hist_wt_dot_diff_##SUF(lbfgs_b200_hist* h, int k, const T* X, int64_t ldx, const T* mean,    \
+                                                        double* R_host, double* nrm_host);                                   \
     /* Cauchy.h:111-129: breakpoints, d = -g on movable coordinates, class bytes.                                      \
      * out5 = { #fixed, #never-bounded, #with a finite breakpoint, d.d, smallest breakpoint } */                       \
     lbfgs_b200_status lbfgs_b200_box_cauchy_breaks_##SUF(lbfgs_b200_box*, const T* x, const T* g, const T* lb, \
@@ -386,6 +396,9 @@ void lbfgs_b200_small_hist_destroy(lbfgs_b200_small_hist* h);
 const void* lbfgs_b200_small_hist_s_col(const lbfgs_b200_small_hist* h, int64_t b, int age);
 const void* lbfgs_b200_small_hist_y_col(const lbfgs_b200_small_hist* h, int64_t b, int age);
 
+/* op of lbfgs_b200_small_hist_factor_apply_*: with H = L L' (include/LBFGSpp/CompactForm.h), L, L', L^-1 or L^-T */
+enum { LBFGS_B200_FACTOR_L = 0, LBFGS_B200_FACTOR_LT = 1, LBFGS_B200_FACTOR_LINV = 2, LBFGS_B200_FACTOR_LINVT = 3 };
+
 #define LBFGS_B200_DECLARE_SMALL_HIST(T, SUF)                                                                                     \
     /* lbfgs_b200_small_minimize_* that also fills `hist`, whose n, m, precision and B must match the solve's             \
      * (LBFGS_B200_ERR_INVALID before anything is launched otherwise).  Everything else is the same launch.            */ \
@@ -423,7 +436,18 @@ const void* lbfgs_b200_small_hist_y_col(const lbfgs_b200_small_hist* h, int64_t 
     lbfgs_b200_status lbfgs_b200_small_hist_sample_##SUF(lbfgs_b200_small_hist* h, uint64_t seed, uint32_t first, int64_t b0,       \
                                                          int64_t count, int k, const T* MEAN, int64_t ldm, T* OUT, int64_t ldo,  \
                                                          int64_t ldop);                                                          \
-    lbfgs_b200_status lbfgs_b200_small_hist_logdet_##SUF(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, double* out_host);
+    lbfgs_b200_status lbfgs_b200_small_hist_logdet_##SUF(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, double* out_host);  \
+    /* Whitening under N(x_b, H_b) (CompactForm.h, compact_factor_t_coef / _inv_coef / _invt_coef): OUT = op(L_b) V with op one  \
+     * of LBFGS_B200_FACTOR_*, in the layouts and with the aliasing rules of factor_times (op L is factor_times).  Asynchronous.   \
+     * log_density: out_host[p*k + j] = log N(x_pj; MEAN + p*ldm, H_b), point j of problem p at X + p*ldxp + j*ldx, from          \
+     * W'(x - mean) and |x - mean|^2 alone (compact_factor_quad); MEAN is required.  Synchronous.  A problem whose pairs fail    \
+     * the check of compact_factor_setup gets NaN outputs.  Errors as small_hist_times, and an op out of range.                */ \
+    lbfgs_b200_status lbfgs_b200_small_hist_factor_apply_##SUF(lbfgs_b200_small_hist* h, int op, int64_t b0, int64_t count, int k, \
+                                                               const T* V, int64_t ldv, int64_t ldvp, T* OUT, int64_t ldo,       \
+                                                               int64_t ldop);                                                    \
+    lbfgs_b200_status lbfgs_b200_small_hist_log_density_##SUF(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, int k,          \
+                                                               const T* X, int64_t ldx, int64_t ldxp, const T* MEAN, int64_t ldm, \
+                                                               double* out_host);
 
 LBFGS_B200_DECLARE_SMALL_HIST(double, f64)
 LBFGS_B200_DECLARE_SMALL_HIST(float, f32)

@@ -138,6 +138,9 @@ def _declare(lib):
         if hasattr(lib, "lbfgs_b200_hist_wt_dot_normal_" + suf):  # the sampler's passes (a test double of the ABI may lack them)
             getattr(lib, "lbfgs_b200_hist_wt_dot_normal_" + suf).argtypes = [vp, C.c_uint64, C.c_uint32, C.c_uint32, ci, pt]
             getattr(lib, "lbfgs_b200_hist_lincomb_normal_" + suf).argtypes = [vp, ct, C.c_uint64, C.c_uint32, C.c_uint32, ci, vp, pt, vp, i64]
+        if hasattr(lib, "lbfgs_b200_hist_s_dot_multi_" + suf):    # the whitening passes (a test double of the ABI may lack them)
+            getattr(lib, "lbfgs_b200_hist_s_dot_multi_" + suf).argtypes = [vp, ci, vp, i64, pt]
+            getattr(lib, "lbfgs_b200_hist_wt_dot_diff_" + suf).argtypes = [vp, ci, vp, i64, vp, C.POINTER(C.c_double), C.POINTER(C.c_double)]
         getattr(lib, "lbfgs_b200_box_cauchy_breaks_" + suf).argtypes = [vp, vp, vp, vp, vp, pt]
         getattr(lib, "lbfgs_b200_box_cauchy_sweep_" + suf).argtypes = [vp, vp, pt, pt, ct, ct, i64, i64, pt]
         getattr(lib, "lbfgs_b200_box_cauchy_build_" + suf).argtypes = [vp, vp, vp, vp, ct, ct, pt]
@@ -180,6 +183,10 @@ def _declare(lib):
                 getattr(lib, "lbfgs_b200_small_hist_factor_times_" + suf).argtypes = [vp, i64, i64, ci, vp, i64, i64, vp, i64, i64]
                 getattr(lib, "lbfgs_b200_small_hist_sample_" + suf).argtypes = [vp, C.c_uint64, C.c_uint32, i64, i64, ci, vp, i64, vp, i64, i64]
                 getattr(lib, "lbfgs_b200_small_hist_logdet_" + suf).argtypes = [vp, i64, i64, C.POINTER(C.c_double)]
+            if hasattr(lib, "lbfgs_b200_small_hist_factor_apply_" + suf):
+                getattr(lib, "lbfgs_b200_small_hist_factor_apply_" + suf).argtypes = [vp, ci, i64, i64, ci, vp, i64, i64, vp, i64, i64]
+                getattr(lib, "lbfgs_b200_small_hist_log_density_" + suf).argtypes = [vp, i64, i64, ci, vp, i64, i64, vp, i64,
+                                                                                     C.POINTER(C.c_double)]
     lib._typed = True
     return lib
 
@@ -299,6 +306,15 @@ def _declare_driver(lib):
         for suf, pt in (("f64", dp), ("f32", fp)):
             getattr(lib, "lbfgsb200_drv_small_batch_hessian_sample_" + suf).argtypes = [ci, ci, cl, cl, pt, pt, pt, cl, ci, prm, pt, ci, pt, pt, u64,
                                                                                        u32, ci, pt, dp, C.POINTER(_SmallItem), err, errlen]
+    # whitening and log densities under N(x*, H) (csrc/driver_hessian_whiten.cpp)
+    if hasattr(lib, "lbfgsb200_drv_solve_hessian_whiten_f64"):
+        lib.lbfgsb200_drv_solve_hessian_whiten_f64.argtypes = [ci, ci, cl, ci, prm, ci, dp, ci, ci, dp, dp, ci, dp, dp, dp, C.POINTER(ci), err,
+                                                               errlen]
+        lib.lbfgsb200_drv_batch_hessian_whiten_f64.argtypes = [ci, ci, cl, ci, dp, ci, prm, ci, ci, ci, dp, dp, ci, dp, dp, dp, dp, err, errlen]
+        lib.lbfgsb200_drv_hist_whiten_f64.argtypes = [ci, cl, ci, ci, dp, dp, ci, ci, dp, dp, ci, dp, dp, dp, err, errlen]
+        for suf, pt in (("f64", dp), ("f32", fp)):
+            getattr(lib, "lbfgsb200_drv_small_batch_hessian_whiten_" + suf).argtypes = [ci, ci, cl, cl, pt, pt, pt, cl, ci, prm, pt, ci, ci, pt, pt,
+                                                                                       ci, pt, pt, dp, cl, C.POINTER(_SmallItem), err, errlen]
     lib._drv_typed = True
     return lib
 
@@ -670,6 +686,24 @@ class History:
             self.h, a0, seed, stream, first, k, mean.ptr if mean is not None else None,
             coef.ctypes.data_as(C.POINTER(self.ct)) if coef.size else None, OUT.ptr, ldo))
 
+    def s_dot_multi(self, V, k, ldv):
+        """S'V for the k columns of the DeviceArray V (lbfgs_b200_hist_s_dot_multi): a (c, k) array, rows s by age."""
+        c = self.ncorr
+        R = (self.ct * max(1, c * k))()
+        self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_hist_s_dot_multi_" + self.suf)(self.h, k, V.ptr, ldv, R))
+        return np.array(R[:c * k], dtype=self.dtype).reshape(c, k)
+
+    def wt_dot_diff(self, X, k, ldx, mean):
+        """[Y S]'(X - mean) and |x_j - mean|^2 for the k columns of the DeviceArray X (lbfgs_b200_hist_wt_dot_diff): a (2c, k)
+        float64 array and k float64 norms, as summed in fp64."""
+        c = self.ncorr
+        R = np.zeros(max(1, 2 * c * k))
+        nrm = np.zeros(k)
+        dp = C.POINTER(C.c_double)
+        self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_hist_wt_dot_diff_" + self.suf)(self.h, k, X.ptr, ldx, mean.ptr, R.ctypes.data_as(dp),
+                                                                                        nrm.ctypes.data_as(dp)))
+        return R[:2 * c * k].reshape(2 * c, k), nrm
+
     def column(self, which, age):
         fn = self.ctx.lib.lbfgs_b200_hist_s_col if which == "s" else self.ctx.lib.lbfgs_b200_hist_y_col
         p = fn(self.h, age)
@@ -1018,6 +1052,158 @@ def small_batch_hessian_sample(objective, X0, V=None, seed=0, first=0, k=0, para
     return res, X, LV, D, ld
 
 
+FACTOR_OPS = {"L": 0, "LT": 1, "LINV": 2, "LINVT": 3}   # LBFGS_B200_FACTOR_*: with H = L L', L, L', L^-1 and L^-T
+
+
+def _op_id(op):
+    return FACTOR_OPS[op] if isinstance(op, str) else int(op)
+
+
+def _rows(A, n, dtype=np.float64):
+    """A as contiguous rows of n values, its row count (0 for None)."""
+    if A is None:
+        return None, 0
+    a = np.ascontiguousarray(A, dtype=dtype).reshape(-1, n)
+    return a, a.shape[0]
+
+
+def _solve_whiten(objective, x0, op, V, X, mean, param, linesearch, resident, device, lib):
+    drv = driver(lib)
+    x = np.array(x0, dtype=np.float64, order="C").copy()
+    n = x.size
+    p = (param if param is not None else LBFGSParam())._c()
+    v, kv = _rows(V, n)
+    P, kx = _rows(X, n)
+    mu = None if mean is None else np.ascontiguousarray(mean, dtype=np.float64)
+    OV = None if v is None else np.zeros_like(v)
+    lp = np.zeros(kx) if kx else None
+    niter = C.c_int(0)
+    _checked("solve_hessian_whiten", lambda *err: drv.lbfgsb200_drv_solve_hessian_whiten_f64(
+        device, objective, n, _ls_id(linesearch), C.byref(p), int(resident), _ptr(x), _op_id(op), kv, _ptr(v), _ptr(OV), kx, _ptr(P), _ptr(mu),
+        _ptr(lp), C.byref(niter), *err))
+    return niter.value, x, OV, lp
+
+
+def solve_hessian_factor(objective, x0, V, op="L", param=None, linesearch="NocedalWright", resident=True, device=0, lib=None):
+    """minimize(), then op(L) V for the rows of V with H = L L' the final approximation (LBFGSSolver::final_approx_inverse_hessian_
+    factor_times / _transpose_times / _solve / _transpose_solve; op one of FACTOR_OPS).  Returns (niter, x, OV)."""
+    niter, x, OV, _ = _solve_whiten(objective, x0, op, V, None, None, param, linesearch, resident, device, lib)
+    return niter, x, OV
+
+
+def solve_hessian_log_density(objective, x0, X, mean=None, param=None, linesearch="NocedalWright", resident=True, device=0, lib=None):
+    """minimize(), then log N(x; mean, H) at the rows of X (LBFGSSolver::final_approx_log_density; mean None: the solution).
+    Returns (niter, x, logp)."""
+    niter, x, _, lp = _solve_whiten(objective, x0, 0, None, X, mean, param, linesearch, resident, device, lib)
+    return niter, x, lp
+
+
+def _batch_whiten(objective, X0, b, op, V, X, mean, param, linesearch, device, lib):
+    drv = driver(lib)
+    X0 = np.ascontiguousarray(X0, dtype=np.float64)
+    B, n = X0.shape
+    p = (param if param is not None else LBFGSParam())._c()
+    v, kv = _rows(V, n)
+    P, kx = _rows(X, n)
+    mu = None if mean is None else np.ascontiguousarray(mean, dtype=np.float64)
+    OV = None if v is None else np.zeros_like(v)
+    lp = np.zeros(kx) if kx else None
+    Xs = np.zeros_like(X0)
+    _checked("batch_hessian_whiten", lambda *err: drv.lbfgsb200_drv_batch_hessian_whiten_f64(
+        device, objective, n, B, _ptr(X0), _ls_id(linesearch), C.byref(p), b, _op_id(op), kv, _ptr(v), _ptr(OV), kx, _ptr(P), _ptr(mu), _ptr(lp),
+        _ptr(Xs), *err))
+    return Xs, OV, lp
+
+
+def batch_hessian_factor(objective, X0, b, V, op="L", param=None, linesearch="MoreThuente", device=0, lib=None):
+    """A batch (rows of X0) minimised by LBFGSBatchSolver, then problem b's op(L) V.  Returns (X, OV)."""
+    Xs, OV, _ = _batch_whiten(objective, X0, b, op, V, None, None, param, linesearch, device, lib)
+    return Xs, OV
+
+
+def batch_hessian_log_density(objective, X0, b, X, mean=None, param=None, linesearch="MoreThuente", device=0, lib=None):
+    """A batch minimised by LBFGSBatchSolver, then log N(x; mean, H_b) at the rows of X (mean None: problem b's solution).
+    Returns (X_solutions, logp)."""
+    Xs, _, lp = _batch_whiten(objective, X0, b, 0, None, X, mean, param, linesearch, device, lib)
+    return Xs, lp
+
+
+def _hist_whiten(S, Y, m, op, V, X, mean, device, lib):
+    drv = driver(lib)
+    S = np.ascontiguousarray(S, dtype=np.float64)
+    Y = np.ascontiguousarray(Y, dtype=np.float64)
+    npairs, n = S.shape
+    v, kv = _rows(V, n)
+    P, kx = _rows(X, n)
+    mu = None if mean is None else np.ascontiguousarray(mean, dtype=np.float64)
+    OV = None if v is None else np.zeros_like(v)
+    lp = np.zeros(kx) if kx else None
+    _checked("hist_whiten", lambda *err: drv.lbfgsb200_drv_hist_whiten_f64(device, n, npairs if m is None else m, npairs, _ptr(S), _ptr(Y),
+                                                                          _op_id(op), kv, _ptr(v), _ptr(OV), kx, _ptr(P), _ptr(mu), _ptr(lp),
+                                                                          *err))
+    return OV, lp
+
+
+def hist_hessian_factor(S, Y, V, op="L", m=None, device=0, lib=None):
+    """BFGSMat's op(L) V on the history built by adding the pairs (S[k], Y[k]) in order to a ring of size m (default: all of them)."""
+    return _hist_whiten(S, Y, m, op, V, None, None, device, lib)[0]
+
+
+def hist_hessian_log_density(S, Y, X, mean, m=None, device=0, lib=None):
+    """BFGSMat::log_density at the rows of X on the history built from (S, Y) as hist_hessian_factor builds it."""
+    return _hist_whiten(S, Y, m, 0, None, X, mean, device, lib)[1]
+
+
+def _small_batch_whiten(objective, X0, op, V, X, means, param, linesearch, dtype, data0, data1, ldd, device, lib, b=None):
+    drv = driver(lib)
+    X0 = np.ascontiguousarray(X0, dtype=dtype)
+    B, n = X0.shape
+    per = B if b is None else 1     # problems whose vectors, points and means are given
+    p = (param if param is not None else LBFGSParam())._c()
+    d0 = None if data0 is None else np.ascontiguousarray(data0, dtype=dtype).reshape(-1)
+    d1 = None if data1 is None else np.ascontiguousarray(data1, dtype=dtype).reshape(-1)
+    v = None if V is None else np.ascontiguousarray(V, dtype=dtype).reshape(per, -1, n)
+    kv = 0 if v is None else v.shape[1]
+    P = None if X is None else np.ascontiguousarray(X, dtype=dtype).reshape(per, -1, n)
+    kx = 0 if P is None else P.shape[1]
+    mu = None if means is None else np.ascontiguousarray(means, dtype=dtype).reshape(per, n)
+    OV = None if v is None else np.zeros_like(v)
+    lp = np.zeros((per, kx)) if kx else None
+    Xs = np.empty_like(X0)
+    items = (_SmallItem * B)()
+    suf = "f32" if np.dtype(dtype) == np.float32 else "f64"
+    err = C.create_string_buffer(256)
+    r = getattr(drv, "lbfgsb200_drv_small_batch_hessian_whiten_" + suf)(device, objective, n, B, _ptr(X0), _ptr(d0), _ptr(d1), int(ldd),
+                                                                       _ls_id(linesearch), C.byref(p), _ptr(Xs), _op_id(op), kv, _ptr(v),
+                                                                       _ptr(OV), kx, _ptr(P), _ptr(mu), _ptr(lp), -1 if b is None else int(b),
+                                                                       items, err, len(err))
+    if r < 0:
+        raise (ValueError if r == -1 else RuntimeError)("small_batch_hessian_whiten failed: %s" % err.value.decode())
+    res = [dict(status=STATUS_NAMES[it.kind], code=it.code, niter=it.niter, nfev=it.nfev, fx=it.fx, gnorm=it.gnorm, rounds=it.rounds)
+           for it in items]
+    if b is not None:
+        OV, lp = None if OV is None else OV[0], None if lp is None else lp[0]
+    return res, Xs, OV, lp
+
+
+def small_batch_hessian_factor(objective, X0, V, op="L", param=None, linesearch="MoreThuente", dtype=np.float64, data0=None, data1=None,
+                               ldd=0, device=0, lib=None, b=None):
+    """solve_small_batch with every problem's final approximation kept, then op(L_b) V_b for all problems at once
+    (LBFGSSmallBatchSolver; V: (B, kv, n)), or with b given for problem b alone through the one-problem forms (V: (kv, n)).
+    Returns (outcomes, X, OV)."""
+    res, Xs, OV, _ = _small_batch_whiten(objective, X0, op, V, None, None, param, linesearch, dtype, data0, data1, ldd, device, lib, b)
+    return res, Xs, OV
+
+
+def small_batch_hessian_log_density(objective, X0, X, means=None, param=None, linesearch="MoreThuente", dtype=np.float64, data0=None,
+                                    data1=None, ldd=0, device=0, lib=None, b=None):
+    """solve_small_batch with the final approximations kept, then log N(x; mean_b, H_b) at the points X (B, kx, n) for all problems at
+    once (means (B, n); None: the solutions), or with b given for problem b alone through the one-problem forms (X: (kx, n), means: one
+    mean or None).  Returns (outcomes, X_solutions, logp (B, kx) or (kx,))."""
+    res, Xs, _, lp = _small_batch_whiten(objective, X0, 0, None, X, means, param, linesearch, dtype, data0, data1, ldd, device, lib, b)
+    return res, Xs, lp
+
+
 def small_max_n(m, objective, dtype=np.float64):
     """Largest n of a problem the small-batch solve takes for history size m and built-in objective `objective` (0 if none)."""
     return int(abi().lbfgs_b200_small_max_n(int(m), np.dtype(dtype).itemsize, int(objective)))
@@ -1172,6 +1358,18 @@ class SmallHistory:
         """lbfgs_b200_small_hist_sample_*: OUT = MEAN_b + L_b z_j, z_j draw first + j of stream b; MEAN a DeviceArray or None."""
         self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_small_hist_sample_" + self.suf)(
             self.h, seed, first, b0, count, k, MEAN.ptr if MEAN is not None else None, ldm, OUT.ptr, ldo, ldop))
+
+    def factor_apply(self, op, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop):
+        """lbfgs_b200_small_hist_factor_apply_*: OUT = op(L_b) V (op one of FACTOR_OPS), on DeviceArrays (asynchronous)."""
+        self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_small_hist_factor_apply_" + self.suf)(self.h, _op_id(op), b0, count, k, V.ptr, ldv,
+                                                                                                ldvp, OUT.ptr, ldo, ldop))
+
+    def log_density(self, b0, count, k, X, ldx, ldxp, MEAN, ldm):
+        """lbfgs_b200_small_hist_log_density_*: log N(x_pj; MEAN_p, H_b) for problems b0 .. b0+count-1, a (count, k) array."""
+        out = np.zeros((count, k))
+        self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_small_hist_log_density_" + self.suf)(
+            self.h, b0, count, k, X.ptr, ldx, ldxp, MEAN.ptr, ldm, out.ctypes.data_as(C.POINTER(C.c_double))))
+        return out
 
     def logdet(self, b0=0, count=None):
         """lbfgs_b200_small_hist_logdet_*: log det H_b for problems b0 .. b0+count-1 (NaN where the pairs fail the check)."""

@@ -127,12 +127,12 @@ static int wt_multi_grid(const lbfgs_b200_hist* h)
     return (int)(nstrips < 4 * h->ctx->sm_count ? nstrips : 4 * h->ctx->sm_count);
 }
 
-// The history's scratch for the k-vector passes, made on first use: partials [grid][2m*kMaxK] | result [2m*kMaxK] |
-// coefficients [2m*kMaxK] (doubles; the coefficients are stored as T)
+// The history's scratch for the k-vector passes, made on first use: partials [grid][(2m+1)*kMaxK] | result [(2m+1)*kMaxK] |
+// coefficients [(2m+1)*kMaxK] (doubles; the coefficients are stored as T).  The extra row holds the squared norms of hist_wt_dot_diff.
 static lbfgs_b200_status multi_scratch(lbfgs_b200_hist* h, double** partials, double** result, void** coef)
 {
     lbfgs_b200_ctx* ctx = h->ctx;
-    const size_t vals = (size_t)2 * h->m * kMaxK;
+    const size_t vals = (size_t)(2 * h->m + 1) * kMaxK;
     if (!h->multi)
     {
         const cudaError_t e = pool_alloc(ctx, &h->multi, sizeof(double) * vals * (wt_multi_grid(h) + 2));
@@ -179,6 +179,61 @@ template <class T> static lbfgs_b200_status do_hist_wt_dot_multi(lbfgs_b200_hist
     CU(ctx, cudaMemcpyAsync(tmp.data(), result, sizeof(double) * w * k, cudaMemcpyDeviceToHost, ctx->stream));
     CU(ctx, cudaStreamSynchronize(ctx->stream));
     for (int e = 0; e < w * k; e++) R_host[e] = (T)tmp[(size_t)e];
+    return LBFGS_B200_OK;
+}
+
+// The whitening forms of the dots pass (k_hist_wt_dot_multi with WtDotSArgs / WtDotDiffArgs): the launch of the loaded form with w
+// staged history columns and ncol dots per vector, the ncol * k results copied to tmp
+template <class T, class A>
+static lbfgs_b200_status run_wt_dots(lbfgs_b200_hist* h, A& a, int w, int ncol, std::vector<double>& tmp, const char* what)
+{
+    lbfgs_b200_ctx* ctx = h->ctx;
+    double *partials, *result;
+    void* coef;
+    if (auto st = multi_scratch(h, &partials, &result, &coef)) return st;
+    a.n = h->n; a.ld = h->ld; a.S = static_cast<const T*>(h->S); a.Y = static_cast<const T*>(h->Y);
+    a.c = h->ncorr; a.partials = partials; a.ticket = ctx->rb.ticket; a.result = result;
+    fill_slots<T>(h, a.slots);
+    auto kernel = k_hist_wt_dot_multi<T, A>;
+    const size_t smem = (size_t)(w + a.k) * kWtPitch * sizeof(T);
+    if (smem > 48 * 1024) CU(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<wt_multi_grid(h), kThreads, smem, ctx->stream>>>(a);
+    if (auto st = post_launch(ctx, what)) return st;
+    tmp.resize((size_t)ncol * a.k);
+    CU(ctx, cudaMemcpyAsync(tmp.data(), result, sizeof(double) * tmp.size(), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(ctx, cudaStreamSynchronize(ctx->stream));
+    return LBFGS_B200_OK;
+}
+
+// R_host[c][k] = S'V (rows: s by age), each dot bit-identical to the s row of that age from hist_wt_dot_multi on the same V
+template <class T> static lbfgs_b200_status do_hist_s_dot_multi(lbfgs_b200_hist* h, int k, const T* V, int64_t ldv, T* R_host)
+{
+    if (auto st = multi_check<T>(h, k, ldv, "hist_s_dot_multi")) return st;
+    REQUIRE(h->ctx, V && R_host, "hist_s_dot_multi: NULL argument");
+    const int c = h->ncorr;
+    if (c == 0) return LBFGS_B200_OK;
+    WtDotSArgs<T> a{};
+    a.V = V; a.ldv = ldv; a.k = k;
+    std::vector<double> tmp;
+    if (auto st = run_wt_dots<T>(h, a, c, c, tmp, "k_hist_s_dot_multi")) return st;
+    for (int e = 0; e < c * k; e++) R_host[e] = (T)tmp[(size_t)e];
+    return LBFGS_B200_OK;
+}
+
+// R_host[2c][k] = [Y S]'(X - mean) and nrm_host[j] = |x_j - mean|^2, both as summed in fp64, the differences formed in the pass
+template <class T>
+static lbfgs_b200_status do_hist_wt_dot_diff(lbfgs_b200_hist* h, int k, const T* X, int64_t ldx, const T* mean, double* R_host,
+                                             double* nrm_host)
+{
+    if (auto st = multi_check<T>(h, k, ldx, "hist_wt_dot_diff")) return st;
+    REQUIRE(h->ctx, X && mean && R_host && nrm_host, "hist_wt_dot_diff: NULL argument");
+    const int w = 2 * h->ncorr;
+    WtDotDiffArgs<T> a{};
+    a.V = X; a.ldv = ldx; a.k = k; a.mean = mean;
+    std::vector<double> tmp;
+    if (auto st = run_wt_dots<T>(h, a, w, w + 1, tmp, "k_hist_wt_dot_diff")) return st;
+    for (int e = 0; e < w * k; e++) R_host[e] = tmp[(size_t)e];
+    for (int j = 0; j < k; j++) nrm_host[j] = tmp[(size_t)(w * k + j)];
     return LBFGS_B200_OK;
 }
 
@@ -617,6 +672,11 @@ void* lbfgs_b200_box_vector(lbfgs_b200_box* b, int which)
                                                            uint32_t first, int k, const T* mean, const T* C_host, T* OUT,    \
                                                            int64_t ldo)                                                      \
     { return do_hist_lincomb_normal<T>(h, a0, seed, stream, first, k, mean, C_host, OUT, ldo); }                            \
+    lbfgs_b200_status lbfgs_b200_hist_s_dot_multi_##SUF(lbfgs_b200_hist* h, int k, const T* V, int64_t ldv, T* R_host)       \
+    { return do_hist_s_dot_multi<T>(h, k, V, ldv, R_host); }                                                                 \
+    lbfgs_b200_status lbfgs_b200_hist_wt_dot_diff_##SUF(lbfgs_b200_hist* h, int k, const T* X, int64_t ldx, const T* mean,   \
+                                                        double* R_host, double* nrm_host)                                    \
+    { return do_hist_wt_dot_diff<T>(h, k, X, ldx, mean, R_host, nrm_host); }                                                 \
     lbfgs_b200_status lbfgs_b200_box_cauchy_breaks_##SUF(lbfgs_b200_box* b, const T* x, const T* g, const T* lb,            \
                                                          const T* ub, T* out5_host)                                         \
     { return do_box_cauchy_breaks<T>(b, x, g, lb, ub, out5_host); }                                                         \

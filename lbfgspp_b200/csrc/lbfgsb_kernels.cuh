@@ -710,20 +710,36 @@ template <class T> struct WtDotNormalArgs : WtDotMultiArgs<T>
     NormalSrc src;
 };
 
+// The whitening forms.  WtDotSArgs: the s columns alone, R[c][k] = S'V by age, each dot summed exactly as the s row of that age in
+// the form above.  WtDotDiffArgs: vector j is staged as x_j - mean (V holds the points x_j), formed in T as the two-operand pass
+// lbfgs_b200_axpy_out(x, -1, mean) forms it, and one more column per vector, the vector row itself, gives |x_j - mean|^2 in the
+// same order; the result holds R[2c][k] and then the k squared norms.
+template <class T> struct WtDotSArgs : WtDotMultiArgs<T>
+{
+};
+template <class T> struct WtDotDiffArgs : WtDotMultiArgs<T>
+{
+    const T* mean;
+};
+
 template <class T, class A = WtDotMultiArgs<T>> __global__ void __launch_bounds__(kThreads) k_hist_wt_dot_multi(A a)
 {
-    constexpr bool kGen = !std::is_same<A, WtDotMultiArgs<T>>::value;
+    constexpr bool kGen = std::is_same<A, WtDotNormalArgs<T>>::value;
+    constexpr bool kSOnly = std::is_same<A, WtDotSArgs<T>>::value;
+    constexpr bool kDiff = std::is_same<A, WtDotDiffArgs<T>>::value;
     extern __shared__ __align__(16) unsigned char wt_smem[];
-    T* rows = reinterpret_cast<T*>(wt_smem);   // [2c + k][kWtPitch]: y by age, s by age, then the k vectors
+    T* rows = reinterpret_cast<T*>(wt_smem);   // [w + k][kWtPitch]: y by age, s by age (S only: s by age), then the k vectors
     __shared__ const T* s_col[kMaxW + kMaxK];
     __shared__ bool s_last;
-    const int w = 2 * a.c, k = a.k, nrows = w + k, tid = threadIdx.x;
+    const int w = kSOnly ? a.c : 2 * a.c, k = a.k, nrows = w + k, tid = threadIdx.x;
+    const int ncol = kDiff ? w + 1 : w;   // dots per vector: the history columns, and for kDiff the vector with itself
     const int nload = kGen ? w : nrows;   // rows staged from memory
     for (int q = tid; q < nload; q += kThreads)
-        s_col[q] = q < a.c ? a.Y + (int64_t)a.slots[q] * a.ld : q < w ? a.S + (int64_t)a.slots[q - a.c] * a.ld : a.V + (int64_t)(q - w) * a.ldv;
+        if constexpr (kSOnly) s_col[q] = q < w ? a.S + (int64_t)a.slots[q] * a.ld : a.V + (int64_t)(q - w) * a.ldv;
+        else s_col[q] = q < a.c ? a.Y + (int64_t)a.slots[q] * a.ld : q < w ? a.S + (int64_t)a.slots[q - a.c] * a.ld : a.V + (int64_t)(q - w) * a.ldv;
     const int groups = kThreads / k, j = tid % k, g = tid / k;
     const bool active = g < groups;
-    constexpr int kMaxOwn = kMaxW / (kThreads / kMaxK);   // columns per thread: ceil(2c / G) <= 8 with G >= 16
+    constexpr int kMaxOwn = kMaxW / (kThreads / kMaxK) + (kDiff ? 1 : 0);   // columns per thread: ceil(ncol / G) with G >= 16
     double acc[kMaxOwn];
 #pragma unroll
     for (int q = 0; q < kMaxOwn; q++) acc[q] = 0.0;
@@ -736,7 +752,8 @@ template <class T, class A = WtDotMultiArgs<T>> __global__ void __launch_bounds_
         {
             const int q = t / kWtRows, r = t % kWtRows;
             const int64_t i = r0 + r;
-            rows[q * kWtPitch + r] = i < a.n ? __ldcs(s_col[q] + i) : T(0);
+            if constexpr (kDiff) rows[q * kWtPitch + r] = i < a.n ? (q < w ? __ldcs(s_col[q] + i) : __ldcs(s_col[q] + i) - a.mean[i]) : T(0);
+            else rows[q * kWtPitch + r] = i < a.n ? __ldcs(s_col[q] + i) : T(0);
         }
         if constexpr (kGen)
             for (int t = tid; t < k * (kWtRows / 2); t += kThreads)   // one generator call per coordinate pair (r0 is even)
@@ -761,7 +778,12 @@ template <class T, class A = WtDotMultiArgs<T>> __global__ void __launch_bounds_
                 const double v = (double)vr[r];
 #pragma unroll
                 for (int q = 0; q < kMaxOwn; q++)
-                    if (g + q * groups < w) s[q] += (double)rows[(g + q * groups) * kWtPitch + r] * v;
+                    if constexpr (kDiff)
+                    {
+                        const int col = g + q * groups;
+                        if (col < ncol) s[q] += (double)rows[(col < w ? col : w + j) * kWtPitch + r] * v;
+                    }
+                    else if (g + q * groups < w) s[q] += (double)rows[(g + q * groups) * kWtPitch + r] * v;
             }
 #pragma unroll
             for (int q = 0; q < kMaxOwn; q++) acc[q] += s[q];
@@ -773,7 +795,7 @@ template <class T, class A = WtDotMultiArgs<T>> __global__ void __launch_bounds_
         for (int q = 0; q < kMaxOwn; q++)
         {
             const int col = g + q * groups;
-            if (col < w) a.partials[(size_t)blockIdx.x * (w * k) + col * k + j] = acc[q];
+            if (col < ncol) a.partials[(size_t)blockIdx.x * (ncol * k) + col * k + j] = acc[q];
         }
     __threadfence();
     __syncthreads();
@@ -781,10 +803,10 @@ template <class T, class A = WtDotMultiArgs<T>> __global__ void __launch_bounds_
     __syncthreads();
     if (!s_last) return;
     __threadfence();
-    for (int e = tid; e < w * k; e += kThreads)
+    for (int e = tid; e < ncol * k; e += kThreads)
     {
         double t = 0.0;
-        for (unsigned b = 0; b < gridDim.x; b++) t += __ldcg(&a.partials[(size_t)b * (w * k) + e]);
+        for (unsigned b = 0; b < gridDim.x; b++) t += __ldcg(&a.partials[(size_t)b * (ncol * k) + e]);
         a.result[e] = t;
     }
     if (tid == 0) *a.ticket = 0u;

@@ -181,12 +181,14 @@ lbfgs_b200_status small_hist_diag(lbfgs_b200_small_hist* h, int inverse, int64_t
 
 template <class T>
 lbfgs_b200_status small_hist_factor(lbfgs_b200_small_hist* h, bool gen, uint64_t seed, uint32_t first, int64_t b0, int64_t count, int k,
-                                    const T* V, int64_t ldv, int64_t ldvp, T* OUT, int64_t ldo, int64_t ldop)
+                                    const T* V, int64_t ldv, int64_t ldvp, T* OUT, int64_t ldo, int64_t ldop, int op = LBFGS_B200_FACTOR_L,
+                                    const char* what = nullptr)
 {
     using namespace lb;
-    const char* what = gen ? "small_hist_sample" : "small_hist_factor_times";
+    if (!what) what = gen ? "small_hist_sample" : "small_hist_factor_times";
     if (auto st = small_hist_check<T>(h, what)) return st;
     lbfgs_b200_ctx* ctx = h->ctx;
+    REQUIRE(ctx, op >= LBFGS_B200_FACTOR_L && op <= LBFGS_B200_FACTOR_LINVT, "%s: op %d is not one of LBFGS_B200_FACTOR_*", what, op);
     const int64_t n = h->n;
     REQUIRE(ctx, OUT && (gen || V), "%s: NULL argument", what);
     REQUIRE(ctx, k >= 1 && (k + kSGroup - 1) / kSGroup <= 65535, "%s: k must be in 1..%d (got %d)", what, 65535 * kSGroup, k);
@@ -212,7 +214,11 @@ lbfgs_b200_status small_hist_factor(lbfgs_b200_small_hist* h, bool gen, uint64_t
     a.hist = static_cast<const T*>(h->data); a.hist_c = h->counts; a.HL = SmallHistLayout{n, h->m};
     a.b0 = b0; a.k = k; a.V = V; a.ldv = ldv; a.ldvp = ldvp; a.OUT = OUT; a.ldo = ldo; a.ldop = ldop; a.seed = seed; a.first = first;
     const size_t smem = small_factor_smem(h->m, (int)sizeof(T));
-    auto kernel = gen ? k_small_hist_factor<T, true> : k_small_hist_factor<T, false>;
+    auto kernel = gen ? k_small_hist_factor<T, true>
+                : op == LBFGS_B200_FACTOR_LT    ? k_small_hist_factor<T, false, LBFGS_B200_FACTOR_LT>
+                : op == LBFGS_B200_FACTOR_LINV  ? k_small_hist_factor<T, false, LBFGS_B200_FACTOR_LINV>
+                : op == LBFGS_B200_FACTOR_LINVT ? k_small_hist_factor<T, false, LBFGS_B200_FACTOR_LINVT>
+                                                : k_small_hist_factor<T, false>;
     CU(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel<<<dim3((unsigned)count, (unsigned)((k + kSGroup - 1) / kSGroup)), small_threads(n), smem, ctx->stream>>>(a);
     CU(ctx, cudaGetLastError());
@@ -242,6 +248,45 @@ template <class T> lbfgs_b200_status small_hist_logdet(lbfgs_b200_small_hist* h,
         ctx->launches++;
     }
     if (e == cudaSuccess) e = cudaMemcpyAsync(out_host, d, sizeof(double) * (size_t)count, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    pool_free(ctx, d);
+    CU(ctx, e);
+    return LBFGS_B200_OK;
+}
+
+template <class T>
+lbfgs_b200_status small_hist_log_density(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, int k, const T* X, int64_t ldx, int64_t ldxp,
+                                         const T* MEAN, int64_t ldm, double* out_host)
+{
+    using namespace lb;
+    const char* what = "small_hist_log_density";
+    if (auto st = small_hist_check<T>(h, what)) return st;
+    lbfgs_b200_ctx* ctx = h->ctx;
+    const int64_t n = h->n;
+    REQUIRE(ctx, X && MEAN && out_host, "%s: NULL argument", what);
+    REQUIRE(ctx, k >= 1 && (k + kSGroup - 1) / kSGroup <= 65535, "%s: k must be in 1..%d (got %d)", what, 65535 * kSGroup, k);
+    REQUIRE(ctx, b0 >= 0 && count >= 1 && count <= h->B - b0, "%s: problems [%lld, %lld) are not within the %lld of the history", what,
+            (long long)b0, (long long)(b0 + count), (long long)h->B);
+    REQUIRE(ctx, ldx >= n, "%s: leading dimension ldx = %lld must be at least n = %lld", what, (long long)ldx, (long long)n);
+    REQUIRE(ctx, ldxp >= 0 && ldm >= 0, "%s: negative problem stride", what);
+    REQUIRE(ctx, ctx->nranks == 1, "%s: one CTA holds a whole problem, so n cannot be sharded (the context has %d ranks)", what, ctx->nranks);
+    double* d = nullptr;
+    const size_t nout = (size_t)count * (size_t)k;
+    cudaError_t e = pool_alloc(ctx, reinterpret_cast<void**>(&d), sizeof(double) * nout);
+    if (e != cudaSuccess)
+        return fail(ctx, e == cudaErrorMemoryAllocation ? LBFGS_B200_ERR_ALLOC : LBFGS_B200_ERR_CUDA, "%s: %s", what, cudaGetErrorString(e));
+    SmallDensityArgs<T> a{};
+    a.hist = static_cast<const T*>(h->data); a.hist_c = h->counts; a.HL = SmallHistLayout{n, h->m};
+    a.b0 = b0; a.k = k; a.X = X; a.ldx = ldx; a.ldxp = ldxp; a.MEAN = MEAN; a.ldm = ldm; a.out = d;
+    const size_t smem = small_density_smem(h->m);
+    e = cudaFuncSetAttribute(k_small_hist_log_density<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess)
+    {
+        k_small_hist_log_density<T><<<dim3((unsigned)count, (unsigned)((k + kSGroup - 1) / kSGroup)), small_threads(n), smem, ctx->stream>>>(a);
+        e = cudaGetLastError();
+        ctx->launches++;
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(out_host, d, sizeof(double) * nout, cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
     pool_free(ctx, d);
     CU(ctx, e);
@@ -329,7 +374,15 @@ const void* lbfgs_b200_small_hist_y_col(const lbfgs_b200_small_hist* h, int64_t 
                                                          int64_t ldop)                                                           \
     { return small_hist_factor<T>(h, true, seed, first, b0, count, k, MEAN, 0, ldm, OUT, ldo, ldop); }                            \
     lbfgs_b200_status lbfgs_b200_small_hist_logdet_##SUF(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, double* out_host)    \
-    { return small_hist_logdet<T>(h, b0, count, out_host); }
+    { return small_hist_logdet<T>(h, b0, count, out_host); }                                                                \
+    lbfgs_b200_status lbfgs_b200_small_hist_factor_apply_##SUF(lbfgs_b200_small_hist* h, int op, int64_t b0, int64_t count, int k, \
+                                                               const T* V, int64_t ldv, int64_t ldvp, T* OUT, int64_t ldo,       \
+                                                               int64_t ldop)                                                     \
+    { return small_hist_factor<T>(h, false, 0, 0, b0, count, k, V, ldv, ldvp, OUT, ldo, ldop, op, "small_hist_factor_apply"); }  \
+    lbfgs_b200_status lbfgs_b200_small_hist_log_density_##SUF(lbfgs_b200_small_hist* h, int64_t b0, int64_t count, int k,          \
+                                                               const T* X, int64_t ldx, int64_t ldxp, const T* MEAN, int64_t ldm, \
+                                                               double* out_host)                                                 \
+    { return small_hist_log_density<T>(h, b0, count, k, X, ldx, ldxp, MEAN, ldm, out_host); }
 
 LBFGS_B200_SMALL_KEEP(double, f64)
 LBFGS_B200_SMALL_KEEP(float, f32)

@@ -718,9 +718,15 @@ inline size_t small_factor_smem(int m, int elem)
     return sizeof(double) * (size_t)kSMaxWarps * kSGroup + (size_t)elem * 4 * (size_t)m * kSGroup + sizeof(double) * 3 * (size_t)m * m;
 }
 
-template <class T, bool GEN>
+// OP (LBFGS_B200_FACTOR_*): L as above; L' and L^-T take the dots of the c s rows only and combine over all 2c columns (a0 V, y by
+// age, s by age), L^-1 takes all 2c dots and combines over the s columns; a0 = 1/sqrt(theta) for L and L', sqrt(theta) for the
+// inverses.  The recursion of each op (compact_factor_t_coef / _inv_coef / _invt_coef, after compact_factor_upper for the inverses)
+// runs in fp64 in a per-thread array.
+template <class T, bool GEN, int OP = LBFGS_B200_FACTOR_L>
 __global__ void __launch_bounds__(kSMaxThreads) k_small_hist_factor(const SmallFactorArgs<T> a)
 {
+    constexpr bool kSDots = OP == LBFGS_B200_FACTOR_LT || OP == LBFGS_B200_FACTOR_LINVT;   // S'V only, combination over W
+    constexpr bool kInv = OP == LBFGS_B200_FACTOR_LINV || OP == LBFGS_B200_FACTOR_LINVT;
     extern __shared__ __align__(16) unsigned char s_smem[];
     __shared__ int s_ok;
     const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5;
@@ -734,7 +740,7 @@ __global__ void __launch_bounds__(kSMaxThreads) k_small_hist_factor(const SmallF
     const int c = a.hist_c[b];
     const T theta = rec[a.HL.theta()];
     const double rsq = 1.0 / sqrt((double)theta);
-    const T a0 = (T)rsq;
+    const T a0 = kInv ? (T)sqrt((double)theta) : (T)rsq;
     double* red = reinterpret_cast<double*>(s_smem);
     T* wv = reinterpret_cast<T*>(red + kSMaxWarps * kSGroup);        // [2c][kSGroup]
     T* C = wv + 2 * m * kSGroup;                                     // [2c][kSGroup]
@@ -758,7 +764,7 @@ __global__ void __launch_bounds__(kSMaxThreads) k_small_hist_factor(const SmallF
     if (c > 0)
     {
         // [Y S]'V, one history row at a time (the sums of k_small_hist_times)
-        for (int r = 0; r < 2 * c; r++)
+        for (int r = kSDots ? c : 0; r < 2 * c; r++)
         {
             const T* h = rec + (r < c ? a.HL.y(r) : a.HL.s(r - c));
             double acc[kSGroup];
@@ -790,13 +796,28 @@ __global__ void __launch_bounds__(kSMaxThreads) k_small_hist_factor(const SmallF
         {
             double ls;
             s_ok = LBFGSpp::compact_factor_setup(c, rec + a.HL.SY(), rec + a.HL.SS(), rec + a.HL.YY(), c, theta, beta, Tm, &ls) == 0;
+            if constexpr (kInv)
+                if (s_ok) LBFGSpp::compact_factor_upper(c, rec + a.HL.SY(), c, Tm);
         }
         __syncthreads();
         ok = s_ok != 0;
-        if (ok && tid < kk) LBFGSpp::compact_factor_coef(c, beta, Tm, rsq, wv + tid, kSGroup, C + tid, kSGroup);
+        if (ok && tid < kk)
+        {
+            if constexpr (OP == LBFGS_B200_FACTOR_L) LBFGSpp::compact_factor_coef(c, beta, Tm, rsq, wv + tid, kSGroup, C + tid, kSGroup);
+            else
+            {
+                double z[kMaxM];
+                const double sq = sqrt((double)theta);
+                if constexpr (OP == LBFGS_B200_FACTOR_LT)
+                    LBFGSpp::compact_factor_t_coef(c, beta, Tm, rsq, wv + c * kSGroup + tid, kSGroup, z, C + tid, kSGroup);
+                else if constexpr (OP == LBFGS_B200_FACTOR_LINV)
+                    LBFGSpp::compact_factor_inv_coef(c, beta, Tm, sq, wv + tid, kSGroup, z, C + tid, kSGroup);
+                else LBFGSpp::compact_factor_invt_coef(c, beta, Tm, sq, wv + c * kSGroup + tid, kSGroup, z, C + tid, kSGroup);
+            }
+        }
         __syncthreads();
     }
-    // OUT = [mean +] a0 V + sum_a cs_a s_a
+    // OUT = [mean +] a0 V [+ sum_a cy_a y_a] + sum_a cs_a s_a
     const T nan = (T)__longlong_as_double(0x7ff8000000000000ll);
     for (int64_t i = tid; i < n; i += nt)
     {
@@ -804,6 +825,13 @@ __global__ void __launch_bounds__(kSMaxThreads) k_small_hist_factor(const SmallF
         const T mi = mean ? mean[i] : T(0);
 #pragma unroll
         for (int j = 0; j < kSGroup; j++) r[j] = j < kk ? (mean ? mi + a0 * V[j * ldv + i] : a0 * V[j * ldv + i]) : T(0);
+        if constexpr (kSDots)
+            for (int q = 0; q < c; q++)
+            {
+                const T yv = rec[a.HL.y(q) + i];
+#pragma unroll
+                for (int j = 0; j < kSGroup; j++) r[j] += C[q * kSGroup + j] * yv;
+            }
         for (int q = 0; q < c; q++)
         {
             const T sv = rec[a.HL.s(q) + i];
@@ -830,6 +858,103 @@ template <class T> __global__ void k_small_hist_logdet(const T* hist, const int*
     double ls = 0.0;
     const int st = LBFGSpp::compact_factor_setup(c, rec + HL.SY(), rec + HL.SS(), rec + HL.YY(), c, theta, beta, beta + 2 * c * c, &ls);
     out[p] = st ? __longlong_as_double(0x7ff8000000000000ll) : -(double)HL.n * log((double)theta) + ls;
+}
+
+// log N(x_pj; mean_p, H_b) for problems b = b0 + p and points j: one CTA per (problem, group of <= kSGroup points), small_threads(n)
+// threads.  v_j = x_j - mean is formed in T; W'v_j and |v_j|^2 are summed in fp64 through the block sums of k_small_hist_factor (a
+// row of W at a time, then the points with themselves), thread 0 runs compact_factor_setup and compact_factor_upper, and thread j
+// the recursion of compact_factor_quad.  Every sum's order depends on n only, so a problem's values do not depend on b0, count, its
+// position or k.  NaN when the check fails.
+template <class T> struct SmallDensityArgs
+{
+    const T* hist;
+    const int* hist_c;
+    SmallHistLayout HL;
+    int64_t b0;
+    int k;
+    const T* X;                 // problem p's point j at X + p*ldxp + j*ldx
+    int64_t ldx, ldxp;
+    const T* MEAN;              // problem p's mean at MEAN + p*ldm
+    int64_t ldm;
+    double* out;                // [count][k]
+};
+
+// dynamic shared memory of k_small_hist_log_density (bytes): block sums, W'v and |v|^2 ((2m + 1) x kSGroup), beta and Tm, all in
+// double.  At most small_times_smem for m >= 2 and under 1 KB for m = 1, so any history small_hist_create accepts fits.
+inline size_t small_density_smem(int m)
+{
+    return sizeof(double) * ((size_t)kSMaxWarps * kSGroup + (2 * (size_t)m + 1) * kSGroup + 3 * (size_t)m * m);
+}
+
+template <class T>
+__global__ void __launch_bounds__(kSMaxThreads) k_small_hist_log_density(const SmallDensityArgs<T> a)
+{
+    extern __shared__ __align__(16) unsigned char s_smem[];
+    __shared__ int s_ok;
+    __shared__ double s_ls;
+    const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5;
+    const int64_t p = blockIdx.x, b = a.b0 + p, n = a.HL.n;
+    const int m = a.HL.m, j0 = blockIdx.y * kSGroup, kk = min(kSGroup, a.k - j0);
+    const T* rec = a.hist + b * a.HL.rec();
+    const T* X = a.X + p * a.ldxp + j0 * a.ldx;
+    const T* mean = a.MEAN + p * a.ldm;
+    const int c = a.hist_c[b];
+    const T theta = rec[a.HL.theta()];
+    double* red = reinterpret_cast<double*>(s_smem);
+    double* wv = red + kSMaxWarps * kSGroup;   // [2c + 1][kSGroup]: W'v, then |v|^2
+    double* beta = wv + (2 * m + 1) * kSGroup;
+    double* Tm = beta + 2 * m * m;
+    for (int r = 0; r <= 2 * c; r++)
+    {
+        const T* h = r < c ? rec + a.HL.y(r) : r < 2 * c ? rec + a.HL.s(r - c) : nullptr;
+        double acc[kSGroup];
+#pragma unroll
+        for (int j = 0; j < kSGroup; j++) acc[j] = 0.0;
+        for (int64_t i = tid; i < n; i += nt)
+        {
+            const T mi = mean[i];
+#pragma unroll
+            for (int j = 0; j < kSGroup; j++)
+                if (j < kk)
+                {
+                    const double v = (double)(X[j * a.ldx + i] - mi);
+                    acc[j] += (h ? (double)h[i] : v) * v;
+                }
+        }
+#pragma unroll
+        for (int j = 0; j < kSGroup; j++)
+        {
+            const double w = warp_sum(acc[j]);
+            if (lane == 0) red[warp * kSGroup + j] = w;
+        }
+        __syncthreads();
+        if (tid < kk)
+        {
+            double t = 0.0;
+            for (int w = 0; w < (nt >> 5); w++) t += red[w * kSGroup + tid];
+            wv[r * kSGroup + tid] = t;
+        }
+        __syncthreads();
+    }
+    if (tid == 0)
+    {
+        double ls = 0.0;
+        s_ok = LBFGSpp::compact_factor_setup(c, rec + a.HL.SY(), rec + a.HL.SS(), rec + a.HL.YY(), c, theta, beta, Tm, &ls) == 0;
+        if (s_ok) LBFGSpp::compact_factor_upper(c, rec + a.HL.SY(), c, Tm);
+        s_ls = ls;
+    }
+    __syncthreads();
+    if (tid < kk)
+    {
+        double z[kMaxM];
+        double r = __longlong_as_double(0x7ff8000000000000ll);
+        if (s_ok)
+        {
+            const double q = LBFGSpp::compact_factor_quad(c, beta, Tm, rec + a.HL.SS(), c, theta, wv + tid, kSGroup, wv[2 * c * kSGroup + tid], z);
+            r = LBFGSpp::compact_log_density(q, -(double)n * log((double)theta) + s_ls, (double)n);
+        }
+        a.out[p * a.k + j0 + tid] = r;
+    }
 }
 
 }  // namespace lb
