@@ -15,6 +15,8 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstdint>
+#include <limits>
 #include <stdexcept>
 #include <vector>
 
@@ -151,6 +153,86 @@ public:
     const Vector& final_grad() const { return m_grad; }
     Scalar final_grad_norm() const { return m_projgnorm; }
     long num_evaluations() const { return m_nfev; }
+
+    // The final quasi-Newton approximation over the whole space, with the names, contracts and exceptions of LBFGSSolver's members
+    // (BFGSMat: dense / hessian_times / hessian_diagonal / inverse_hessian_factor_* / sample / inverse_hessian_logdet / log_density).
+    // The last step's pair is not in the history (the loop returns before update()); after an in-loop BFGS reset the history may be
+    // empty, and then B = theta I and H = I/theta.  std::logic_error before the first minimize().
+    SmallMatrix<Scalar> final_approx_hessian() { m_bfgs.require_history(); return m_bfgs.dense(false); }
+    SmallMatrix<Scalar> final_approx_inverse_hessian() { m_bfgs.require_history(); return m_bfgs.dense(true); }
+    void final_approx_hessian_times(const Vector& V, Vector& OUT) { m_bfgs.require_history(); m_bfgs.hessian_times(V, count(V), OUT); }
+    void final_approx_inverse_hessian_times(const Vector& V, Vector& OUT) { m_bfgs.require_history(); m_bfgs.inverse_hessian_times(V, count(V), OUT); }
+    void final_approx_hessian_diagonal(Vector& out) { m_bfgs.require_history(); m_bfgs.hessian_diagonal(out); }
+    void final_approx_inverse_hessian_diagonal(Vector& out) { m_bfgs.require_history(); m_bfgs.inverse_hessian_diagonal(out); }
+    void final_approx_inverse_hessian_factor_times(const Vector& V, Vector& OUT)
+    {
+        m_bfgs.require_history();
+        m_bfgs.inverse_hessian_factor_times(V, count(V), OUT);
+    }
+    void final_approx_inverse_hessian_factor_transpose_times(const Vector& V, Vector& OUT)
+    {
+        m_bfgs.require_history();
+        m_bfgs.inverse_hessian_factor_transpose_times(V, count(V), OUT);
+    }
+    void final_approx_inverse_hessian_factor_solve(const Vector& V, Vector& OUT)
+    {
+        m_bfgs.require_history();
+        m_bfgs.inverse_hessian_factor_solve(V, count(V), OUT);
+    }
+    void final_approx_inverse_hessian_factor_transpose_solve(const Vector& V, Vector& OUT)
+    {
+        m_bfgs.require_history();
+        m_bfgs.inverse_hessian_factor_transpose_solve(V, count(V), OUT);
+    }
+    void final_approx_sample(const Vector& mean, unsigned long long seed, uint32_t first, int k, Vector& OUT)
+    {
+        m_bfgs.require_history();
+        m_bfgs.sample(&mean, seed, 0u, first, k, OUT);
+    }
+    double final_approx_inverse_hessian_logdet() { m_bfgs.require_history(); return m_bfgs.inverse_hessian_logdet(); }
+    std::vector<double> final_approx_log_density(const Vector& mean, const Vector& X)
+    {
+        m_bfgs.require_history();
+        return m_bfgs.log_density(mean, X, count(X));
+    }
+
+    // The approximation on the free variables F at the solution: B_F = Z'BZ and H_F = (Z'BZ)^-1, Z selecting F.  H_F is the
+    // covariance of N(x*, H) conditioned on the fixed coordinates staying where they are: the Laplace approximation on the face the
+    // solver stopped on.  final_approx_free_set marks F at x (normally the solution) and returns n_F: coordinate i is fixed when
+    // lb_i == ub_i or x_i lies within tol max(1, |bound|) of a finite bound (the solver does not clamp at exit, so x can miss a bound by
+    // an ulp), free otherwise.  The set lasts until the next minimize().  Then, with the rows outside F written as 0:
+    //   final_approx_free_hessian_times / _inverse_hessian_times: OUT = B_F V or H_F V for V holding k = V.size()/n vectors;
+    //   final_approx_free_hessian_diagonal / _inverse_hessian_diagonal: diag B_F, diag H_F (standard errors sqrt(diag H_F));
+    //   final_approx_free_inverse_hessian_logdet: log det H_F;
+    //   final_approx_free_sample: mean + L_F z_j on F and mean_i elsewhere for the k draws first .. first+k-1 of stream 0 (L_F L_F = H_F);
+    //   final_approx_free_log_density: log N(x_F; mean_F, H_F) for the k points of X; the fixed coordinates are ignored.
+    // std::logic_error before minimize() or before final_approx_free_set after the latest minimize(); when H_F cannot be formed,
+    // std::runtime_error from the products and the sampler and NaN from the log-determinant and the densities (BFGSMat::free_*).
+    int final_approx_free_set(const Vector& x, const Vector& lb, const Vector& ub, Scalar tol = 4 * std::numeric_limits<Scalar>::epsilon())
+    {
+        m_bfgs.require_history();
+        return int(m_bfgs.free_set(x, lb, ub, tol));
+    }
+    void final_approx_free_hessian_times(const Vector& V, Vector& OUT) { m_bfgs.free_hessian_times(V, free_count(V), OUT); }
+    void final_approx_free_inverse_hessian_times(const Vector& V, Vector& OUT) { m_bfgs.free_inverse_hessian_times(V, free_count(V), OUT); }
+    void final_approx_free_hessian_diagonal(Vector& out) { m_bfgs.free_hessian_diagonal(out); }
+    void final_approx_free_inverse_hessian_diagonal(Vector& out) { m_bfgs.free_inverse_hessian_diagonal(out); }
+    double final_approx_free_inverse_hessian_logdet() { return m_bfgs.free_inverse_hessian_logdet(); }
+    void final_approx_free_sample(const Vector& mean, unsigned long long seed, uint32_t first, int k, Vector& OUT)
+    {
+        m_bfgs.free_sample(&mean, seed, 0u, first, k, OUT);
+    }
+    std::vector<double> final_approx_free_log_density(const Vector& mean, const Vector& X) { return m_bfgs.free_log_density(mean, X, free_count(X)); }
+
+private:
+    int count(const Vector& V) const { return BFGSMat<Scalar, true>::block_count(V.size(), m_bfgs.dim()); }
+    // the block count after the free-set check, so that a call before the free set reports std::logic_error
+    int free_count(const Vector& V) const
+    {
+        m_bfgs.require_history();
+        if (m_bfgs.free_count() < 0) throw std::logic_error("LBFGSBSolver: no free set since the last minimize() (call final_approx_free_set)");
+        return count(V);
+    }
 };
 
 }  // namespace LBFGSpp

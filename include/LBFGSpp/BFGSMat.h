@@ -39,7 +39,7 @@ class BFGSMat
     BFGSMat& operator=(const BFGSMat&);
 
 public:
-    BFGSMat() : m_dev(nullptr), m_hist(nullptr), m_owned(true), m_n(0), m_m(0), m_algo(LBFGS_B200_HV_AUTO), m_theta_host(1), m_c_host(0), m_box(nullptr) {}
+    BFGSMat() : m_dev(nullptr), m_hist(nullptr), m_owned(true), m_n(0), m_m(0), m_algo(LBFGS_B200_HV_AUTO), m_theta_host(1), m_c_host(0), m_box(nullptr), m_nfree(-1) {}
     ~BFGSMat()
     {
         lbfgs_b200_box_destroy(m_box);
@@ -65,6 +65,7 @@ public:
         m_dev = &dev;
         m_n = n;
         m_m = m;
+        mark_free(-1);
         if (!m_hist)
             dev.check(lbfgs_b200_hist_create(dev.ctx(), &m_hist, n, m, int(sizeof(Scalar))));
         else
@@ -81,6 +82,7 @@ public:
         if (m_owned) lbfgs_b200_hist_destroy(m_hist);
         m_hist = hist;
         m_owned = false;
+        mark_free(-1);
         m_dev = &dev;
         m_n = n;
         m_m = m;
@@ -95,12 +97,14 @@ public:
     // BFGSMat.h:81-97
     void add_correction(const Vector& s, const Vector& y)
     {
+        m_free.level = 0;
         m_dev->check(detail::Abi<Scalar>::hist_add(m_hist, s.data(), y.data()));
     }
 
     // LBFGS.h:159-162 in one kernel; returns whether the pair passed the curvature gate
     bool update(const Vector& x, const Vector& xp, const Vector& g, const Vector& gp)
     {
+        m_free.level = 0;
         int accepted = 0;
         m_dev->check(detail::Abi<Scalar>::hist_update(m_hist, x.data(), xp.data(), g.data(), gp.data(),
                                                       std::numeric_limits<Scalar>::epsilon(), &accepted, nullptr));
@@ -128,6 +132,7 @@ public:
     Scalar update_apply_Hv_dot(const Vector& x, const Vector& xp, const Vector& g, const Vector& gp, const Scalar& a, Vector& res,
                                bool* accepted = nullptr)
     {
+        m_free.level = 0;
         res.resize(g.size());
         int acc = 0;
         Scalar vr = Scalar(0);
@@ -150,6 +155,17 @@ private:
     SmallMatrix<Scalar> m_Minv, m_M, m_SS, m_SY;
     BKLDLT<Scalar> m_Msolver;  // Minv is symmetric indefinite (reference BFGSMat.h:47,134-146)
     lbfgs_b200_box* m_box;
+    int64_t m_nfree;           // size of the free set marked by free_set(); -1: none since the last reset()
+    // the free-set setup kept between calls (free_setup): level 0 none, 1 K_B, 2 also K_HF, E and log det H_F; b_ok / h_ok: whether B_F /
+    // H_F could be formed
+    struct FreeSetup
+    {
+        int level = 0, c = 0;
+        bool b_ok = false, h_ok = false;
+        double theta = 1.0, logdet = 0.0;
+        std::vector<double> SY, SS, Minv, KB, KH, E;
+    };
+    FreeSetup m_free;
 
 public:
     lbfgs_b200_hist* handle() const { return m_hist; }
@@ -231,14 +247,7 @@ public:
         SmallMatrix<Scalar> G(2 * c, 2 * c);
         m_dev->check(detail::BoxAbi<Scalar>::hist_masked_gram(m_hist, box(), lbfgs_b200_box_classes(box()), mask, G.data()));
         SmallMatrix<Scalar> mid(2 * c, 2 * c);
-        for (int a = 0; a < c; a++)
-            for (int b = 0; b < c; b++)
-            {
-                mid(a, b) = m_Minv(a, b) - G(a, b) / theta;
-                mid(c + a, b) = m_Minv(c + a, b) - G(c + a, b);
-                mid(b, c + a) = mid(c + a, b);
-                mid(c + a, c + b) = theta * (m_SS(a, b) - G(c + a, c + b));
-            }
+        compact_free_mid(c, m_Minv.data(), m_SS.data(), c, G.data(), theta, mid.data());
         BKLDLT<Scalar> midsolver(mid);  // reference BFGSMat.h:551
         std::vector<Scalar> z = Wt_dot(v_dev);      // [Y_P'v ; theta*S_P'v]
         midsolver.solve_inplace(z);
@@ -270,6 +279,245 @@ public:
         lincomb(Scalar(0), nullptr, coef, mask, out_dev);
     }
 
+    //========== the final approximation on the free variables F of a bound-constrained solve ==========
+    // B_F = Z'BZ and H_F = (Z'BZ)^-1 (CompactForm.h, compact_free_mid / compact_free_kh / compact_free_sqrt; the 2c x 2c algebra in fp64
+    // whatever Scalar is), F the coordinates whose class byte carries LBFGS_B200_CLS_FINAL.  free_set marks F at a point x (see
+    // lbfgs_b200_box_final_classes) and returns n_F; free_set_classes takes F from n class bytes on the host instead.  Every other member
+    // works on the rows of F through the masked passes (lbfgs_b200_hist_*_masked), in groups of 16 vectors, with the rows outside F
+    // written as 0 (products, diagonals) or mean_i (draws):
+    //   free_hessian_times / free_inverse_hessian_times: OUT = B_F V or H_F V (V's rows outside F are not read);
+    //   free_hessian_diagonal / free_inverse_hessian_diagonal: diag B_F = diag B on F, diag H_F;
+    //   free_inverse_hessian_logdet: log det H_F = -n_F log theta + sum_i log(1 + sigma_i);
+    //   free_sample: mean + L_F z_j on F for the k draws first .. first+k-1 of stream `stream`, L_F the symmetric square root of H_F;
+    //   free_log_density: log N(x_F; mean_F, H_F) of the k points of X, from the masked dots of x_j - mean alone.
+    // The setup (K_B; for H_F also the masked Gram pass, K_HF, the square root and log det H_F) is formed on first use and kept until the
+    // free set or the history changes.  std::logic_error before free_set / free_set_classes (after a reset()).  When H_F cannot be formed
+    // (a singular middle matrix, or some 1 + sigma_i not positive and finite): std::runtime_error from the H_F products, diag H_F and the
+    // sampler, NaN from the log-determinant and the densities; when M itself cannot be formed, the B_F members throw as well.
+    int64_t free_set(const Vector& x, const Vector& lb, const Vector& ub, Scalar tol)
+    {
+        require_history();
+        if (x.size() != m_n || lb.size() != m_n || ub.size() != m_n) throw std::invalid_argument("x, lb and ub must hold n values");
+        int64_t nf = 0;
+        m_dev->check(detail::BoxAbi<Scalar>::final_classes(box(), x.data(), lb.data(), ub.data(), tol, &nf));
+        mark_free(nf);
+        return nf;
+    }
+    int64_t free_set_classes(const unsigned char* cls_host)
+    {
+        require_history();
+        m_dev->check(lbfgs_b200_memcpy_h2d(m_dev->ctx(), const_cast<unsigned char*>(lbfgs_b200_box_classes(box())), cls_host, size_t(m_n)));
+        int64_t nf = 0;
+        for (std::ptrdiff_t i = 0; i < m_n; i++) nf += (cls_host[i] & LBFGS_B200_CLS_FINAL) ? 1 : 0;
+        mark_free(nf);
+        return nf;
+    }
+    int64_t free_count() const { return m_nfree; }
+
+    void free_hessian_times(const Vector& V, int k, Vector& OUT) { free_times(V, k, OUT, false); }
+    void free_inverse_hessian_times(const Vector& V, int k, Vector& OUT) { free_times(V, k, OUT, true); }
+    void free_hessian_diagonal(Vector& out) { free_diagonal(out, false); }
+    void free_inverse_hessian_diagonal(Vector& out) { free_diagonal(out, true); }
+    double free_inverse_hessian_logdet() { return free_setup(true).logdet; }
+    void free_sample(const Vector* mean, unsigned long long seed, uint32_t stream, uint32_t first, int k, Vector& OUT)
+    {
+        require_free();
+        if (mean && mean->size() != m_n) throw std::invalid_argument("mean must hold n values");
+        if (k < 1 || uint64_t(first) + uint64_t(k) > (uint64_t(1) << 32)) throw std::invalid_argument("need k >= 1 and first + k <= 2^32");
+        const FreeSetup& f = free_setup(true);
+        if (!f.h_ok) throw std::runtime_error("BFGSMat: the kept pairs do not define a positive definite H_F");
+        const int c = f.c, w = 2 * c, kGroup = 16;
+        const double rsq = 1.0 / std::sqrt(f.theta);
+        OUT.resize(std::ptrdiff_t(k) * m_n);
+        std::vector<Scalar> Wv, C;
+        for (int j0 = 0; j0 < k; j0 += kGroup)
+        {
+            const int kk = std::min(kGroup, k - j0);
+            C.assign(size_t(std::max(1, w * kk)), Scalar(0));
+            if (c > 0)
+            {
+                Wv.assign(size_t(w * kk), Scalar(0));
+                m_dev->check(detail::BoxAbi<Scalar>::hist_wt_dot_normal_masked(m_hist, box(), classes(), LBFGS_B200_CLS_FINAL, seed, stream,
+                                                                                first + uint32_t(j0), kk, Wv.data()));
+                coef_times(w, kk, f.E.data(), rsq, Wv.data(), C.data());
+            }
+            m_dev->check(detail::BoxAbi<Scalar>::hist_lincomb_normal_masked(m_hist, box(), classes(), LBFGS_B200_CLS_FINAL, Scalar(rsq), seed,
+                                                                             stream, first + uint32_t(j0), kk, mean ? mean->data() : nullptr,
+                                                                             c > 0 ? C.data() : nullptr, OUT.data() + std::ptrdiff_t(j0) * m_n, m_n));
+        }
+    }
+    std::vector<double> free_log_density(const Vector& mean, const Vector& X, int k)
+    {
+        require_free();
+        if (mean.size() != m_n) throw std::invalid_argument("mean must hold n values");
+        if (block_count(X.size(), m_n) != k) throw std::invalid_argument("X.size() must be k * n");
+        const FreeSetup& f = free_setup(true);
+        std::vector<double> out(static_cast<size_t>(k), std::numeric_limits<double>::quiet_NaN());
+        if (!f.h_ok) return out;
+        const int w = 2 * f.c, kGroup = 16;
+        std::vector<double> Wv, nrm;
+        for (int j0 = 0; j0 < k; j0 += kGroup)
+        {
+            const int kk = std::min(kGroup, k - j0);
+            Wv.assign(size_t(std::max(1, w * kk)), 0.0);
+            nrm.assign(size_t(kk), 0.0);
+            m_dev->check(detail::BoxAbi<Scalar>::hist_wt_dot_diff_masked(m_hist, box(), classes(), LBFGS_B200_CLS_FINAL, kk,
+                                                                          X.data() + std::ptrdiff_t(j0) * m_n, m_n, mean.data(), Wv.data(), nrm.data()));
+            for (int j = 0; j < kk; j++)
+            {
+                double q = f.theta * nrm[size_t(j)];   // v_F'B_F v_F = theta |v_F|^2 + r'K_B r, r = W_F'v
+                for (int p = 0; p < w; p++)
+                {
+                    double kr = 0.0;
+                    for (int r = 0; r < w; r++) kr += f.KB[size_t(p * w + r)] * Wv[size_t(r * kk + j)];
+                    q += Wv[size_t(p * kk + j)] * kr;
+                }
+                out[size_t(j0 + j)] = compact_log_density(q, f.logdet, double(m_nfree));
+            }
+        }
+        return out;
+    }
+
+private:
+    const unsigned char* classes() { return lbfgs_b200_box_classes(box()); }
+    void require_free() const
+    {
+        require_history();
+        if (m_nfree < 0) throw std::logic_error("BFGSMat: no free set marked since the last minimize() (call final_approx_free_set)");
+    }
+    void mark_free(int64_t nf)
+    {
+        m_nfree = nf;
+        m_free.level = 0;
+    }
+
+    // C[p][j] = a * sum_q K[p][q] R[q][j] for kk vectors (K w x w in double, R and C [w][kk])
+    template <class TR>
+    static void coef_times(int w, int kk, const double* K, double a, const TR* R, Scalar* C)
+    {
+        for (int p = 0; p < w; p++)
+            for (int j = 0; j < kk; j++)
+            {
+                double acc = 0.0;
+                for (int q = 0; q < w; q++) acc += K[p * w + q] * double(R[q * kk + j]);
+                C[p * kk + j] = Scalar(a * acc);
+            }
+    }
+
+    // The kept setup, at level 1 (K_B) or 2 (also K_HF, E and log det H_F, which need the masked Gram pass); formed on first use.
+    const FreeSetup& free_setup(bool h)
+    {
+        require_free();
+        FreeSetup& f = m_free;
+        if (f.level >= (h ? 2 : 1)) return f;
+        refresh_middle();
+        const int c = m_c_host, w = 2 * c;
+        const size_t ww = size_t(std::max(1, w * w)), cc = static_cast<size_t>(c * c), ws = static_cast<size_t>(w);
+        if (f.level == 0)
+        {
+            f.c = c;
+            f.theta = double(m_theta_host);
+            f.KB.assign(ww, 0.0);
+            f.SY.assign(std::max<size_t>(1, cc), 0.0);
+            f.SS.assign(std::max<size_t>(1, cc), 0.0);
+            f.Minv.assign(ww, 0.0);
+            f.b_ok = true;
+            if (c > 0)
+            {
+                std::vector<double> M(ww), z(ws), unit(2 * ws - 1, 0.0);
+                for (size_t e = 0; e < cc; e++) { f.SY[e] = double(m_SY.data()[e]); f.SS[e] = double(m_SS.data()[e]); }
+                compact_minv(c, f.SY.data(), f.SS.data(), c, f.theta, f.Minv.data());
+                std::vector<int> order(ws);
+                std::vector<unsigned char> tag(ws);
+                std::vector<double> fac(f.Minv);
+                f.b_ok = bk_factor(fac.data(), w, order.data(), tag.data()) == 0;
+                if (f.b_ok)
+                {
+                    for (int r = 0; r < w; r++)
+                    {
+                        for (int i = 0; i < w; i++) M[size_t(i * w + r)] = i == r ? 1.0 : 0.0;
+                        bk_solve(fac.data(), w, order.data(), tag.data(), M.data() + r, w, z.data());
+                    }
+                    unit[ws - 1] = 1.0;
+                    compact_kb(c, M.data(), f.theta, unit.data(), 0, 1, f.KB.data());
+                    compact_k_symmetrise(w, f.KB.data(), 0, 1);
+                    for (size_t e = 0; e < ww; e++) f.b_ok = f.b_ok && std::isfinite(f.KB[e]);
+                }
+            }
+            f.level = 1;
+        }
+        if (h)
+        {
+            f.KH.assign(ww, 0.0);
+            f.E.assign(ww, 0.0);
+            f.h_ok = f.b_ok;
+            double ls = 0.0;
+            if (c > 0 && f.h_ok)
+            {
+                std::vector<double> G(ww), mid(ww), z(ws), scratch(size_t(5 * w * w + 3 * w));
+                std::vector<int> order(ws);
+                std::vector<unsigned char> tag(ws);
+                std::vector<Scalar> Gs(ww);
+                m_dev->check(detail::BoxAbi<Scalar>::hist_masked_gram(m_hist, box(), classes(), LBFGS_B200_CLS_FINAL, Gs.data()));
+                for (size_t e = 0; e < ww; e++) G[e] = double(Gs[e]);
+                compact_free_mid(c, f.Minv.data(), f.SS.data(), c, G.data(), f.theta, mid.data());
+                f.h_ok = compact_free_kh(c, mid.data(), f.theta, order.data(), tag.data(), z.data(), f.KH.data()) == 0 &&
+                         compact_free_sqrt(w, G.data(), f.KH.data(), f.theta, f.E.data(), &ls, scratch.data()) == 0;
+            }
+            f.logdet = -double(m_nfree) * std::log(f.theta) + ls;
+            f.h_ok = f.h_ok && std::isfinite(f.logdet);
+            for (size_t e = 0; e < ww && f.h_ok; e++) f.h_ok = std::isfinite(f.KH[e]) && std::isfinite(f.E[e]);
+            if (!f.h_ok) f.logdet = std::numeric_limits<double>::quiet_NaN();
+            f.level = 2;
+        }
+        return f;
+    }
+
+    const FreeSetup& checked_setup(bool inverse)
+    {
+        const FreeSetup& f = free_setup(inverse);
+        if (inverse ? !f.h_ok : !f.b_ok)
+            throw std::runtime_error(inverse ? "BFGSMat: the kept pairs do not define a positive definite H_F" : "BFGSMat: singular middle matrix");
+        return f;
+    }
+
+    void free_diagonal(Vector& out, bool inverse)
+    {
+        const FreeSetup& f = checked_setup(inverse);
+        const int w = 2 * f.c;
+        std::vector<Scalar> K(size_t(std::max(1, w * w)));
+        for (int e = 0; e < w * w; e++) K[size_t(e)] = Scalar(inverse ? f.KH[size_t(e)] : f.KB[size_t(e)]);
+        out.resize(m_n);
+        m_dev->check(detail::BoxAbi<Scalar>::hist_quad_diag_masked(m_hist, box(), classes(), LBFGS_B200_CLS_FINAL,
+                                                                    Scalar(inverse ? 1.0 / f.theta : f.theta), w > 0 ? K.data() : nullptr, out.data()));
+    }
+
+    void free_times(const Vector& V, int k, Vector& OUT, bool inverse)
+    {
+        require_free();
+        if (block_count(V.size(), m_n) != k) throw std::invalid_argument("V.size() must be k * n");
+        const FreeSetup& f = checked_setup(inverse);
+        const int c = f.c, w = 2 * c, kGroup = 16;
+        OUT.resize(V.size());
+        std::vector<Scalar> Wv, C;
+        for (int j0 = 0; j0 < k; j0 += kGroup)
+        {
+            const int kk = std::min(kGroup, k - j0);
+            const Scalar* v = V.data() + std::ptrdiff_t(j0) * m_n;
+            C.assign(size_t(std::max(1, w * kk)), Scalar(0));
+            if (c > 0)
+            {
+                Wv.assign(size_t(w * kk), Scalar(0));
+                m_dev->check(detail::BoxAbi<Scalar>::hist_wt_dot_multi_masked(m_hist, box(), classes(), LBFGS_B200_CLS_FINAL, kk, v, m_n, Wv.data()));
+                coef_times(w, kk, inverse ? f.KH.data() : f.KB.data(), 1.0, Wv.data(), C.data());
+            }
+            m_dev->check(detail::BoxAbi<Scalar>::hist_lincomb_multi_masked(m_hist, box(), classes(), LBFGS_B200_CLS_FINAL,
+                                                                            Scalar(inverse ? 1.0 / f.theta : f.theta), kk, v, m_n,
+                                                                            c > 0 ? C.data() : nullptr, OUT.data() + std::ptrdiff_t(j0) * m_n, m_n));
+        }
+    }
+
+public:
     // Explicit n x n approximations for small n (final_approx_hessian / final_approx_inverse_hessian of the reference,
     // BFGSMat.h:150-271), through the compact representation:
     //   B = theta*I - W M W'                with the Minv above,

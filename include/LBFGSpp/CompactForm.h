@@ -421,6 +421,161 @@ LBFGS_HD inline double compact_log_density(double q, double logdet, double n)
     return -0.5 * q - 0.5 * logdet - 0.5 * n * 1.8378770664093453;   // log(2 pi)
 }
 
+// ---- the approximation restricted to a set F of coordinates: B_F = Z'BZ and H_F = (Z'BZ)^-1, Z selecting F -----------------------
+// With G = W_F'W_F the Gram matrix of the rows of F (raw W = [Y S] by age, 2c x 2c), Woodbury on B_F = theta I - W_F M W_F' (W in
+// [Y, theta S]) gives H_F = I/theta + W_F mid^-1 W_F' / theta^2 with
+//     mid = Minv - W_F'W_F / theta   (in W's [Y, theta S] convention; solve_PtBP's inv(P'BP))
+// and over the raw columns, with D = diag(I, theta I):
+//     B_F = theta I + W_F K_B W_F',  K_B = -D M D (compact_kb);     H_F = I/theta + W_F K_HF W_F',  K_HF = D mid^-1 D / theta^2.
+// diag B_F is diag B on F (a principal submatrix), diag H_F_i = 1/theta + r_i' K_HF r_i.  H_F is also the covariance of N(x*, H)
+// conditioned on the coordinates outside F.
+
+// mid [2c x 2c] row-major from Minv, the S'S block by age (leading dimension ldg) and the masked Gram G [2c x 2c]
+template <typename T>
+LBFGS_HD inline void compact_free_mid(int c, const T* Minv, const T* SS, int ldg, const T* G, T theta, T* mid)
+{
+    const int w = 2 * c;
+    for (int a = 0; a < c; a++)
+        for (int b = 0; b < c; b++)
+        {
+            mid[a * w + b] = Minv[a * w + b] - G[a * w + b] / theta;
+            mid[(c + a) * w + b] = Minv[(c + a) * w + b] - G[(c + a) * w + b];
+            mid[b * w + c + a] = mid[(c + a) * w + b];
+            mid[(c + a) * w + c + b] = theta * (SS[a * ldg + b] - G[(c + a) * w + c + b]);
+        }
+}
+
+// Host only: K_HF [2c x 2c] = D mid^-1 D / theta^2, symmetrised.  mid is factorised in place; order, tag, z: 2c elements of scratch each.
+// Returns bk_factor's status (0, or 2 when mid is singular: K is then not written).
+inline int compact_free_kh(int c, double* mid, double theta, int* order, unsigned char* tag, double* z, double* K)
+{
+    const int w = 2 * c;
+    if (const int st = bk_factor(mid, w, order, tag)) return st;
+    for (int r = 0; r < w; r++)
+    {
+        for (int i = 0; i < w; i++) K[i * w + r] = i == r ? 1.0 : 0.0;
+        bk_solve(mid, w, order, tag, K + r, w, z);
+        const double dr = r < c ? 1.0 : theta;
+        for (int i = 0; i < w; i++) K[i * w + r] *= dr * (i < c ? 1.0 : theta) / (theta * theta);
+    }
+    compact_k_symmetrise(w, K, 0, 1);
+    return 0;
+}
+
+// Host only: A = V diag(lam) V' for a symmetric n x n A (row-major, destroyed) by cyclic Jacobi rotations; V row-major, eigenvector j in column j.
+inline void sym_eig_jacobi(int n, double* A, double* V, double* lam)
+{
+    for (int i = 0; i < n * n; i++) V[i] = 0.0;
+    for (int i = 0; i < n; i++) V[i * n + i] = 1.0;
+    for (int sweep = 0; sweep < 100; sweep++)
+    {
+        double off = 0.0, tot = 0.0;
+        for (int i = 0; i < n; i++)
+            for (int j = 0; j < n; j++) (i == j ? tot : off) += A[i * n + j] * A[i * n + j];
+        if (!(off > 1e-30 * (tot + off))) break;
+        for (int p = 0; p < n - 1; p++)
+            for (int q = p + 1; q < n; q++)
+            {
+                const double apq = A[p * n + q];
+                if (apq == 0.0) continue;
+                const double tau = (A[q * n + q] - A[p * n + p]) / (2.0 * apq);
+                const double t = (tau >= 0.0 ? 1.0 : -1.0) / (std::fabs(tau) + std::sqrt(1.0 + tau * tau));
+                const double cs = 1.0 / std::sqrt(1.0 + t * t), sn = t * cs;
+                for (int k = 0; k < n; k++)   // A <- J'A J with J the rotation in the (p, q) plane
+                {
+                    const double akp = A[k * n + p], akq = A[k * n + q];
+                    A[k * n + p] = cs * akp - sn * akq;
+                    A[k * n + q] = sn * akp + cs * akq;
+                }
+                for (int k = 0; k < n; k++)
+                {
+                    const double apk = A[p * n + k], aqk = A[q * n + k];
+                    A[p * n + k] = cs * apk - sn * aqk;
+                    A[q * n + k] = sn * apk + cs * aqk;
+                }
+                for (int k = 0; k < n; k++)
+                {
+                    const double vkp = V[k * n + p], vkq = V[k * n + q];
+                    V[k * n + p] = cs * vkp - sn * vkq;
+                    V[k * n + q] = sn * vkp + cs * vkq;
+                }
+            }
+    }
+    for (int i = 0; i < n; i++) lam[i] = A[i * n + i];
+}
+
+// Host only: a symmetric square root of H_F: L_F = (I + W_F E W_F') / sqrt(theta) with L_F L_F = H_F, and log det H_F = -n_F log theta + *logsum.
+// G = W_F'W_F is equilibrated first, Gs = D G D with D = diag(G)^-1/2 (0 for a column that is zero on F): the y and s columns differ in
+// size by the curvature (|y| ~ theta |s|), and a cut on the raw G would drop the directions of the smaller set once theta is far
+// from 1.  Gs = V Lambda V' (eigenvalues <= 2c 2^-52 lambda_max dropped: W_F may be rank-deficient, e.g. n_F < 2c), Q = D^-1 V
+// Lambda^1/2, A = theta Q' K_HF Q = U Sigma U', R = D V Lambda^-1/2 U, E = R (sqrt(1 + Sigma) - 1) R', *logsum = sum log(1 + sigma).
+// G, K: w x w (w = 2c), E written w x w; scratch: 5 w^2 + 3 w doubles.  Returns 0, or 2 when some 1 + sigma_i is not positive and
+// finite (E is then not written).
+inline int compact_free_sqrt(int w, const double* G, const double* K, double theta, double* E, double* logsum, double* scratch)
+{
+    double *A = scratch, *V = A + w * w, *U = V + w * w, *Q = U + w * w, *R = Q + w * w, *lam = R + w * w, *sig = lam + w, *dg = sig + w;
+    for (int i = 0; i < w; i++) dg[i] = G[i * w + i] > 0.0 ? std::sqrt(G[i * w + i]) : 0.0;   // D^-1
+    for (int i = 0; i < w; i++)
+        for (int j = 0; j < w; j++) A[i * w + j] = dg[i] > 0.0 && dg[j] > 0.0 ? G[i * w + j] / (dg[i] * dg[j]) : 0.0;
+    sym_eig_jacobi(w, A, V, lam);
+    double lmax = 0.0;
+    for (int i = 0; i < w; i++) lmax = lam[i] > lmax ? lam[i] : lmax;
+    auto kept = [&](int i) { return lmax > 0.0 && lam[i] > double(w) * 2.220446049250313e-16 * lmax; };
+    int r = 0;   // Q = D^-1 V_r Lambda_r^1/2 and R without U: D V_r Lambda_r^-1/2 (w x r, columns packed; rows of zero columns are 0)
+    for (int i = 0; i < w; i++)
+        if (kept(i))
+        {
+            const double sl = std::sqrt(lam[i]);
+            for (int k = 0; k < w; k++)
+            {
+                Q[k * w + r] = dg[k] * V[k * w + i] * sl;
+                R[k * w + r] = dg[k] > 0.0 ? V[k * w + i] / (dg[k] * sl) : 0.0;
+            }
+            r++;
+        }
+    for (int a = 0; a < r; a++)   // A = theta Q' K Q  (r x r, leading dimension r)
+        for (int b = 0; b < r; b++)
+        {
+            double acc = 0.0;
+            for (int p = 0; p < w; p++)
+            {
+                double kq = 0.0;
+                for (int q = 0; q < w; q++) kq += K[p * w + q] * Q[q * w + b];
+                acc += Q[p * w + a] * kq;
+            }
+            A[a * r + b] = theta * acc;
+        }
+    for (int a = 0; a < r; a++)
+        for (int b = a + 1; b < r; b++) A[a * r + b] = A[b * r + a] = 0.5 * (A[a * r + b] + A[b * r + a]);
+    sym_eig_jacobi(r, A, U, sig);
+    *logsum = 0.0;
+    for (int i = 0; i < r; i++)
+    {
+        const double d = 1.0 + sig[i];
+        if (!(d > 0.0 && d <= 1.7976931348623157e308)) return 2;
+        *logsum += std::log1p(sig[i]);
+    }
+    for (int k = 0; k < w; k++)   // R <- R U
+    {
+        double row[128];
+        for (int j = 0; j < r; j++)
+        {
+            double acc = 0.0;
+            for (int i = 0; i < r; i++) acc += R[k * w + i] * U[i * r + j];
+            row[j] = acc;
+        }
+        for (int j = 0; j < r; j++) R[k * w + j] = row[j];
+    }
+    for (int p = 0; p < w; p++)
+        for (int q = 0; q < w; q++)
+        {
+            double acc = 0.0;
+            for (int j = 0; j < r; j++) acc += R[p * w + j] * (std::sqrt(1.0 + sig[j]) - 1.0) * R[q * w + j];
+            E[p * w + q] = acc;
+        }
+    return 0;
+}
+
 }  // namespace LBFGSpp
 
 #endif  // LBFGSPP_B200_COMPACT_FORM_H

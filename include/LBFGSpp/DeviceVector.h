@@ -133,6 +133,13 @@ template <class Scalar> struct BoxAbi;
         static lbfgs_b200_status hist_s_dot_multi(lbfgs_b200_hist* h, int k, const T* V, int64_t ldv, T* R) { return lbfgs_b200_hist_s_dot_multi_##SUF(h, k, V, ldv, R); } \
         static lbfgs_b200_status hist_wt_dot_diff(lbfgs_b200_hist* h, int k, const T* X, int64_t ldx, const T* mean, double* R, double* nrm) { return lbfgs_b200_hist_wt_dot_diff_##SUF(h, k, X, ldx, mean, R, nrm); } \
         static lbfgs_b200_status hist_lincomb_normal(lbfgs_b200_hist* h, T a0, uint64_t seed, uint32_t stream, uint32_t first, int k, const T* mean, const T* C, T* OUT, int64_t ldo) { return lbfgs_b200_hist_lincomb_normal_##SUF(h, a0, seed, stream, first, k, mean, C, OUT, ldo); } \
+        static lbfgs_b200_status hist_wt_dot_multi_masked(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, int mask, int k, const T* V, int64_t ldv, T* R) { return lbfgs_b200_hist_wt_dot_multi_masked_##SUF(h, b, cls, mask, k, V, ldv, R); } \
+        static lbfgs_b200_status hist_wt_dot_diff_masked(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, int mask, int k, const T* X, int64_t ldx, const T* mean, double* R, double* nrm) { return lbfgs_b200_hist_wt_dot_diff_masked_##SUF(h, b, cls, mask, k, X, ldx, mean, R, nrm); } \
+        static lbfgs_b200_status hist_wt_dot_normal_masked(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, int mask, uint64_t seed, uint32_t stream, uint32_t first, int k, T* R) { return lbfgs_b200_hist_wt_dot_normal_masked_##SUF(h, b, cls, mask, seed, stream, first, k, R); } \
+        static lbfgs_b200_status hist_lincomb_multi_masked(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, int mask, T a0, int k, const T* V, int64_t ldv, const T* C, T* OUT, int64_t ldo) { return lbfgs_b200_hist_lincomb_multi_masked_##SUF(h, b, cls, mask, a0, k, V, ldv, C, OUT, ldo); } \
+        static lbfgs_b200_status hist_lincomb_normal_masked(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, int mask, T a0, uint64_t seed, uint32_t stream, uint32_t first, int k, const T* mean, const T* C, T* OUT, int64_t ldo) { return lbfgs_b200_hist_lincomb_normal_masked_##SUF(h, b, cls, mask, a0, seed, stream, first, k, mean, C, OUT, ldo); } \
+        static lbfgs_b200_status hist_quad_diag_masked(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, int mask, T a0, const T* K, T* out) { return lbfgs_b200_hist_quad_diag_masked_##SUF(h, b, cls, mask, a0, K, out); } \
+        static lbfgs_b200_status final_classes(lbfgs_b200_box* b, const T* x, const T* lb, const T* ub, T tol, int64_t* nfree) { return lbfgs_b200_box_final_classes_##SUF(b, x, lb, ub, tol, nfree); } \
         static lbfgs_b200_status cauchy_breaks(lbfgs_b200_box* b, const T* x, const T* g, const T* lb, const T* ub, T* o5) { return lbfgs_b200_box_cauchy_breaks_##SUF(b, x, g, lb, ub, o5); } \
         static lbfgs_b200_status cauchy_sweep(lbfgs_b200_box* b, const T* g, const T* M, const T* p0, T theta, T gt, int64_t nord, int64_t ninf, T* out) { return lbfgs_b200_box_cauchy_sweep_##SUF(b, g, M, p0, theta, gt, nord, ninf, out); } \
         static lbfgs_b200_status cauchy_build(lbfgs_b200_box* b, const T* x, const T* lb, const T* ub, T tc, T tf, T* cnt) { return lbfgs_b200_box_cauchy_build_##SUF(b, x, lb, ub, tc, tf, cnt); } \

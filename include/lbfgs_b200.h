@@ -186,6 +186,8 @@ enum { LBFGS_B200_SUB_INIT = 0, LBFGS_B200_SUB_ACT_DIR = 1, LBFGS_B200_SUB_ADD_G
        LBFGS_B200_SUB_CHECK_BOUNDS = 4, LBFGS_B200_SUB_CLASSIFY = 5, LBFGS_B200_SUB_LU_VEC = 6, LBFGS_B200_SUB_RHS_P = 7,
        LBFGS_B200_SUB_FREE_VEC = 8, LBFGS_B200_SUB_MULTIPLIERS = 9, LBFGS_B200_SUB_CONVERGED = 10,
        LBFGS_B200_SUB_WRITE_DRT = 11 };
+/* class bit of the free set at a solution (lbfgs_b200_box_final_classes); bits 1 to 32 belong to Cauchy and the subspace step */
+enum { LBFGS_B200_CLS_FINAL = 64 };
 /* work vectors of the box workspace, for lbfgs_b200_box_vector() */
 enum { LBFGS_B200_BOXV_VECC = 0, LBFGS_B200_BOXV_VECY = 1, LBFGS_B200_BOXV_LAMBDA = 2, LBFGS_B200_BOXV_MU = 3,
        LBFGS_B200_BOXV_TMP = 4, LBFGS_B200_BOXV_TMP2 = 5, LBFGS_B200_BOXV_YFB = 6, LBFGS_B200_BOXV_DVEC = 7,
@@ -259,6 +261,36 @@ void* lbfgs_b200_box_vector(lbfgs_b200_box* b, int which);               /* LBFG
     lbfgs_b200_status lbfgs_b200_hist_s_dot_multi_##SUF(lbfgs_b200_hist* h, int k, const T* V, int64_t ldv, T* R_host);      \
     lbfgs_b200_status lbfgs_b200_hist_wt_dot_diff_##SUF(lbfgs_b200_hist* h, int k, const T* X, int64_t ldx, const T* mean,    \
                                                         double* R_host, double* nrm_host);                                   \
+    /* The final approximation on the free variables of a bound-constrained solve (LBFGSBSolver::final_approx_free_*): the     \
+     * passes above restricted to the rows i with (cls_i & mask) != 0, cls the class bytes of box b (of history h).  Each keeps  \
+     * its twin's order, so with every row in the mask it computes its twin's bits, and follows its twin's rules (1 <= k <= 16,  \
+     * leading dimensions, replicas only).  wt_dot_multi / wt_dot_diff / wt_dot_normal: the vector rows outside the mask count   \
+     * as 0 (the norms of wt_dot_diff too).  lincomb_multi: OUT rows outside the mask are written as 0.  lincomb_normal: reads   \
+     * every row of C_host (y and s), OUT rows outside the mask are mean_i (0 when mean is NULL).  quad_diag: out_i = 0 outside  \
+     * the mask.                                                                                                                */ \
+    lbfgs_b200_status lbfgs_b200_hist_wt_dot_multi_masked_##SUF(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, \
+                                                                int mask, int k, const T* V, int64_t ldv, T* R_host);          \
+    lbfgs_b200_status lbfgs_b200_hist_wt_dot_diff_masked_##SUF(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls,  \
+                                                               int mask, int k, const T* X, int64_t ldx, const T* mean,        \
+                                                               double* R_host, double* nrm_host);                              \
+    lbfgs_b200_status lbfgs_b200_hist_wt_dot_normal_masked_##SUF(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, \
+                                                                 int mask, uint64_t seed, uint32_t stream, uint32_t first,     \
+                                                                 int k, T* R_host);                                            \
+    lbfgs_b200_status lbfgs_b200_hist_lincomb_multi_masked_##SUF(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, \
+                                                                 int mask, T a0, int k, const T* V, int64_t ldv,               \
+                                                                 const T* C_host, T* OUT, int64_t ldo);                        \
+    lbfgs_b200_status lbfgs_b200_hist_lincomb_normal_masked_##SUF(lbfgs_b200_hist* h, lbfgs_b200_box* b,                      \
+                                                                  const unsigned char* cls, int mask, T a0, uint64_t seed,     \
+                                                                  uint32_t stream, uint32_t first, int k, const T* mean,      \
+                                                                  const T* C_host, T* OUT, int64_t ldo);                       \
+    lbfgs_b200_status lbfgs_b200_hist_quad_diag_masked_##SUF(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls,   \
+                                                             int mask, T a0, const T* K_host, T* out);                         \
+    /* The free set at a solution x: LBFGS_B200_CLS_FINAL set in the class bytes of the free coordinates and cleared elsewhere   \
+     * (the other bits are kept).  Coordinate i is fixed when lb_i == ub_i, x_i <= lb_i + tol max(1, |lb_i|) or                 \
+     * x_i >= ub_i - tol max(1, |ub_i|) (infinite bounds never fix); *nfree_host = the number of free ones.  Cauchy rebuilds   \
+     * the class bytes, so the set lasts until the next iteration of a solve.                                                  */ \
+    lbfgs_b200_status lbfgs_b200_box_final_classes_##SUF(lbfgs_b200_box* b, const T* x, const T* lb, const T* ub, T tol,      \
+                                                         int64_t* nfree_host);                                                 \
     /* Cauchy.h:111-129: breakpoints, d = -g on movable coordinates, class bytes.                                      \
      * out5 = { #fixed, #never-bounded, #with a finite breakpoint, d.d, smallest breakpoint } */                       \
     lbfgs_b200_status lbfgs_b200_box_cauchy_breaks_##SUF(lbfgs_b200_box*, const T* x, const T* g, const T* lb, \

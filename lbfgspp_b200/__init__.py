@@ -141,6 +141,16 @@ def _declare(lib):
         if hasattr(lib, "lbfgs_b200_hist_s_dot_multi_" + suf):    # the whitening passes (a test double of the ABI may lack them)
             getattr(lib, "lbfgs_b200_hist_s_dot_multi_" + suf).argtypes = [vp, ci, vp, i64, pt]
             getattr(lib, "lbfgs_b200_hist_wt_dot_diff_" + suf).argtypes = [vp, ci, vp, i64, vp, C.POINTER(C.c_double), C.POINTER(C.c_double)]
+        if hasattr(lib, "lbfgs_b200_box_final_classes_" + suf):   # the free-set passes (a test double of the ABI may lack them)
+            u64, u32, cls = C.c_uint64, C.c_uint32, C.POINTER(C.c_ubyte)
+            getattr(lib, "lbfgs_b200_hist_wt_dot_multi_masked_" + suf).argtypes = [vp, vp, vp, ci, ci, vp, i64, pt]
+            getattr(lib, "lbfgs_b200_hist_wt_dot_diff_masked_" + suf).argtypes = [vp, vp, vp, ci, ci, vp, i64, vp, C.POINTER(C.c_double),
+                                                                                  C.POINTER(C.c_double)]
+            getattr(lib, "lbfgs_b200_hist_wt_dot_normal_masked_" + suf).argtypes = [vp, vp, vp, ci, u64, u32, u32, ci, pt]
+            getattr(lib, "lbfgs_b200_hist_lincomb_multi_masked_" + suf).argtypes = [vp, vp, vp, ci, ct, ci, vp, i64, pt, vp, i64]
+            getattr(lib, "lbfgs_b200_hist_lincomb_normal_masked_" + suf).argtypes = [vp, vp, vp, ci, ct, u64, u32, u32, ci, vp, pt, vp, i64]
+            getattr(lib, "lbfgs_b200_hist_quad_diag_masked_" + suf).argtypes = [vp, vp, vp, ci, ct, pt, vp]
+            getattr(lib, "lbfgs_b200_box_final_classes_" + suf).argtypes = [vp, vp, vp, vp, ct, C.POINTER(i64)]
         getattr(lib, "lbfgs_b200_box_cauchy_breaks_" + suf).argtypes = [vp, vp, vp, vp, vp, pt]
         getattr(lib, "lbfgs_b200_box_cauchy_sweep_" + suf).argtypes = [vp, vp, pt, pt, ct, ct, i64, i64, pt]
         getattr(lib, "lbfgs_b200_box_cauchy_build_" + suf).argtypes = [vp, vp, vp, vp, ct, ct, pt]
@@ -315,6 +325,14 @@ def _declare_driver(lib):
         for suf, pt in (("f64", dp), ("f32", fp)):
             getattr(lib, "lbfgsb200_drv_small_batch_hessian_whiten_" + suf).argtypes = [ci, ci, cl, cl, pt, pt, pt, cl, ci, prm, pt, ci, ci, pt, pt,
                                                                                        ci, pt, pt, dp, cl, C.POINTER(_SmallItem), err, errlen]
+    # the final approximation of a bound-constrained solve (csrc/driver_box_hessian.cpp)
+    if hasattr(lib, "lbfgsb200_drv_box_hessian_f64"):
+        u64, u32 = C.c_uint64, C.c_uint32
+        for suf, pt in (("f64", dp), ("f32", fp)):
+            getattr(lib, "lbfgsb200_drv_box_hessian_" + suf).argtypes = [ci, ci, cl, prm, pt, pt, pt, ci, C.c_double, ci, ci, pt, pt, C.c_ulonglong,
+                                                                         C.c_uint, pt, dp, dp, C.POINTER(cl), C.POINTER(ci), err, errlen]
+        lib.lbfgsb200_drv_box_hist_hessian_f64.argtypes = [ci, cl, ci, ci, dp, dp, ci, C.POINTER(C.c_ubyte), ci, ci, dp, dp, C.c_ulonglong,
+                                                           C.c_uint, dp, dp, dp, C.POINTER(cl), err, errlen]
     lib._drv_typed = True
     return lib
 
@@ -704,6 +722,52 @@ class History:
                                                                                         nrm.ctypes.data_as(dp)))
         return R[:2 * c * k].reshape(2 * c, k), nrm
 
+    # The masked forms (lbfgs_b200_hist_*_masked): the passes above on the rows whose class byte in `box` (a Box of this history)
+    # intersects `mask`; the vector rows outside count as 0, output rows outside are 0 (mean_i for lincomb_normal_masked).
+    def _masked(self, name):
+        return getattr(self.ctx.lib, "lbfgs_b200_hist_%s_masked_%s" % (name, self.suf))
+
+    def _cls(self, box):
+        return box._ptr("cls")
+
+    def wt_dot_multi_masked(self, box, mask, V, k, ldv):
+        c = self.ncorr
+        R = (self.ct * max(1, 2 * c * k))()
+        self.ctx.check(self._masked("wt_dot_multi")(self.h, box.h, self._cls(box), mask, k, V.ptr, ldv, R))
+        return np.array(R[:2 * c * k], dtype=self.dtype).reshape(2 * c, k)
+
+    def wt_dot_diff_masked(self, box, mask, X, k, ldx, mean):
+        c = self.ncorr
+        R = np.zeros(max(1, 2 * c * k))
+        nrm = np.zeros(k)
+        dp = C.POINTER(C.c_double)
+        self.ctx.check(self._masked("wt_dot_diff")(self.h, box.h, self._cls(box), mask, k, X.ptr, ldx, mean.ptr, R.ctypes.data_as(dp),
+                                                   nrm.ctypes.data_as(dp)))
+        return R[:2 * c * k].reshape(2 * c, k), nrm
+
+    def wt_dot_normal_masked(self, box, mask, seed, stream, first, k):
+        c = self.ncorr
+        R = (self.ct * max(1, 2 * c * k))()
+        self.ctx.check(self._masked("wt_dot_normal")(self.h, box.h, self._cls(box), mask, seed, stream, first, k, R))
+        return np.array(R[:2 * c * k], dtype=self.dtype).reshape(2 * c, k)
+
+    def lincomb_multi_masked(self, box, mask, a0, V, k, ldv, C_coef, OUT, ldo):
+        coef = np.ascontiguousarray(C_coef, dtype=self.dtype).reshape(-1)
+        self.ctx.check(self._masked("lincomb_multi")(self.h, box.h, self._cls(box), mask, a0, k, V.ptr, ldv,
+                                                     coef.ctypes.data_as(C.POINTER(self.ct)) if coef.size else None, OUT.ptr, ldo))
+
+    def lincomb_normal_masked(self, box, mask, a0, seed, stream, first, k, mean, C_coef, OUT, ldo):
+        """OUT[:, j] = mean + a0 z_j + sum_a C[a, j] y_a + C[c + a, j] s_a on the rows of the mask, mean_i elsewhere."""
+        coef = np.ascontiguousarray(C_coef, dtype=self.dtype).reshape(-1)
+        self.ctx.check(self._masked("lincomb_normal")(self.h, box.h, self._cls(box), mask, a0, seed, stream, first, k,
+                                                      mean.ptr if mean is not None else None,
+                                                      coef.ctypes.data_as(C.POINTER(self.ct)) if coef.size else None, OUT.ptr, ldo))
+
+    def quad_diag_masked(self, box, mask, a0, K, out):
+        Kc = np.ascontiguousarray(K, dtype=self.dtype).reshape(-1)
+        self.ctx.check(self._masked("quad_diag")(self.h, box.h, self._cls(box), mask, a0,
+                                                 Kc.ctypes.data_as(C.POINTER(self.ct)) if Kc.size else None, out.ptr))
+
     def column(self, which, age):
         fn = self.ctx.lib.lbfgs_b200_hist_s_col if which == "s" else self.ctx.lib.lbfgs_b200_hist_y_col
         p = fn(self.h, age)
@@ -713,7 +777,7 @@ class History:
 
 
 BOXV_VECC, BOXV_VECY, BOXV_LAMBDA, BOXV_MU, BOXV_TMP, BOXV_TMP2, BOXV_YFB, BOXV_DVEC, BOXV_BRK, BOXV_XCP = range(10)
-CLS_FIXED, CLS_ACT, CLS_FREE, SUB_L, SUB_U, SUB_P = 1, 2, 4, 8, 16, 32
+CLS_FIXED, CLS_ACT, CLS_FREE, SUB_L, SUB_U, SUB_P, CLS_FINAL = 1, 2, 4, 8, 16, 32, 64
 
 
 class Box:
@@ -750,6 +814,15 @@ class Box:
         assert host.size == n
         self.ctx.check(self.ctx.lib.lbfgs_b200_memcpy_h2d(self.ctx.h, self._ptr(which), host.ctypes.data_as(C.c_void_p), host.nbytes))
         self.ctx.sync()
+
+    def final_classes(self, x, lb, ub, tol=None):
+        """CLS_FINAL on the free coordinates of the DeviceArray x against the DeviceArrays lb, ub (lbfgs_b200_box_final_classes);
+        returns their number.  tol: 4 eps of the storage type by default."""
+        tol = 4 * np.finfo(self.dtype).eps if tol is None else tol
+        nf = C.c_int64(0)
+        self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_box_final_classes_" + ("f64" if self.dtype == np.float64 else "f32"))(
+            self.h, x.ptr, lb.ptr, ub.ptr, tol, C.byref(nf)))
+        return nf.value
 
 
 class Session:
@@ -1202,6 +1275,104 @@ def small_batch_hessian_log_density(objective, X0, X, means=None, param=None, li
     mean or None).  Returns (outcomes, X_solutions, logp (B, kx) or (kx,))."""
     res, Xs, _, lp = _small_batch_whiten(objective, X0, 0, None, X, means, param, linesearch, dtype, data0, data1, ldd, device, lib, b)
     return res, Xs, lp
+
+
+BOX_OPS = {"B": 0, "H": 1, "diagB": 2, "diagH": 3, "sample": 4, "log_density": 5, "logdet": 6, "L": 7, "LT": 8, "LINV": 9, "LINVT": 10,
+           "denseB": 11, "denseH": 12}
+
+
+def box_solve_hessian(objective, x0, lb, ub, op, V=None, mean=None, seed=0, first=0, k=0, free=True, tol=None, param=None, dtype=np.float64,
+                      device=0, lib=None):
+    """LBFGSBSolver<Scalar>::minimize on a built-in objective, then one operation (BOX_OPS) on the final approximation: on the free set at
+    the solution (free=True: B_F, H_F, ...) or over the whole space.  V: (k, n) vectors for products and factor ops, points for the log
+    density; mean: the draws' and densities' mean (None: the solution); k: the number of draws.  Returns a dict with x, niter, nfree
+    (free only), logdet (log det H_F or H), and out: the (k, n) products or draws, the n-diagonal, the (n, n) matrix or the log densities."""
+    drv = driver(lib)
+    dt = np.dtype(dtype)
+    opid = BOX_OPS[op] if isinstance(op, str) else int(op)
+    x = np.array(x0, dtype=dt, order="C").copy()
+    n = x.size
+    lbv = np.ascontiguousarray(np.broadcast_to(lb, n), dtype=dt)
+    ubv = np.ascontiguousarray(np.broadcast_to(ub, n), dtype=dt)
+    Vr = None if V is None else np.ascontiguousarray(np.atleast_2d(V), dtype=dt)
+    kv = k if opid == BOX_OPS["sample"] else (0 if Vr is None else Vr.shape[0])
+    mu = None if mean is None else np.ascontiguousarray(mean, dtype=dt)
+    out = np.zeros(n * n if opid >= BOX_OPS["denseB"] else max(kv, 1) * n, dtype=dt)
+    dout = np.zeros(max(kv, 1))
+    logdet, nfree, niter = C.c_double(0.0), C.c_long(-1), C.c_int(0)
+    p = (param if param is not None else LBFGSBParam())._c()
+    fn = drv.lbfgsb200_drv_box_hessian_f64 if dt == np.float64 else drv.lbfgsb200_drv_box_hessian_f32
+    _checked("box_solve_hessian", lambda e, el: fn(device, objective, n, C.byref(p), _ptr(x), _ptr(lbv), _ptr(ubv), int(bool(free)),
+                                                   -1.0 if tol is None else float(tol), opid, kv, _ptr(Vr), _ptr(mu), seed, first, _ptr(out),
+                                                   _ptr(dout), C.byref(logdet), C.byref(nfree), C.byref(niter), e, el))
+    if opid >= BOX_OPS["denseB"]:
+        res = out.reshape(n, n)
+    elif opid in (BOX_OPS["diagB"], BOX_OPS["diagH"]):
+        res = out[:n]
+    elif opid == BOX_OPS["log_density"]:
+        res = dout[:kv]
+    elif opid == BOX_OPS["logdet"]:
+        res = logdet.value
+    else:
+        res = out[:kv * n].reshape(kv, n)
+    return dict(x=x, niter=niter.value, nfree=nfree.value if free else None, logdet=logdet.value, out=res)
+
+
+def box_solve_hessian_times(objective, x0, lb, ub, V, inverse=False, free=True, **kw):
+    """B_F V or H_F V (free=False: B V or H V) after a bound-constrained solve; see box_solve_hessian."""
+    return box_solve_hessian(objective, x0, lb, ub, "H" if inverse else "B", V=V, free=free, **kw)
+
+
+def box_solve_hessian_diagonal(objective, x0, lb, ub, inverse=False, free=True, **kw):
+    """diag B_F or diag H_F (free=False: diag B or diag H), 0 off the free set; see box_solve_hessian."""
+    return box_solve_hessian(objective, x0, lb, ub, "diagH" if inverse else "diagB", free=free, **kw)
+
+
+def box_solve_hessian_sample(objective, x0, lb, ub, k, seed=0, first=0, mean=None, free=True, **kw):
+    """k draws of N(mean, H_F) on the free set, mean_i on the fixed coordinates (free=False: N(mean, H)), stream 0."""
+    return box_solve_hessian(objective, x0, lb, ub, "sample", k=k, seed=seed, first=first, mean=mean, free=free, **kw)
+
+
+def box_solve_hessian_log_density(objective, x0, lb, ub, X, mean=None, free=True, **kw):
+    """log N(x_F; mean_F, H_F) of the rows of X (free=False: log N(x; mean, H)); see box_solve_hessian."""
+    return box_solve_hessian(objective, x0, lb, ub, "log_density", V=X, mean=mean, free=free, **kw)
+
+
+def box_solve_hessian_logdet(objective, x0, lb, ub, free=True, **kw):
+    """log det H_F (free=False: log det H) and n_F; see box_solve_hessian."""
+    return box_solve_hessian(objective, x0, lb, ub, "logdet", free=free, **kw)
+
+
+def box_hist_hessian(S, Y, op, cls=None, m=None, V=None, mean=None, seed=0, first=0, k=0, device=0, lib=None):
+    """The same operations on an explicit history (pairs S[k], Y[k] added in order to a ring of size m <= 20, fp64); cls: n class bytes
+    whose CLS_FINAL bit marks the free set (None: the whole space).  Returns the dict of box_solve_hessian without x and niter."""
+    drv = driver(lib)
+    S = np.ascontiguousarray(np.atleast_2d(S), dtype=np.float64)
+    Y = np.ascontiguousarray(np.atleast_2d(Y), dtype=np.float64)
+    npairs, n = S.shape
+    m = m if m is not None else max(1, npairs)
+    opid = BOX_OPS[op] if isinstance(op, str) else int(op)
+    Vr = None if V is None else np.ascontiguousarray(np.atleast_2d(V), dtype=np.float64)
+    kv = k if opid == BOX_OPS["sample"] else (0 if Vr is None else Vr.shape[0])
+    mu = None if mean is None else np.ascontiguousarray(mean, dtype=np.float64)
+    cb = None if cls is None else np.ascontiguousarray(cls, dtype=np.uint8)
+    out = np.zeros(n * n if opid >= BOX_OPS["denseB"] else max(kv, 1) * n)
+    dout = np.zeros(max(kv, 1))
+    logdet, nfree = C.c_double(0.0), C.c_long(-1)
+    _checked("box_hist_hessian", lambda e, el: drv.lbfgsb200_drv_box_hist_hessian_f64(
+        device, n, m, npairs, _ptr(S), _ptr(Y), int(cb is not None), None if cb is None else cb.ctypes.data_as(C.POINTER(C.c_ubyte)), opid, kv,
+        _ptr(Vr), _ptr(mu), seed, first, _ptr(out), _ptr(dout), C.byref(logdet), C.byref(nfree), e, el))
+    if opid >= BOX_OPS["denseB"]:
+        res = out.reshape(n, n)
+    elif opid in (BOX_OPS["diagB"], BOX_OPS["diagH"]):
+        res = out[:n]
+    elif opid == BOX_OPS["log_density"]:
+        res = dout[:kv]
+    elif opid == BOX_OPS["logdet"]:
+        res = logdet.value
+    else:
+        res = out[:kv * n].reshape(kv, n)
+    return dict(nfree=nfree.value if cb is not None else None, logdet=logdet.value, out=res)
 
 
 def small_max_n(m, objective, dtype=np.float64):

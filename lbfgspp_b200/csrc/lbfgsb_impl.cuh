@@ -324,7 +324,8 @@ static lbfgs_b200_status do_hist_lincomb_normal(lbfgs_b200_hist* h, T a0, uint64
 
 // out_i = a0 + r_i' K r_i (see k_hist_quad_diag): K's upper triangle is packed, off-diagonal entries doubled, on the host (exact
 // in binary floating point), and the kernel's width is chosen from c alone, so a row's arithmetic depends on c, K and the row only
-template <class T> static lbfgs_b200_status do_hist_quad_diag(lbfgs_b200_hist* h, T a0, const T* K_host, T* out)
+template <class T, class A = QuadDiagArgs<T>>
+static lbfgs_b200_status do_hist_quad_diag(lbfgs_b200_hist* h, T a0, const T* K_host, T* out, const unsigned char* fcls = nullptr, int fmask = 0)
 {
     if (auto st = hist_check<T>(h)) return st;
     lbfgs_b200_ctx* ctx = h->ctx;
@@ -346,9 +347,11 @@ template <class T> static lbfgs_b200_status do_hist_quad_diag(lbfgs_b200_hist* h
         CU(ctx, cudaMemcpyAsync(h->quad, kp.data(), sizeof(double) * (size_t)nk, cudaMemcpyHostToDevice, ctx->stream));
         CU(ctx, cudaStreamSynchronize(ctx->stream));   // kp is freed on return
     }
-    QuadDiagArgs<T> a{};
+    A a{};
     a.n = h->n; a.ld = h->ld; a.S = static_cast<const T*>(h->S); a.Y = static_cast<const T*>(h->Y);
     a.Kp = static_cast<const double*>(h->quad); a.a0 = (double)a0; a.out = out; a.c = c;
+    if constexpr (unmasked<A>::masked) { a.fcls = fcls; a.fmask = (unsigned char)fmask; }
+    else (void)fcls, (void)fmask;
     fill_slots<T>(h, a.slots);
     const size_t smem = sizeof(double) * (size_t)nk;
     auto launch = [&](auto kernel, int rpt) -> lbfgs_b200_status {
@@ -357,10 +360,11 @@ template <class T> static lbfgs_b200_status do_hist_quad_diag(lbfgs_b200_hist* h
         kernel<<<(int)(want < 1 ? 1 : want < cap ? want : cap), kThreads, smem, ctx->stream>>>(a);
         return post_launch(ctx, "k_hist_quad_diag");
     };
-    if (w <= 16) return launch(k_hist_quad_diag<T, 16>, quad_diag_rpt<16>());
-    if (w <= 32) return launch(k_hist_quad_diag<T, 32>, quad_diag_rpt<32>());
-    if (w <= 64) return launch(k_hist_quad_diag<T, 64>, quad_diag_rpt<64>());
-    return launch(k_hist_quad_diag<T, kMaxW>, quad_diag_rpt<kMaxW>());
+    if (w <= 16) return launch(k_hist_quad_diag<T, 16, A>, quad_diag_rpt<16>());
+    if (w <= 32) return launch(k_hist_quad_diag<T, 32, A>, quad_diag_rpt<32>());
+    if (w <= 64) return launch(k_hist_quad_diag<T, 64, A>, quad_diag_rpt<64>());
+    if constexpr (unmasked<A>::masked) return fail(ctx, LBFGS_B200_ERR_INVALID, "hist_quad_diag_masked: the box path keeps m <= 20");
+    else return launch(k_hist_quad_diag<T, kMaxW>, quad_diag_rpt<kMaxW>());
 }
 
 // G[(2c)x(2c)] over rows with (cls & mask) != 0, ordering [Y by age, S by age]   (WP'WP of BFGSMat.h:529-565)
@@ -387,6 +391,151 @@ static lbfgs_b200_status do_hist_masked_gram(lbfgs_b200_hist* h, lbfgs_b200_box*
     CU(ctx, cudaMemcpyAsync(tmp.data(), b->mg_result, sizeof(double) * w * w, cudaMemcpyDeviceToHost, ctx->stream));
     CU(ctx, cudaStreamSynchronize(ctx->stream));
     for (int e = 0; e < w * w; e++) G_host[e] = (T)tmp[e];
+    return LBFGS_B200_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ the masked k-vector passes
+// The passes above restricted to the rows with (cls & mask) != 0 (k_hist_wt_dot_multi / k_hist_lincomb / k_hist_quad_diag with
+// Masked<A>): the final approximation on the free variables of a bound-constrained solve.  Each follows its twin's rules (replicas
+// only, 1 <= k <= 16) and needs the history's box workspace and class bytes.
+static lbfgs_b200_status mask_check(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, const char* what)
+{
+    REQUIRE(h->ctx, b && b->h == h && cls, "%s: NULL argument or a box of another history", what);
+    return LBFGS_B200_OK;
+}
+
+template <class T>
+static lbfgs_b200_status do_hist_wt_dot_multi_masked(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, int mask, int k,
+                                                     const T* V, int64_t ldv, T* R_host)
+{
+    if (auto st = multi_check<T>(h, k, ldv, "hist_wt_dot_multi_masked")) return st;
+    if (auto st = mask_check(h, b, cls, "hist_wt_dot_multi_masked")) return st;
+    REQUIRE(h->ctx, V && R_host, "hist_wt_dot_multi_masked: NULL argument");
+    const int w = 2 * h->ncorr;
+    if (w == 0) return LBFGS_B200_OK;
+    Masked<WtDotMultiArgs<T>> a{};
+    a.V = V; a.ldv = ldv; a.k = k; a.fcls = cls; a.fmask = (unsigned char)mask;
+    std::vector<double> tmp;
+    if (auto st = run_wt_dots<T>(h, a, w, w, tmp, "k_hist_wt_dot_multi_masked")) return st;
+    for (int e = 0; e < w * k; e++) R_host[e] = (T)tmp[(size_t)e];
+    return LBFGS_B200_OK;
+}
+
+template <class T>
+static lbfgs_b200_status do_hist_wt_dot_diff_masked(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, int mask, int k, const T* X,
+                                                    int64_t ldx, const T* mean, double* R_host, double* nrm_host)
+{
+    if (auto st = multi_check<T>(h, k, ldx, "hist_wt_dot_diff_masked")) return st;
+    if (auto st = mask_check(h, b, cls, "hist_wt_dot_diff_masked")) return st;
+    REQUIRE(h->ctx, X && mean && R_host && nrm_host, "hist_wt_dot_diff_masked: NULL argument");
+    const int w = 2 * h->ncorr;
+    Masked<WtDotDiffArgs<T>> a{};
+    a.V = X; a.ldv = ldx; a.k = k; a.mean = mean; a.fcls = cls; a.fmask = (unsigned char)mask;
+    std::vector<double> tmp;
+    if (auto st = run_wt_dots<T>(h, a, w, w + 1, tmp, "k_hist_wt_dot_diff_masked")) return st;
+    for (int e = 0; e < w * k; e++) R_host[e] = tmp[(size_t)e];
+    for (int j = 0; j < k; j++) nrm_host[j] = tmp[(size_t)(w * k + j)];
+    return LBFGS_B200_OK;
+}
+
+template <class T>
+static lbfgs_b200_status do_hist_wt_dot_normal_masked(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, int mask, uint64_t seed,
+                                                      uint32_t stream, uint32_t first, int k, T* R_host)
+{
+    if (auto st = normal_check<T>(h, k, first, "hist_wt_dot_normal_masked")) return st;
+    if (auto st = mask_check(h, b, cls, "hist_wt_dot_normal_masked")) return st;
+    REQUIRE(h->ctx, R_host, "hist_wt_dot_normal_masked: NULL argument");
+    const int w = 2 * h->ncorr;
+    if (w == 0) return LBFGS_B200_OK;
+    Masked<WtDotNormalArgs<T>> a{};
+    a.V = nullptr; a.ldv = 0; a.k = k; a.src = NormalSrc{(unsigned long long)seed, stream, first}; a.fcls = cls; a.fmask = (unsigned char)mask;
+    std::vector<double> tmp;
+    if (auto st = run_wt_dots<T>(h, a, w, w, tmp, "k_hist_wt_dot_normal_masked")) return st;
+    for (int e = 0; e < w * k; e++) R_host[e] = (T)tmp[(size_t)e];
+    return LBFGS_B200_OK;
+}
+
+// the coefficients [2c][k] to the scratch of the k-vector passes (C_host may be a stack array of the caller)
+template <class T> static lbfgs_b200_status upload_coef(lbfgs_b200_hist* h, int k, const T* C_host, void** coef, const char* what)
+{
+    double *partials, *result;
+    if (auto st = multi_scratch(h, &partials, &result, coef)) return st;
+    lbfgs_b200_ctx* ctx = h->ctx;
+    if (h->ncorr > 0)
+    {
+        REQUIRE(ctx, C_host != nullptr, "%s: NULL argument", what);
+        CU(ctx, cudaMemcpyAsync(*coef, C_host, sizeof(T) * 2 * h->ncorr * k, cudaMemcpyHostToDevice, ctx->stream));
+        CU(ctx, cudaStreamSynchronize(ctx->stream));
+    }
+    return LBFGS_B200_OK;
+}
+
+template <class T>
+static lbfgs_b200_status do_hist_lincomb_multi_masked(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, int mask, T a0, int k,
+                                                      const T* V, int64_t ldv, const T* C_host, T* OUT, int64_t ldo)
+{
+    if (auto st = multi_check<T>(h, k, ldv, "hist_lincomb_multi_masked")) return st;
+    if (auto st = mask_check(h, b, cls, "hist_lincomb_multi_masked")) return st;
+    lbfgs_b200_ctx* ctx = h->ctx;
+    REQUIRE(ctx, V && OUT, "hist_lincomb_multi_masked: NULL argument");
+    REQUIRE(ctx, ldo >= h->n, "hist_lincomb_multi_masked: leading dimension %lld is smaller than n = %lld", (long long)ldo, (long long)h->n);
+    void* coef;
+    if (auto st = upload_coef<T>(h, k, C_host, &coef, "hist_lincomb_multi_masked")) return st;
+    Masked<LincombArgs<T>> a{};
+    a.n = h->n; a.ld = h->ld; a.ldv = ldv; a.ldo = ldo; a.S = static_cast<const T*>(h->S); a.Y = static_cast<const T*>(h->Y);
+    a.V = V; a.a0 = a0; a.coef = static_cast<const T*>(coef); a.cls = nullptr; a.mask = 0; a.out = OUT; a.c = h->ncorr; a.k = k;
+    a.fcls = cls; a.fmask = (unsigned char)mask;
+    fill_slots<T>(h, a.slots);
+    if (k == 1) k_hist_lincomb<T, 1, Masked<LincombArgs<T>>><<<grid_for(ctx, h->n * 4, 4), kThreads, 0, ctx->stream>>>(a);
+    else k_hist_lincomb<T, kMaxK, Masked<LincombArgs<T>>><<<grid_for(ctx, h->n * 4, 4), kThreads, 0, ctx->stream>>>(a);
+    return post_launch(ctx, "k_hist_lincomb_masked");
+}
+
+template <class T>
+static lbfgs_b200_status do_hist_lincomb_normal_masked(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, int mask, T a0,
+                                                       uint64_t seed, uint32_t stream, uint32_t first, int k, const T* mean, const T* C_host,
+                                                       T* OUT, int64_t ldo)
+{
+    if (auto st = normal_check<T>(h, k, first, "hist_lincomb_normal_masked")) return st;
+    if (auto st = mask_check(h, b, cls, "hist_lincomb_normal_masked")) return st;
+    lbfgs_b200_ctx* ctx = h->ctx;
+    REQUIRE(ctx, OUT, "hist_lincomb_normal_masked: NULL argument");
+    REQUIRE(ctx, ldo >= h->n, "hist_lincomb_normal_masked: leading dimension %lld is smaller than n = %lld", (long long)ldo, (long long)h->n);
+    void* coef;
+    if (auto st = upload_coef<T>(h, k, C_host, &coef, "hist_lincomb_normal_masked")) return st;
+    Masked<LincombNormalArgs<T>> a{};
+    a.n = h->n; a.ld = h->ld; a.ldv = 0; a.ldo = ldo; a.S = static_cast<const T*>(h->S); a.Y = static_cast<const T*>(h->Y);
+    a.V = nullptr; a.a0 = a0; a.coef = static_cast<const T*>(coef); a.cls = nullptr; a.mask = 0; a.out = OUT; a.c = h->ncorr; a.k = k;
+    a.mean = mean; a.src = NormalSrc{(unsigned long long)seed, stream, first}; a.fcls = cls; a.fmask = (unsigned char)mask;
+    fill_slots<T>(h, a.slots);
+    const int64_t npairs = (h->n + 1) / 2;
+    if (k == 1) k_hist_lincomb<T, 1, Masked<LincombNormalArgs<T>>><<<grid_for(ctx, npairs * 4, 4), kThreads, 0, ctx->stream>>>(a);
+    else k_hist_lincomb<T, kMaxK, Masked<LincombNormalArgs<T>>><<<grid_for(ctx, npairs * 4, 4), kThreads, 0, ctx->stream>>>(a);
+    return post_launch(ctx, "k_hist_lincomb_normal_masked");
+}
+
+template <class T>
+static lbfgs_b200_status do_hist_quad_diag_masked(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, int mask, T a0, const T* K_host,
+                                                  T* out)
+{
+    if (auto st = hist_check<T>(h)) return st;
+    if (auto st = mask_check(h, b, cls, "hist_quad_diag_masked")) return st;
+    return do_hist_quad_diag<T, Masked<QuadDiagArgs<T>>>(h, a0, K_host, out, cls, mask);
+}
+
+// CLS_FINAL on the free coordinates of x (k_box_final_classes); *nfree_host = their number
+template <class T>
+static lbfgs_b200_status do_box_final_classes(lbfgs_b200_box* b, const T* x, const T* lb, const T* ub, T tol, int64_t* nfree_host)
+{
+    if (auto st = box_check<T>(b)) return st;
+    lbfgs_b200_ctx* ctx = b->h->ctx;
+    REQUIRE(ctx, x && lb && ub && nfree_host, "box_final_classes: NULL argument");
+    REQUIRE(ctx, tol >= T(0), "box_final_classes: tol must be >= 0");
+    const ReduceBuf rb = next_rb(ctx, true);
+    k_box_final_classes<T><<<grid_for(ctx, b->n * 4, 4), kThreads, 0, ctx->stream>>>(b->n, x, lb, ub, tol, b->cls, rb);
+    if (auto st = post_launch(ctx, "k_box_final_classes")) return st;
+    if (auto st = receive(ctx, 1)) return st;
+    *nfree_host = (int64_t)ctx->h_result[0];
     return LBFGS_B200_OK;
 }
 
@@ -677,6 +826,32 @@ void* lbfgs_b200_box_vector(lbfgs_b200_box* b, int which)
     lbfgs_b200_status lbfgs_b200_hist_wt_dot_diff_##SUF(lbfgs_b200_hist* h, int k, const T* X, int64_t ldx, const T* mean,   \
                                                         double* R_host, double* nrm_host)                                    \
     { return do_hist_wt_dot_diff<T>(h, k, X, ldx, mean, R_host, nrm_host); }                                                 \
+    lbfgs_b200_status lbfgs_b200_hist_wt_dot_multi_masked_##SUF(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, \
+                                                                int mask, int k, const T* V, int64_t ldv, T* R_host)          \
+    { return do_hist_wt_dot_multi_masked<T>(h, b, cls, mask, k, V, ldv, R_host); }                                           \
+    lbfgs_b200_status lbfgs_b200_hist_wt_dot_diff_masked_##SUF(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls,  \
+                                                               int mask, int k, const T* X, int64_t ldx, const T* mean,        \
+                                                               double* R_host, double* nrm_host)                               \
+    { return do_hist_wt_dot_diff_masked<T>(h, b, cls, mask, k, X, ldx, mean, R_host, nrm_host); }                            \
+    lbfgs_b200_status lbfgs_b200_hist_wt_dot_normal_masked_##SUF(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, \
+                                                                 int mask, uint64_t seed, uint32_t stream, uint32_t first,     \
+                                                                 int k, T* R_host)                                             \
+    { return do_hist_wt_dot_normal_masked<T>(h, b, cls, mask, seed, stream, first, k, R_host); }                             \
+    lbfgs_b200_status lbfgs_b200_hist_lincomb_multi_masked_##SUF(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls, \
+                                                                 int mask, T a0, int k, const T* V, int64_t ldv,               \
+                                                                 const T* C_host, T* OUT, int64_t ldo)                         \
+    { return do_hist_lincomb_multi_masked<T>(h, b, cls, mask, a0, k, V, ldv, C_host, OUT, ldo); }                            \
+    lbfgs_b200_status lbfgs_b200_hist_lincomb_normal_masked_##SUF(lbfgs_b200_hist* h, lbfgs_b200_box* b,                      \
+                                                                  const unsigned char* cls, int mask, T a0, uint64_t seed,     \
+                                                                  uint32_t stream, uint32_t first, int k, const T* mean,      \
+                                                                  const T* C_host, T* OUT, int64_t ldo)                        \
+    { return do_hist_lincomb_normal_masked<T>(h, b, cls, mask, a0, seed, stream, first, k, mean, C_host, OUT, ldo); }         \
+    lbfgs_b200_status lbfgs_b200_hist_quad_diag_masked_##SUF(lbfgs_b200_hist* h, lbfgs_b200_box* b, const unsigned char* cls,   \
+                                                             int mask, T a0, const T* K_host, T* out)                          \
+    { return do_hist_quad_diag_masked<T>(h, b, cls, mask, a0, K_host, out); }                                                \
+    lbfgs_b200_status lbfgs_b200_box_final_classes_##SUF(lbfgs_b200_box* b, const T* x, const T* lb, const T* ub, T tol,      \
+                                                         int64_t* nfree_host)                                                  \
+    { return do_box_final_classes<T>(b, x, lb, ub, tol, nfree_host); }                                                       \
     lbfgs_b200_status lbfgs_b200_box_cauchy_breaks_##SUF(lbfgs_b200_box* b, const T* x, const T* g, const T* lb,            \
                                                          const T* ub, T* out5_host)                                         \
     { return do_box_cauchy_breaks<T>(b, x, g, lb, ub, out5_host); }                                                         \

@@ -21,7 +21,27 @@
 
 namespace lb {
 
-enum : unsigned char { CLS_FIXED = 1, CLS_ACT = 2, CLS_FREE = 4, SUB_L = 8, SUB_U = 16, SUB_P = 32 };
+// CLS_FINAL: the free set at the solution (k_box_final_classes); Cauchy rebuilds the other bits on every iteration and leaves it be
+enum : unsigned char { CLS_FIXED = 1, CLS_ACT = 2, CLS_FREE = 4, SUB_L = 8, SUB_U = 16, SUB_P = 32, CLS_FINAL = 64 };
+
+// The masked forms of the history passes (the final approximation on the free variables): Masked<A> is the pass of argument form A
+// restricted to the rows i with (fcls_i & fmask) != 0.  Each form keeps the order of A, so with every row in the mask it computes
+// A's bits; unmasked<A> names A and says whether a form is masked.
+template <class A> struct Masked : A
+{
+    const unsigned char* fcls;
+    unsigned char fmask;
+};
+template <class A> struct unmasked
+{
+    using type = A;
+    static constexpr bool masked = false;
+};
+template <class A> struct unmasked<Masked<A>>
+{
+    using type = A;
+    static constexpr bool masked = true;
+};
 
 // ---------------------------------------------------------------- reductions with max slots
 // like grid_reduce, but slots whose bit is set in `maxmask` take the maximum instead of the sum (exact, order-free)
@@ -111,6 +131,26 @@ template <class T> __global__ void __launch_bounds__(kThreads) k_box_dirinfo(int
     }
     double acc[2] = {(double)dot, negmin};
     grid_reduce_mixed<2>(acc, rb, 2u);
+}
+
+// The free set at the solution: coordinate i is fixed when lb_i == ub_i or x_i lies within tol * max(1, |bound|) of a finite bound
+// (the solver does not clamp at exit, so a point on a bound can miss it by an ulp); every other one is free and gets CLS_FINAL.
+// out = { number of free coordinates }
+template <class T> __global__ void __launch_bounds__(kThreads) k_box_final_classes(int64_t n, const T* __restrict__ x, const T* __restrict__ lb,
+                                                                                  const T* __restrict__ ub, T tol, unsigned char* __restrict__ cls,
+                                                                                  ReduceBuf rb)
+{
+    double nfree = 0;
+    const T inf = (T)INFINITY;
+    for (int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x; i < n; i += (int64_t)gridDim.x * kThreads)
+    {
+        const T xi = x[i], li = lb[i], ui = ub[i];
+        const bool fixed = li == ui || (li > -inf && xi <= li + tol * fmax(T(1), fabs(li))) || (ui < inf && xi >= ui - tol * fmax(T(1), fabs(ui)));
+        cls[i] = fixed ? (unsigned char)(cls[i] & ~CLS_FINAL) : (unsigned char)(cls[i] | CLS_FINAL);
+        nfree += fixed ? 0.0 : 1.0;
+    }
+    double acc[1] = {nfree};
+    grid_reduce_mixed<1>(acc, rb, 0u);
 }
 
 // ---------------------------------------------------------------- Cauchy point, phase 1 (Cauchy.h:111-129)
@@ -509,13 +549,18 @@ template <class T> struct LincombNormalArgs : LincombArgs<T>
     NormalSrc src;
 };
 
-template <class T, int KMAX> __device__ __forceinline__ void k_hist_lincomb_normal(const LincombNormalArgs<T>& a)
+// Masked<LincombNormalArgs>: the draws of N(mean, H_F) on the free rows (mean_i elsewhere), so the y rows of C are read too: per element
+// mean, a0*z, y by age, s by age; with zero y rows and every row in the mask, the bits of the unmasked form.
+template <class T, int KMAX, class A> __device__ __forceinline__ void k_hist_lincomb_normal(const A& a)
 {
+    constexpr bool kMask = unmasked<A>::masked;
     __shared__ T s_coef[kMaxW * KMAX];
-    __shared__ const T* s_s[kMaxM];
+    __shared__ const T* s_s[kMask ? 2 * kMaxM : kMaxM];   // masked: the y columns at kMaxM + age
     const int k = KMAX == 1 ? 1 : a.k;
     for (int e = threadIdx.x; e < 2 * a.c * k; e += kThreads) s_coef[e] = a.coef[e];
     for (int j = threadIdx.x; j < a.c; j += kThreads) s_s[j] = a.S + (int64_t)a.slots[j] * a.ld;
+    if constexpr (kMask)
+        for (int j = threadIdx.x; j < a.c; j += kThreads) s_s[kMaxM + j] = a.Y + (int64_t)a.slots[j] * a.ld;
     __syncthreads();
     const int64_t npairs = (a.n + 1) / 2;
     for (int64_t q = (int64_t)blockIdx.x * kThreads + threadIdx.x; q < npairs; q += (int64_t)gridDim.x * kThreads)
@@ -533,6 +578,18 @@ template <class T, int KMAX> __device__ __forceinline__ void k_hist_lincomb_norm
                 r0[j] = a.mean ? m0 + a.a0 * (T)z0 : a.a0 * (T)z0;
                 r1[j] = a.mean ? m1 + a.a0 * (T)z1 : a.a0 * (T)z1;
             }
+        if constexpr (kMask)
+            for (int p = 0; p < a.c; p++)
+            {
+                const T y0 = s_s[kMaxM + p][i0], y1 = two ? s_s[kMaxM + p][i0 + 1] : T(0);
+#pragma unroll
+                for (int j = 0; j < KMAX; j++)
+                    if (j < k)
+                    {
+                        r0[j] += s_coef[p * k + j] * y0;
+                        r1[j] += s_coef[p * k + j] * y1;
+                    }
+            }
         for (int p = 0; p < a.c; p++)
         {
             const T s0 = s_s[p][i0], s1 = two ? s_s[p][i0 + 1] : T(0);
@@ -544,20 +601,28 @@ template <class T, int KMAX> __device__ __forceinline__ void k_hist_lincomb_norm
                     r1[j] += s_coef[(a.c + p) * k + j] * s1;
                 }
         }
+        bool in0 = true, in1 = true;
+        if constexpr (kMask)
+        {
+            in0 = (a.fcls[i0] & a.fmask) != 0;
+            in1 = two && (a.fcls[i0 + 1] & a.fmask) != 0;
+        }
 #pragma unroll
         for (int j = 0; j < KMAX; j++)
             if (j < k)
             {
-                a.out[j * a.ldo + i0] = r0[j];
-                if (two) a.out[j * a.ldo + i0 + 1] = r1[j];
+                a.out[j * a.ldo + i0] = in0 ? r0[j] : m0;
+                if (two) a.out[j * a.ldo + i0 + 1] = in1 ? r1[j] : m1;
             }
     }
 }
 
-// KMAX: 1 (the L-BFGS-B pass) or kMaxK; the k running sums of an element stay in registers
+// KMAX: 1 (the L-BFGS-B pass, and any k = 1 call) or kMaxK; the k running sums of an element stay in registers.  Masked<LincombArgs>:
+// rows outside the mask are written as 0 instead of being skipped.
 template <class T, int KMAX, class A = LincombArgs<T>> __global__ void __launch_bounds__(kThreads) k_hist_lincomb(A a)
 {
-    if constexpr (!std::is_same<A, LincombArgs<T>>::value)
+    constexpr bool kMask = unmasked<A>::masked;
+    if constexpr (!std::is_same<typename unmasked<A>::type, LincombArgs<T>>::value)
     {
         k_hist_lincomb_normal<T, KMAX>(a);
         return;
@@ -577,7 +642,17 @@ template <class T, int KMAX, class A = LincombArgs<T>> __global__ void __launch_
     __syncthreads();
     for (int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x; i < a.n; i += (int64_t)gridDim.x * kThreads)
     {
-        if (a.cls && !(a.cls[i] & a.mask)) continue;
+        if constexpr (kMask)
+        {
+            if (!(a.fcls[i] & a.fmask))
+            {
+#pragma unroll
+                for (int j = 0; j < KMAX; j++)
+                    if (j < k) a.out[j * a.ldo + i] = T(0);
+                continue;
+            }
+        }
+        else if (a.cls && !(a.cls[i] & a.mask)) continue;
         T r[KMAX];
 #pragma unroll
         for (int j = 0; j < KMAX; j++)
@@ -625,7 +700,8 @@ template <class T> struct QuadDiagArgs
 
 template <int WMAX> __host__ __device__ constexpr int quad_diag_rpt() { return WMAX <= 32 ? 64 / WMAX : 1; }
 
-template <class T, int WMAX> __global__ void __launch_bounds__(kThreads) k_hist_quad_diag(QuadDiagArgs<T> a)
+// Masked<QuadDiagArgs>: out_i = 0 on the rows outside the mask
+template <class T, int WMAX, class A = QuadDiagArgs<T>> __global__ void __launch_bounds__(kThreads) k_hist_quad_diag(A a)
 {
     constexpr int RPT = quad_diag_rpt<WMAX>();
     constexpr int UNROLL = WMAX <= 64 ? WMAX : 1;
@@ -678,7 +754,11 @@ template <class T, int WMAX> __global__ void __launch_bounds__(kThreads) k_hist_
         for (int j = 0; j < RPT; j++)
         {
             const int64_t i = i0 + (int64_t)j * kThreads;
-            if (i < a.n) a.out[i] = (T)(a.a0 + acc[j]);
+            if constexpr (unmasked<A>::masked)
+            {
+                if (i < a.n) a.out[i] = (a.fcls[i] & a.fmask) ? (T)(a.a0 + acc[j]) : T(0);
+            }
+            else if (i < a.n) a.out[i] = (T)(a.a0 + acc[j]);
         }
     }
 }
@@ -722,15 +802,21 @@ template <class T> struct WtDotDiffArgs : WtDotMultiArgs<T>
     const T* mean;
 };
 
+// Masked<WtDotMultiArgs / WtDotDiffArgs / WtDotNormalArgs>: the vector rows outside the mask (loaded, differences or generated) are
+// staged as 0, the history rows as always, so every dot and norm is taken over the rows of the mask in the order above.
 template <class T, class A = WtDotMultiArgs<T>> __global__ void __launch_bounds__(kThreads) k_hist_wt_dot_multi(A a)
 {
-    constexpr bool kGen = std::is_same<A, WtDotNormalArgs<T>>::value;
-    constexpr bool kSOnly = std::is_same<A, WtDotSArgs<T>>::value;
-    constexpr bool kDiff = std::is_same<A, WtDotDiffArgs<T>>::value;
+    using B = typename unmasked<A>::type;
+    constexpr bool kMask = unmasked<A>::masked;
+    constexpr bool kGen = std::is_same<B, WtDotNormalArgs<T>>::value;
+    constexpr bool kSOnly = std::is_same<B, WtDotSArgs<T>>::value;
+    constexpr bool kDiff = std::is_same<B, WtDotDiffArgs<T>>::value;
+    static_assert(!(kMask && kSOnly), "no masked S-only form");
     extern __shared__ __align__(16) unsigned char wt_smem[];
     T* rows = reinterpret_cast<T*>(wt_smem);   // [w + k][kWtPitch]: y by age, s by age (S only: s by age), then the k vectors
     __shared__ const T* s_col[kMaxW + kMaxK];
     __shared__ bool s_last;
+    __shared__ bool s_in[kMask ? kWtRows : 1];   // masked: whether row r of the strip is in the mask
     const int w = kSOnly ? a.c : 2 * a.c, k = a.k, nrows = w + k, tid = threadIdx.x;
     const int ncol = kDiff ? w + 1 : w;   // dots per vector: the history columns, and for kDiff the vector with itself
     const int nload = kGen ? w : nrows;   // rows staged from memory
@@ -748,13 +834,28 @@ template <class T, class A = WtDotMultiArgs<T>> __global__ void __launch_bounds_
     for (int64_t strip = blockIdx.x; strip < nstrips; strip += gridDim.x)
     {
         const int64_t r0 = strip * kWtRows;
-        for (int t = tid; t < nload * kWtRows; t += kThreads)
+        if constexpr (kMask)
         {
-            const int q = t / kWtRows, r = t % kWtRows;
-            const int64_t i = r0 + r;
-            if constexpr (kDiff) rows[q * kWtPitch + r] = i < a.n ? (q < w ? __ldcs(s_col[q] + i) : __ldcs(s_col[q] + i) - a.mean[i]) : T(0);
-            else rows[q * kWtPitch + r] = i < a.n ? __ldcs(s_col[q] + i) : T(0);
+            for (int r = tid; r < kWtRows; r += kThreads) s_in[r] = r0 + r < a.n && (a.fcls[r0 + r] & a.fmask) != 0;
+            __syncthreads();
+            for (int t = tid; t < nload * kWtRows; t += kThreads)   // every load issued as in the unmasked form, then selected
+            {
+                const int q = t / kWtRows, r = t % kWtRows;
+                const int64_t i = r0 + r;
+                T v;
+                if constexpr (kDiff) v = i < a.n ? (q < w ? __ldcs(s_col[q] + i) : __ldcs(s_col[q] + i) - a.mean[i]) : T(0);
+                else v = i < a.n ? __ldcs(s_col[q] + i) : T(0);
+                rows[q * kWtPitch + r] = (q < w || s_in[r]) ? v : T(0);
+            }
         }
+        else
+            for (int t = tid; t < nload * kWtRows; t += kThreads)
+            {
+                const int q = t / kWtRows, r = t % kWtRows;
+                const int64_t i = r0 + r;
+                if constexpr (kDiff) rows[q * kWtPitch + r] = i < a.n ? (q < w ? __ldcs(s_col[q] + i) : __ldcs(s_col[q] + i) - a.mean[i]) : T(0);
+                else rows[q * kWtPitch + r] = i < a.n ? __ldcs(s_col[q] + i) : T(0);
+            }
         if constexpr (kGen)
             for (int t = tid; t < k * (kWtRows / 2); t += kThreads)   // one generator call per coordinate pair (r0 is even)
             {
@@ -762,8 +863,16 @@ template <class T, class A = WtDotMultiArgs<T>> __global__ void __launch_bounds_
                 const int64_t i = r0 + r;
                 double z0, z1;
                 normal_pair(a.src.seed, a.src.stream, a.src.first + (uint32_t)jv, (unsigned long long)(i / 2), z0, z1);
-                rows[(w + jv) * kWtPitch + r] = i < a.n ? (T)z0 : T(0);
-                rows[(w + jv) * kWtPitch + r + 1] = i + 1 < a.n ? (T)z1 : T(0);
+                if constexpr (kMask)
+                {
+                    rows[(w + jv) * kWtPitch + r] = s_in[r] ? (T)z0 : T(0);
+                    rows[(w + jv) * kWtPitch + r + 1] = s_in[r + 1] ? (T)z1 : T(0);
+                }
+                else
+                {
+                    rows[(w + jv) * kWtPitch + r] = i < a.n ? (T)z0 : T(0);
+                    rows[(w + jv) * kWtPitch + r + 1] = i + 1 < a.n ? (T)z1 : T(0);
+                }
             }
         __syncthreads();
         if (active)
