@@ -354,9 +354,10 @@ int lbfgs_b200_solver_batch(const lbfgs_b200_solver* s);
  * indexed by the pass a round ran: 0 = rounds in which the problems of a batch ran different passes, 1 FIRST, 2 TRIAL, 3 DOTS_FORM,
  * 4 DOTS_PLAIN, 5 COMBINE, 6 COMBINE_TRIAL, 7 RESTORE, 8 MATERIALIZE (9 unused).  ms_by_op10: the kernel's time split by round (CTA 0's cycle counter scaled
  * to kernel_ms; includes each round's synchronisation); alg_bytes_by_op10: algorithmic bytes of those passes (whole vectors read and
- * written: FIRST 4n, TRIAL 2n, DOTS_FORM (c+2)n, DOTS_PLAIN (c+2)n, COMBINE (c+2)n, COMBINE_TRIAL (c+2)n, MATERIALIZE 4n or 3n
- * words (the point on the ray; the search's start point or the point already in x: the gradient is evaluated from x, not stored, between
- * FIRST and MATERIALIZE, and the history ring holds the c+1 iterates of c chained pairs, not the pairs); for the neighbour-coupled
+ * written: FIRST 2n, TRIAL 2n (first search 1n), DOTS_FORM (c+2)n (iteration 1 (c+1)n), DOTS_PLAIN (c+2)n, COMBINE (c+2)n,
+ * COMBINE_TRIAL (c+2)n, MATERIALIZE 4n (first search 3n) or 3n words (the point on the ray; the search's start point or the point
+ * already in x: the gradient is evaluated from x, not stored, before MATERIALIZE, the first search's direction -grad f(x0) is evaluated
+ * from x0, not stored, and the history ring holds the c+1 iterates of c chained pairs, not the pairs); for the neighbour-coupled
  * objectives, whose trials store their points, whose passes read the stored gradient and whose ring holds S|Y: FIRST 3n, TRIAL 4n,
  * DOTS_FORM (2c+4)n, DOTS_PLAIN (2c+1)n, COMBINE (2c+2)n, COMBINE_TRIAL (2c+5)n, MATERIALIZE 4n, RESTORE 4n; + the objective's
  * data vectors per evaluation); sync_ms[3]: { the part of kernel_ms between CTA 0's arrival at a grid barrier and its release, the part of that spent waiting for

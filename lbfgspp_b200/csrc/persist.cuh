@@ -5,7 +5,7 @@
 //
 // The kernel is a "phase machine".  One CTA per SM (768 threads), all co-resident (cooperative launch).  Work proceeds in ROUNDS;
 // in a round every problem that is still running executes the ONE streaming pass its state asks for:
-//     FIRST          g = grad f(x0), d = -g                      ; {f, g.g, x.x}                            LBFGS.h:91-108
+//     FIRST          g = grad f(x0), d = -g (stored: HALO only)  ; {f, g.g, x.x}                            LBFGS.h:91-108
 //     TRIAL          x = xp + step*d, g = grad f(x)              ; {f, g.d, g.g, x.x}                       LineSearch*.h trial, LBFGS.h:130,137
 //     DOTS_FORM      s = x - xp, y = g - gp -> free ring slot    ; [S Y]'[g s y] (6 dots per column pair)   LBFGS.h:159-162, BFGSMat.h:85-92 + apply_Hv pass 1
 //     DOTS_PLAIN     (pair rejected by the curvature gate)       ; [S Y]'g over the old history
@@ -21,9 +21,12 @@
 // arithmetic, bit for bit, writes x, and forms the pair from it.  Nor is g itself stored between passes: the passes that need the
 // gradient of a stored point (gp = grad f(xp) in DOTS_FORM, g = grad f(x) in DOTS_PLAIN and COMBINE) evaluate it from that point
 // with the same arithmetic, bit for bit the g a pass would have stored; that spares DOTS_FORM the read of gp and the write of g and
-// COMBINE the read of g.  Only FIRST and MATERIALIZE write g: a problem that stops anywhere but at FIRST takes one MATERIALIZE round
-// for the point it stopped at -- on the ray, its search's start point, or the point in x (arming the next search failed).  The kept
-// best trial of a search is its step, so there is no x_lo/g_lo and no RESTORE pass.
+// COMBINE the read of g.  Only MATERIALIZE writes g: a problem that stops takes one MATERIALIZE round for the point it stopped at --
+// on the ray, its search's start point, or the point in x (it converged at x0, or arming the next search failed).  The direction of
+// the first search, d = -grad f(x0), is not stored either: FIRST writes x0 to its point row only, and while PRound::d_implied is
+// set (k == 1: until the first combination pass writes d) TRIAL, MATERIALIZE on the ray and the first DOTS_FORM evaluate d = T(-1) *
+// grad f(xp) from xp, bit for bit the d FIRST would have stored, instead of reading it.  The kept best trial of a search is its
+// step, so there is no x_lo/g_lo and no RESTORE pass.
 // History of iterates.  For the same objectives a pair is a function of its two endpoints (s = x - xp, y = grad f(x) - grad f(xp)),
 // and consecutive accepted pairs share one: the ring holds iterates (PState::pts), x and xp are rows of it, and the dots and
 // combination passes stage the c + 1 endpoints of c chained pairs instead of 2c columns and rebuild each pair where they read it,
@@ -70,6 +73,7 @@ template <class T> struct alignas(128) PRound
     int op, c_round, head, pending, gram_cur;
     int at_start;               // DOTS_FORM / MATERIALIZE of an implied point: which point (PT_RAY, PT_START, PT_X)
     int px, pxp;                // objectives without neighbour coupling: the point rows of x and xp in the ring
+    int d_implied;              // ... and the first search (k == 1): d = -grad f(xp) is not stored, the passes that read d evaluate it
 };
 static_assert(sizeof(PRound<double>) == 128 && sizeof(PRound<float>) == 128, "a round descriptor is one 128-byte line");
 
@@ -181,60 +185,69 @@ template <int NV> __device__ __forceinline__ void block_sums(const double (&acc)
 }
 
 // ---- FIRST / TRIAL -------------------------------------------------------------------------------------------------------------
-// MODE 0: FIRST (evaluate at the flat x, write g, d = -g and x into point row `pout` of the ring) ; MODE 1: TRIAL (evaluate at
-// x = xp + step*d, xp = point row `pin`, store nothing: the point is rebuilt by the pass that needs it) ; MODE 2: MATERIALIZE of a ray
-// point (x = xp + step*d, write the flat x and g; no sums) ; MODE 3: MATERIALIZE of a stored point (evaluate at point row `pin`,
-// write the flat x and g; no sums).  Operands stream through registers with 128-bit loads/stores (a shared-memory staged variant
-// measured slower for this 1:1 read/write pass); a pack never crosses a block of the ring (BT >= 32).  Objectives without neighbour
-// coupling only: the coupled ones take p_trial_halo.
+// MODE 0: FIRST (evaluate at the flat x, write x into point row `pout` of the ring: neither g nor d = -g is stored) ; MODE 1: TRIAL
+// (evaluate at x = xp + step*d, xp = point row `pin`, store nothing: the point is rebuilt by the pass that needs it) ; MODE 2:
+// MATERIALIZE of a ray point (x = xp + step*d, write the flat x and g; no sums) ; MODE 3: MATERIALIZE of a stored point (evaluate at
+// point row `pin`, write the flat x and g; no sums).  d_implied (MODES 1, 2 in the first search): d is not read but evaluated as
+// T(-1) * grad f(xp) with FIRST's expressions, bit for bit the d FIRST would have stored; a run-time flag, not a template parameter:
+// two more inlined copies of the pass made the dots and combination passes of the kernel 1-2 % slower per round (C5 -1.1 %), measured,
+// and unrolling the flag's loop 4x instead of 2x gained nothing (0.0577 against 0.0581 ms per trial round).  Operands stream through
+// registers with 128-bit loads/stores (a shared-memory staged variant measured slower for this 1:1 read/write pass); a pack never crosses a block of
+// the ring (BT >= 32).  Objectives without neighbour coupling only: the coupled ones take p_trial_halo.
 template <class T, class OBJ, int MODE>
 __device__ __forceinline__ void p_trial(const OBJ& obj, const Own& own, const PHist<T>& h, int pin, const T* __restrict__ d, T step,
-                                        T* __restrict__ x, T* __restrict__ g, T* __restrict__ dout, int pout, PShared& sh, double* dst, int G,
-                                        bool evict_first)
+                                        T* __restrict__ x, T* __restrict__ g, int pout, PShared& sh, double* dst, int G, bool evict_first,
+                                        bool d_implied = false)
 {
     static_assert(!OBJ::kHalo, "neighbour-coupled objectives take p_trial_halo");
     T acc[4] = {T(0), T(0), T(0), T(0)};
     const int64_t n = own.n;
     const int64_t p1 = (own.c1 + 3) >> 2;
+    auto store = [&](T* base, int64_t i0, int cnt, const Pack<T>& v) {
+        if (evict_first) store4<T, Hint::Stream, true>(base, i0, cnt, v);
+        else store4<T, Hint::Plain, true>(base, i0, cnt, v);
+    };
     auto body = [&](int64_t q) {
         const int64_t i0 = q << 2;
         const int cnt = (n - i0 >= 4) ? 4 : int(n - i0);
         T xv[4], dv[4] = {T(0), T(0), T(0), T(0)}, gv[4];
         const T* xin = (MODE == 0) ? x + i0 : h.pt_at(pin, i0);
-        if (MODE == 1 || MODE == 2)
+        const Pack<T> px = load4<T, Hint::Stream, true>(xin, 0, cnt);
+        if constexpr (MODE == 1 || MODE == 2)
         {
-            const Pack<T> px = load4<T, Hint::Stream, true>(xin, 0, cnt), pd = load4<T, Hint::Stream, true>(d, i0, cnt);
+            if (d_implied)
+            {
+                T gp[4];
+                obj.eval(i0, cnt, px.v, T(0), T(0), gp);   // grad f(xp): FIRST's evaluation of the same point
 #pragma unroll
-            for (int k = 0; k < 4; k++) { dv[k] = pd.v[k]; xv[k] = px.v[k] + step * pd.v[k]; }
+                for (int k = 0; k < 4; k++) dv[k] = (k < cnt) ? T(-1) * gp[k] : T(0);
+            }
+            else
+            {
+                const Pack<T> pd = load4<T, Hint::Stream, true>(d, i0, cnt);
+#pragma unroll
+                for (int k = 0; k < 4; k++) dv[k] = pd.v[k];
+            }
+#pragma unroll
+            for (int k = 0; k < 4; k++) xv[k] = px.v[k] + step * dv[k];
         }
         else
         {
-            const Pack<T> px = load4<T, Hint::Stream, true>(xin, 0, cnt);
 #pragma unroll
             for (int k = 0; k < 4; k++) xv[k] = px.v[k];
         }
         eval_pack(obj, i0, cnt, xv, T(0), T(0), dv, gv, acc);
-        if constexpr (MODE != 1)
+        Pack<T> pxo;
+#pragma unroll
+        for (int k = 0; k < 4; k++) pxo.v[k] = xv[k];
+        if constexpr (MODE == 0) store(h.pt_at(pout, i0), 0, cnt, pxo);
+        if constexpr (MODE >= 2)
         {
-            Pack<T> pg, po;
+            Pack<T> pg;
 #pragma unroll
-            for (int k = 0; k < 4; k++) { pg.v[k] = gv[k]; po.v[k] = (MODE >= 2) ? xv[k] : T(-1) * gv[k]; }
-            T* const out0 = (MODE >= 2) ? x : dout;
-            Pack<T> pxo;
-#pragma unroll
-            for (int k = 0; k < 4; k++) pxo.v[k] = xv[k];
-            if (evict_first)
-            {
-                store4<T, Hint::Stream, true>(out0, i0, cnt, po);
-                store4<T, Hint::Stream, true>(g, i0, cnt, pg);
-                if (MODE == 0) store4<T, Hint::Stream, true>(h.pt_at(pout, i0), 0, cnt, pxo);
-            }
-            else
-            {
-                store4<T, Hint::Plain, true>(out0, i0, cnt, po);
-                store4<T, Hint::Plain, true>(g, i0, cnt, pg);
-                if (MODE == 0) store4<T, Hint::Plain, true>(h.pt_at(pout, i0), 0, cnt, pxo);
-            }
+            for (int k = 0; k < 4; k++) pg.v[k] = gv[k];
+            store(x, i0, cnt, pxo);
+            store(g, i0, cnt, pg);
         }
     };
 #pragma unroll 2
@@ -512,7 +525,8 @@ __device__ __forceinline__ void stage_points(T* dstt, int TE, int nrhs, int nloa
 //                                                    step*d and g = grad f(x) with the trial's own arithmetic (or x = xp, g = gp when
 //                                                    the search ended on its start point), s = x - xp, y = g - gp; x is written to its
 //                                                    point row (g is not stored: the next pass evaluates it from x; nor is the pair:
-//                                                    its readers rebuild it from its endpoints)
+//                                                    its readers rebuild it from its endpoints).  Iteration 1 (d_implied): d is not
+//                                                    staged but taken as T(-1) * gp, FIRST's d
 //     FORM,  stored point (neighbour-coupled)        staged g, x, gp, xp: s = x - xp, y = g - gp, written to ring slot `new_slot`
 //                                                    (row 0 stays g)
 //     PLAIN, no neighbour coupling                   the points: g = grad f(x)
@@ -539,6 +553,7 @@ template <class T> struct PDots
     T step;              // FORM of an implied point: its step (PT_RAY), or the start point (PT_START)
     int at_start;
     int px;              // FORM of an implied point: the point row it is written to
+    bool d_implied;      // FORM of an implied point: d = -grad f(xp) is not stored (iteration 1); the d row is not loaded
 };
 
 template <class T, class OBJ, int ROUNDS, bool FORM>
@@ -548,7 +563,7 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const 
     constexpr int EPT = 16 / (int)sizeof(T);
     constexpr bool HALO = OBJ::kHalo;
     constexpr int NRHS = !FORM ? 1 : (HALO ? 4 : 3);             // right-hand rows: g / (formed) ; FORM: g, x, gp, xp / d, (formed) x 2
-    constexpr int NLOAD = HALO ? NRHS : (FORM ? 1 : 0);          // ... of which the bulk copies fill the first NLOAD
+    const int nload = HALO ? NRHS : (FORM && !a.d_implied ? 1 : 0);   // ... of which the bulk copies fill the first nload
     __shared__ uint64_t formed_bar[kPMaxStages], empty_bar[kPMaxStages];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int TE = a.h.BT();
@@ -578,8 +593,8 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const 
     __syncthreads();   // sh.vecs / sh.slots and the barriers are in place, the staging ring is free
     int64_t next_tile = 0;
     auto stage_one = [&](T* dstt, int64_t t, uint64_t* bar) {
-        if constexpr (HALO) stage_tiled<T>(dstt, TE, NRHS, NLOAD, own.start(t, TE), own.len(t, TE), a.h, runs, sh, bar);
-        else stage_points<T>(dstt, TE, NRHS, NLOAD, own.start(t, TE), own.len(t, TE), a.h, sh, bar);
+        if constexpr (HALO) stage_tiled<T>(dstt, TE, NRHS, NRHS, own.start(t, TE), own.len(t, TE), a.h, runs, sh, bar);
+        else stage_points<T>(dstt, TE, NRHS, nload, own.start(t, TE), own.len(t, TE), a.h, sh, bar);
     };
     for (int s = 0; s < stages; s++, next_tile++)
         if (next_tile < ntl) stage_one(tiles + (size_t)s * nrows * TE, next_tile, &full_bar[s]);
@@ -619,12 +634,18 @@ __device__ __forceinline__ void p_dots(const PDots<T>& a, const OBJ& obj, const 
                         }
                         else
                         {
-                            const Unit<T> ud = lds_unit<T>(base + off);
                             uxp = lds_unit<T>(hist + (size_t)sh.xrow * TE + off);
                             ugp = grad_unit(obj, e0 + off, cnt, uxp);
                             if (a.at_start) { ux = uxp; ug = ugp; }
                             else
                             {
+                                Unit<T> ud;
+                                if (a.d_implied)   // FIRST's d = T(-1) * grad f(x0)
+                                {
+#pragma unroll
+                                    for (int k = 0; k < EPT; k++) ud.v[k] = T(-1) * ugp.v[k];
+                                }
+                                else ud = lds_unit<T>(base + off);
                                 // the trial's arithmetic (p_trial, and p_combine's first trial with step 1 on the stored d)
 #pragma unroll
                                 for (int k = 0; k < EPT; k++) ux.v[k] = (k < cnt) ? uxp.v[k] + a.step * ud.v[k] : T(0);
@@ -1195,16 +1216,17 @@ __device__ __forceinline__ void st_release_gpu_u32(unsigned* p, unsigned v)
 // trials store their points, every pass reads the stored g and the ring holds the c pairs as 2c columns (neighbour-coupled
 // objectives).  Otherwise g is evaluated from x wherever it is needed, only FIRST and MATERIALIZE write it, and the ring holds
 // points: c chained pairs are c + 1 of them (a chain broken by the curvature gate stages up to c more, not counted here).  pt: the
-// point a MATERIALIZE writes (PT_*)
-__device__ __forceinline__ double words_of(int op, int c, int data_vectors, bool stored, int pt)
+// point a MATERIALIZE writes (PT_*); d_implied: the first search's d = -grad f(xp) is evaluated, not read
+__device__ __forceinline__ double words_of(int op, int c, int data_vectors, bool stored, int pt, bool d_implied)
 {
+    const double dw = d_implied ? 0.0 : 1.0;
     switch (op)
     {
-    case POP_FIRST: return (stored ? 3.0 : 4.0) + data_vectors;   // R x ; W g, d (, x to its point row)
-    case POP_TRIAL: return (stored ? 4.0 : 2.0) + data_vectors;   // R xp, d (; W x, g)
+    case POP_FIRST: return (stored ? 3.0 : 2.0) + data_vectors;   // R x ; W g, d  /  R x ; W x to its point row
+    case POP_TRIAL: return (stored ? 4.0 : 1.0 + dw) + data_vectors;   // R xp, d (; W x, g)
     case POP_RESTORE: return 4.0;                           // R xp, gp ; W x, g
-    case POP_MATERIALIZE: return stored || pt == PT_RAY ? 4.0 : 3.0;   // R xp, d / xp / x ; W x, g
-    case POP_DOTS_FORM: return stored ? 2.0 * c + 4.0 : c + 2.0;   // R x, xp, g, gp, 2(c-1) columns ; W s, y  /  R d, c points ; W x
+    case POP_MATERIALIZE: return stored ? 4.0 : (pt == PT_RAY ? 3.0 + dw : 3.0);   // R xp, d / xp / x ; W x, g
+    case POP_DOTS_FORM: return stored ? 2.0 * c + 4.0 : c + 1.0 + dw;   // R x, xp, g, gp, 2(c-1) columns ; W s, y  /  R d, c points ; W x
     case POP_DOTS_PLAIN: return stored ? 2.0 * c + 1.0 : c + 2.0;  // R g, 2c columns  /  R x, c + 1 points
     case POP_COMBINE: return stored ? 2.0 * c + 2.0 : c + 2.0;     // R g, 2c columns / c + 1 points ; W d
     case POP_COMBINE_TRIAL: return (stored ? 2.0 * c + 5.0 : c + 2.0) + data_vectors;   // R g, x, 2c columns / c + 1 points ; W d (, x1, g1)
@@ -1330,7 +1352,7 @@ __device__ int leader_round(const PArgs<T>& a, int G, PShared& sh, PState<T>* ca
             PRound<T>* rd = a.rounds + b;
             rd->x = st->x; rd->xp = st->xp; rd->g = st->g; rd->gp = st->gp; rd->drt = st->drt;
             rd->step = st->step; rd->at_start = st->at_start;
-            if (!HALO) { rd->px = st->px; rd->pxp = st->pxp; }
+            if (!HALO) { rd->px = st->px; rd->pxp = st->pxp; rd->d_implied = st->k == 1; }
             rd->c_round = st->c_round; rd->head = st->head; rd->pending = st->pending; rd->gram_cur = st->gram_cur;
             rd->op = st->op;
             running = st->op != POP_IDLE;
@@ -1487,20 +1509,21 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
             const int c_round = ldv(&rd->c_round), head = ldv(&rd->head), pending = ldv(&rd->pending), gram_cur = ldv(&rd->gram_cur);
             const int at_start = ldv(&rd->at_start);
             const int px = HALO ? 0 : ldv(&rd->px), pxp = HALO ? 0 : ldv(&rd->pxp);
+            const bool d_implied = HALO ? false : ldv(&rd->d_implied) != 0;
             if (op == POP_IDLE) continue;
             acct_bucket = (acct_bucket == -1 || acct_bucket == op) ? op : 0;
-            acct_words += words_of(op, c_round, kDataVectors, HALO, at_start);
+            acct_words += words_of(op, c_round, kDataVectors, HALO, at_start, d_implied);
             double* dst = a.partials + (size_t)b * a.pstride * G + cta;
             const OBJ obj{ObjGeom<T>{a.n, a.index_offset, a.n_global, (HALO && a.xc != nullptr) ? st->halo : nullptr, st->data0, st->data1}};
             switch (op)
             {
             case POP_FIRST:
                 if constexpr (HALO) p_trial_halo<T, OBJ, 0>(obj, own, nullptr, nullptr, T(0), vx, vg, vd, tiles, sh, phase_bits, dst, G);
-                else p_trial<T, OBJ, 0>(obj, own, st->hist, 0, nullptr, T(0), vx, vg, vd, px, sh, dst, G, a.evict_first_stores);
+                else p_trial<T, OBJ, 0>(obj, own, st->hist, 0, nullptr, T(0), vx, nullptr, px, sh, dst, G, a.evict_first_stores);
                 break;
             case POP_TRIAL:
                 if constexpr (HALO) p_trial_halo<T, OBJ, 1>(obj, own, vxp, vd, step, vx, vg, nullptr, tiles, sh, phase_bits, dst, G);
-                else p_trial<T, OBJ, 1>(obj, own, st->hist, pxp, vd, step, nullptr, nullptr, nullptr, 0, sh, dst, G, a.evict_first_stores);
+                else p_trial<T, OBJ, 1>(obj, own, st->hist, pxp, vd, step, nullptr, nullptr, 0, sh, dst, G, a.evict_first_stores, d_implied);
                 break;
             case POP_RESTORE:
                 p_restore<T>(own, vxp, vgp, vx, vg);
@@ -1508,9 +1531,9 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
             case POP_MATERIALIZE:
                 if constexpr (!HALO)
                 {
-                    if (at_start == PT_RAY) p_trial<T, OBJ, 2>(obj, own, st->hist, pxp, vd, step, vx, vg, nullptr, 0, sh, dst, G, a.evict_first_stores);
+                    if (at_start == PT_RAY) p_trial<T, OBJ, 2>(obj, own, st->hist, pxp, vd, step, vx, vg, 0, sh, dst, G, a.evict_first_stores, d_implied);
                     else   // PT_START: x = xp ; PT_X: x = x (its point row) ; g = grad f(x)
-                        p_trial<T, OBJ, 3>(obj, own, st->hist, at_start == PT_START ? pxp : px, nullptr, T(0), vx, vg, nullptr, 0, sh, dst, G, a.evict_first_stores);
+                        p_trial<T, OBJ, 3>(obj, own, st->hist, at_start == PT_START ? pxp : px, nullptr, T(0), vx, vg, 0, sh, dst, G, a.evict_first_stores);
                 }
                 break;
             case POP_DOTS_FORM:
@@ -1522,7 +1545,7 @@ __global__ void __launch_bounds__(kPThreads, 1) k_persist(PArgs<T> a)
                 d.end = head;                                   // the old columns: the slots below the free slot `head`
                 d.cnt_old = form ? c_round - 1 : c_round;
                 d.new_slot = form ? head : -1;
-                d.step = step; d.at_start = at_start; d.px = px;
+                d.step = step; d.at_start = at_start; d.px = px; d.d_implied = d_implied;
                 dots_geometry(d.c, d.h.BT() / (16 / (int)sizeof(T)), d.split, d.cols_per_round);
                 __syncthreads();   // sh.slots / sh.vecs may still be read by the previous problem's pass
                 if constexpr (!HALO)

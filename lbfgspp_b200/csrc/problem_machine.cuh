@@ -197,9 +197,10 @@ template <class T, bool G_IMPLIED = false, bool POINTS = false> __device__ __for
     return true;
 }
 
-// G_IMPLIED (the resident solve, objectives without neighbour coupling): g is stored by FIRST and MATERIALIZE only; every other pass
-// that needs grad f of a stored point evaluates it from x, bit for bit the g that would have been stored.  POINTS (the same solve):
-// the ring holds iterates (see PState::pts)
+// G_IMPLIED (the resident solve, objectives without neighbour coupling): g is stored by MATERIALIZE only; every other pass that needs
+// grad f of a stored point evaluates it from x, bit for bit the g that would have been stored, and the first search's direction
+// -grad f(x0) (k == 1: until the first combination pass writes d) is evaluated from x0 as well.  So every stop, at FIRST too, takes
+// one MATERIALIZE round.  POINTS (the same solve): the ring holds iterates (see PState::pts)
 template <class T, bool STORED, bool G_IMPLIED = false, bool POINTS = false> __device__ void advance_problem(PState<T>* st, const double* vals)
 {
     st->rounds++;
@@ -214,9 +215,14 @@ template <class T, bool STORED, bool G_IMPLIED = false, bool POINTS = false> __d
         st->k = 1;
         if (st->past > 0) st->fx_hist[0] = fx;
         st->gnorm = std::sqrt(gg);
-        if (LBFGSpp::gradient_converged(st->gnorm, xx, st->epsilon, st->epsilon_rel)) { finish(st, 1); return; }
+        if (LBFGSpp::gradient_converged(st->gnorm, xx, st->epsilon, st->epsilon_rel))
+        {
+            if (G_IMPLIED) st->at_start = PT_X;   // FIRST wrote x0 to point row px only
+            finish(st, 1, 0, G_IMPLIED);
+            return;
+        }
         st->rec.dg = -gg;                   // grad . (-grad)
-        begin_search<T, false, POINTS>(st, T(1) / st->gnorm); // LBFGS.h:108
+        begin_search<T, G_IMPLIED, POINTS>(st, T(1) / st->gnorm); // LBFGS.h:108
         return;
     }
     case POP_TRIAL:
