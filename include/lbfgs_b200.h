@@ -173,6 +173,40 @@ const void* lbfgs_b200_hist_y_col(const lbfgs_b200_hist* h, int age);
 LBFGS_B200_DECLARE_HIST(double, f64)
 LBFGS_B200_DECLARE_HIST(float, f32)
 
+/* ---------------------------------------------------------------- L1-regularised path (OWLQNSolver, include/OWLQN.h)
+ * OWL-QN (Andrew & Gao, "Scalable training of L1-regularized log-linear models", ICML 2007) for F(x) = f(x) + lam |x|_1.  The
+ * pseudo-gradient pg(x, g; lam) (g = grad f(x)) is never stored: every pass forms it from x and g with the expressions of
+ * include/LBFGSpp/OWLQNCore.h (owlqn_pg, owlqn_orthant, owlqn_project, owlqn_constrain).  Every entry refuses (LBFGS_B200_ERR_INVALID)
+ * a lam that is not positive and finite and a context with more than one rank (no n-sharding); the history entry also refuses a
+ * history of the other precision. */
+#define LBFGS_B200_DECLARE_OWLQN(T, SUF)                                                                       \
+    /* The paper's projected line-search trial (section 3.2, "projected line search") for a built-in objective, ONE kernel:     \
+     *   x = pi(xp + step*d; xi), xi_i = sign(xp_i) or, at xp_i = 0, sign(-pgp_i), pgp = pg(xp, gp);  g = grad f(x);           \
+     *   out5 = { f(x), |x|_1, pgp.(x - xp), pg.pg, x.x }.  Neighbour-coupled objectives see the projected neighbours.          \
+     * 5 words per coordinate (+ data vectors). */                                                             \
+    lbfgs_b200_status lbfgs_b200_owlqn_trial_##SUF(lbfgs_b200_ctx*, int objective, const T* data0, const T* data1,   \
+                                                   int64_t n, const T* xp, const T* d, const T* gp, T step, T lam,    \
+                                                   T* x, T* g, T* out5_host);                                        \
+    /* The same projection for any objective (the user functor then evaluates f and g at x):                     \
+     * x = pi(xp + step*d; xi);  out2 = { |x|_1, pgp.(x - xp) }.  4 words per coordinate. */                     \
+    lbfgs_b200_status lbfgs_b200_owlqn_project_##SUF(lbfgs_b200_ctx*, int64_t n, const T* xp, const T* d,         \
+                                                     const T* gp, T step, T lam, T* x, T* out2_host);              \
+    /* The sums at a point (x, g): out3 = { |x|_1, pg.pg, x.x }.  With d != NULL also the first search's direction   \
+     * d = -pg (the paper's steepest-descent start; LBFGS.h:106-108 with pg in place of g).  d may not alias x or g. */ \
+    lbfgs_b200_status lbfgs_b200_owlqn_sums_##SUF(lbfgs_b200_ctx*, int64_t n, const T* x, const T* g, T lam, T* d, \
+                                                  T* out3_host);                                                    \
+    /* The paper's direction (section 3.2, "choosing a direction") after the pair update: the curvature-gated pair  \
+     * s = x - xp, y = g - gp (smooth gradients) formed into the ring inside the Gram dots pass, whose right-hand vector is \
+     * pg(x, g) formed from the staged x and g tiles; then d = -H pg in the Gram form with d_i = 0 wherever d_i pg_i >= 0, and \
+     * dg_host = pg.d over the constrained d.  x, xp, g, gp on 4-element boundaries (lbfgs_b200_malloc); d may not alias them. \
+     * accepted_host (optional) = the gate's verdict. */                                                        \
+    lbfgs_b200_status lbfgs_b200_owlqn_update_dir_##SUF(lbfgs_b200_hist* h, const T* x, const T* xp, const T* g,  \
+                                                        const T* gp, T eps, T lam, T* d, int* accepted_host,       \
+                                                        T* dg_host);
+
+LBFGS_B200_DECLARE_OWLQN(double, f64)
+LBFGS_B200_DECLARE_OWLQN(float, f32)
+
 /* ---------------------------------------------------------------- bound-constrained path (LBFGSBSolver, config 4)
  * Index sets of the reference (std::vector<int> free / active / L / U / P sets of Cauchy.h and SubspaceMin.h) are bits of
  * a per-coordinate class byte; W = [Y, theta*S] is never gathered: every W-product is a masked pass over the S/Y columns.

@@ -112,6 +112,11 @@ def _declare(lib):
         getattr(lib, "lbfgs_b200_hist_apply_Hv_" + suf).argtypes = [vp, vp, ct, vp, ci, pt]
         getattr(lib, "lbfgs_b200_hist_update_apply_Hv_" + suf).argtypes = [vp, vp, vp, vp, vp, ct, ct, vp, ci, C.POINTER(ci), pt]
         getattr(lib, "lbfgs_b200_hist_scalars_" + suf).argtypes = [vp, pt, pt, pt]
+        if hasattr(lib, "lbfgs_b200_owlqn_trial_" + suf):
+            getattr(lib, "lbfgs_b200_owlqn_trial_" + suf).argtypes = [vp, ci, vp, vp, i64, vp, vp, vp, ct, ct, vp, vp, pt]
+            getattr(lib, "lbfgs_b200_owlqn_project_" + suf).argtypes = [vp, i64, vp, vp, vp, ct, ct, vp, pt]
+            getattr(lib, "lbfgs_b200_owlqn_sums_" + suf).argtypes = [vp, i64, vp, vp, ct, vp, pt]
+            getattr(lib, "lbfgs_b200_owlqn_update_dir_" + suf).argtypes = [vp, vp, vp, vp, vp, ct, ct, vp, C.POINTER(ci), pt]
     # bound-constrained path
     lib.lbfgs_b200_box_create.argtypes = [vp, C.POINTER(vp)]
     lib.lbfgs_b200_box_destroy.argtypes = [vp]
@@ -237,6 +242,11 @@ class _DrvResult(C.Structure):
                 ("d2h_bytes", C.c_long)]
 
 
+class _OwlqnResult(C.Structure):
+    _fields_ = [("status", C.c_int), ("msg", C.c_char * 200), ("niter", C.c_int), ("nfev", C.c_long), ("fx", C.c_double),
+                ("gnorm", C.c_double), ("seconds", C.c_double)]
+
+
 def driver(lib=None):
     """liblbfgs_b200_driver.so, or `lib` (a library exporting the same entry points, e.g. built on a test double), typed."""
     if lib is not None:
@@ -333,6 +343,10 @@ def _declare_driver(lib):
                                                                          C.c_uint, pt, dp, dp, C.POINTER(cl), C.POINTER(ci), err, errlen]
         lib.lbfgsb200_drv_box_hist_hessian_f64.argtypes = [ci, cl, ci, ci, dp, dp, ci, C.POINTER(C.c_ubyte), ci, ci, dp, dp, C.c_ulonglong,
                                                            C.c_uint, dp, dp, dp, C.POINTER(cl), err, errlen]
+    # the L1-regularised solve (csrc/driver_owlqn.cpp)
+    if hasattr(lib, "lbfgsb200_drv_owlqn_f64"):
+        for suf, pt in (("f64", dp), ("f32", fp)):
+            getattr(lib, "lbfgsb200_drv_owlqn_" + suf).argtypes = [ci, ci, pt, pt, cl, prm, C.c_double, ci, pt, pt, C.POINTER(_OwlqnResult)]
     lib._drv_typed = True
     return lib
 
@@ -383,6 +397,39 @@ class LBFGSParam:
     def _c(self):
         return _DrvParam(self.m, self.epsilon, self.epsilon_rel, self.past, self.delta, self.max_iterations,
                          self.linesearch, 10, self.max_linesearch, self.min_step, self.max_step, self.ftol, self.wolfe)
+
+
+class OWLQNSolver:
+    """LBFGSpp::OWLQNSolver<Scalar> on the GPU (include/OWLQN.h): minimises f(x) + lam |x|_1, host buffers in and out.
+
+    minimize(objective, x0) returns dict(status, msg, niter, nfev, fx = F(x), gnorm = ||pg||, x, grad = grad f(x), seconds = the
+    synchronised minimize() alone); with
+    raise_errors=True the exceptions come back as ValueError / ArithmeticError / RuntimeError as for LBFGSSolver.  plain=True runs the
+    objective as a plain device functor (projection kernel -> objective -> sums kernel) instead of the fused projected trial.
+    From param it uses m, epsilon, epsilon_rel, past, delta, max_iterations, max_linesearch, min_step, max_step and ftol.
+    """
+
+    def __init__(self, param=None, lam=1.0, dtype=np.float64, device=0, lib=None):
+        self.param = param if param is not None else LBFGSParam()
+        self.lam = float(lam)
+        self.dtype = np.dtype(dtype)
+        self.device = device
+        self.lib = lib
+
+    def minimize(self, objective, x0, data0=None, data1=None, plain=False, raise_errors=False):
+        drv = driver(self.lib)
+        dt = self.dtype
+        x = np.array(x0, dtype=dt, order="C").copy()
+        grad = np.zeros(x.size, dtype=dt)
+        d0, d1 = (None if a is None else np.ascontiguousarray(a, dtype=dt) for a in (data0, data1))
+        res = _OwlqnResult()
+        p = self.param._c()
+        fn = drv.lbfgsb200_drv_owlqn_f64 if dt == np.float64 else drv.lbfgsb200_drv_owlqn_f32
+        fn(self.device, objective, _ptr(d0), _ptr(d1), x.size, C.byref(p), self.lam, 0 if plain else 1, _ptr(x), _ptr(grad), C.byref(res))
+        if res.status and raise_errors:
+            raise _EXC.get(res.status, RuntimeError)(res.msg.decode())
+        return dict(status=STATUS_NAMES[res.status], msg=res.msg.decode(), niter=res.niter, nfev=res.nfev, fx=res.fx, gnorm=res.gnorm,
+                    x=x, grad=grad, seconds=res.seconds)
 
 
 class LBFGSBParam:
@@ -579,6 +626,27 @@ class Context:
         return list(out)
 
 
+    # OWL-QN kernels (include/lbfgs_b200.h, lbfgs_b200_owlqn_*): F = f + lam |x|_1
+    def owlqn_trial(self, kind, xp, d, gp, step, lam, x, g, data0=None, data1=None):
+        """Fused projected trial of a built-in objective: writes x, g; -> [f, |x|_1, pgp.(x - xp), pg.pg, x.x]"""
+        out = (x.ct * 5)()
+        self.check(self._fn("owlqn_trial", x.dtype)(self.h, kind, data0.ptr if data0 else None, data1.ptr if data1 else None, xp.n,
+                                                    xp.ptr, d.ptr, gp.ptr, step, lam, x.ptr, g.ptr, out))
+        return list(out)
+
+    def owlqn_project(self, xp, d, gp, step, lam, x):
+        """x = pi(xp + step d; xi); -> [|x|_1, pgp.(x - xp)]"""
+        out = (x.ct * 2)()
+        self.check(self._fn("owlqn_project", x.dtype)(self.h, xp.n, xp.ptr, d.ptr, gp.ptr, step, lam, x.ptr, out))
+        return list(out)
+
+    def owlqn_sums(self, x, g, lam, d=None):
+        """-> [|x|_1, pg.pg, x.x]; with d also writes d = -pg"""
+        out = (x.ct * 3)()
+        self.check(self._fn("owlqn_sums", x.dtype)(self.h, x.n, x.ptr, g.ptr, lam, d.ptr if d is not None else None, out))
+        return list(out)
+
+
 class DeviceArray:
     def __init__(self, ctx, host=None, dtype=None, n=None, offset_elems=0):
         self.ctx = ctx
@@ -653,6 +721,15 @@ class History:
         out = (self.ct * 1)()
         self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_hist_update_apply_Hv_" + self.suf)(
             self.h, x.ptr, xp.ptr, g.ptr, gp.ptr, eps, a, res.ptr, algo, C.byref(acc), out))
+        return bool(acc.value), out[0]
+
+    def owlqn_update_dir(self, x, xp, g, gp, lam, d, eps=None):
+        """OWL-QN: pair update + d = the orthant-constrained -H pg(x, g); -> (accepted, pg.d)"""
+        eps = np.finfo(self.dtype).eps if eps is None else eps
+        acc = C.c_int(0)
+        out = (self.ct * 1)()
+        self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_owlqn_update_dir_" + self.suf)(
+            self.h, x.ptr, xp.ptr, g.ptr, gp.ptr, eps, lam, d.ptr, C.byref(acc), out))
         return bool(acc.value), out[0]
 
     def apply_Hv(self, v, a, res, algo=HV_AUTO, want_dot=False):

@@ -64,7 +64,7 @@ def build_kernels(force=False, verbose=False):
 
 
 DRIVER_UNITS = ["driver.cpp", "driver_hessian_ops.cpp", "driver_small_batch.cpp", "driver_hessian_diag.cpp",
-               "driver_hessian_sample.cpp", "driver_hessian_whiten.cpp", "driver_box_hessian.cpp"]   # g++ units of the driver library
+               "driver_hessian_sample.cpp", "driver_hessian_whiten.cpp", "driver_box_hessian.cpp", "driver_owlqn.cpp"]   # g++ units of the driver library
 
 
 def build_driver(force=False):

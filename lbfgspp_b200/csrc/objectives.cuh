@@ -22,6 +22,7 @@
 #include <stdint.h>
 
 #include "device_utils.cuh"
+#include "../../include/LBFGSpp/OWLQNCore.h"
 
 namespace lb {
 
@@ -183,6 +184,38 @@ __device__ __forceinline__ void eval_pack(const OBJ& obj, int64_t i0, int cnt, c
         acc[1] += g[k] * d[k];
         acc[2] += g[k] * g[k];
         acc[3] += (k < cnt) ? x[k] * x[k] : T(0);
+    }
+}
+
+// OWL-QN (LBFGSpp/OWLQNCore.h): one pack of the projected trial x = pi(xp + step d; xi), whose start point xp, direction d and start
+// gradient gp the caller loaded; x and g of the pack into x, g, and its {f, |x|_1, pgp.(x - xp), pg.pg, x.x} over the cnt valid
+// lanes added to acc[0..4].  The neighbours of a coupled objective are the projected trial coordinates, which `at(j)` returns from
+// the three input vectors with the same expression (owlqn_point).  One GPU only: no halo.
+template <class T, class OBJ, class At>
+__device__ __forceinline__ void eval_pack_owlqn(const OBJ& obj, int64_t i0, int64_t n, int cnt, const T (&xp)[4], const T (&d)[4],
+                                                const T (&gp)[4], T step, T lam, At at, T (&x)[4], T (&g)[4], T* acc)
+{
+    T pgp[4];
+#pragma unroll
+    for (int k = 0; k < 4; k++)
+    {
+        pgp[k] = LBFGSpp::owlqn_pg(xp[k], gp[k], lam);
+        x[k] = (k < cnt) ? LBFGSpp::owlqn_project(xp[k] + step * d[k], LBFGSpp::owlqn_orthant(xp[k], pgp[k])) : T(0);
+    }
+    T xl = T(0), xr = T(0);
+    if constexpr (OBJ::kHalo) pack_neighbours<false>(obj, i0, n, step, at, xl, xr);
+    acc[0] += obj.eval(i0, cnt, x, xl, xr, g);
+#pragma unroll
+    for (int k = 0; k < 4; k++)
+    {
+        if (k < cnt)
+        {
+            const T pg = LBFGSpp::owlqn_pg(x[k], g[k], lam);
+            acc[1] += x[k] < T(0) ? -x[k] : x[k];
+            acc[2] += pgp[k] * (x[k] - xp[k]);
+            acc[3] += pg * pg;
+            acc[4] += x[k] * x[k];
+        }
     }
 }
 

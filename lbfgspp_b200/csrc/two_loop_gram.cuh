@@ -21,6 +21,7 @@
 #pragma once
 
 #include "device_utils.cuh"
+#include "../../include/LBFGSpp/OWLQNCore.h"
 
 namespace lb {
 
@@ -115,11 +116,14 @@ __device__ __forceinline__ Pack<float> lds_pack(const float* p, int)
 }
 
 // FORM ("update + dots"): forms the newest pair from (x, xp, g, gp) while it computes [S Y]'[g s_new y_new]  (see GramDotsArgs)
-template <class T, int ROUNDS, bool FORM>
-__global__ void __launch_bounds__(kGramMaxThreads, 1) k_gram_dots(GramDotsArgs<T> a, double* partials, unsigned* ticket, double* result, const XComm* xc, unsigned long long epoch)
+// PG (OWL-QN, FORM only): the right-hand vector is the pseudo-gradient pg(x, g; lam) (LBFGSpp/OWLQNCore.h), formed per element
+// from the staged x and g tiles before they become s and y: [S Y]'[pg s_new y_new], the same HBM traffic as FORM
+template <class T, int ROUNDS, bool FORM, bool PG>
+__device__ __forceinline__ void gram_dots_body(unsigned char* gram_smem, const GramDotsArgs<T>& a, T lam, double* partials, unsigned* ticket,
+                                               double* result, const XComm* xc, unsigned long long epoch)
 {
+    static_assert(FORM || !PG, "the pseudo-gradient is formed from the staged x and g of the FORM variant");
     constexpr int NT = FORM ? 4 : 3;                             // staged vectors per tile: v, s_new, y_new (+ xp while forming)
-    extern __shared__ __align__(128) unsigned char gram_smem[];
     T* tiles = reinterpret_cast<T*>(gram_smem);                  // [stage][NT][TE]
     __shared__ __align__(8) uint64_t full_bar[kGramStages];
     __shared__ double s_red[kGramMaxWarps][ROUNDS * kGramVals];
@@ -182,7 +186,8 @@ __global__ void __launch_bounds__(kGramMaxThreads, 1) k_gram_dots(GramDotsArgs<T
                     const T gv = ok ? a.v[e0 + i] : T(0);
                     const T sv = ok ? a.fx[e0 + i] - a.fxp[e0 + i] : T(0);
                     const T yv = ok ? gv - a.fgp[e0 + i] : T(0);
-                    dst[i] = gv;
+                    if constexpr (PG) dst[i] = ok ? LBFGSpp::owlqn_pg(a.fx[e0 + i], gv, lam) : T(0);
+                    else dst[i] = gv;
                     dst[kGramTE + i] = sv;
                     dst[2 * kGramTE + i] = yv;
                     if (ok) { a.s_out[e0 + i] = sv; a.y_out[e0 + i] = yv; }
@@ -225,15 +230,21 @@ __global__ void __launch_bounds__(kGramMaxThreads, 1) k_gram_dots(GramDotsArgs<T
         const int64_t e0f = tile * kGramTE;
         for (int i = tid * 4; i < kGramTE; i += nthreads * 4)
         {
-            Pack<T> ps, py;
+            Pack<T> ps, py, pp;
 #pragma unroll
             for (int k = 0; k < 4; k++)
             {
                 ps.v[k] = t0[kGramTE + i + k] - t0[3 * kGramTE + i + k];
                 py.v[k] = t0[i + k] - t0[2 * kGramTE + i + k];
+                if constexpr (PG) pp.v[k] = LBFGSpp::owlqn_pg(t0[kGramTE + i + k], t0[i + k], lam);
             }
 #pragma unroll
-            for (int k = 0; k < 4; k++) { t0[kGramTE + i + k] = ps.v[k]; t0[2 * kGramTE + i + k] = py.v[k]; }
+            for (int k = 0; k < 4; k++)
+            {
+                t0[kGramTE + i + k] = ps.v[k];
+                t0[2 * kGramTE + i + k] = py.v[k];
+                if constexpr (PG) t0[i + k] = pp.v[k];
+            }
             st_pack<Hint::Plain>(a.s_out + e0f + i, ps);
             st_pack<Hint::Plain>(a.y_out + e0f + i, py);
         }
@@ -381,6 +392,22 @@ __global__ void __launch_bounds__(kGramMaxThreads, 1) k_gram_dots(GramDotsArgs<T
         __threadfence();
         xrank_allreduce(result, nvals, xc, epoch);
     }
+}
+
+template <class T, int ROUNDS, bool FORM>
+__global__ void __launch_bounds__(kGramMaxThreads, 1) k_gram_dots(GramDotsArgs<T> a, double* partials, unsigned* ticket, double* result, const XComm* xc, unsigned long long epoch)
+{
+    extern __shared__ __align__(128) unsigned char gram_smem[];
+    gram_dots_body<T, ROUNDS, FORM, false>(gram_smem, a, T(0), partials, ticket, result, xc, epoch);
+}
+
+// OWL-QN: the pair-forming dots with pg(x, g; lam) as the right-hand vector (the FORM variant's staging, see gram_dots_body)
+template <class T, int ROUNDS>
+__global__ void __launch_bounds__(kGramMaxThreads, 1) k_gram_dots_pg(GramDotsArgs<T> a, T lam, double* partials, unsigned* ticket, double* result,
+                                                                     const XComm* xc, unsigned long long epoch)
+{
+    extern __shared__ __align__(128) unsigned char gram_smem[];
+    gram_dots_body<T, ROUNDS, true, true>(gram_smem, a, lam, partials, ticket, result, xc, epoch);
 }
 
 // ---- the O(c^2) recursion on coefficients ---------------------------------------------------------------------
@@ -579,6 +606,71 @@ __global__ void __launch_bounds__(kThreads) k_gram_combine(GramCombineArgs<T> a,
         {
             out.v[k] = r[k];
             dot += (k < cnt) ? pv.v[k] * r[k] : T(0);
+        }
+        store4<T, Hint::Plain, VEC>(a.res, i0, cnt, out);
+    }
+    if (a.want_dot)
+    {
+        double dacc[1] = {(double)dot};
+        grid_reduce<1>(dacc, rb);
+    }
+}
+
+// OWL-QN: k_gram_combine with v = pg(x, g; lam) formed per element from x and g = a.v, res = the orthant-constrained combination
+// (owlqn_constrain against pg: d = -H pg projected, with a = -1) and the dot pg.res over the constrained res
+template <class T, bool VEC>
+__global__ void __launch_bounds__(kThreads) k_gram_combine_pg(GramCombineArgs<T> a, const T* x, T lam, ReduceBuf rb)
+{
+    extern __shared__ __align__(16) unsigned char comb_smem[];
+    T* sm = reinterpret_cast<T*>(comb_smem);
+    const int c = a.solve.c;
+    gram_solve_in_smem<T>(a.solve, sm, blockIdx.x == 0);
+    const T* s_coef = sm + 2 * c * c;
+    __shared__ const T* s_ycol[kMaxM];
+    __shared__ const T* s_scol[kMaxM];
+    for (int j = threadIdx.x; j < c; j += kThreads)
+    {
+        s_ycol[j] = a.Y + (int64_t)a.solve.slots[j] * a.ld;
+        s_scol[j] = a.S + (int64_t)a.solve.slots[j] * a.ld;
+    }
+    __syncthreads();
+    const T cv = s_coef[0];
+    T dot = T(0);
+    const int64_t packs = (a.n + 3) >> 2, stride = (int64_t)gridDim.x * kThreads;
+    for (int64_t p = (int64_t)blockIdx.x * kThreads + threadIdx.x; p < packs; p += stride)
+    {
+        const int64_t i0 = p << 2;
+        const int cnt = (a.n - i0 >= 4) ? 4 : int(a.n - i0);
+        const Pack<T> px = load4<T, Hint::Stream, VEC>(x, i0, cnt);
+        Pack<T> pv = load4<T, Hint::Stream, VEC>(a.v, i0, cnt);
+#pragma unroll
+        for (int k = 0; k < 4; k++) pv.v[k] = LBFGSpp::owlqn_pg(px.v[k], pv.v[k], lam);
+        T r[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) r[k] = cv * pv.v[k];
+        // y terms newest -> oldest, then s terms oldest -> newest (the order the recursion would add them)
+#pragma unroll 4
+        for (int j = 0; j < c; j++)
+        {
+            const Pack<T> py = load4<T, Hint::Stream, VEC>(s_ycol[j], i0, cnt);
+            const T cy = s_coef[1 + j];
+#pragma unroll
+            for (int k = 0; k < 4; k++) r[k] += cy * py.v[k];
+        }
+#pragma unroll 4
+        for (int j = c - 1; j >= 0; j--)
+        {
+            const Pack<T> ps = load4<T, Hint::Stream, VEC>(s_scol[j], i0, cnt);
+            const T cs = s_coef[1 + c + j];
+#pragma unroll
+            for (int k = 0; k < 4; k++) r[k] += cs * ps.v[k];
+        }
+        Pack<T> out;
+#pragma unroll
+        for (int k = 0; k < 4; k++)
+        {
+            out.v[k] = LBFGSpp::owlqn_constrain(r[k], pv.v[k]);
+            dot += (k < cnt) ? pv.v[k] * out.v[k] : T(0);
         }
         store4<T, Hint::Plain, VEC>(a.res, i0, cnt, out);
     }
