@@ -53,6 +53,38 @@ LBFGS_HD inline T owlqn_constrain(T d, T pg)
     return (d * pg >= T(0)) ? T(0) : d;
 }
 
+// Per-coordinate weights, F = f + lambda sum_i w_i |x_i|: coordinate i carries lam_i = lambda * w_i, rounded once in T
+// (owlqn_lam_i).  Where lam_i > 0 the expressions above apply with lam_i in place of lambda; where lam_i == 0 (w_i = 0, or a w_i so
+// small that lambda * w_i underflows) the coordinate is smooth: pg_i = g_i (owlqn_pg at lam = 0), the trial coordinate is not
+// projected and the direction is not constrained.
+template <typename T>
+LBFGS_HD inline T owlqn_lam_i(T lam, T w)
+{
+    return lam * w;
+}
+
+// one coordinate of the weighted trial point: pi(xp + step d; xi) where lam_i > 0, xp + step d where lam_i == 0
+template <typename T>
+LBFGS_HD inline T owlqn_point_w(T xp, T d, T gp, T step, T lam_i)
+{
+    return lam_i > T(0) ? owlqn_point(xp, d, gp, step, lam_i) : xp + step * d;
+}
+
+// the weighted direction constraint: owlqn_constrain where lam_i > 0, d unchanged where lam_i == 0
+template <typename T>
+LBFGS_HD inline T owlqn_constrain_w(T d, T pg, T lam_i)
+{
+    return lam_i > T(0) ? owlqn_constrain(d, pg) : d;
+}
+
+// a weight the solver accepts: w >= 0, finite, and lambda * w finite (v - v is 0 exactly for a finite v, NaN otherwise)
+template <typename T>
+LBFGS_HD inline bool owlqn_weight_ok(T lam, T w)
+{
+    const T lw = owlqn_lam_i(lam, w);
+    return w >= T(0) && w - w == T(0) && lw - lw == T(0);
+}
+
 // The projected backtracking search of OWL-QN as a resumable core (the shape of the four cores of LineSearchCore.h):
 //     int init(opts, F0, dg0, step0)   dg0 = pg(xp).d; returns 0 or an error code
 //     int advance(F, dirder)           F = F(x) at the trial, dirder = pg(xp).(x - xp); LSC_EVALUATE at the new `step`,

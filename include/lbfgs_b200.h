@@ -202,7 +202,27 @@ LBFGS_B200_DECLARE_HIST(float, f32)
      * accepted_host (optional) = the gate's verdict. */                                                        \
     lbfgs_b200_status lbfgs_b200_owlqn_update_dir_##SUF(lbfgs_b200_hist* h, const T* x, const T* xp, const T* g,  \
                                                         const T* gp, T eps, T lam, T* d, int* accepted_host,       \
-                                                        T* dg_host);
+                                                        T* dg_host);                                                \
+    /* Per-coordinate weights, F(x) = f(x) + lam sum_i w_i |x_i|: each entry above with w (n entries, device memory) after   \
+     * lam.  Coordinate i carries lam_i = lam * w_i rounded once in T; where lam_i > 0 the expressions above apply with lam_i, \
+     * where lam_i == 0 (w_i = 0, or a w_i so small that lam * w_i underflows) the coordinate is smooth: pg_i = g_i, the trial \
+     * coordinate is xp_i + step d_i unprojected, d_i is not constrained.  The sums report sum_i w_i |x_i| in place of       \
+     * |x|_1.  Each refuses a NULL w, and update_dir a w off the 4-element boundary it asks of x.  The sums entry checks     \
+     * every weight in its pass: any w_i negative or not finite, or with lam * w_i not finite, makes it return               \
+     * LBFGS_B200_ERR_INVALID with their count in the error message; the other entries trust w.  One more word per         \
+     * coordinate in each pass. */                                                                              \
+    lbfgs_b200_status lbfgs_b200_owlqn_weighted_trial_##SUF(lbfgs_b200_ctx*, int objective, const T* data0,       \
+                                                            const T* data1, int64_t n, const T* xp, const T* d,   \
+                                                            const T* gp, T step, T lam, const T* w, T* x, T* g,   \
+                                                            T* out5_host);                                          \
+    lbfgs_b200_status lbfgs_b200_owlqn_weighted_project_##SUF(lbfgs_b200_ctx*, int64_t n, const T* xp, const T* d, \
+                                                              const T* gp, T step, T lam, const T* w, T* x,       \
+                                                              T* out2_host);                                        \
+    lbfgs_b200_status lbfgs_b200_owlqn_weighted_sums_##SUF(lbfgs_b200_ctx*, int64_t n, const T* x, const T* g, T lam, \
+                                                           const T* w, T* d, T* out3_host);                        \
+    lbfgs_b200_status lbfgs_b200_owlqn_weighted_update_dir_##SUF(lbfgs_b200_hist* h, const T* x, const T* xp,     \
+                                                                 const T* g, const T* gp, T eps, T lam, const T* w, \
+                                                                 T* d, int* accepted_host, T* dg_host);
 
 LBFGS_B200_DECLARE_OWLQN(double, f64)
 LBFGS_B200_DECLARE_OWLQN(float, f32)

@@ -117,6 +117,11 @@ def _declare(lib):
             getattr(lib, "lbfgs_b200_owlqn_project_" + suf).argtypes = [vp, i64, vp, vp, vp, ct, ct, vp, pt]
             getattr(lib, "lbfgs_b200_owlqn_sums_" + suf).argtypes = [vp, i64, vp, vp, ct, vp, pt]
             getattr(lib, "lbfgs_b200_owlqn_update_dir_" + suf).argtypes = [vp, vp, vp, vp, vp, ct, ct, vp, C.POINTER(ci), pt]
+        if hasattr(lib, "lbfgs_b200_owlqn_weighted_trial_" + suf):
+            getattr(lib, "lbfgs_b200_owlqn_weighted_trial_" + suf).argtypes = [vp, ci, vp, vp, i64, vp, vp, vp, ct, ct, vp, vp, vp, pt]
+            getattr(lib, "lbfgs_b200_owlqn_weighted_project_" + suf).argtypes = [vp, i64, vp, vp, vp, ct, ct, vp, vp, pt]
+            getattr(lib, "lbfgs_b200_owlqn_weighted_sums_" + suf).argtypes = [vp, i64, vp, vp, ct, vp, vp, pt]
+            getattr(lib, "lbfgs_b200_owlqn_weighted_update_dir_" + suf).argtypes = [vp, vp, vp, vp, vp, ct, ct, vp, vp, C.POINTER(ci), pt]
     # bound-constrained path
     lib.lbfgs_b200_box_create.argtypes = [vp, C.POINTER(vp)]
     lib.lbfgs_b200_box_destroy.argtypes = [vp]
@@ -346,7 +351,8 @@ def _declare_driver(lib):
     # the L1-regularised solve (csrc/driver_owlqn.cpp)
     if hasattr(lib, "lbfgsb200_drv_owlqn_f64"):
         for suf, pt in (("f64", dp), ("f32", fp)):
-            getattr(lib, "lbfgsb200_drv_owlqn_" + suf).argtypes = [ci, ci, pt, pt, cl, prm, C.c_double, ci, pt, pt, C.POINTER(_OwlqnResult)]
+            getattr(lib, "lbfgsb200_drv_owlqn_" + suf).argtypes = [ci, ci, pt, pt, cl, prm, C.c_double, pt, ci, pt, pt,
+                                                                   C.POINTER(_OwlqnResult)]
     lib._drv_typed = True
     return lib
 
@@ -407,25 +413,31 @@ class OWLQNSolver:
     raise_errors=True the exceptions come back as ValueError / ArithmeticError / RuntimeError as for LBFGSSolver.  plain=True runs the
     objective as a plain device functor (projection kernel -> objective -> sums kernel) instead of the fused projected trial.
     From param it uses m, epsilon, epsilon_rel, past, delta, max_iterations, max_linesearch, min_step, max_step and ftol.
+    weights (n entries, or None): F = f(x) + lam sum_i w_i |x_i|, w_i >= 0; a coordinate with lam * w_i == 0 is not penalised.
     """
 
-    def __init__(self, param=None, lam=1.0, dtype=np.float64, device=0, lib=None):
+    def __init__(self, param=None, lam=1.0, weights=None, dtype=np.float64, device=0, lib=None):
         self.param = param if param is not None else LBFGSParam()
         self.lam = float(lam)
+        self.weights = weights
         self.dtype = np.dtype(dtype)
         self.device = device
         self.lib = lib
 
     def minimize(self, objective, x0, data0=None, data1=None, plain=False, raise_errors=False):
-        drv = driver(self.lib)
         dt = self.dtype
         x = np.array(x0, dtype=dt, order="C").copy()
+        w = None if self.weights is None else np.ascontiguousarray(self.weights, dtype=dt)
+        if w is not None and w.shape != (x.size,):
+            raise ValueError("weights must have one entry per coordinate of x0 (got %s for n = %d)" % (w.shape, x.size))
+        drv = driver(self.lib)
         grad = np.zeros(x.size, dtype=dt)
         d0, d1 = (None if a is None else np.ascontiguousarray(a, dtype=dt) for a in (data0, data1))
         res = _OwlqnResult()
         p = self.param._c()
         fn = drv.lbfgsb200_drv_owlqn_f64 if dt == np.float64 else drv.lbfgsb200_drv_owlqn_f32
-        fn(self.device, objective, _ptr(d0), _ptr(d1), x.size, C.byref(p), self.lam, 0 if plain else 1, _ptr(x), _ptr(grad), C.byref(res))
+        fn(self.device, objective, _ptr(d0), _ptr(d1), x.size, C.byref(p), self.lam, _ptr(w), 0 if plain else 1, _ptr(x), _ptr(grad),
+           C.byref(res))
         if res.status and raise_errors:
             raise _EXC.get(res.status, RuntimeError)(res.msg.decode())
         return dict(status=STATUS_NAMES[res.status], msg=res.msg.decode(), niter=res.niter, nfev=res.nfev, fx=res.fx, gnorm=res.gnorm,
@@ -646,6 +658,29 @@ class Context:
         self.check(self._fn("owlqn_sums", x.dtype)(self.h, x.n, x.ptr, g.ptr, lam, d.ptr if d is not None else None, out))
         return list(out)
 
+    # the same under per-coordinate weights w (F = f + lam sum_i w_i |x_i|; lbfgs_b200_owlqn_weighted_*)
+    def owlqn_weighted_trial(self, kind, xp, d, gp, step, lam, w, x, g, data0=None, data1=None):
+        """-> [f, sum w_i |x_i|, pgp.(x - xp), pg.pg, x.x]; writes x, g"""
+        out = (x.ct * 5)()
+        self.check(self._fn("owlqn_weighted_trial", x.dtype)(self.h, kind, data0.ptr if data0 else None, data1.ptr if data1 else None,
+                                                             xp.n, xp.ptr, d.ptr, gp.ptr, step, lam, w.ptr if w is not None else None,
+                                                             x.ptr, g.ptr, out))
+        return list(out)
+
+    def owlqn_weighted_project(self, xp, d, gp, step, lam, w, x):
+        """-> [sum w_i |x_i|, pgp.(x - xp)]; writes x"""
+        out = (x.ct * 2)()
+        self.check(self._fn("owlqn_weighted_project", x.dtype)(self.h, xp.n, xp.ptr, d.ptr, gp.ptr, step, lam,
+                                                               w.ptr if w is not None else None, x.ptr, out))
+        return list(out)
+
+    def owlqn_weighted_sums(self, x, g, lam, w, d=None):
+        """-> [sum w_i |x_i|, pg.pg, x.x]; with d also writes d = -pg; refuses (LbfgsB200Error) any bad weight"""
+        out = (x.ct * 3)()
+        self.check(self._fn("owlqn_weighted_sums", x.dtype)(self.h, x.n, x.ptr, g.ptr, lam, w.ptr if w is not None else None,
+                                                            d.ptr if d is not None else None, out))
+        return list(out)
+
 
 class DeviceArray:
     def __init__(self, ctx, host=None, dtype=None, n=None, offset_elems=0):
@@ -730,6 +765,15 @@ class History:
         out = (self.ct * 1)()
         self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_owlqn_update_dir_" + self.suf)(
             self.h, x.ptr, xp.ptr, g.ptr, gp.ptr, eps, lam, d.ptr, C.byref(acc), out))
+        return bool(acc.value), out[0]
+
+    def owlqn_weighted_update_dir(self, x, xp, g, gp, lam, w, d, eps=None):
+        """OWL-QN under per-coordinate weights w: pair update + the weighted constrained -H pg(x, g); -> (accepted, pg.d)"""
+        eps = np.finfo(self.dtype).eps if eps is None else eps
+        acc = C.c_int(0)
+        out = (self.ct * 1)()
+        self.ctx.check(getattr(self.ctx.lib, "lbfgs_b200_owlqn_weighted_update_dir_" + self.suf)(
+            self.h, x.ptr, xp.ptr, g.ptr, gp.ptr, eps, lam, w.ptr if w is not None else None, d.ptr, C.byref(acc), out))
         return bool(acc.value), out[0]
 
     def apply_Hv(self, v, a, res, algo=HV_AUTO, want_dot=False):

@@ -343,12 +343,122 @@ __global__ void __launch_bounds__(kThreads) k_owlqn_sums(int64_t n, const T* __r
     grid_reduce<3>(dacc, rb);
 }
 
+// Per-coordinate weights (F = f + lam sum_i w_i |x_i|): each pass above has a weighted twin that reads w on the same packs (one more
+// word per coordinate), forms lam_i = lam * w_i (owlqn_lam_i), reports sum w_i |x_i| in place of |x|_1, and leaves the coordinates
+// with lam_i == 0 unprojected and unconstrained (owlqn_point_w, owlqn_constrain_w).  The twins keep the launch geometry, element
+// ownership and summation order, so w = 1 reproduces the unweighted bits.  They are kernels of their own: one body behind a weight
+// flag moved the registers of the unweighted kernels (see DESIGN.md, section 8h).
+//
+// weighted fused projected trial                                                                   [R 4 + W 2 (+data)]
+template <class T, class OBJ, bool VEC>
+__global__ void __launch_bounds__(kThreads) k_owlqn_trial_w(OBJ obj, int64_t n, const T* __restrict__ xp, const T* __restrict__ d,
+                                                            const T* __restrict__ gp, T step, T lam, const T* __restrict__ w,
+                                                            T* __restrict__ x, T* __restrict__ g, ReduceBuf rb)
+{
+    T acc[5] = {T(0), T(0), T(0), T(0), T(0)};
+    const int64_t packs = (n + 3) >> 2, stride = (int64_t)gridDim.x * kThreads;
+#pragma unroll 2
+    for (int64_t p = (int64_t)blockIdx.x * kThreads + threadIdx.x; p < packs; p += stride)
+    {
+        const int64_t i0 = p << 2;
+        const int cnt = (n - i0 >= 4) ? 4 : int(n - i0);
+        const Pack<T> pxp = load4<T, Hint::Stream, VEC>(xp, i0, cnt), pd = load4<T, Hint::Stream, VEC>(d, i0, cnt),
+                      pgp = load4<T, Hint::Stream, VEC>(gp, i0, cnt), pw = load4<T, Hint::Stream, VEC>(w, i0, cnt);
+        T xv[4], gv[4];
+        // the neighbours of a coupled objective are projected under their own weights
+        const auto at = [&](int j) {
+            return LBFGSpp::owlqn_point_w(xp[i0 + j], d[i0 + j], gp[i0 + j], step, LBFGSpp::owlqn_lam_i(lam, w[i0 + j]));
+        };
+        eval_pack_owlqn_w(obj, i0, n, cnt, pxp.v, pd.v, pgp.v, pw.v, step, lam, at, xv, gv, acc);
+        Pack<T> pg, pxo;
+#pragma unroll
+        for (int k = 0; k < 4; k++) { pg.v[k] = gv[k]; pxo.v[k] = xv[k]; }
+        store4<T, Hint::Plain, VEC>(x, i0, cnt, pxo);
+        store4<T, Hint::Plain, VEC>(g, i0, cnt, pg);
+    }
+    double dacc[5] = {(double)acc[0], (double)acc[1], (double)acc[2], (double)acc[3], (double)acc[4]};
+    grid_reduce<5>(dacc, rb);
+}
+
+// weighted projection: {sum w_i |x_i|, pgp.(x - xp)}                                                 [R 4 + W 1]
+template <class T, bool VEC>
+__global__ void __launch_bounds__(kThreads) k_owlqn_project_w(int64_t n, const T* __restrict__ xp, const T* __restrict__ d,
+                                                              const T* __restrict__ gp, T step, T lam, const T* __restrict__ w,
+                                                              T* __restrict__ x, ReduceBuf rb)
+{
+    T acc[2] = {T(0), T(0)};
+    const int64_t packs = (n + 3) >> 2, stride = (int64_t)gridDim.x * kThreads;
+#pragma unroll 2
+    for (int64_t p = (int64_t)blockIdx.x * kThreads + threadIdx.x; p < packs; p += stride)
+    {
+        const int64_t i0 = p << 2;
+        const int cnt = (n - i0 >= 4) ? 4 : int(n - i0);
+        const Pack<T> pxp = load4<T, Hint::Stream, VEC>(xp, i0, cnt), pd = load4<T, Hint::Stream, VEC>(d, i0, cnt),
+                      pgp = load4<T, Hint::Stream, VEC>(gp, i0, cnt), pw = load4<T, Hint::Stream, VEC>(w, i0, cnt);
+        Pack<T> px;
+#pragma unroll
+        for (int k = 0; k < 4; k++)
+        {
+            const T lk = LBFGSpp::owlqn_lam_i(lam, pw.v[k]);
+            const T pgk = LBFGSpp::owlqn_pg(pxp.v[k], pgp.v[k], lk);
+            px.v[k] = (k < cnt) ? (lk > T(0) ? LBFGSpp::owlqn_project(pxp.v[k] + step * pd.v[k], LBFGSpp::owlqn_orthant(pxp.v[k], pgk))
+                                             : pxp.v[k] + step * pd.v[k])
+                                : T(0);
+            acc[0] += pw.v[k] * (px.v[k] < T(0) ? -px.v[k] : px.v[k]);
+            acc[1] += pgk * (px.v[k] - pxp.v[k]);
+        }
+        store4<T, Hint::Plain, VEC>(x, i0, cnt, px);
+    }
+    double dacc[2] = {(double)acc[0], (double)acc[1]};
+    grid_reduce<2>(dacc, rb);
+}
+
+// weighted sums: {sum w_i |x_i|, pg.pg, x.x, the number of weights owlqn_weight_ok refuses}; START writes d = -pg  [R 3 (+W 1)]
+template <class T, bool START, bool VEC>
+__global__ void __launch_bounds__(kThreads) k_owlqn_sums_w(int64_t n, const T* __restrict__ x, const T* __restrict__ g, T lam,
+                                                           const T* __restrict__ w, T* __restrict__ d, ReduceBuf rb)
+{
+    T acc[4] = {T(0), T(0), T(0), T(0)};
+    const int64_t packs = (n + 3) >> 2, stride = (int64_t)gridDim.x * kThreads;
+#pragma unroll 2
+    for (int64_t p = (int64_t)blockIdx.x * kThreads + threadIdx.x; p < packs; p += stride)
+    {
+        const int64_t i0 = p << 2;
+        const int cnt = (n - i0 >= 4) ? 4 : int(n - i0);
+        const Pack<T> px = load4<T, Hint::Stream, VEC>(x, i0, cnt), pg = load4<T, Hint::Stream, VEC>(g, i0, cnt),
+                      pw = load4<T, Hint::Stream, VEC>(w, i0, cnt);
+        Pack<T> pd;
+#pragma unroll
+        for (int k = 0; k < 4; k++)
+        {
+            const T pgk = LBFGSpp::owlqn_pg(px.v[k], pg.v[k], LBFGSpp::owlqn_lam_i(lam, pw.v[k]));
+            pd.v[k] = -pgk;
+            acc[0] += pw.v[k] * (px.v[k] < T(0) ? -px.v[k] : px.v[k]);
+            acc[1] += pgk * pgk;
+            acc[2] += px.v[k] * px.v[k];
+            acc[3] += LBFGSpp::owlqn_weight_ok(lam, pw.v[k]) ? T(0) : T(1);   // the lanes past cnt read w = 0
+        }
+        if (START) store4<T, Hint::Plain, VEC>(d, i0, cnt, pd);
+    }
+    double dacc[4] = {(double)acc[0], (double)acc[1], (double)acc[2], (double)acc[3]};
+    grid_reduce<4>(dacc, rb);
+}
+
 // pg(x, g) into out (the spare ring column), for the dots round that follows a pair the curvature gate refused      [R 2 + W 1]
 template <class T>
 __global__ void __launch_bounds__(kThreads) k_owlqn_pg(int64_t n, const T* __restrict__ x, const T* __restrict__ g, T lam, T* __restrict__ out)
 {
     const int64_t stride = (int64_t)gridDim.x * kThreads;
     for (int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x; i < n; i += stride) out[i] = LBFGSpp::owlqn_pg(x[i], g[i], lam);
+}
+// the same under per-coordinate weights                                                                               [R 3 + W 1]
+template <class T>
+__global__ void __launch_bounds__(kThreads) k_owlqn_pg_w(int64_t n, const T* __restrict__ x, const T* __restrict__ g, T lam,
+                                                         const T* __restrict__ w, T* __restrict__ out)
+{
+    const int64_t stride = (int64_t)gridDim.x * kThreads;
+    for (int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x; i < n; i += stride)
+        out[i] = LBFGSpp::owlqn_pg(x[i], g[i], LBFGSpp::owlqn_lam_i(lam, w[i]));
 }
 
 // =====================================================================================================
@@ -1332,74 +1442,126 @@ template <class T> static lbfgs_b200_status owlqn_receive(lbfgs_b200_ctx* ctx, i
     return LBFGS_B200_OK;
 }
 
+// The weighted entries (w != nullptr) refuse a NULL w, and a w off the alignment x must have.  Only the sums entry reads every
+// weight for validity (its count of refused weights costs no extra pass); the others trust w.
+template <class T> static lbfgs_b200_status owlqn_weights(lbfgs_b200_ctx* ctx, bool weighted, const T* w, const char* what)
+{
+    REQUIRE(ctx, !weighted || w, "%s: NULL weights", what);
+    return LBFGS_B200_OK;
+}
+
 template <class T>
 static lbfgs_b200_status do_owlqn_trial(lbfgs_b200_ctx* ctx, int objective, const T* data0, const T* data1, int64_t n, const T* xp,
-                                        const T* d, const T* gp, T step, T lam, T* x, T* g, T* out5)
+                                        const T* d, const T* gp, T step, T lam, const T* w, bool weighted, T* x, T* g, T* out5)
 {
     REQUIRE(ctx, ctx && xp && d && gp && x && g && out5 && n >= 1, "owlqn_trial: bad arguments");
+    if (auto st = owlqn_weights<T>(ctx, weighted, w, "owlqn_weighted_trial")) return st;
     if (auto st = owlqn_check<T>(ctx, lam)) return st;
     return with_objective<T>(ctx, objective, [&](auto tag) -> lbfgs_b200_status {
         using OBJ = decltype(tag);
         ObjGeom<T> geo;
         if (auto st = objective_geometry<OBJ>(ctx, n, data0, data1, geo)) return st;
-        ProfSpan span(ctx, PH_TRIAL, double(sizeof(T)) * double(n) * (5.0 + OBJ::kDataVectors));
+        ProfSpan span(ctx, PH_TRIAL, double(sizeof(T)) * double(n) * ((weighted ? 6.0 : 5.0) + OBJ::kDataVectors));
         const int grid = grid_for(ctx, n, 2);
         const ReduceBuf rb = next_rb(ctx, true);
-        if (all_aligned<T>({xp, d, gp, x, g}))
+        const bool vec = all_aligned<T>({xp, d, gp, x, g}) && (!weighted || all_aligned<T>({w}));
+        if (weighted)
+        {
+            if (vec) k_owlqn_trial_w<T, OBJ, true><<<grid, kThreads, 0, ctx->stream>>>(OBJ{geo}, n, xp, d, gp, step, lam, w, x, g, rb);
+            else k_owlqn_trial_w<T, OBJ, false><<<grid, kThreads, 0, ctx->stream>>>(OBJ{geo}, n, xp, d, gp, step, lam, w, x, g, rb);
+        }
+        else if (vec)
             k_owlqn_trial<T, OBJ, true><<<grid, kThreads, 0, ctx->stream>>>(OBJ{geo}, n, xp, d, gp, step, lam, x, g, rb);
         else
             k_owlqn_trial<T, OBJ, false><<<grid, kThreads, 0, ctx->stream>>>(OBJ{geo}, n, xp, d, gp, step, lam, x, g, rb);
-        if (auto st = post_launch(ctx, "k_owlqn_trial")) return st;
+        if (auto st = post_launch(ctx, weighted ? "k_owlqn_trial_w" : "k_owlqn_trial")) return st;
         span.stop();
         return owlqn_receive<T>(ctx, 5, out5);
     });
 }
 
 template <class T>
-static lbfgs_b200_status do_owlqn_project(lbfgs_b200_ctx* ctx, int64_t n, const T* xp, const T* d, const T* gp, T step, T lam, T* x, T* out2)
+static lbfgs_b200_status do_owlqn_project(lbfgs_b200_ctx* ctx, int64_t n, const T* xp, const T* d, const T* gp, T step, T lam, const T* w,
+                                          bool weighted, T* x, T* out2)
 {
     REQUIRE(ctx, ctx && xp && d && gp && x && out2 && n >= 1, "owlqn_project: bad arguments");
+    if (auto st = owlqn_weights<T>(ctx, weighted, w, "owlqn_weighted_project")) return st;
     if (auto st = owlqn_check<T>(ctx, lam)) return st;
     const int grid = grid_for(ctx, n);
     const ReduceBuf rb = next_rb(ctx, true);
-    if (all_aligned<T>({xp, d, gp, x})) k_owlqn_project<T, true><<<grid, kThreads, 0, ctx->stream>>>(n, xp, d, gp, step, lam, x, rb);
+    const bool vec = all_aligned<T>({xp, d, gp, x}) && (!weighted || all_aligned<T>({w}));
+    if (weighted)
+    {
+        if (vec) k_owlqn_project_w<T, true><<<grid, kThreads, 0, ctx->stream>>>(n, xp, d, gp, step, lam, w, x, rb);
+        else k_owlqn_project_w<T, false><<<grid, kThreads, 0, ctx->stream>>>(n, xp, d, gp, step, lam, w, x, rb);
+    }
+    else if (vec) k_owlqn_project<T, true><<<grid, kThreads, 0, ctx->stream>>>(n, xp, d, gp, step, lam, x, rb);
     else k_owlqn_project<T, false><<<grid, kThreads, 0, ctx->stream>>>(n, xp, d, gp, step, lam, x, rb);
-    if (auto st = post_launch(ctx, "k_owlqn_project")) return st;
+    if (auto st = post_launch(ctx, weighted ? "k_owlqn_project_w" : "k_owlqn_project")) return st;
     return owlqn_receive<T>(ctx, 2, out2);
 }
 
+template <class T, bool START, bool VEC>
+static void launch_owlqn_sums(lbfgs_b200_ctx* ctx, int grid, int64_t n, const T* x, const T* g, T lam, const T* w, bool weighted, T* d,
+                              const ReduceBuf& rb)
+{
+    if (weighted) k_owlqn_sums_w<T, START, VEC><<<grid, kThreads, 0, ctx->stream>>>(n, x, g, lam, w, d, rb);
+    else k_owlqn_sums<T, START, VEC><<<grid, kThreads, 0, ctx->stream>>>(n, x, g, lam, d, rb);
+}
+
+// weighted: the kernel also counts the weights owlqn_weight_ok refuses; any such weight makes the entry return
+// LBFGS_B200_ERR_INVALID with that count (out3 is written all the same)
 template <class T>
-static lbfgs_b200_status do_owlqn_sums(lbfgs_b200_ctx* ctx, int64_t n, const T* x, const T* g, T lam, T* d, T* out3)
+static lbfgs_b200_status do_owlqn_sums(lbfgs_b200_ctx* ctx, int64_t n, const T* x, const T* g, T lam, const T* w, bool weighted, T* d, T* out3)
 {
     REQUIRE(ctx, ctx && x && g && out3 && n >= 1, "owlqn_sums: bad arguments");
     REQUIRE(ctx, d != x && d != g, "owlqn_sums: d aliases x or g");
+    if (auto st = owlqn_weights<T>(ctx, weighted, w, "owlqn_weighted_sums")) return st;
     if (auto st = owlqn_check<T>(ctx, lam)) return st;
     const int grid = grid_for(ctx, n);
     const ReduceBuf rb = next_rb(ctx, true);
-    const bool vec = all_aligned<T>({x, g, d});
+    const bool vec = all_aligned<T>({x, g, d}) && (!weighted || all_aligned<T>({w}));
     if (d)
     {
-        if (vec) k_owlqn_sums<T, true, true><<<grid, kThreads, 0, ctx->stream>>>(n, x, g, lam, d, rb);
-        else k_owlqn_sums<T, true, false><<<grid, kThreads, 0, ctx->stream>>>(n, x, g, lam, d, rb);
+        if (vec) launch_owlqn_sums<T, true, true>(ctx, grid, n, x, g, lam, w, weighted, d, rb);
+        else launch_owlqn_sums<T, true, false>(ctx, grid, n, x, g, lam, w, weighted, d, rb);
     }
     else
     {
-        if (vec) k_owlqn_sums<T, false, true><<<grid, kThreads, 0, ctx->stream>>>(n, x, g, lam, nullptr, rb);
-        else k_owlqn_sums<T, false, false><<<grid, kThreads, 0, ctx->stream>>>(n, x, g, lam, nullptr, rb);
+        if (vec) launch_owlqn_sums<T, false, true>(ctx, grid, n, x, g, lam, w, weighted, nullptr, rb);
+        else launch_owlqn_sums<T, false, false>(ctx, grid, n, x, g, lam, w, weighted, nullptr, rb);
     }
-    if (auto st = post_launch(ctx, "k_owlqn_sums")) return st;
-    return owlqn_receive<T>(ctx, 3, out3);
+    if (auto st = post_launch(ctx, weighted ? "k_owlqn_sums_w" : "k_owlqn_sums")) return st;
+    if (!weighted) return owlqn_receive<T>(ctx, 3, out3);
+    if (auto st = receive(ctx, 4)) return st;
+    for (int k = 0; k < 3; k++) out3[k] = (T)ctx->h_result[k];
+    const double bad = ctx->h_result[3];
+    REQUIRE(ctx, bad == 0.0, "owlqn_weighted_sums: %.0f weights are negative, not finite, or make lambda * w overflow", bad);
+    return LBFGS_B200_OK;
 }
 
 // d = the orthant-constrained -H pg and pg.d, after the new pair's update: the Gram form of do_hist_update_apply_Hv with
 // pg(x, g; lam) as the right-hand vector.  The pair (s, y) = (x - xp, g - gp) is formed in the dots pass (k_gram_dots_pg); if the
 // curvature gate refuses it, the dots of the kept history are taken again against pg written into the spare ring column.
+// Weighted: k_gram_dots_pg_w / k_gram_combine_pg_w / k_owlqn_pg_w, the same passes with one more word per coordinate each.
 template <class T>
-static lbfgs_b200_status launch_gram_dots_pg(lbfgs_b200_ctx* ctx, const GramDotsArgs<T>& a, T lam, int rounds, int grid, int threads, size_t smem)
+static lbfgs_b200_status launch_gram_dots_pg(lbfgs_b200_ctx* ctx, const GramDotsArgs<T>& a, T lam, const T* w, int rounds, int grid, int threads,
+                                             size_t smem)
 {
     const int r = rounds <= 1 ? 1 : rounds == 2 ? 2 : 3;
+    const unsigned bit = 1u << ((w ? 24 : 16) + (sizeof(T) == 8 ? 0 : 4) + r);
+    if (w)
+    {
+        const auto kernel = r == 1 ? k_gram_dots_pg_w<T, 1> : r == 2 ? k_gram_dots_pg_w<T, 2> : k_gram_dots_pg_w<T, 3>;
+        if (!(ctx->smem_optin & bit))
+        {
+            CU(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            ctx->smem_optin |= bit;
+        }
+        kernel<<<grid, threads, smem, ctx->stream>>>(a, lam, w, ctx->gram_partials, ctx->rb.ticket, ctx->gram_raw);
+        return post_launch(ctx, "k_gram_dots_pg_w");
+    }
     const auto kernel = r == 1 ? k_gram_dots_pg<T, 1> : r == 2 ? k_gram_dots_pg<T, 2> : k_gram_dots_pg<T, 3>;
-    const unsigned bit = 1u << (16 + (sizeof(T) == 8 ? 0 : 4) + r);
     if (!(ctx->smem_optin & bit))
     {
         CU(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1409,20 +1571,37 @@ static lbfgs_b200_status launch_gram_dots_pg(lbfgs_b200_ctx* ctx, const GramDots
     return post_launch(ctx, "k_gram_dots_pg");
 }
 
+template <class T, bool VEC>
+static lbfgs_b200_status launch_gram_combine_pg(lbfgs_b200_ctx* ctx, const GramCombineArgs<T>& k, const T* x, T lam, const T* w, int grid,
+                                                size_t smem)
+{
+    if (smem > 40 * 1024)
+    {
+        if (w) CU(ctx, cudaFuncSetAttribute(k_gram_combine_pg_w<T, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        else CU(ctx, cudaFuncSetAttribute(k_gram_combine_pg<T, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    }
+    const ReduceBuf rb = next_rb(ctx, true);
+    if (w) k_gram_combine_pg_w<T, VEC><<<grid, kThreads, smem, ctx->stream>>>(k, x, lam, w, rb);
+    else k_gram_combine_pg<T, VEC><<<grid, kThreads, smem, ctx->stream>>>(k, x, lam, rb);
+    return post_launch(ctx, w ? "k_gram_combine_pg_w" : "k_gram_combine_pg");
+}
+
 template <class T>
-static lbfgs_b200_status do_owlqn_update_dir(lbfgs_b200_hist* h, const T* x, const T* xp, const T* g, const T* gp, T eps, T lam, T* d,
-                                             int* accepted_host, T* dg_host)
+static lbfgs_b200_status do_owlqn_update_dir(lbfgs_b200_hist* h, const T* x, const T* xp, const T* g, const T* gp, T eps, T lam, const T* w,
+                                             bool weighted, T* d, int* accepted_host, T* dg_host)
 {
     if (auto st = hist_check<T>(h)) return st;
     lbfgs_b200_ctx* ctx = h->ctx;
     REQUIRE(ctx, x && xp && g && gp && d && dg_host, "owlqn_update_dir: NULL argument");
     REQUIRE(ctx, d != g && d != x && d != xp && d != gp, "owlqn_update_dir: d aliases an input");
     REQUIRE(ctx, all_aligned<T>({x, xp, g, gp}), "owlqn_update_dir: x, xp, g and gp must start on %zu-byte boundaries", 4 * sizeof(T));
+    if (auto st = owlqn_weights<T>(ctx, weighted, w, "owlqn_weighted_update_dir")) return st;
+    REQUIRE(ctx, !weighted || all_aligned<T>({w}), "owlqn_weighted_update_dir: w must start on a %zu-byte boundary, like x", 4 * sizeof(T));
     if (auto st = owlqn_check<T>(ctx, lam)) return st;
     if (h->pending >= 0)
         if (auto st = gram_refresh<T>(h)) return st;
     const int c_new = h->ncorr < h->m ? h->ncorr + 1 : h->m;
-    ProfSpan span(ctx, PH_APPLY_HV, double(sizeof(T)) * double(h->n) * (4.0 * c_new + 3.0 + 7.0));
+    ProfSpan span(ctx, PH_APPLY_HV, double(sizeof(T)) * double(h->n) * (4.0 * c_new + 3.0 + (weighted ? 9.0 : 7.0)));
     // the FORM dots of gram_dots(), with pg in place of g
     GramDotsArgs<T> a{};
     a.n = h->n; a.ld = h->ld; a.v = g;
@@ -1440,15 +1619,18 @@ static lbfgs_b200_status do_owlqn_update_dir(lbfgs_b200_hist* h, const T* x, con
     const int rounds = (c_new + a.cols_per_round - 1) / a.cols_per_round;
     const int64_t ntiles = (h->n + kGramTE - 1) / kGramTE;
     const int grid = (int)(ntiles < ctx->sm_count ? ntiles : ctx->sm_count);
-    if (auto st = launch_gram_dots_pg<T>(ctx, a, lam, rounds, grid, a.cols_per_round * split * 32, (size_t)kGramStages * 4 * kGramTE * sizeof(T)))
+    const T* wk = weighted ? w : nullptr;
+    if (auto st = launch_gram_dots_pg<T>(ctx, a, lam, wk, rounds, grid, a.cols_per_round * split * 32,
+                                         (size_t)kGramStages * 4 * kGramTE * sizeof(T)))
         return st;
     int ok = 0;
     if (auto st = commit_pair<T>(h, eps, 1, &ok, nullptr, ctx->gram_raw + 2)) return st;   // age-0 column: [2] = s'y, [3] = y'y
     if (!ok && h->ncorr > 0)
     {
         T* pg = h->s_col<T>(h->head);   // the refused pair's column is free again
-        k_owlqn_pg<T><<<grid_for(ctx, h->n), kThreads, 0, ctx->stream>>>(h->n, x, g, lam, pg);
-        if (auto st = post_launch(ctx, "k_owlqn_pg")) return st;
+        if (weighted) k_owlqn_pg_w<T><<<grid_for(ctx, h->n), kThreads, 0, ctx->stream>>>(h->n, x, g, lam, w, pg);
+        else k_owlqn_pg<T><<<grid_for(ctx, h->n), kThreads, 0, ctx->stream>>>(h->n, x, g, lam, pg);
+        if (auto st = post_launch(ctx, weighted ? "k_owlqn_pg_w" : "k_owlqn_pg")) return st;
         if (auto st = gram_dots<T>(h, pg)) return st;
     }
     // the combination: with no pair kept, H = I / theta and the recursion runs on no columns
@@ -1459,16 +1641,8 @@ static lbfgs_b200_status do_owlqn_update_dir(lbfgs_b200_hist* h, const T* x, con
     k.solve = make_solve_args<T>(h, T(-1), true);
     const int cgrid = grid_for(ctx, h->n, 1);
     const size_t smem = gram_solve_smem_elems(h->ncorr) * sizeof(T);
-    const bool vec = all_aligned<T>({d});
-    if (smem > 40 * 1024)
-    {
-        if (vec) CU(ctx, cudaFuncSetAttribute(k_gram_combine_pg<T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        else CU(ctx, cudaFuncSetAttribute(k_gram_combine_pg<T, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    }
-    const ReduceBuf rb = next_rb(ctx, true);
-    if (vec) k_gram_combine_pg<T, true><<<cgrid, kThreads, smem, ctx->stream>>>(k, x, lam, rb);
-    else k_gram_combine_pg<T, false><<<cgrid, kThreads, smem, ctx->stream>>>(k, x, lam, rb);
-    if (auto st = post_launch(ctx, "k_gram_combine_pg")) return st;
+    if (all_aligned<T>({d})) { if (auto st = launch_gram_combine_pg<T, true>(ctx, k, x, lam, wk, cgrid, smem)) return st; }
+    else if (auto st = launch_gram_combine_pg<T, false>(ctx, k, x, lam, wk, cgrid, smem)) return st;
     gram_folded(h);
     span.stop();
     if (accepted_host) *accepted_host = ok;
@@ -1595,15 +1769,30 @@ DEFINE_HIST(float, f32)
 #define DEFINE_OWLQN(T, SUF)                                                                                   \
     lbfgs_b200_status lbfgs_b200_owlqn_trial_##SUF(lbfgs_b200_ctx* c, int obj, const T* d0, const T* d1, int64_t n, \
                                                    const T* xp, const T* d, const T* gp, T step, T lam, T* x, T* g, \
-                                                   T* out5) { return do_owlqn_trial<T>(c, obj, d0, d1, n, xp, d, gp, step, lam, x, g, out5); } \
+                                                   T* out5)                                                     \
+    { return do_owlqn_trial<T>(c, obj, d0, d1, n, xp, d, gp, step, lam, nullptr, false, x, g, out5); }         \
     lbfgs_b200_status lbfgs_b200_owlqn_project_##SUF(lbfgs_b200_ctx* c, int64_t n, const T* xp, const T* d, const T* gp, \
                                                      T step, T lam, T* x, T* out2)                              \
-    { return do_owlqn_project<T>(c, n, xp, d, gp, step, lam, x, out2); }                                       \
+    { return do_owlqn_project<T>(c, n, xp, d, gp, step, lam, nullptr, false, x, out2); }                       \
     lbfgs_b200_status lbfgs_b200_owlqn_sums_##SUF(lbfgs_b200_ctx* c, int64_t n, const T* x, const T* g, T lam, T* d, \
-                                                  T* out3) { return do_owlqn_sums<T>(c, n, x, g, lam, d, out3); } \
+                                                  T* out3) { return do_owlqn_sums<T>(c, n, x, g, lam, nullptr, false, d, out3); } \
     lbfgs_b200_status lbfgs_b200_owlqn_update_dir_##SUF(lbfgs_b200_hist* h, const T* x, const T* xp, const T* g,  \
                                                         const T* gp, T eps, T lam, T* d, int* acc, T* dg)       \
-    { return do_owlqn_update_dir<T>(h, x, xp, g, gp, eps, lam, d, acc, dg); }
+    { return do_owlqn_update_dir<T>(h, x, xp, g, gp, eps, lam, nullptr, false, d, acc, dg); }                  \
+    lbfgs_b200_status lbfgs_b200_owlqn_weighted_trial_##SUF(lbfgs_b200_ctx* c, int obj, const T* d0, const T* d1, int64_t n, \
+                                                            const T* xp, const T* d, const T* gp, T step, T lam, const T* w, \
+                                                            T* x, T* g, T* out5)                                \
+    { return do_owlqn_trial<T>(c, obj, d0, d1, n, xp, d, gp, step, lam, w, true, x, g, out5); }                \
+    lbfgs_b200_status lbfgs_b200_owlqn_weighted_project_##SUF(lbfgs_b200_ctx* c, int64_t n, const T* xp, const T* d, \
+                                                              const T* gp, T step, T lam, const T* w, T* x, T* out2) \
+    { return do_owlqn_project<T>(c, n, xp, d, gp, step, lam, w, true, x, out2); }                              \
+    lbfgs_b200_status lbfgs_b200_owlqn_weighted_sums_##SUF(lbfgs_b200_ctx* c, int64_t n, const T* x, const T* g, T lam, \
+                                                           const T* w, T* d, T* out3)                           \
+    { return do_owlqn_sums<T>(c, n, x, g, lam, w, true, d, out3); }                                            \
+    lbfgs_b200_status lbfgs_b200_owlqn_weighted_update_dir_##SUF(lbfgs_b200_hist* h, const T* x, const T* xp, const T* g, \
+                                                                 const T* gp, T eps, T lam, const T* w, T* d, int* acc, \
+                                                                 T* dg)                                         \
+    { return do_owlqn_update_dir<T>(h, x, xp, g, gp, eps, lam, w, true, d, acc, dg); }
 
 DEFINE_OWLQN(double, f64)
 DEFINE_OWLQN(float, f32)

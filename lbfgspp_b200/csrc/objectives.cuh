@@ -219,4 +219,37 @@ __device__ __forceinline__ void eval_pack_owlqn(const OBJ& obj, int64_t i0, int6
     }
 }
 
+// eval_pack_owlqn under per-coordinate weights w[0..3] of the pack: lam_i = lam * w_i (owlqn_lam_i), the trial coordinates are
+// owlqn_point_w, acc[1] takes sum w_i |x_i|, and `at(j)` returns the neighbour's owlqn_point_w under the neighbour's own weight
+template <class T, class OBJ, class At>
+__device__ __forceinline__ void eval_pack_owlqn_w(const OBJ& obj, int64_t i0, int64_t n, int cnt, const T (&xp)[4], const T (&d)[4],
+                                                  const T (&gp)[4], const T (&w)[4], T step, T lam, At at, T (&x)[4], T (&g)[4], T* acc)
+{
+    T pgp[4], lw[4];
+#pragma unroll
+    for (int k = 0; k < 4; k++)
+    {
+        lw[k] = LBFGSpp::owlqn_lam_i(lam, w[k]);
+        pgp[k] = LBFGSpp::owlqn_pg(xp[k], gp[k], lw[k]);
+        x[k] = (k < cnt) ? (lw[k] > T(0) ? LBFGSpp::owlqn_project(xp[k] + step * d[k], LBFGSpp::owlqn_orthant(xp[k], pgp[k]))
+                                         : xp[k] + step * d[k])
+                         : T(0);
+    }
+    T xl = T(0), xr = T(0);
+    if constexpr (OBJ::kHalo) pack_neighbours<false>(obj, i0, n, step, at, xl, xr);
+    acc[0] += obj.eval(i0, cnt, x, xl, xr, g);
+#pragma unroll
+    for (int k = 0; k < 4; k++)
+    {
+        if (k < cnt)
+        {
+            const T pg = LBFGSpp::owlqn_pg(x[k], g[k], lw[k]);
+            acc[1] += w[k] * (x[k] < T(0) ? -x[k] : x[k]);
+            acc[2] += pgp[k] * (x[k] - xp[k]);
+            acc[3] += pg * pg;
+            acc[4] += x[k] * x[k];
+        }
+    }
+}
+
 }  // namespace lb

@@ -118,11 +118,14 @@ __device__ __forceinline__ Pack<float> lds_pack(const float* p, int)
 // FORM ("update + dots"): forms the newest pair from (x, xp, g, gp) while it computes [S Y]'[g s_new y_new]  (see GramDotsArgs)
 // PG (OWL-QN, FORM only): the right-hand vector is the pseudo-gradient pg(x, g; lam) (LBFGSpp/OWLQNCore.h), formed per element
 // from the staged x and g tiles before they become s and y: [S Y]'[pg s_new y_new], the same HBM traffic as FORM
-template <class T, int ROUNDS, bool FORM, bool PG>
+// W (PG only): per-coordinate weights, lam_i = lam * w[i] (owlqn_lam_i).  w is not staged (a fifth staged vector does not fit the
+// shared memory of three fp64 stages): each element's weight is a plain streaming load by the thread that forms that element's pg.
+template <class T, int ROUNDS, bool FORM, bool PG, bool W = false>
 __device__ __forceinline__ void gram_dots_body(unsigned char* gram_smem, const GramDotsArgs<T>& a, T lam, double* partials, unsigned* ticket,
-                                               double* result, const XComm* xc, unsigned long long epoch)
+                                               double* result, const XComm* xc, unsigned long long epoch, const T* w = nullptr)
 {
     static_assert(FORM || !PG, "the pseudo-gradient is formed from the staged x and g of the FORM variant");
+    static_assert(PG || !W, "weights apply to the pseudo-gradient");
     constexpr int NT = FORM ? 4 : 3;                             // staged vectors per tile: v, s_new, y_new (+ xp while forming)
     T* tiles = reinterpret_cast<T*>(gram_smem);                  // [stage][NT][TE]
     __shared__ __align__(8) uint64_t full_bar[kGramStages];
@@ -186,7 +189,8 @@ __device__ __forceinline__ void gram_dots_body(unsigned char* gram_smem, const G
                     const T gv = ok ? a.v[e0 + i] : T(0);
                     const T sv = ok ? a.fx[e0 + i] - a.fxp[e0 + i] : T(0);
                     const T yv = ok ? gv - a.fgp[e0 + i] : T(0);
-                    if constexpr (PG) dst[i] = ok ? LBFGSpp::owlqn_pg(a.fx[e0 + i], gv, lam) : T(0);
+                    if constexpr (W) dst[i] = ok ? LBFGSpp::owlqn_pg(a.fx[e0 + i], gv, LBFGSpp::owlqn_lam_i(lam, w[e0 + i])) : T(0);
+                    else if constexpr (PG) dst[i] = ok ? LBFGSpp::owlqn_pg(a.fx[e0 + i], gv, lam) : T(0);
                     else dst[i] = gv;
                     dst[kGramTE + i] = sv;
                     dst[2 * kGramTE + i] = yv;
@@ -230,13 +234,15 @@ __device__ __forceinline__ void gram_dots_body(unsigned char* gram_smem, const G
         const int64_t e0f = tile * kGramTE;
         for (int i = tid * 4; i < kGramTE; i += nthreads * 4)
         {
-            Pack<T> ps, py, pp;
+            Pack<T> ps, py, pp, pw;
+            if constexpr (W) pw = ld_pack<Hint::Stream>(w + e0f + i);
 #pragma unroll
             for (int k = 0; k < 4; k++)
             {
                 ps.v[k] = t0[kGramTE + i + k] - t0[3 * kGramTE + i + k];
                 py.v[k] = t0[i + k] - t0[2 * kGramTE + i + k];
-                if constexpr (PG) pp.v[k] = LBFGSpp::owlqn_pg(t0[kGramTE + i + k], t0[i + k], lam);
+                if constexpr (W) pp.v[k] = LBFGSpp::owlqn_pg(t0[kGramTE + i + k], t0[i + k], LBFGSpp::owlqn_lam_i(lam, pw.v[k]));
+                else if constexpr (PG) pp.v[k] = LBFGSpp::owlqn_pg(t0[kGramTE + i + k], t0[i + k], lam);
             }
 #pragma unroll
             for (int k = 0; k < 4; k++)
@@ -408,6 +414,15 @@ __global__ void __launch_bounds__(kGramMaxThreads, 1) k_gram_dots_pg(GramDotsArg
 {
     extern __shared__ __align__(128) unsigned char gram_smem[];
     gram_dots_body<T, ROUNDS, true, true>(gram_smem, a, lam, partials, ticket, result, xc, epoch);
+}
+
+// OWL-QN with per-coordinate weights: k_gram_dots_pg with lam_i = lam * w[i] (w on the alignment of x)
+template <class T, int ROUNDS>
+__global__ void __launch_bounds__(kGramMaxThreads, 1) k_gram_dots_pg_w(GramDotsArgs<T> a, T lam, const T* __restrict__ w, double* partials,
+                                                                       unsigned* ticket, double* result)
+{
+    extern __shared__ __align__(128) unsigned char gram_smem[];
+    gram_dots_body<T, ROUNDS, true, true, true>(gram_smem, a, lam, partials, ticket, result, nullptr, 0ull, w);
 }
 
 // ---- the O(c^2) recursion on coefficients ---------------------------------------------------------------------
@@ -670,6 +685,77 @@ __global__ void __launch_bounds__(kThreads) k_gram_combine_pg(GramCombineArgs<T>
         for (int k = 0; k < 4; k++)
         {
             out.v[k] = LBFGSpp::owlqn_constrain(r[k], pv.v[k]);
+            dot += (k < cnt) ? pv.v[k] * out.v[k] : T(0);
+        }
+        store4<T, Hint::Plain, VEC>(a.res, i0, cnt, out);
+    }
+    if (a.want_dot)
+    {
+        double dacc[1] = {(double)dot};
+        grid_reduce<1>(dacc, rb);
+    }
+}
+
+// OWL-QN with per-coordinate weights: k_gram_combine_pg with lam_i = lam * w[i] (owlqn_lam_i) in pg and in the constraint
+// (owlqn_constrain_w), w read on the packs of x.  A kernel of its own: a shared body moved the registers of k_gram_combine_pg.
+template <class T, bool VEC>
+__global__ void __launch_bounds__(kThreads) k_gram_combine_pg_w(GramCombineArgs<T> a, const T* x, T lam, const T* w, ReduceBuf rb)
+{
+    extern __shared__ __align__(16) unsigned char comb_smem[];
+    T* sm = reinterpret_cast<T*>(comb_smem);
+    const int c = a.solve.c;
+    gram_solve_in_smem<T>(a.solve, sm, blockIdx.x == 0);
+    const T* s_coef = sm + 2 * c * c;
+    __shared__ const T* s_ycol[kMaxM];
+    __shared__ const T* s_scol[kMaxM];
+    for (int j = threadIdx.x; j < c; j += kThreads)
+    {
+        s_ycol[j] = a.Y + (int64_t)a.solve.slots[j] * a.ld;
+        s_scol[j] = a.S + (int64_t)a.solve.slots[j] * a.ld;
+    }
+    __syncthreads();
+    const T cv = s_coef[0];
+    T dot = T(0);
+    const int64_t packs = (a.n + 3) >> 2, stride = (int64_t)gridDim.x * kThreads;
+    for (int64_t p = (int64_t)blockIdx.x * kThreads + threadIdx.x; p < packs; p += stride)
+    {
+        const int64_t i0 = p << 2;
+        const int cnt = (a.n - i0 >= 4) ? 4 : int(a.n - i0);
+        const Pack<T> px = load4<T, Hint::Stream, VEC>(x, i0, cnt);
+        Pack<T> pv = load4<T, Hint::Stream, VEC>(a.v, i0, cnt);
+        const Pack<T> pw = load4<T, Hint::Stream, VEC>(w, i0, cnt);
+        T lw[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++)
+        {
+            lw[k] = LBFGSpp::owlqn_lam_i(lam, pw.v[k]);
+            pv.v[k] = LBFGSpp::owlqn_pg(px.v[k], pv.v[k], lw[k]);
+        }
+        T r[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) r[k] = cv * pv.v[k];
+        // y terms newest -> oldest, then s terms oldest -> newest (the order the recursion would add them)
+#pragma unroll 4
+        for (int j = 0; j < c; j++)
+        {
+            const Pack<T> py = load4<T, Hint::Stream, VEC>(s_ycol[j], i0, cnt);
+            const T cy = s_coef[1 + j];
+#pragma unroll
+            for (int k = 0; k < 4; k++) r[k] += cy * py.v[k];
+        }
+#pragma unroll 4
+        for (int j = c - 1; j >= 0; j--)
+        {
+            const Pack<T> ps = load4<T, Hint::Stream, VEC>(s_scol[j], i0, cnt);
+            const T cs = s_coef[1 + c + j];
+#pragma unroll
+            for (int k = 0; k < 4; k++) r[k] += cs * ps.v[k];
+        }
+        Pack<T> out;
+#pragma unroll
+        for (int k = 0; k < 4; k++)
+        {
+            out.v[k] = LBFGSpp::owlqn_constrain_w(r[k], pv.v[k], lw[k]);
             dot += (k < cnt) ? pv.v[k] * out.v[k] : T(0);
         }
         store4<T, Hint::Plain, VEC>(a.res, i0, cnt, out);

@@ -11,7 +11,11 @@ it nonzero).  Both arms run the same number of iterations (--iters, both must re
              words-per-coordinate model the library records with each span (DESIGN.md §8h)
 Prints one JSON line per workload.
 
-    python tools/owlqn_bench.py [--n N] [--iters K] [--window S] [--reps R]
+--weights unit: the arms are instead OWLQNSolver(param, lam, w = 1) and OWLQNSolver(param, lam), which take the same iteration path
+bit for bit (checked), so the difference is the cost of the weight vector: one more word per coordinate in the trial (6 against 5)
+and in the direction (4c + 11 against 4c + 9).
+
+    python tools/owlqn_bench.py [--n N] [--iters K] [--window S] [--reps R] [--weights unit]
 """
 import argparse
 import ctypes as C
@@ -78,6 +82,7 @@ def main():
     ap.add_argument("--iters", type=int, default=30)
     ap.add_argument("--window", type=float, default=1.0)
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--weights", choices=["unit"], default=None)
     a = ap.parse_args()
     n = a.n
     d0, d1 = tridiag_data(n)
@@ -92,18 +97,25 @@ def main():
     for name, (obj, lam, d0, d1, x0) in work.items():
         prm = lb.LBFGSParam(m=10, epsilon=1e-30, epsilon_rel=0.0, max_iterations=a.iters)
         owl = lb.OWLQNSolver(prm, lam)
-        ref = lb.LBFGSSolver(prm, "Backtracking", resident=False)
-        arms = {"owlqn": lambda: owl.minimize(obj, x0, d0, d1), "lbfgs_lam0": lambda: ref.minimize(obj, x0, d0, d1)}
+        if a.weights:
+            owl_w = lb.OWLQNSolver(prm, lam, weights=np.ones(n))
+            arms = {"owlqn": lambda: owl.minimize(obj, x0, d0, d1), "owlqn_w1": lambda: owl_w.minimize(obj, x0, d0, d1)}
+        else:
+            ref = lb.LBFGSSolver(prm, "Backtracking", resident=False)
+            arms = {"owlqn": lambda: owl.minimize(obj, x0, d0, d1), "lbfgs_lam0": lambda: ref.minimize(obj, x0, d0, d1)}
+        other = "owlqn_w1" if a.weights else "lbfgs_lam0"
         last = {k: run() for k, run in arms.items()}             # warm-up of both arms
+        if a.weights:
+            assert last["owlqn"]["fx"] == last["owlqn_w1"]["fx"] and np.array_equal(last["owlqn"]["x"], last["owlqn_w1"]["x"])
         rates = {k: [] for k in arms}
         for _ in range(a.reps):
             for k, run in arms.items():
                 its, t, last[k] = window(run, a.window)
                 rates[k].append(its / t)
-        assert last["owlqn"]["niter"] == last["lbfgs_lam0"]["niter"] == a.iters, "both arms must run --iters iterations"
+        assert last["owlqn"]["niter"] == last[other]["niter"] == a.iters, "both arms must run --iters iterations"
         phases = {k: profiled(abi, h, run)[0] for k, run in arms.items()}
         print(json.dumps(dict(workload=name, n=n, m=10, lam=lam, card=info, iterations=a.iters, nfev_owlqn=last["owlqn"]["nfev"],
-                              nfev_lbfgs=last["lbfgs_lam0"]["nfev"], nonzeros=int(np.count_nonzero(last["owlqn"]["x"])),
+                              **{"nfev_w1" if a.weights else "nfev_lbfgs": last[other]["nfev"]}, nonzeros=int(np.count_nonzero(last["owlqn"]["x"])),
                               it_s={k: sorted(v) for k, v in rates.items()}, phases=phases)))
 
 
