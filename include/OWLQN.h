@@ -39,31 +39,33 @@
 namespace LBFGSpp {
 
 namespace detail {
+// one function per pass: the weighted entry when w is given, the unweighted one when w is nullptr
 template <class S> struct OwlqnAbi;
 #define LBFGSPP_B200_OWLQNABI(T, SUF)                                                                                                   \
     template <> struct OwlqnAbi<T>                                                                                                      \
     {                                                                                                                                   \
         static lbfgs_b200_status trial(lbfgs_b200_ctx* c, int obj, const T* d0, const T* d1, int64_t n, const T* xp, const T* d,        \
-                                       const T* gp, T step, T lam, T* x, T* g, T* o5)                                                   \
-        { return lbfgs_b200_owlqn_trial_##SUF(c, obj, d0, d1, n, xp, d, gp, step, lam, x, g, o5); }                                     \
-        static lbfgs_b200_status project(lbfgs_b200_ctx* c, int64_t n, const T* xp, const T* d, const T* gp, T step, T lam, T* x, T* o2) \
-        { return lbfgs_b200_owlqn_project_##SUF(c, n, xp, d, gp, step, lam, x, o2); }                                                   \
-        static lbfgs_b200_status sums(lbfgs_b200_ctx* c, int64_t n, const T* x, const T* g, T lam, T* d, T* o3)                         \
-        { return lbfgs_b200_owlqn_sums_##SUF(c, n, x, g, lam, d, o3); }                                                                 \
-        static lbfgs_b200_status update_dir(lbfgs_b200_hist* h, const T* x, const T* xp, const T* g, const T* gp, T eps, T lam, T* d,   \
-                                            int* acc, T* dg)                                                                           \
-        { return lbfgs_b200_owlqn_update_dir_##SUF(h, x, xp, g, gp, eps, lam, d, acc, dg); }                                            \
-        static lbfgs_b200_status trial(lbfgs_b200_ctx* c, int obj, const T* d0, const T* d1, int64_t n, const T* xp, const T* d,        \
                                        const T* gp, T step, T lam, const T* w, T* x, T* g, T* o5)                                       \
-        { return lbfgs_b200_owlqn_weighted_trial_##SUF(c, obj, d0, d1, n, xp, d, gp, step, lam, w, x, g, o5); }                         \
+        {                                                                                                                               \
+            return w ? lbfgs_b200_owlqn_weighted_trial_##SUF(c, obj, d0, d1, n, xp, d, gp, step, lam, w, x, g, o5)                      \
+                     : lbfgs_b200_owlqn_trial_##SUF(c, obj, d0, d1, n, xp, d, gp, step, lam, x, g, o5);                                 \
+        }                                                                                                                               \
         static lbfgs_b200_status project(lbfgs_b200_ctx* c, int64_t n, const T* xp, const T* d, const T* gp, T step, T lam,           \
                                          const T* w, T* x, T* o2)                                                                       \
-        { return lbfgs_b200_owlqn_weighted_project_##SUF(c, n, xp, d, gp, step, lam, w, x, o2); }                                       \
+        {                                                                                                                               \
+            return w ? lbfgs_b200_owlqn_weighted_project_##SUF(c, n, xp, d, gp, step, lam, w, x, o2)                                    \
+                     : lbfgs_b200_owlqn_project_##SUF(c, n, xp, d, gp, step, lam, x, o2);                                               \
+        }                                                                                                                               \
         static lbfgs_b200_status sums(lbfgs_b200_ctx* c, int64_t n, const T* x, const T* g, T lam, const T* w, T* d, T* o3)             \
-        { return lbfgs_b200_owlqn_weighted_sums_##SUF(c, n, x, g, lam, w, d, o3); }                                                     \
+        {                                                                                                                               \
+            return w ? lbfgs_b200_owlqn_weighted_sums_##SUF(c, n, x, g, lam, w, d, o3) : lbfgs_b200_owlqn_sums_##SUF(c, n, x, g, lam, d, o3); \
+        }                                                                                                                               \
         static lbfgs_b200_status update_dir(lbfgs_b200_hist* h, const T* x, const T* xp, const T* g, const T* gp, T eps, T lam,         \
                                             const T* w, T* d, int* acc, T* dg)                                                         \
-        { return lbfgs_b200_owlqn_weighted_update_dir_##SUF(h, x, xp, g, gp, eps, lam, w, d, acc, dg); }                                \
+        {                                                                                                                               \
+            return w ? lbfgs_b200_owlqn_weighted_update_dir_##SUF(h, x, xp, g, gp, eps, lam, w, d, acc, dg)                             \
+                     : lbfgs_b200_owlqn_update_dir_##SUF(h, x, xp, g, gp, eps, lam, d, acc, dg);                                        \
+        }                                                                                                                               \
     };
 LBFGSPP_B200_OWLQNABI(double, f64)
 LBFGSPP_B200_OWLQNABI(float, f32)
@@ -96,13 +98,8 @@ private:
     {
         Device& dev = x.device();
         Scalar o[5];
-        if (m_weights)
-            dev.check(detail::OwlqnAbi<Scalar>::trial(dev.ctx(), f.builtin_kind(), f.builtin_data0(), f.builtin_data1(), x.size(),
-                                                      m_xp.data(), m_drt.data(), m_gradp.data(), step, m_lambda, m_weights->data(), x.data(),
-                                                      m_grad.data(), o));
-        else
-            dev.check(detail::OwlqnAbi<Scalar>::trial(dev.ctx(), f.builtin_kind(), f.builtin_data0(), f.builtin_data1(), x.size(),
-                                                      m_xp.data(), m_drt.data(), m_gradp.data(), step, m_lambda, x.data(), m_grad.data(), o));
+        dev.check(detail::OwlqnAbi<Scalar>::trial(dev.ctx(), f.builtin_kind(), f.builtin_data0(), f.builtin_data1(), x.size(), m_xp.data(),
+                                                  m_drt.data(), m_gradp.data(), step, m_lambda, w(), x.data(), m_grad.data(), o));
         f.add_calls(1);
         return Trial{o[0] + m_lambda * o[1], o[2], o[3], o[4]};
     }
@@ -113,11 +110,7 @@ private:
         Device& dev = x.device();
         const std::ptrdiff_t n = x.size();
         Scalar p[2], s[3];
-        if (m_weights)
-            dev.check(detail::OwlqnAbi<Scalar>::project(dev.ctx(), n, m_xp.data(), m_drt.data(), m_gradp.data(), step, m_lambda,
-                                                        m_weights->data(), x.data(), p));
-        else
-            dev.check(detail::OwlqnAbi<Scalar>::project(dev.ctx(), n, m_xp.data(), m_drt.data(), m_gradp.data(), step, m_lambda, x.data(), p));
+        dev.check(detail::OwlqnAbi<Scalar>::project(dev.ctx(), n, m_xp.data(), m_drt.data(), m_gradp.data(), step, m_lambda, w(), x.data(), p));
         const Scalar fx = f(static_cast<const Vector&>(x), m_grad);
         sums(dev, x, nullptr, s);
         return Trial{fx + m_lambda * p[0], p[1], s[1], s[2]};
@@ -125,11 +118,10 @@ private:
     // {|x|_1 (weighted: sum w_i |x_i|), pg.pg, x.x} at (x, m_grad), and d = -pg when d is given; the weighted entry refuses bad weights
     void sums(Device& dev, const Vector& x, Scalar* d, Scalar* s)
     {
-        if (m_weights)
-            dev.check(detail::OwlqnAbi<Scalar>::sums(dev.ctx(), x.size(), x.data(), m_grad.data(), m_lambda, m_weights->data(), d, s));
-        else
-            dev.check(detail::OwlqnAbi<Scalar>::sums(dev.ctx(), x.size(), x.data(), m_grad.data(), m_lambda, d, s));
+        dev.check(detail::OwlqnAbi<Scalar>::sums(dev.ctx(), x.size(), x.data(), m_grad.data(), m_lambda, w(), d, s));
     }
+    // the weights' device storage, or nullptr when every coordinate weighs 1
+    const Scalar* w() const { return m_weights ? m_weights->data() : nullptr; }
 
 public:
     // lambda: the weight of |x|_1; std::invalid_argument unless it is positive and finite
@@ -205,13 +197,8 @@ public:
                 return k;
 
             int accepted = 0;
-            if (m_weights)
-                dev.check(detail::OwlqnAbi<Scalar>::update_dir(m_bfgs.handle(), x.data(), m_xp.data(), m_grad.data(), m_gradp.data(),
-                                                               std::numeric_limits<Scalar>::epsilon(), m_lambda, m_weights->data(),
-                                                               m_drt.data(), &accepted, &dg));
-            else
-                dev.check(detail::OwlqnAbi<Scalar>::update_dir(m_bfgs.handle(), x.data(), m_xp.data(), m_grad.data(), m_gradp.data(),
-                                                               std::numeric_limits<Scalar>::epsilon(), m_lambda, m_drt.data(), &accepted, &dg));
+            dev.check(detail::OwlqnAbi<Scalar>::update_dir(m_bfgs.handle(), x.data(), m_xp.data(), m_grad.data(), m_gradp.data(),
+                                                           std::numeric_limits<Scalar>::epsilon(), m_lambda, w(), m_drt.data(), &accepted, &dg));
             if (!(dg < Scalar(0))) ls_throw(LSE_NOT_DESCENT);
             step = Scalar(1);
             k++;

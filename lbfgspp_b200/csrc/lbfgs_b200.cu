@@ -255,6 +255,11 @@ __global__ void __launch_bounds__(kThreads) k_trial(OBJ obj, int64_t n, const T*
 // =====================================================================================================
 // OWL-QN (F = f + lam |x|_1; the expressions of LBFGSpp/OWLQNCore.h).  The pseudo-gradient is never stored: each pass forms it from
 // the x and g it reads.
+// Per-coordinate weights (F = f + lam sum_i w_i |x_i|): each pass has a weighted form (the _w kernels) that reads w on the same packs,
+// one more word per coordinate, forms lam_i = lam * w_i (owlqn_lam_i), reports sum w_i |x_i| in place of |x|_1, and leaves the
+// coordinates with lam_i == 0 unprojected and unconstrained (owlqn_point_w, owlqn_constrain_w).  Both forms keep the launch geometry,
+// element ownership and summation order, so w = 1 reproduces the unweighted bits.  The projection, the sums and the pseudo-gradient
+// passes are one body each, compiled without weights (W = false: lam on every coordinate, w never read) and with them.
 // =====================================================================================================
 // fused projected trial for a built-in objective: x = pi(xp + step d; xi(xp, pgp)); g = grad f(x);
 // {f, |x|_1, pgp.(x - xp), pg.pg, x.x}                                                              [R 3 + W 2 (+data)]
@@ -285,69 +290,8 @@ __global__ void __launch_bounds__(kThreads) k_owlqn_trial(OBJ obj, int64_t n, co
     grid_reduce<5>(dacc, rb);
 }
 
-// the projection alone, for any objective: x = pi(xp + step d; xi(xp, pgp)); {|x|_1, pgp.(x - xp)}    [R 3 + W 1]
-template <class T, bool VEC>
-__global__ void __launch_bounds__(kThreads) k_owlqn_project(int64_t n, const T* __restrict__ xp, const T* __restrict__ d,
-                                                            const T* __restrict__ gp, T step, T lam, T* __restrict__ x, ReduceBuf rb)
-{
-    T acc[2] = {T(0), T(0)};
-    const int64_t packs = (n + 3) >> 2, stride = (int64_t)gridDim.x * kThreads;
-#pragma unroll 2
-    for (int64_t p = (int64_t)blockIdx.x * kThreads + threadIdx.x; p < packs; p += stride)
-    {
-        const int64_t i0 = p << 2;
-        const int cnt = (n - i0 >= 4) ? 4 : int(n - i0);
-        const Pack<T> pxp = load4<T, Hint::Stream, VEC>(xp, i0, cnt), pd = load4<T, Hint::Stream, VEC>(d, i0, cnt),
-                      pgp = load4<T, Hint::Stream, VEC>(gp, i0, cnt);
-        Pack<T> px;
-#pragma unroll
-        for (int k = 0; k < 4; k++)
-        {
-            const T pgk = LBFGSpp::owlqn_pg(pxp.v[k], pgp.v[k], lam);
-            px.v[k] = (k < cnt) ? LBFGSpp::owlqn_project(pxp.v[k] + step * pd.v[k], LBFGSpp::owlqn_orthant(pxp.v[k], pgk)) : T(0);
-            acc[0] += px.v[k] < T(0) ? -px.v[k] : px.v[k];
-            acc[1] += pgk * (px.v[k] - pxp.v[k]);
-        }
-        store4<T, Hint::Plain, VEC>(x, i0, cnt, px);
-    }
-    double dacc[2] = {(double)acc[0], (double)acc[1]};
-    grid_reduce<2>(dacc, rb);
-}
-
-// the sums at a point: {|x|_1, pg.pg, x.x}; START also writes the first search's direction d = -pg    [R 2 (+W 1)]
-template <class T, bool START, bool VEC>
-__global__ void __launch_bounds__(kThreads) k_owlqn_sums(int64_t n, const T* __restrict__ x, const T* __restrict__ g, T lam,
-                                                         T* __restrict__ d, ReduceBuf rb)
-{
-    T acc[3] = {T(0), T(0), T(0)};
-    const int64_t packs = (n + 3) >> 2, stride = (int64_t)gridDim.x * kThreads;
-#pragma unroll 2
-    for (int64_t p = (int64_t)blockIdx.x * kThreads + threadIdx.x; p < packs; p += stride)
-    {
-        const int64_t i0 = p << 2;
-        const int cnt = (n - i0 >= 4) ? 4 : int(n - i0);
-        const Pack<T> px = load4<T, Hint::Stream, VEC>(x, i0, cnt), pg = load4<T, Hint::Stream, VEC>(g, i0, cnt);
-        Pack<T> pd;
-#pragma unroll
-        for (int k = 0; k < 4; k++)
-        {
-            const T pgk = LBFGSpp::owlqn_pg(px.v[k], pg.v[k], lam);
-            pd.v[k] = -pgk;
-            acc[0] += px.v[k] < T(0) ? -px.v[k] : px.v[k];
-            acc[1] += pgk * pgk;
-            acc[2] += px.v[k] * px.v[k];
-        }
-        if (START) store4<T, Hint::Plain, VEC>(d, i0, cnt, pd);
-    }
-    double dacc[3] = {(double)acc[0], (double)acc[1], (double)acc[2]};
-    grid_reduce<3>(dacc, rb);
-}
-
-// Per-coordinate weights (F = f + lam sum_i w_i |x_i|): each pass above has a weighted twin that reads w on the same packs (one more
-// word per coordinate), forms lam_i = lam * w_i (owlqn_lam_i), reports sum w_i |x_i| in place of |x|_1, and leaves the coordinates
-// with lam_i == 0 unprojected and unconstrained (owlqn_point_w, owlqn_constrain_w).  The twins keep the launch geometry, element
-// ownership and summation order, so w = 1 reproduces the unweighted bits.  They are kernels of their own: one body behind a weight
-// flag moved the registers of the unweighted kernels (see DESIGN.md, section 8h).
+// The weighted trial is a kernel of its own beside the unweighted one: one body behind the weight flag took the vectorised fp32
+// tridiagonal trial from 5 to 4 CTAs per SM and the vectorised fp64 chained-Rosenbrock weighted trial from 3 to 2 (DESIGN.md, §8h).
 //
 // weighted fused projected trial                                                                   [R 4 + W 2 (+data)]
 template <class T, class OBJ, bool VEC>
@@ -380,11 +324,10 @@ __global__ void __launch_bounds__(kThreads) k_owlqn_trial_w(OBJ obj, int64_t n, 
     grid_reduce<5>(dacc, rb);
 }
 
-// weighted projection: {sum w_i |x_i|, pgp.(x - xp)}                                                 [R 4 + W 1]
-template <class T, bool VEC>
-__global__ void __launch_bounds__(kThreads) k_owlqn_project_w(int64_t n, const T* __restrict__ xp, const T* __restrict__ d,
-                                                              const T* __restrict__ gp, T step, T lam, const T* __restrict__ w,
-                                                              T* __restrict__ x, ReduceBuf rb)
+// the projection alone, for any objective: x = pi(xp + step d; xi(xp, pgp)); {|x|_1, pgp.(x - xp)}    [R 3 (+W 1) + W 1]
+template <class T, bool VEC, bool W>
+__device__ __forceinline__ void owlqn_project_body(int64_t n, const T* xp, const T* d, const T* gp, T step, T lam, const T* w, T* x,
+                                                   const ReduceBuf& rb)
 {
     T acc[2] = {T(0), T(0)};
     const int64_t packs = (n + 3) >> 2, stride = (int64_t)gridDim.x * kThreads;
@@ -394,17 +337,20 @@ __global__ void __launch_bounds__(kThreads) k_owlqn_project_w(int64_t n, const T
         const int64_t i0 = p << 2;
         const int cnt = (n - i0 >= 4) ? 4 : int(n - i0);
         const Pack<T> pxp = load4<T, Hint::Stream, VEC>(xp, i0, cnt), pd = load4<T, Hint::Stream, VEC>(d, i0, cnt),
-                      pgp = load4<T, Hint::Stream, VEC>(gp, i0, cnt), pw = load4<T, Hint::Stream, VEC>(w, i0, cnt);
+                      pgp = load4<T, Hint::Stream, VEC>(gp, i0, cnt);
+        Pack<T> pw;
+        if constexpr (W) pw = load4<T, Hint::Stream, VEC>(w, i0, cnt);
         Pack<T> px;
 #pragma unroll
         for (int k = 0; k < 4; k++)
         {
-            const T lk = LBFGSpp::owlqn_lam_i(lam, pw.v[k]);
+            const T lk = W ? LBFGSpp::owlqn_lam_i(lam, pw.v[k]) : lam;
             const T pgk = LBFGSpp::owlqn_pg(pxp.v[k], pgp.v[k], lk);
-            px.v[k] = (k < cnt) ? (lk > T(0) ? LBFGSpp::owlqn_project(pxp.v[k] + step * pd.v[k], LBFGSpp::owlqn_orthant(pxp.v[k], pgk))
-                                             : pxp.v[k] + step * pd.v[k])
+            px.v[k] = (k < cnt) ? (!W || lk > T(0) ? LBFGSpp::owlqn_project(pxp.v[k] + step * pd.v[k], LBFGSpp::owlqn_orthant(pxp.v[k], pgk))
+                                                   : pxp.v[k] + step * pd.v[k])
                                 : T(0);
-            acc[0] += pw.v[k] * (px.v[k] < T(0) ? -px.v[k] : px.v[k]);
+            const T ax = px.v[k] < T(0) ? -px.v[k] : px.v[k];
+            acc[0] += W ? pw.v[k] * ax : ax;
             acc[1] += pgk * (px.v[k] - pxp.v[k]);
         }
         store4<T, Hint::Plain, VEC>(x, i0, cnt, px);
@@ -412,53 +358,88 @@ __global__ void __launch_bounds__(kThreads) k_owlqn_project_w(int64_t n, const T
     double dacc[2] = {(double)acc[0], (double)acc[1]};
     grid_reduce<2>(dacc, rb);
 }
-
-// weighted sums: {sum w_i |x_i|, pg.pg, x.x, the number of weights owlqn_weight_ok refuses}; START writes d = -pg  [R 3 (+W 1)]
-template <class T, bool START, bool VEC>
-__global__ void __launch_bounds__(kThreads) k_owlqn_sums_w(int64_t n, const T* __restrict__ x, const T* __restrict__ g, T lam,
-                                                           const T* __restrict__ w, T* __restrict__ d, ReduceBuf rb)
+template <class T, bool VEC>
+__global__ void __launch_bounds__(kThreads) k_owlqn_project(int64_t n, const T* __restrict__ xp, const T* __restrict__ d,
+                                                            const T* __restrict__ gp, T step, T lam, T* __restrict__ x, ReduceBuf rb)
 {
-    T acc[4] = {T(0), T(0), T(0), T(0)};
+    owlqn_project_body<T, VEC, false>(n, xp, d, gp, step, lam, nullptr, x, rb);
+}
+template <class T, bool VEC>
+__global__ void __launch_bounds__(kThreads) k_owlqn_project_w(int64_t n, const T* __restrict__ xp, const T* __restrict__ d,
+                                                              const T* __restrict__ gp, T step, T lam, const T* __restrict__ w,
+                                                              T* __restrict__ x, ReduceBuf rb)
+{
+    owlqn_project_body<T, VEC, true>(n, xp, d, gp, step, lam, w, x, rb);
+}
+
+// the sums at a point: {|x|_1, pg.pg, x.x}, with W also the number of weights owlqn_weight_ok refuses; START also writes the first
+// search's direction d = -pg                                                                             [R 2 (+W 1) (+W 1)]
+template <class T, bool START, bool VEC, bool W>
+__device__ __forceinline__ void owlqn_sums_body(int64_t n, const T* x, const T* g, T lam, const T* w,
+                                                T* d, const ReduceBuf& rb)
+{
+    constexpr int NS = W ? 4 : 3;
+    T acc[NS] = {T(0), T(0), T(0)};
     const int64_t packs = (n + 3) >> 2, stride = (int64_t)gridDim.x * kThreads;
 #pragma unroll 2
     for (int64_t p = (int64_t)blockIdx.x * kThreads + threadIdx.x; p < packs; p += stride)
     {
         const int64_t i0 = p << 2;
         const int cnt = (n - i0 >= 4) ? 4 : int(n - i0);
-        const Pack<T> px = load4<T, Hint::Stream, VEC>(x, i0, cnt), pg = load4<T, Hint::Stream, VEC>(g, i0, cnt),
-                      pw = load4<T, Hint::Stream, VEC>(w, i0, cnt);
+        const Pack<T> px = load4<T, Hint::Stream, VEC>(x, i0, cnt), pg = load4<T, Hint::Stream, VEC>(g, i0, cnt);
+        Pack<T> pw;
+        if constexpr (W) pw = load4<T, Hint::Stream, VEC>(w, i0, cnt);
         Pack<T> pd;
 #pragma unroll
         for (int k = 0; k < 4; k++)
         {
-            const T pgk = LBFGSpp::owlqn_pg(px.v[k], pg.v[k], LBFGSpp::owlqn_lam_i(lam, pw.v[k]));
+            const T pgk = LBFGSpp::owlqn_pg(px.v[k], pg.v[k], W ? LBFGSpp::owlqn_lam_i(lam, pw.v[k]) : lam);
             pd.v[k] = -pgk;
-            acc[0] += pw.v[k] * (px.v[k] < T(0) ? -px.v[k] : px.v[k]);
+            const T ax = px.v[k] < T(0) ? -px.v[k] : px.v[k];
+            acc[0] += W ? pw.v[k] * ax : ax;
             acc[1] += pgk * pgk;
             acc[2] += px.v[k] * px.v[k];
-            acc[3] += LBFGSpp::owlqn_weight_ok(lam, pw.v[k]) ? T(0) : T(1);   // the lanes past cnt read w = 0
+            if constexpr (W) acc[3] += LBFGSpp::owlqn_weight_ok(lam, pw.v[k]) ? T(0) : T(1);   // the lanes past cnt read w = 0
         }
         if (START) store4<T, Hint::Plain, VEC>(d, i0, cnt, pd);
     }
-    double dacc[4] = {(double)acc[0], (double)acc[1], (double)acc[2], (double)acc[3]};
-    grid_reduce<4>(dacc, rb);
+    double dacc[NS];
+#pragma unroll
+    for (int k = 0; k < NS; k++) dacc[k] = (double)acc[k];
+    grid_reduce<NS>(dacc, rb);
+}
+template <class T, bool START, bool VEC>
+__global__ void __launch_bounds__(kThreads) k_owlqn_sums(int64_t n, const T* __restrict__ x, const T* __restrict__ g, T lam,
+                                                         T* __restrict__ d, ReduceBuf rb)
+{
+    owlqn_sums_body<T, START, VEC, false>(n, x, g, lam, nullptr, d, rb);
+}
+template <class T, bool START, bool VEC>
+__global__ void __launch_bounds__(kThreads) k_owlqn_sums_w(int64_t n, const T* __restrict__ x, const T* __restrict__ g, T lam,
+                                                           const T* __restrict__ w, T* __restrict__ d, ReduceBuf rb)
+{
+    owlqn_sums_body<T, START, VEC, true>(n, x, g, lam, w, d, rb);
 }
 
-// pg(x, g) into out (the spare ring column), for the dots round that follows a pair the curvature gate refused      [R 2 + W 1]
+// pg(x, g) into out (the spare ring column), for the dots round that follows a pair the curvature gate refused     [R 2 (+W 1) + W 1]
+template <class T, bool W>
+__device__ __forceinline__ void owlqn_pg_body(int64_t n, const T* x, const T* g, T lam, const T* w,
+                                              T* out)
+{
+    const int64_t stride = (int64_t)gridDim.x * kThreads;
+    for (int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x; i < n; i += stride)
+        out[i] = LBFGSpp::owlqn_pg(x[i], g[i], W ? LBFGSpp::owlqn_lam_i(lam, w[i]) : lam);
+}
 template <class T>
 __global__ void __launch_bounds__(kThreads) k_owlqn_pg(int64_t n, const T* __restrict__ x, const T* __restrict__ g, T lam, T* __restrict__ out)
 {
-    const int64_t stride = (int64_t)gridDim.x * kThreads;
-    for (int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x; i < n; i += stride) out[i] = LBFGSpp::owlqn_pg(x[i], g[i], lam);
+    owlqn_pg_body<T, false>(n, x, g, lam, nullptr, out);
 }
-// the same under per-coordinate weights                                                                               [R 3 + W 1]
 template <class T>
 __global__ void __launch_bounds__(kThreads) k_owlqn_pg_w(int64_t n, const T* __restrict__ x, const T* __restrict__ g, T lam,
                                                          const T* __restrict__ w, T* __restrict__ out)
 {
-    const int64_t stride = (int64_t)gridDim.x * kThreads;
-    for (int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x; i < n; i += stride)
-        out[i] = LBFGSpp::owlqn_pg(x[i], g[i], LBFGSpp::owlqn_lam_i(lam, w[i]));
+    owlqn_pg_body<T, true>(n, x, g, lam, w, out);
 }
 
 // =====================================================================================================
@@ -1426,9 +1407,12 @@ static lbfgs_b200_status do_hist_scalars(lbfgs_b200_hist* h, T* theta_host, T* y
 }
 
 // ----------------------------------------------------------------------------- OWL-QN
-// Every entry refuses a lambda that is not positive and finite, and a context with more than one rank (no n-sharding).
-template <class T> static lbfgs_b200_status owlqn_check(lbfgs_b200_ctx* ctx, T lam)
+// Every entry refuses a lambda that is not positive and finite, and a context with more than one rank (no n-sharding).  The weighted
+// entries (`weighted`, named `what`) first refuse a NULL w; past this check w != nullptr selects the weighted kernels.  Only the
+// sums entry reads every weight for validity (its count of refused weights costs no extra pass); the others trust w.
+template <class T> static lbfgs_b200_status owlqn_check(lbfgs_b200_ctx* ctx, T lam, bool weighted, const T* w, const char* what)
 {
+    REQUIRE(ctx, !weighted || w, "%s: NULL weights", what);
     REQUIRE(ctx, lam > T(0) && lam <= std::numeric_limits<T>::max(), "owlqn: lambda must be positive and finite (got %g)", double(lam));
     REQUIRE(ctx, ctx->nranks == 1, "owlqn: one rank only, the vectors cannot be sharded (the context has %d)", ctx->nranks);
     return LBFGS_B200_OK;
@@ -1442,12 +1426,24 @@ template <class T> static lbfgs_b200_status owlqn_receive(lbfgs_b200_ctx* ctx, i
     return LBFGS_B200_OK;
 }
 
-// The weighted entries (w != nullptr) refuse a NULL w, and a w off the alignment x must have.  Only the sums entry reads every
-// weight for validity (its count of refused weights costs no extra pass); the others trust w.
-template <class T> static lbfgs_b200_status owlqn_weights(lbfgs_b200_ctx* ctx, bool weighted, const T* w, const char* what)
+// launch(W, VEC) with the weight and vector-width choices as std::bool_constant: one place turns them into template arguments
+template <class F> static void owlqn_variant(bool weighted, bool vec, F&& launch)
 {
-    REQUIRE(ctx, !weighted || w, "%s: NULL weights", what);
-    return LBFGS_B200_OK;
+    if (weighted)
+    {
+        if (vec) launch(std::true_type{}, std::true_type{});
+        else launch(std::true_type{}, std::false_type{});
+    }
+    else if (vec) launch(std::false_type{}, std::true_type{});
+    else launch(std::false_type{}, std::false_type{});
+}
+
+template <class T, class OBJ, bool W, bool VEC>
+static void launch_owlqn_trial(lbfgs_b200_ctx* ctx, int grid, const ObjGeom<T>& geo, int64_t n, const T* xp, const T* d, const T* gp,
+                               T step, T lam, const T* w, T* x, T* g, const ReduceBuf& rb)
+{
+    if constexpr (W) k_owlqn_trial_w<T, OBJ, VEC><<<grid, kThreads, 0, ctx->stream>>>(OBJ{geo}, n, xp, d, gp, step, lam, w, x, g, rb);
+    else k_owlqn_trial<T, OBJ, VEC><<<grid, kThreads, 0, ctx->stream>>>(OBJ{geo}, n, xp, d, gp, step, lam, x, g, rb);
 }
 
 template <class T>
@@ -1455,29 +1451,29 @@ static lbfgs_b200_status do_owlqn_trial(lbfgs_b200_ctx* ctx, int objective, cons
                                         const T* d, const T* gp, T step, T lam, const T* w, bool weighted, T* x, T* g, T* out5)
 {
     REQUIRE(ctx, ctx && xp && d && gp && x && g && out5 && n >= 1, "owlqn_trial: bad arguments");
-    if (auto st = owlqn_weights<T>(ctx, weighted, w, "owlqn_weighted_trial")) return st;
-    if (auto st = owlqn_check<T>(ctx, lam)) return st;
+    if (auto st = owlqn_check<T>(ctx, lam, weighted, w, "owlqn_weighted_trial")) return st;
     return with_objective<T>(ctx, objective, [&](auto tag) -> lbfgs_b200_status {
         using OBJ = decltype(tag);
         ObjGeom<T> geo;
         if (auto st = objective_geometry<OBJ>(ctx, n, data0, data1, geo)) return st;
-        ProfSpan span(ctx, PH_TRIAL, double(sizeof(T)) * double(n) * ((weighted ? 6.0 : 5.0) + OBJ::kDataVectors));
+        ProfSpan span(ctx, PH_TRIAL, double(sizeof(T)) * double(n) * ((w ? 6.0 : 5.0) + OBJ::kDataVectors));
         const int grid = grid_for(ctx, n, 2);
         const ReduceBuf rb = next_rb(ctx, true);
-        const bool vec = all_aligned<T>({xp, d, gp, x, g}) && (!weighted || all_aligned<T>({w}));
-        if (weighted)
-        {
-            if (vec) k_owlqn_trial_w<T, OBJ, true><<<grid, kThreads, 0, ctx->stream>>>(OBJ{geo}, n, xp, d, gp, step, lam, w, x, g, rb);
-            else k_owlqn_trial_w<T, OBJ, false><<<grid, kThreads, 0, ctx->stream>>>(OBJ{geo}, n, xp, d, gp, step, lam, w, x, g, rb);
-        }
-        else if (vec)
-            k_owlqn_trial<T, OBJ, true><<<grid, kThreads, 0, ctx->stream>>>(OBJ{geo}, n, xp, d, gp, step, lam, x, g, rb);
-        else
-            k_owlqn_trial<T, OBJ, false><<<grid, kThreads, 0, ctx->stream>>>(OBJ{geo}, n, xp, d, gp, step, lam, x, g, rb);
-        if (auto st = post_launch(ctx, weighted ? "k_owlqn_trial_w" : "k_owlqn_trial")) return st;
+        owlqn_variant(w != nullptr, all_aligned<T>({xp, d, gp, x, g, w}), [&](auto W, auto VEC) {
+            launch_owlqn_trial<T, OBJ, W, VEC>(ctx, grid, geo, n, xp, d, gp, step, lam, w, x, g, rb);
+        });
+        if (auto st = post_launch(ctx, w ? "k_owlqn_trial_w" : "k_owlqn_trial")) return st;
         span.stop();
         return owlqn_receive<T>(ctx, 5, out5);
     });
+}
+
+template <class T, bool W, bool VEC>
+static void launch_owlqn_project(lbfgs_b200_ctx* ctx, int grid, int64_t n, const T* xp, const T* d, const T* gp, T step, T lam, const T* w,
+                                 T* x, const ReduceBuf& rb)
+{
+    if constexpr (W) k_owlqn_project_w<T, VEC><<<grid, kThreads, 0, ctx->stream>>>(n, xp, d, gp, step, lam, w, x, rb);
+    else k_owlqn_project<T, VEC><<<grid, kThreads, 0, ctx->stream>>>(n, xp, d, gp, step, lam, x, rb);
 }
 
 template <class T>
@@ -1485,27 +1481,20 @@ static lbfgs_b200_status do_owlqn_project(lbfgs_b200_ctx* ctx, int64_t n, const 
                                           bool weighted, T* x, T* out2)
 {
     REQUIRE(ctx, ctx && xp && d && gp && x && out2 && n >= 1, "owlqn_project: bad arguments");
-    if (auto st = owlqn_weights<T>(ctx, weighted, w, "owlqn_weighted_project")) return st;
-    if (auto st = owlqn_check<T>(ctx, lam)) return st;
+    if (auto st = owlqn_check<T>(ctx, lam, weighted, w, "owlqn_weighted_project")) return st;
     const int grid = grid_for(ctx, n);
     const ReduceBuf rb = next_rb(ctx, true);
-    const bool vec = all_aligned<T>({xp, d, gp, x}) && (!weighted || all_aligned<T>({w}));
-    if (weighted)
-    {
-        if (vec) k_owlqn_project_w<T, true><<<grid, kThreads, 0, ctx->stream>>>(n, xp, d, gp, step, lam, w, x, rb);
-        else k_owlqn_project_w<T, false><<<grid, kThreads, 0, ctx->stream>>>(n, xp, d, gp, step, lam, w, x, rb);
-    }
-    else if (vec) k_owlqn_project<T, true><<<grid, kThreads, 0, ctx->stream>>>(n, xp, d, gp, step, lam, x, rb);
-    else k_owlqn_project<T, false><<<grid, kThreads, 0, ctx->stream>>>(n, xp, d, gp, step, lam, x, rb);
-    if (auto st = post_launch(ctx, weighted ? "k_owlqn_project_w" : "k_owlqn_project")) return st;
+    owlqn_variant(w != nullptr, all_aligned<T>({xp, d, gp, x, w}), [&](auto W, auto VEC) {
+        launch_owlqn_project<T, W, VEC>(ctx, grid, n, xp, d, gp, step, lam, w, x, rb);
+    });
+    if (auto st = post_launch(ctx, w ? "k_owlqn_project_w" : "k_owlqn_project")) return st;
     return owlqn_receive<T>(ctx, 2, out2);
 }
 
-template <class T, bool START, bool VEC>
-static void launch_owlqn_sums(lbfgs_b200_ctx* ctx, int grid, int64_t n, const T* x, const T* g, T lam, const T* w, bool weighted, T* d,
-                              const ReduceBuf& rb)
+template <class T, bool W, bool VEC, bool START>
+static void launch_owlqn_sums(lbfgs_b200_ctx* ctx, int grid, int64_t n, const T* x, const T* g, T lam, const T* w, T* d, const ReduceBuf& rb)
 {
-    if (weighted) k_owlqn_sums_w<T, START, VEC><<<grid, kThreads, 0, ctx->stream>>>(n, x, g, lam, w, d, rb);
+    if constexpr (W) k_owlqn_sums_w<T, START, VEC><<<grid, kThreads, 0, ctx->stream>>>(n, x, g, lam, w, d, rb);
     else k_owlqn_sums<T, START, VEC><<<grid, kThreads, 0, ctx->stream>>>(n, x, g, lam, d, rb);
 }
 
@@ -1516,23 +1505,15 @@ static lbfgs_b200_status do_owlqn_sums(lbfgs_b200_ctx* ctx, int64_t n, const T* 
 {
     REQUIRE(ctx, ctx && x && g && out3 && n >= 1, "owlqn_sums: bad arguments");
     REQUIRE(ctx, d != x && d != g, "owlqn_sums: d aliases x or g");
-    if (auto st = owlqn_weights<T>(ctx, weighted, w, "owlqn_weighted_sums")) return st;
-    if (auto st = owlqn_check<T>(ctx, lam)) return st;
+    if (auto st = owlqn_check<T>(ctx, lam, weighted, w, "owlqn_weighted_sums")) return st;
     const int grid = grid_for(ctx, n);
     const ReduceBuf rb = next_rb(ctx, true);
-    const bool vec = all_aligned<T>({x, g, d}) && (!weighted || all_aligned<T>({w}));
-    if (d)
-    {
-        if (vec) launch_owlqn_sums<T, true, true>(ctx, grid, n, x, g, lam, w, weighted, d, rb);
-        else launch_owlqn_sums<T, true, false>(ctx, grid, n, x, g, lam, w, weighted, d, rb);
-    }
-    else
-    {
-        if (vec) launch_owlqn_sums<T, false, true>(ctx, grid, n, x, g, lam, w, weighted, nullptr, rb);
-        else launch_owlqn_sums<T, false, false>(ctx, grid, n, x, g, lam, w, weighted, nullptr, rb);
-    }
-    if (auto st = post_launch(ctx, weighted ? "k_owlqn_sums_w" : "k_owlqn_sums")) return st;
-    if (!weighted) return owlqn_receive<T>(ctx, 3, out3);
+    owlqn_variant(w != nullptr, all_aligned<T>({x, g, d, w}), [&](auto W, auto VEC) {
+        if (d) launch_owlqn_sums<T, W, VEC, true>(ctx, grid, n, x, g, lam, w, d, rb);
+        else launch_owlqn_sums<T, W, VEC, false>(ctx, grid, n, x, g, lam, w, nullptr, rb);
+    });
+    if (auto st = post_launch(ctx, w ? "k_owlqn_sums_w" : "k_owlqn_sums")) return st;
+    if (!w) return owlqn_receive<T>(ctx, 3, out3);
     if (auto st = receive(ctx, 4)) return st;
     for (int k = 0; k < 3; k++) out3[k] = (T)ctx->h_result[k];
     const double bad = ctx->h_result[3];
@@ -1544,46 +1525,48 @@ static lbfgs_b200_status do_owlqn_sums(lbfgs_b200_ctx* ctx, int64_t n, const T* 
 // pg(x, g; lam) as the right-hand vector.  The pair (s, y) = (x - xp, g - gp) is formed in the dots pass (k_gram_dots_pg); if the
 // curvature gate refuses it, the dots of the kept history are taken again against pg written into the spare ring column.
 // Weighted: k_gram_dots_pg_w / k_gram_combine_pg_w / k_owlqn_pg_w, the same passes with one more word per coordinate each.
-template <class T>
+template <class T, bool W>
 static lbfgs_b200_status launch_gram_dots_pg(lbfgs_b200_ctx* ctx, const GramDotsArgs<T>& a, T lam, const T* w, int rounds, int grid, int threads,
                                              size_t smem)
 {
     const int r = rounds <= 1 ? 1 : rounds == 2 ? 2 : 3;
-    const unsigned bit = 1u << ((w ? 24 : 16) + (sizeof(T) == 8 ? 0 : 4) + r);
-    if (w)
-    {
-        const auto kernel = r == 1 ? k_gram_dots_pg_w<T, 1> : r == 2 ? k_gram_dots_pg_w<T, 2> : k_gram_dots_pg_w<T, 3>;
-        if (!(ctx->smem_optin & bit))
-        {
-            CU(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            ctx->smem_optin |= bit;
-        }
-        kernel<<<grid, threads, smem, ctx->stream>>>(a, lam, w, ctx->gram_partials, ctx->rb.ticket, ctx->gram_raw);
-        return post_launch(ctx, "k_gram_dots_pg_w");
-    }
-    const auto kernel = r == 1 ? k_gram_dots_pg<T, 1> : r == 2 ? k_gram_dots_pg<T, 2> : k_gram_dots_pg<T, 3>;
+    const unsigned bit = 1u << ((W ? 24 : 16) + (sizeof(T) == 8 ? 0 : 4) + r);
+    const auto kernel = [r] {
+        if constexpr (W) return r == 1 ? k_gram_dots_pg_w<T, 1> : r == 2 ? k_gram_dots_pg_w<T, 2> : k_gram_dots_pg_w<T, 3>;
+        else return r == 1 ? k_gram_dots_pg<T, 1> : r == 2 ? k_gram_dots_pg<T, 2> : k_gram_dots_pg<T, 3>;
+    }();
     if (!(ctx->smem_optin & bit))
     {
         CU(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         ctx->smem_optin |= bit;
     }
-    kernel<<<grid, threads, smem, ctx->stream>>>(a, lam, ctx->gram_partials, ctx->rb.ticket, ctx->gram_raw, nullptr, 0ull);
-    return post_launch(ctx, "k_gram_dots_pg");
+    if constexpr (W) kernel<<<grid, threads, smem, ctx->stream>>>(a, lam, w, ctx->gram_partials, ctx->rb.ticket, ctx->gram_raw);
+    else kernel<<<grid, threads, smem, ctx->stream>>>(a, lam, ctx->gram_partials, ctx->rb.ticket, ctx->gram_raw, nullptr, 0ull);
+    return post_launch(ctx, W ? "k_gram_dots_pg_w" : "k_gram_dots_pg");
 }
 
-template <class T, bool VEC>
+template <class T, bool W, bool VEC>
 static lbfgs_b200_status launch_gram_combine_pg(lbfgs_b200_ctx* ctx, const GramCombineArgs<T>& k, const T* x, T lam, const T* w, int grid,
                                                 size_t smem)
 {
-    if (smem > 40 * 1024)
-    {
-        if (w) CU(ctx, cudaFuncSetAttribute(k_gram_combine_pg_w<T, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        else CU(ctx, cudaFuncSetAttribute(k_gram_combine_pg<T, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    }
+    const auto kernel = [] {
+        if constexpr (W) return k_gram_combine_pg_w<T, VEC>;
+        else return k_gram_combine_pg<T, VEC>;
+    }();
+    if (smem > 40 * 1024) CU(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const ReduceBuf rb = next_rb(ctx, true);
-    if (w) k_gram_combine_pg_w<T, VEC><<<grid, kThreads, smem, ctx->stream>>>(k, x, lam, w, rb);
-    else k_gram_combine_pg<T, VEC><<<grid, kThreads, smem, ctx->stream>>>(k, x, lam, rb);
-    return post_launch(ctx, w ? "k_gram_combine_pg_w" : "k_gram_combine_pg");
+    if constexpr (W) kernel<<<grid, kThreads, smem, ctx->stream>>>(k, x, lam, w, rb);
+    else kernel<<<grid, kThreads, smem, ctx->stream>>>(k, x, lam, rb);
+    return post_launch(ctx, W ? "k_gram_combine_pg_w" : "k_gram_combine_pg");
+}
+
+// pg(x, g) into out, for the dots round that follows a refused pair
+template <class T, bool W>
+static lbfgs_b200_status launch_owlqn_pg(lbfgs_b200_ctx* ctx, int64_t n, const T* x, const T* g, T lam, const T* w, T* out)
+{
+    if constexpr (W) k_owlqn_pg_w<T><<<grid_for(ctx, n), kThreads, 0, ctx->stream>>>(n, x, g, lam, w, out);
+    else k_owlqn_pg<T><<<grid_for(ctx, n), kThreads, 0, ctx->stream>>>(n, x, g, lam, out);
+    return post_launch(ctx, W ? "k_owlqn_pg_w" : "k_owlqn_pg");
 }
 
 template <class T>
@@ -1595,13 +1578,12 @@ static lbfgs_b200_status do_owlqn_update_dir(lbfgs_b200_hist* h, const T* x, con
     REQUIRE(ctx, x && xp && g && gp && d && dg_host, "owlqn_update_dir: NULL argument");
     REQUIRE(ctx, d != g && d != x && d != xp && d != gp, "owlqn_update_dir: d aliases an input");
     REQUIRE(ctx, all_aligned<T>({x, xp, g, gp}), "owlqn_update_dir: x, xp, g and gp must start on %zu-byte boundaries", 4 * sizeof(T));
-    if (auto st = owlqn_weights<T>(ctx, weighted, w, "owlqn_weighted_update_dir")) return st;
-    REQUIRE(ctx, !weighted || all_aligned<T>({w}), "owlqn_weighted_update_dir: w must start on a %zu-byte boundary, like x", 4 * sizeof(T));
-    if (auto st = owlqn_check<T>(ctx, lam)) return st;
+    REQUIRE(ctx, all_aligned<T>({w}), "owlqn_weighted_update_dir: w must start on a %zu-byte boundary, like x", 4 * sizeof(T));
+    if (auto st = owlqn_check<T>(ctx, lam, weighted, w, "owlqn_weighted_update_dir")) return st;
     if (h->pending >= 0)
         if (auto st = gram_refresh<T>(h)) return st;
     const int c_new = h->ncorr < h->m ? h->ncorr + 1 : h->m;
-    ProfSpan span(ctx, PH_APPLY_HV, double(sizeof(T)) * double(h->n) * (4.0 * c_new + 3.0 + (weighted ? 9.0 : 7.0)));
+    ProfSpan span(ctx, PH_APPLY_HV, double(sizeof(T)) * double(h->n) * (4.0 * c_new + 3.0 + (w ? 9.0 : 7.0)));
     // the FORM dots of gram_dots(), with pg in place of g
     GramDotsArgs<T> a{};
     a.n = h->n; a.ld = h->ld; a.v = g;
@@ -1619,18 +1601,17 @@ static lbfgs_b200_status do_owlqn_update_dir(lbfgs_b200_hist* h, const T* x, con
     const int rounds = (c_new + a.cols_per_round - 1) / a.cols_per_round;
     const int64_t ntiles = (h->n + kGramTE - 1) / kGramTE;
     const int grid = (int)(ntiles < ctx->sm_count ? ntiles : ctx->sm_count);
-    const T* wk = weighted ? w : nullptr;
-    if (auto st = launch_gram_dots_pg<T>(ctx, a, lam, wk, rounds, grid, a.cols_per_round * split * 32,
-                                         (size_t)kGramStages * 4 * kGramTE * sizeof(T)))
+    const size_t dots_smem = (size_t)kGramStages * 4 * kGramTE * sizeof(T);
+    if (auto st = w ? launch_gram_dots_pg<T, true>(ctx, a, lam, w, rounds, grid, a.cols_per_round * split * 32, dots_smem)
+                    : launch_gram_dots_pg<T, false>(ctx, a, lam, w, rounds, grid, a.cols_per_round * split * 32, dots_smem))
         return st;
     int ok = 0;
     if (auto st = commit_pair<T>(h, eps, 1, &ok, nullptr, ctx->gram_raw + 2)) return st;   // age-0 column: [2] = s'y, [3] = y'y
     if (!ok && h->ncorr > 0)
     {
         T* pg = h->s_col<T>(h->head);   // the refused pair's column is free again
-        if (weighted) k_owlqn_pg_w<T><<<grid_for(ctx, h->n), kThreads, 0, ctx->stream>>>(h->n, x, g, lam, w, pg);
-        else k_owlqn_pg<T><<<grid_for(ctx, h->n), kThreads, 0, ctx->stream>>>(h->n, x, g, lam, pg);
-        if (auto st = post_launch(ctx, weighted ? "k_owlqn_pg_w" : "k_owlqn_pg")) return st;
+        if (auto st = w ? launch_owlqn_pg<T, true>(ctx, h->n, x, g, lam, w, pg) : launch_owlqn_pg<T, false>(ctx, h->n, x, g, lam, w, pg))
+            return st;
         if (auto st = gram_dots<T>(h, pg)) return st;
     }
     // the combination: with no pair kept, H = I / theta and the recursion runs on no columns
@@ -1641,8 +1622,11 @@ static lbfgs_b200_status do_owlqn_update_dir(lbfgs_b200_hist* h, const T* x, con
     k.solve = make_solve_args<T>(h, T(-1), true);
     const int cgrid = grid_for(ctx, h->n, 1);
     const size_t smem = gram_solve_smem_elems(h->ncorr) * sizeof(T);
-    if (all_aligned<T>({d})) { if (auto st = launch_gram_combine_pg<T, true>(ctx, k, x, lam, wk, cgrid, smem)) return st; }
-    else if (auto st = launch_gram_combine_pg<T, false>(ctx, k, x, lam, wk, cgrid, smem)) return st;
+    lbfgs_b200_status st = LBFGS_B200_OK;
+    owlqn_variant(w != nullptr, all_aligned<T>({d}), [&](auto W, auto VEC) {
+        st = launch_gram_combine_pg<T, W, VEC>(ctx, k, x, lam, w, cgrid, smem);
+    });
+    if (st) return st;
     gram_folded(h);
     span.stop();
     if (accepted_host) *accepted_host = ok;

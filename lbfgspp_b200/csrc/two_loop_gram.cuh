@@ -632,11 +632,13 @@ __global__ void __launch_bounds__(kThreads) k_gram_combine(GramCombineArgs<T> a,
 }
 
 // OWL-QN: k_gram_combine with v = pg(x, g; lam) formed per element from x and g = a.v, res = the orthant-constrained combination
-// (owlqn_constrain against pg: d = -H pg projected, with a = -1) and the dot pg.res over the constrained res
-template <class T, bool VEC>
-__global__ void __launch_bounds__(kThreads) k_gram_combine_pg(GramCombineArgs<T> a, const T* x, T lam, ReduceBuf rb)
+// (owlqn_constrain against pg: d = -H pg projected, with a = -1) and the dot pg.res over the constrained res.
+// W (k_gram_combine_pg_w): per-coordinate weights read on the packs of x, lam_i = lam * w[i] (owlqn_lam_i) in pg and in the
+// constraint (owlqn_constrain_w).  Without W, w is not read.
+template <class T, bool VEC, bool W>
+__device__ __forceinline__ void gram_combine_pg_body(unsigned char* comb_smem, const GramCombineArgs<T>& a, const T* x, T lam, const T* w,
+                                                     const ReduceBuf& rb)
 {
-    extern __shared__ __align__(16) unsigned char comb_smem[];
     T* sm = reinterpret_cast<T*>(comb_smem);
     const int c = a.solve.c;
     gram_solve_in_smem<T>(a.solve, sm, blockIdx.x == 0);
@@ -658,77 +660,13 @@ __global__ void __launch_bounds__(kThreads) k_gram_combine_pg(GramCombineArgs<T>
         const int cnt = (a.n - i0 >= 4) ? 4 : int(a.n - i0);
         const Pack<T> px = load4<T, Hint::Stream, VEC>(x, i0, cnt);
         Pack<T> pv = load4<T, Hint::Stream, VEC>(a.v, i0, cnt);
-#pragma unroll
-        for (int k = 0; k < 4; k++) pv.v[k] = LBFGSpp::owlqn_pg(px.v[k], pv.v[k], lam);
-        T r[4];
-#pragma unroll
-        for (int k = 0; k < 4; k++) r[k] = cv * pv.v[k];
-        // y terms newest -> oldest, then s terms oldest -> newest (the order the recursion would add them)
-#pragma unroll 4
-        for (int j = 0; j < c; j++)
-        {
-            const Pack<T> py = load4<T, Hint::Stream, VEC>(s_ycol[j], i0, cnt);
-            const T cy = s_coef[1 + j];
-#pragma unroll
-            for (int k = 0; k < 4; k++) r[k] += cy * py.v[k];
-        }
-#pragma unroll 4
-        for (int j = c - 1; j >= 0; j--)
-        {
-            const Pack<T> ps = load4<T, Hint::Stream, VEC>(s_scol[j], i0, cnt);
-            const T cs = s_coef[1 + c + j];
-#pragma unroll
-            for (int k = 0; k < 4; k++) r[k] += cs * ps.v[k];
-        }
-        Pack<T> out;
-#pragma unroll
-        for (int k = 0; k < 4; k++)
-        {
-            out.v[k] = LBFGSpp::owlqn_constrain(r[k], pv.v[k]);
-            dot += (k < cnt) ? pv.v[k] * out.v[k] : T(0);
-        }
-        store4<T, Hint::Plain, VEC>(a.res, i0, cnt, out);
-    }
-    if (a.want_dot)
-    {
-        double dacc[1] = {(double)dot};
-        grid_reduce<1>(dacc, rb);
-    }
-}
-
-// OWL-QN with per-coordinate weights: k_gram_combine_pg with lam_i = lam * w[i] (owlqn_lam_i) in pg and in the constraint
-// (owlqn_constrain_w), w read on the packs of x.  A kernel of its own: a shared body moved the registers of k_gram_combine_pg.
-template <class T, bool VEC>
-__global__ void __launch_bounds__(kThreads) k_gram_combine_pg_w(GramCombineArgs<T> a, const T* x, T lam, const T* w, ReduceBuf rb)
-{
-    extern __shared__ __align__(16) unsigned char comb_smem[];
-    T* sm = reinterpret_cast<T*>(comb_smem);
-    const int c = a.solve.c;
-    gram_solve_in_smem<T>(a.solve, sm, blockIdx.x == 0);
-    const T* s_coef = sm + 2 * c * c;
-    __shared__ const T* s_ycol[kMaxM];
-    __shared__ const T* s_scol[kMaxM];
-    for (int j = threadIdx.x; j < c; j += kThreads)
-    {
-        s_ycol[j] = a.Y + (int64_t)a.solve.slots[j] * a.ld;
-        s_scol[j] = a.S + (int64_t)a.solve.slots[j] * a.ld;
-    }
-    __syncthreads();
-    const T cv = s_coef[0];
-    T dot = T(0);
-    const int64_t packs = (a.n + 3) >> 2, stride = (int64_t)gridDim.x * kThreads;
-    for (int64_t p = (int64_t)blockIdx.x * kThreads + threadIdx.x; p < packs; p += stride)
-    {
-        const int64_t i0 = p << 2;
-        const int cnt = (a.n - i0 >= 4) ? 4 : int(a.n - i0);
-        const Pack<T> px = load4<T, Hint::Stream, VEC>(x, i0, cnt);
-        Pack<T> pv = load4<T, Hint::Stream, VEC>(a.v, i0, cnt);
-        const Pack<T> pw = load4<T, Hint::Stream, VEC>(w, i0, cnt);
+        Pack<T> pw;
+        if constexpr (W) pw = load4<T, Hint::Stream, VEC>(w, i0, cnt);
         T lw[4];
 #pragma unroll
         for (int k = 0; k < 4; k++)
         {
-            lw[k] = LBFGSpp::owlqn_lam_i(lam, pw.v[k]);
+            lw[k] = W ? LBFGSpp::owlqn_lam_i(lam, pw.v[k]) : lam;
             pv.v[k] = LBFGSpp::owlqn_pg(px.v[k], pv.v[k], lw[k]);
         }
         T r[4];
@@ -755,7 +693,7 @@ __global__ void __launch_bounds__(kThreads) k_gram_combine_pg_w(GramCombineArgs<
 #pragma unroll
         for (int k = 0; k < 4; k++)
         {
-            out.v[k] = LBFGSpp::owlqn_constrain_w(r[k], pv.v[k], lw[k]);
+            out.v[k] = W ? LBFGSpp::owlqn_constrain_w(r[k], pv.v[k], lw[k]) : LBFGSpp::owlqn_constrain(r[k], pv.v[k]);
             dot += (k < cnt) ? pv.v[k] * out.v[k] : T(0);
         }
         store4<T, Hint::Plain, VEC>(a.res, i0, cnt, out);
@@ -765,6 +703,20 @@ __global__ void __launch_bounds__(kThreads) k_gram_combine_pg_w(GramCombineArgs<
         double dacc[1] = {(double)dot};
         grid_reduce<1>(dacc, rb);
     }
+}
+
+template <class T, bool VEC>
+__global__ void __launch_bounds__(kThreads) k_gram_combine_pg(GramCombineArgs<T> a, const T* x, T lam, ReduceBuf rb)
+{
+    extern __shared__ __align__(16) unsigned char comb_smem[];
+    gram_combine_pg_body<T, VEC, false>(comb_smem, a, x, lam, nullptr, rb);
+}
+
+template <class T, bool VEC>
+__global__ void __launch_bounds__(kThreads) k_gram_combine_pg_w(GramCombineArgs<T> a, const T* x, T lam, const T* w, ReduceBuf rb)
+{
+    extern __shared__ __align__(16) unsigned char comb_smem[];
+    gram_combine_pg_body<T, VEC, true>(comb_smem, a, x, lam, w, rb);
 }
 
 }  // namespace lb

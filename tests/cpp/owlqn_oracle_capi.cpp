@@ -1,5 +1,6 @@
-// owlqn_oracle_capi.cpp -- C entry points of the OWL-QN checker (owlqn_oracle.hpp) for the tests, in the result layout of the driver's
-// lbfgsb200_drv_owlqn_* (status, msg, niter, nfev, fx, gnorm).  TEST INFRASTRUCTURE ONLY.
+// owlqn_oracle_capi.cpp -- C entry points of the OWL-QN checker (owlqn_oracle.hpp) for the tests, unweighted (owlqn_oracle_*) and with
+// per-coordinate weights (owlqn_oracle_weighted_*), in the result layout of the driver's lbfgsb200_drv_owlqn_* (status, msg, niter, nfev,
+// fx, gnorm).  TEST INFRASTRUCTURE ONLY.
 #include <cstring>
 #include <stdexcept>
 
@@ -22,7 +23,8 @@ typedef struct
 namespace {
 
 template <class T>
-int run(int objective, const T* d0, const T* d1, long n, const orc_param* p, double lam, int sum_mode, T* x, T* grad, owlqn_oracle_result* out)
+int run(int objective, const T* d0, const T* d1, long n, const orc_param* p, double lam, const T* w, int sum_mode, T* x, T* grad,
+        owlqn_oracle_result* out)
 {
     std::memset(out, 0, sizeof(*out));
     std::vector<T> g(n);
@@ -33,7 +35,7 @@ int run(int objective, const T* d0, const T* d1, long n, const orc_param* p, dou
     };
     try
     {
-        const orc_owlqn::Outcome o = orc_owlqn::minimize<T>(objective, d0, d1, n, *p, T(lam), orc::Blas1<T>(sum_mode, 1), x, g.data(), nfev);
+        const orc_owlqn::Outcome o = orc_owlqn::minimize<T>(objective, d0, d1, n, *p, T(lam), w, orc::Blas1<T>(sum_mode, 1), x, g.data(), nfev);
         out->niter = o.niter;
         out->fx = o.fx;
         out->gnorm = o.gnorm;
@@ -54,12 +56,23 @@ extern "C" {
 int owlqn_oracle_f64(int objective, const double* d0, const double* d1, long n, const orc_param* p, double lam, int sum_mode, double* x,
                      double* grad, owlqn_oracle_result* out)
 {
-    return run<double>(objective, d0, d1, n, p, lam, sum_mode, x, grad, out);
+    return run<double>(objective, d0, d1, n, p, lam, nullptr, sum_mode, x, grad, out);
 }
 int owlqn_oracle_f32(int objective, const float* d0, const float* d1, long n, const orc_param* p, double lam, int sum_mode, float* x,
                      float* grad, owlqn_oracle_result* out)
 {
-    return run<float>(objective, d0, d1, n, p, lam, sum_mode, x, grad, out);
+    return run<float>(objective, d0, d1, n, p, lam, nullptr, sum_mode, x, grad, out);
+}
+// the same with w: n weights
+int owlqn_oracle_weighted_f64(int objective, const double* d0, const double* d1, long n, const orc_param* p, double lam, const double* w,
+                              int sum_mode, double* x, double* grad, owlqn_oracle_result* out)
+{
+    return run<double>(objective, d0, d1, n, p, lam, w, sum_mode, x, grad, out);
+}
+int owlqn_oracle_weighted_f32(int objective, const float* d0, const float* d1, long n, const orc_param* p, double lam, const float* w,
+                              int sum_mode, float* x, float* grad, owlqn_oracle_result* out)
+{
+    return run<float>(objective, d0, d1, n, p, lam, w, sum_mode, x, grad, out);
 }
 
 }  // extern "C"

@@ -1,5 +1,5 @@
 """OWLQNSolver(param, lam, w) (include/OWLQN.h) and the driver's weighted lbfgsb200_drv_owlqn_* on the host-memory test double
-(tests/cpp/mock_abi_owlqn_weighted.cpp) against the weighted C++ checker (tests/cpp/owlqn_oracle_weighted.hpp) bit for bit: seeded runs of the four
+(tests/cpp/mock_abi_owlqn.cpp) against the C++ checker (tests/cpp/owlqn_oracle.hpp) with weights bit for bit: seeded runs of the four
 built-in objectives, both routes, both precisions, under unit, mixed and all-zero weights; unit weights against the unweighted solver;
 and the refusal of bad weights before any trial."""
 import ctypes as C
@@ -18,7 +18,7 @@ from test_owlqn_front_cpu import CASES, CPP, ORC_SUM_SEQUENTIAL
 def weighted_checker(tmp_path_factory):
     """liblbfgs-free build of the weighted C++ checker's entry points (owlqn_oracle_weighted_f64 / _f32), typed"""
     so = str(tmp_path_factory.mktemp("owlqn_oracle_weighted") / "owlqn_oracle_weighted.so")
-    subprocess.run(CXX + ["-fPIC", "-shared", "-o", so, os.path.join(CPP, "owlqn_oracle_weighted_capi.cpp")], check=True)
+    subprocess.run(CXX + ["-fPIC", "-shared", "-o", so, os.path.join(CPP, "owlqn_oracle_capi.cpp")], check=True)
     lib = C.CDLL(so)
     for suf, pt in (("f64", C.POINTER(C.c_double)), ("f32", C.POINTER(C.c_float))):
         getattr(lib, "owlqn_oracle_weighted_" + suf).argtypes = [C.c_int, pt, pt, C.c_long, C.POINTER(lb._DrvParam), C.c_double, pt, C.c_int,
@@ -33,7 +33,7 @@ def checker(tmp_path_factory):
 
 @pytest.fixture(scope="module")
 def front(tmp_path_factory):
-    return driver_on(tmp_path_factory, os.path.join(CPP, "mock_abi_owlqn_weighted.cpp"), "front_on_owlqn_mock_weighted")
+    return driver_on(tmp_path_factory, os.path.join(CPP, "mock_abi_owlqn.cpp"), "front_on_owlqn_mock_weighted")
 
 
 def checker_run_w(lib, obj, x0, lam, w, prm, dtype, d0=None, d1=None, mode=ORC_SUM_SEQUENTIAL):
@@ -139,7 +139,7 @@ def test_bad_weights_refused_before_any_trial(front, checker, plain, dtype):
 def test_front_refuses_weights_of_another_size_or_device(tmp_path_factory):
     """OWLQNSolver(param, lambda, w).minimize() throws std::invalid_argument before any evaluation when w's size or device is not x's."""
     so = str(tmp_path_factory.mktemp("owlqn_wcheck") / "owlqn_wcheck.so")
-    subprocess.run(CXX + DRIVER_FLAGS + ["-o", so] + [os.path.join(CPP, "owlqn_weights_front_check.cpp"), os.path.join(CPP, "mock_abi_owlqn_weighted.cpp"),
+    subprocess.run(CXX + DRIVER_FLAGS + ["-o", so] + [os.path.join(CPP, "owlqn_weights_front_check.cpp"), os.path.join(CPP, "mock_abi_owlqn.cpp"),
                                                      "-pthread"], check=True)
     fn = C.CDLL(so).owlqn_weights_front_check
     fn.argtypes = [C.c_long, C.c_long, C.c_int]
